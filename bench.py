@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the CycleDiffusion hot path on N B200s of one node.
+"""bench.py -- images/sec of the CycleDiffusion hot path on N H100s of one node.
 
 One "step" = one full cycle over one batch of synthetic (image, source-text, target-text) triplets per GPU.  Default workload
 = BASELINE.json configs[1] (the configuration the metric is quoted on):
@@ -18,6 +18,9 @@ buffers (H2D of image / conditioning / noise and D2H of the result inside the ti
 untimed profiling pass (CUDA events around every launch of each kernel family, inside libcdx); `cpu_baseline` times the CPU
 oracle on a bounded sample on rank 0; `fast_path` is the separately reported reduced-precision mode (mma_mode 4) with its
 measured |delta pixel| against the fp32-faithful result of the same short cycle.
+
+`--dump-outputs DIR` writes what the last timed step returned (the decoded images, float32) as DIR/images.npy; inputs, weights and
+noise are all seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -27,6 +30,7 @@ import sys
 import threading
 import time
 
+sys.dont_write_bytecode = True      # the source tree may be read-only: nothing is written there
 ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
@@ -58,11 +62,11 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm_gbs=p['hbm_gbs'], tflops=p['bf16_tflops'], tflops_sustained=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json: copy GB/s, cuBLAS bf16 TF/s)')
-    return dict(hbm_gbs=6650.0, tflops=1590.0, tflops_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_sustained=989.0, source='H100 SXM data sheet (dense bf16, 700 W card; not measured)')
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -124,9 +128,10 @@ def timed(eng, fn, steps, warmup, world, dist):
     torch.cuda.synchronize()
     l0 = eng.launches
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    out = None
     e0.record()
     for _ in range(steps):
-        fn()
+        out = fn()
     e1.record()
     torch.cuda.synchronize()
     if world > 1:
@@ -134,7 +139,7 @@ def timed(eng, fn, steps, warmup, world, dist):
     ms = torch.tensor([e0.elapsed_time(e1)], device=d)
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-    return float(ms.item()), eng.launches - l0
+    return float(ms.item()), eng.launches - l0, out
 
 
 def time_call(fn, reps=3, warm=2):
@@ -173,12 +178,7 @@ def roofline_of(families, pk, value, tflop_per_image, mma_label):
     top = max(tensor_fams, key=lambda k: tensor_fams[k]['ms'])
     f = tensor_fams[top]
     ach = f['flops'] / (f['ms'] * 1e-3) / 1e12
-    traffic = None      # DRAM bytes of one captured launch of this family (ncu --set full; profiles/ncu_traffic.json)
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'ncu_traffic.json')) as fh:
-            traffic = json.load(fh).get(top)
-    except (OSError, ValueError):
-        pass
+    traffic = None      # DRAM bytes per launch: not measured (no hardware-counter profiler on the measuring hosts)
     return {'kernel': top, 'bound': 'tensor', 'achieved': round(ach, 2), 'peak': pk['tflops_sustained'], 'unit': 'TFLOP/s',
             'frac': round(ach / pk['tflops_sustained'], 4),
             # the fp32-faithful path issues 3 fp16 MMAs per product (hi*hi + lo*hi + hi*lo): its own ceiling is peak / 3
@@ -188,8 +188,8 @@ def roofline_of(families, pk, value, tflop_per_image, mma_label):
             'whole_job_tflops': round(value * tflop_per_image, 2)}
 
 
-MMA_LABELS = {None: 'tcgen05 3x fp16-split (fp32-faithful)', 0: 'ffma-fp32', 1: 'tcgen05 3x fp16-split (fp32-faithful)', 2: 'tcgen05 3x fp16-split, unfused attention',
-              3: 'tcgen05 3xTF32 (fp32-faithful, round-1 scheme)', 4: 'tcgen05 1x fp16 (FAST PATH, not fp32-faithful)'}
+MMA_LABELS = {None: 'wgmma 3x fp16-split (fp32-faithful)', 0: 'ffma-fp32', 1: 'wgmma 3x fp16-split (fp32-faithful)', 2: 'wgmma 3x fp16-split, unfused attention',
+              3: 'wgmma 3xTF32 (fp32-faithful, round-1 scheme)', 4: 'wgmma 1x fp16 (FAST PATH, not fp32-faithful)'}
 
 
 # ================================================================================================ our arm
@@ -307,7 +307,8 @@ def run_ours(args):
         src, tgt = nets
         psched = PixelSchedule('ddim', S, S, ETA, 999)
         n_rec = S - 1
-        noise_dev = torch.randn(n_rec + 1, B, 3, RES, RES, device=d)       # resident arm: noise lives in HBM (1.5 GB at B=8)
+        noise_dev = torch.randn(n_rec + 1, B, 3, RES, RES, device=d,       # resident arm: noise lives in HBM (1.5 GB at B=8)
+                                generator=torch.Generator(device=d).manual_seed(7 + rank))
         last_dev = torch.zeros(1, B, 3, RES, RES, device=d)
         img_dev = image.to(d)
 
@@ -335,10 +336,15 @@ def run_ours(args):
 
     clocks = ClockSampler(local)
     clocks.start()
-    ms_total, launches = timed(eng, cycle_resident, args.steps, args.warmup, world, dist)
+    ms_total, launches, last_out = timed(eng, cycle_resident, args.steps, args.warmup, world, dist)
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'images.npy'), last_out.float().cpu().numpy())
+    del last_out
     e2e_steps = max(1, min(args.steps, 2))
-    ms_e2e, _ = timed(eng, cycle_e2e, e2e_steps, 1, world, dist)
+    ms_e2e, _, _ = timed(eng, cycle_e2e, e2e_steps, 1, world, dist)
     value = world * B * args.steps / (ms_total / 1e3)
     e2e_value = world * B * e2e_steps / (ms_e2e / 1e3)
 
@@ -414,12 +420,12 @@ def run_ours(args):
 
     if rank == 0:
         line = {
-            'metric': cfg['metric'] + ' at 1/2/4/8 B200; ms/U-Net-call', 'value': round(value, 4), 'unit': UNIT, 'n_gpus': world, 'steps': args.steps,
+            'metric': cfg['metric'] + ' at 1/2/4/8 H100; ms/U-Net-call', 'value': round(value, 4), 'unit': UNIT, 'n_gpus': world, 'steps': args.steps,
             'warmup': args.warmup, 'ms_per_step': round(ms_total / args.steps, 2), 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
             'dtype': 'fp32', 'data': 'synthetic (images U[0,1], conditioning N(0,1), random-init weights of the named topology)',
             'config': {'workload': cfg['name'], 'global_batch': world * B, 'steps_encode': S, 'steps_decode': S, 'eta': ETA,
                        'parallelism': f'dp{world} (images sharded, one NCCL weight broadcast)', 'mma_mode': MMA_LABELS.get(args.mma, str(args.mma)),
-                       'l2': 'no flush: GBs of weights + >1 GB activations per U-Net call are streamed every call (>> 126 MB L2)',
+                       'l2': 'no flush: GBs of weights + >1 GB activations per U-Net call are streamed every call (>> 50 MB L2)',
                        'loop': ('lock-step: one U-Net call per step on [source | target uncond | target cond] (3B samples), recovered noise '
                                 'consumed in the same step' if latent else 'two-phase: source-model encode, target-model decode'),
                        'unet_calls_per_step': (S if latent else 2 * S - 1), 'unet_ms': unet_ms, 'stage_ms_two_phase': stage_ms,
@@ -528,7 +534,7 @@ def run_reference(args):
     v = sum(x['value'] for x in vals) / len(vals)
     cpu = dict(vals[-1])
     cpu['value'] = round(v, 6)
-    line = {'impl': 'reference', 'metric': cfg['metric'] + ' at 1/2/4/8 B200; ms/U-Net-call', 'value': round(v, 6), 'unit': UNIT, 'n_gpus': args.gpus,
+    line = {'impl': 'reference', 'metric': cfg['metric'] + ' at 1/2/4/8 H100; ms/U-Net-call', 'value': round(v, 6), 'unit': UNIT, 'n_gpus': args.gpus,
             'steps': len(vals), 'warmup': args.warmup, 'ms_per_step': round(1e3 * cfg['B'] / v, 1), 'higher_is_better': True, 'scaling': 'weak',
             'vs_baseline': None, 'dtype': 'fp32', 'data': 'synthetic',
             'config': {'workload': cfg['name'] + ' -- CPU path on a bounded sample',
@@ -544,9 +550,10 @@ def build_parser():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--config', type=int, default=2, choices=[2, 4, 5], help='BASELINE.json configuration (2 = configs[1], the headline)')
-    ap.add_argument('--mma', type=int, default=None, help='0 FFMA fp32, 1 tcgen05 fp16-split (default), 3 tcgen05 3xTF32, 4 fast path')
+    ap.add_argument('--mma', type=int, default=None, help='0 FFMA fp32, 1 wgmma fp16-split (default), 3 wgmma 3xTF32, 4 fast path')
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-fast', action='store_true', help='skip the fast-path probe')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the last timed step\'s images to DIR/images.npy (float32)')
     return ap
 
 

@@ -1,7 +1,7 @@
-"""In-tree build of libcdx.so (nvcc, sm_100a only).  Used by __graft_entry__.build() and by the tests.
+"""In-tree build of libcdx.so (nvcc, sm_90a only).  Used by __graft_entry__.build() and by the tests.
 
-The shared library lands next to this file (cycle_diffusion_b200/libcdx.so) so that it travels to the
-GPU box with the repo snapshot; it is git-ignored.
+The shared library lands next to this file (cycle_diffusion_b200/libcdx.so), so the package imports from the source
+tree; it is git-ignored.
 """
 import hashlib
 import os
@@ -13,8 +13,9 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libcdx.so')
 STAMP = os.path.join(HERE, '.libcdx.stamp')
 
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']      # H100 (Hopper): wgmma / TMA / setmaxnreg need the 'a' target
 SOURCES = ['engine.cu', 'kernels_gemm.cu', 'kernels_tc.cu', 'kernels_attn.cu', 'kernels_norm.cu', 'kernels_elem.cu', 'nets.cu', 'cabi.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '--use_fast_math=false',
+NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17', '--use_fast_math=false',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-O2', '--expt-relaxed-constexpr', '-Xptxas', '-v']
 
 
@@ -37,7 +38,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into libcdx.so (object files under build/). Returns the path."""
+    """Compile every CUDA source for sm_90a into libcdx.so (object files under build/). Returns the path."""
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(STAMP) and open(STAMP).read().strip() == dig:
         return LIB
@@ -64,7 +65,7 @@ def build(force=False, verbose=False):
         errs = [l for l in '\n'.join(log).splitlines() if 'error' in l.lower()]
         sys.stderr.write('\n'.join(errs[:40]) + '\n')
         raise RuntimeError('nvcc failed; see cycle_diffusion_b200/build/build.log')
-    link = [_nvcc(), '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart_static', '-lpthread', '-ldl', '-lrt']
+    link = [_nvcc(), '-shared', '-o', LIB] + objs + ARCH + ['-lcudart_static', '-lpthread', '-ldl', '-lrt']
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -113,7 +113,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f'{LIB_PATH} is missing: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-            f'(nvcc, sm_100a).  The engine has no CPU fallback.')
+            f'(nvcc, sm_90a).  The engine has no CPU fallback.')
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)      # AttributeError here = header / library mismatch

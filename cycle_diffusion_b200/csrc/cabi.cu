@@ -237,6 +237,9 @@ int cdx_engine_create(int device, cdx_engine** out) {
     CDX_CUDA(cudaGetDeviceProperties(&prop, device));
     cdx_engine* eng = new cdx_engine();
     eng->e.device = device;
+    if (prop.major != 9 || prop.minor != 0)
+      throw Error(CDX_E_CUDA, "libcdx is built for sm_90a (H100) only; device " + std::to_string(device) + " is sm_" +
+                                  std::to_string(prop.major) + std::to_string(prop.minor));
     eng->e.num_sms = prop.multiProcessorCount;
     *out = eng;
   });
@@ -255,7 +258,7 @@ uint64_t cdx_engine_launch_count(const cdx_engine* e) { return e ? e->e.launches
 int cdx_engine_set_mma_mode(cdx_engine* e, int mode) {
   return guard([&] {
     CDX_CHECK(e != nullptr && mode >= 0 && mode <= 5, "set_mma_mode: bad arguments");
-    e->e.mma_mode = mode == 0 ? 0 : 1;       // 2 = tcgen05 contractions but unfused attention (A/B comparisons)
+    e->e.mma_mode = mode == 0 ? 0 : 1;       // 2 = tensor-core contractions but unfused attention (A/B comparisons)
     e->e.flash_attn = mode != 2 && mode != 0;
     e->e.tc_kind = mode == 3 ? 0 : mode == 4 ? 2 : 1;    // 3 = 3xTF32 contractions, 4 = single-term fp16 (fast path), else fp16 split
   });

@@ -71,10 +71,10 @@ struct Profiler {
 struct Engine {
   Profiler prof;
   int device = 0;
-  int num_sms = 148;
-  bool flash_attn = true;        // fused tcgen05 attention kernel (kernels_attn.cu); false -> unfused QK^T / softmax / PV
-  int mma_mode = 1;              // 0 SIMT FFMA (exact fp32), 1 tcgen05
-  int tc_kind = 1;               // tcgen05 product scheme: 0 3xTF32, 1 3x fp16-split at the kind::f16 rate (default), 2 1x fp16 (fast, not fp32-faithful)
+  int num_sms = 132;
+  bool flash_attn = true;        // fused wgmma attention kernel (kernels_attn.cu); false -> unfused QK^T / softmax / PV
+  int mma_mode = 1;              // 0 SIMT FFMA (exact fp32), 1 tensor cores (wgmma)
+  int tc_kind = 1;               // tensor-core product scheme: 0 3xTF32, 1 3x fp16-split at the f16 rate (default), 2 1x fp16 (fast, not fp32-faithful)
   // tracked |max| scalars of activation tensors (operand range of the fp16-split GEMMs): a pool of device floats, handed out
   // per tensor by the graph executors and zeroed at the start of every network call
   float* amax_pool = nullptr;
@@ -127,7 +127,7 @@ inline Tensor alloc_tensor(Engine& e, int B, int H, int W, int C) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// dense contraction (implicit GEMM) arguments, shared by the SIMT and tcgen05 back ends
+// dense contraction (implicit GEMM) arguments, shared by the SIMT and wgmma back ends
 //   C[m,n] = alpha * sum_k A(m,k) * W(n,k)  (+ bias[n]) (+ rowvec[m / rows_per_batch, n]) (+ residual[m,n])
 // A is either a dense row matrix (two channel-concatenated sources allowed) or the implicit im2col of
 // a 3x3 convolution over an NHWC tensor (k = tap*Cin + c).
@@ -152,7 +152,7 @@ struct GemmArgs {
   const float* gn_ab = nullptr; int gn_silu = 0;
   double* c_stats = nullptr;         // optional: += per-(image, channel) {sum, sum sq} of C (rows_per_batch rows per image), zeroed by the caller
   float* Cout = nullptr; int ldc = 0;
-  float* Cout_lo = nullptr;           // if set: Cout receives rn_tf32(C) and Cout_lo rn_tf32(C - hi) (operand planes for tcgen05)
+  float* Cout_lo = nullptr;           // if set: Cout receives rn_tf32(C) and Cout_lo rn_tf32(C - hi) (operand planes for the tensor-core kernels)
   // optional: columns n >= t_col0 are stored TRANSPOSED as TF32 planes, Ct_hi / Ct_lo [(n - t_col0) * ldt + m] (dense mode,
   // no split-K): the value projection of a fused q|k|v GEMM lands directly as the K-major V^T operand of the attention kernel
   float* Ct_hi = nullptr; float* Ct_lo = nullptr; int t_col0 = 0; long long ldt = 0;
@@ -168,7 +168,7 @@ struct GemmArgs {
   long long sA_b = 0, sA_h = 0, sB_b = 0, sB_h = 0, sC_b = 0, sC_h = 0;
 };
 void gemm(Engine& e, const GemmArgs& a, cudaStream_t s);
-// tcgen05 back end (kernels_tc.cu); returns false when the shape is not eligible
+// wgmma back end (kernels_tc.cu); returns false when the shape is not eligible
 bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done = nullptr);   // side_done bit 0: c_amax fused, bit 1: c_stats fused
 bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
                         const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int heads, int d,

@@ -1,4 +1,4 @@
-// kernels_attn.cu -- fused self- / cross-attention on tcgen05 (flash-style, fp32-faithful three-term products).
+// kernels_attn.cu -- fused self- / cross-attention on sm_90a wgmma (flash-style, fp32-faithful three-term products).
 //
 //   out[b, q, h*d + c] = sum_j softmax_j( scale * <Q[b,q,h,:], K[b,j,h,:]> ) * V[b,j,h,c]
 // replaces CrossAttention.forward's two einsums + softmax (ldm/modules/attention.py:178-192), which materialise a
@@ -6,23 +6,16 @@
 //
 // Inputs are hi / lo planes of q, k [rows, ld] and of the transposed values V^T [C, B*N] (see nets.cu), so every operand tile arrives
 // by TMA ready for the tensor core.  Default (F16): fp16 planes of x * 2^e, e from the tensor's tracked range (split_rows_h16 /
-// split_transpose_h16 at the end of this file), three kind::f16 MMAs per 16-wide K step; F16 = false: TF32 planes (rn_tf32(x),
-// rn_tf32(x - hi)) written by the projection's epilogue, three kind::tf32 per 8-wide step (the round-1 scheme, --mma 3).
+// split_transpose_h16 at the end of this file), three wgmma .f16 per 16-wide K step; F16 = false: TF32 planes (rn_tf32(x),
+// rn_tf32(x - hi)) written by the projection's epilogue, three wgmma .tf32 per 8-wide step (--mma 3).
 //
-// One CTA = 128 queries of one (batch, head); keys are walked in blocks of 64.  128 + 32 * 4 * NSUB threads (640 for d <= 40):
-//   warp 0    TMA producer: Q planes once (through a staging buffer that aliases the last K stage), then K and V^T hi+lo tiles into
-//             3-4 deep rings.
-//   warp 1    MMA issuer of the Q.K^T stream: S_j = Q K_j^T as TS-mode MMAs (Q hi/lo live in TMEM, K tiles in smem):
-//             lo*hi + hi*lo + hi*hi, M=128, N=64, K=d.
-//   warps 2-3 MMA issuers of the P.V stream (even / odd key blocks when there are two P/O buffers): O_j = P_j V_j with P hi/lo in
-//             TMEM and V^T tiles in smem, M=128, N=round16(d), K=64, written FRESH into TMEM for every key block.
-//   warps 4.. softmax + accumulation, NSUB threads per query row (64/NSUB key columns and 1/NSUB of the O columns each; the row max
-//             is exchanged through smem; a first profile showed 4 softmax warps issue-bound at 30 % tensor activity):
-//             tcgen05.ld S -> online max / exp2 / row sum in registers -> split P into hi/lo (F16: fp16(p * 2^10) pairs) ->
-//             tcgen05.st into TMEM; O_total = O_total * corr + O_j with round-to-nearest fp32 adds in registers (the tensor core's
-//             accumulation truncates, see kernels_tc.cu; accumulating per block in registers also makes the online-softmax rescale
-//             free).  Final O / l -> global.
-// TMEM columns (<= 512): [S x SB][P hi|lo x PB][O x PB][Q_hi][Q_lo], see ACfg.
+// One CTA = 128 queries of one (batch, head); keys are walked in blocks of 64.  384 threads = 3 warpgroups:
+//   warpgroup 0     TMA producer (one thread): Q planes once, then K and V^T hi+lo tiles into KS / VS deep rings.
+//   warpgroups 1-2  64 query rows each: S_j = Q K_j^T (lo*hi + hi*lo + hi*hi, both operands from smem, m64n64) -> online max / exp2 /
+//                   row sum in registers -> P split into hi / lo in registers (the accumulator layout of S is the A-fragment layout
+//                   of the next wgmma; F16: fp16(p * 2^10)) -> O_j = P_j V_j (m64nNV, V^T tiles from smem) written fresh per block ->
+//                   O_total = O_total * corr + O_j with round-to-nearest fp32 adds (the tensor core's accumulation truncates, see
+//                   kernels_tc.cu; accumulating per block in registers also makes the online-softmax rescale free).  Final O / l -> global.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -34,53 +27,32 @@ using namespace tc;
 
 constexpr int AQ = 128;        // queries per CTA
 constexpr int AKV = 64;        // keys per block
+constexpr int ATHREADS = 384;
 
-// F16: operands are fp16 hi / lo planes (x * 2^e split as in kernels_tc.cu's MODE_H16) and the three product terms run as
-// kind::f16 MMAs (K = 16 per instruction): half the tensor-pipe time and half the operand bytes of the TF32 planes.  P is split as
+// F16: operands are fp16 hi / lo planes (x * 2^e split as in kernels_tc.cu's KIND_H16) and the three product terms run as
+// wgmma .f16 (K = 16 per instruction): half the tensor-pipe time and half the operand bytes of the TF32 planes.  P is split as
 // fp16(p * 2^10): the scale keeps the lo term out of fp16's subnormal range and cancels in O / l.
 template <int D, bool F16>
 struct ACfg {
-  // softmax warps per TMEM lane quadrant (each takes AKV / NSUB score columns and NV / NSUB output columns of its 32 rows):
-  // 4 (16 softmax warps) hides the tcgen05.ld / MUFU / barrier latencies of the softmax chain better than 2 (a profile of the
-  // 2-per-quadrant version had the tensor pipe 50 % active with 36 % issue utilisation); D >= 64 has no smem left for the wider
-  // max exchange and keeps 2
-  static constexpr int NSUB = (D <= 40) ? 4 : 2;
-  static constexpr int THREADS = 128 + 4 * NSUB * 32;       // TMA warp, three MMA issuer warps (QK, PV even / odd blocks), softmax warps
-  static constexpr int KD = F16 ? (D + 15) / 16 * 16 : D;    // head dim as the QK MMAs see it (F16: zero-padded to K = 16 steps by the TMA fill)
+  static constexpr int KD = F16 ? (D + 15) / 16 * 16 : D;    // head dim as the QK products see it (F16: zero-padded to K = 16 steps by the TMA fill)
   static constexpr int KW = F16 ? 64 : 32;                  // elements per 128-byte k-block row
   static constexpr int KB2 = (D + KW - 1) / KW;             // 128-byte k-blocks covering the head dim
-  static constexpr int NG = F16 ? KD / 16 : D / 8;          // 8-column TMEM groups of a Q plane == MMA K steps of Q.K^T
-  static constexpr int QC = F16 ? KD / 2 : D;               // TMEM columns of one Q plane
-  static constexpr int PW = F16 ? AKV / 2 : AKV;            // TMEM columns of one P plane
-  static constexpr int NV = (D + 15) / 16 * 16;             // PV MMA N (rows of the V^T tile)
+  static constexpr int NG = F16 ? KD / 16 : D / 8;          // K steps of Q.K^T (4 per 128-byte k-block)
+  static constexpr int NV = (D + 15) / 16 * 16;             // PV N (rows of the V^T tile)
   static constexpr int KTILE = AKV * 128;                   // one k-block tile of K: 64 rows x 128 B
   static constexpr int K_STAGE = 2 * KB2 * KTILE;           // hi + lo
   static constexpr int VTILE = NV * 128;                    // one 128-byte block of V^T (32 keys; F16: 64 keys): NV rows x 128 B
   static constexpr int V_STAGE = (F16 ? 1 : 2) * 2 * VTILE; // (key sub-blocks) x (hi + lo)
-  static constexpr int Q_STAGE = KB2 * AQ * 128;            // one plane of Q (== K_STAGE)
-  // ring depths: the prefetch distance must cover the TMA latency (a first profile with 2-deep rings had the MMA thread
-  // spinning on k_full); the Q staging buffer is the LAST K stage, which is first needed KS-1 blocks into the loop
-  static constexpr int KS = (D <= 64) ? 4 : 3;
-  static constexpr int VS = (D <= 64) ? 3 : 2;
-  static constexpr int OFF_K = 0;
-  static constexpr int OFF_V = KS * K_STAGE;
-  static constexpr int OFF_Q = (KS - 1) * K_STAGE;
+  static constexpr int Q_PLANE = KB2 * AQ * 128;            // one plane of Q
+  // ring depth 2 where shared memory allows (TF32 at d = 80 has room for one K and one V stage only)
+  static constexpr int RING = (2 * Q_PLANE + 2 * (K_STAGE + V_STAGE) + 2048 <= 232448) ? 2 : 1;
+  static constexpr int KS = RING, VS = RING;
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = 2 * Q_PLANE;
+  static constexpr int OFF_V = OFF_K + KS * K_STAGE;
   static constexpr int OFF_BAR = OFF_V + VS * V_STAGE;
-  static_assert(Q_STAGE == K_STAGE, "Q staging aliases a K stage");
-  static constexpr int OFF_XCHG = OFF_BAR + 256;            // float xchg[2 buffers][NSUB parts][128 rows]
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 2 * NSUB * 512 + 512;   // 512 B slack: the dynamic window is declared __align__(1024)
-  // TMEM buffering.  D <= 40 (the N=4096 level, ~90 % of the attention work): ONE score buffer but TWO P and O buffers, so
-  // P_{j+1} is written without waiting for PV_j and the O accumulation of block j leaves the critical path (a profile of the
-  // (2 S, 1 P, 1 O) scheme showed the softmax warps 47 % stalled on s_full / pv_done with the tensor pipe 30 % active).
-  // Larger head dims do not have the TMEM columns for that and keep (2 S, 1 P, 1 O).
-  static constexpr int SB = (D <= 40) ? 1 : 2;
-  static constexpr int PB = (D <= 40) ? 2 : 1;            // P buffers == O buffers
-  static constexpr int COL_S = 0;
-  static constexpr int COL_P = SB * AKV;                    // buffer b: hi at COL_P + b*2*PW, lo at + PW
-  static constexpr int COL_O = COL_P + PB * 2 * PW;         // buffer b at COL_O + b*NV
-  static constexpr int COL_QH = COL_O + PB * NV, COL_QL = COL_QH + QC;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;   // 1 KB slack: the tiles are placed at the next 1024-byte boundary
   static_assert(D % 8 == 0 && D >= 16 && D <= 80, "head dim must be a multiple of 8 in [16, 80]");
-  static_assert(COL_QL + QC <= 512, "TMEM overflow");
   static_assert(SMEM_BYTES <= 232448, "smem overflow");
   static_assert(NV % 16 == 0, "NV");
 };
@@ -92,419 +64,245 @@ struct AttnParams {
   const float *q_amax, *k_amax, *v_amax;   // F16: tracked max |q|, |k|, |v| (the planes hold x * 2^h16_exp_of(amax))
 };
 
-#define TMEM_LD(NUM, ...) asm volatile("tcgen05.ld.sync.aligned.32x32b.x" #NUM ".b32 " __VA_ARGS__)
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                 "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
+__device__ __forceinline__ void split_h16_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __half2 hh = __floats2half2_rn(x0, x1);          // .x (low half) = even key
+  const float2 hf2 = __half22float2(hh);
+  const __half2 ll = __floats2half2_rn(x0 - hf2.x, x1 - hf2.y);
+  hi = *reinterpret_cast<const uint32_t*>(&hh);
+  lo = *reinterpret_cast<const uint32_t*>(&ll);
+}
+
 template <int D, bool F16>
-__global__ void __launch_bounds__(ACfg<D, F16>::THREADS, 1)
+__global__ void __launch_bounds__(ATHREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_constant__ CUtensorMap mapQl,
                   const __grid_constant__ CUtensorMap mapKh, const __grid_constant__ CUtensorMap mapKl,
                   const __grid_constant__ CUtensorMap mapVh, const __grid_constant__ CUtensorMap mapVl, const AttnParams p) {
   using C = ACfg<D, F16>;
-  constexpr int KB2 = C::KB2, NV = C::NV, NSUB = C::NSUB, KW = C::KW, PW = C::PW;
+  constexpr int KB2 = C::KB2, NV = C::NV, KW = C::KW, KS = C::KS, VS = C::VS;
+  constexpr int NO = NV / 2;                       // O accumulators per thread (m64nNV)
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bars = base + C::OFF_BAR;
-  // barriers (8 B each)
-  const uint32_t bar_q_full = bars + 0;          // TMA: a Q plane landed in the staging buffer (2 phases)
-  const uint32_t bar_q_free = bars + 8;          // softmax warps: staging buffer consumed (plane 0)
-  const uint32_t bar_q_ready = bars + 16;        // softmax warps: Q hi/lo complete in TMEM
-  constexpr int KS = C::KS, VS = C::VS;
-  auto bar_k_full = [&](int s) { return bars + 24u + 8u * s; };      // 4 slots
-  auto bar_k_empty = [&](int s) { return bars + 56u + 8u * s; };     // 4 slots
-  auto bar_v_full = [&](int s) { return bars + 88u + 8u * s; };      // 3 slots
-  auto bar_v_empty = [&](int s) { return bars + 112u + 8u * s; };    // 3 slots
-  auto bar_s_full = [&](int s) { return bars + 136u + 8u * s; };
-  auto bar_s_empty = [&](int s) { return bars + 152u + 8u * s; };
-  auto bar_p_full = [&](int s) { return bars + 168u + 8u * s; };
-  auto bar_pv_done = [&](int s) { return bars + 184u + 8u * s; };
-  auto bar_o_empty = [&](int s) { return bars + 200u + 8u * s; };
-  const uint32_t tmem_slot = bars + 216;
-  constexpr int SB = C::SB, PB = C::PB;
+  const uint32_t bar_q_full = bars;
+  auto bar_k_full = [&](int s) { return bars + 8u + 8u * s; };
+  auto bar_k_empty = [&](int s) { return bars + 24u + 8u * s; };
+  auto bar_v_full = [&](int s) { return bars + 40u + 8u * s; };
+  auto bar_v_empty = [&](int s) { return bars + 56u + 8u * s; };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AQ, h = blockIdx.y, b = blockIdx.z;
   const int nb = (p.Nk + AKV - 1) / AKV;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(bar_q_full, 1);
-    mbar_init(bar_q_free, 4);
-    mbar_init(bar_q_ready, 4);
-    for (int s = 0; s < KS; ++s) {
-      mbar_init(bar_k_full(s), 1);
-      mbar_init(bar_k_empty(s), 1);
-    }
-    for (int s = 0; s < VS; ++s) {
-      mbar_init(bar_v_full(s), 1);
-      mbar_init(bar_v_empty(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_s_full(s), 1);
-      mbar_init(bar_s_empty(s), 4 * NSUB);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_p_full(s), 4 * NSUB);
-      mbar_init(bar_pv_done(s), 1);
-      mbar_init(bar_o_empty(s), 4 * NSUB);
-    }
+    for (int s = 0; s < KS; ++s) { mbar_init(bar_k_full(s), 1); mbar_init(bar_k_empty(s), 8); }
+    for (int s = 0; s < VS; ++s) { mbar_init(bar_v_full(s), 1); mbar_init(bar_v_empty(s), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  pdl_wait();                     // everything above touched shared memory / TMEM only
+  pdl_wait();                     // everything above touched shared memory only
 
-  if (warp == 0) {
-    // =========================================================================== TMA producer (whole warp, elected issue)
-    {
+  if (warp < 4) {
+    // =========================================================================== TMA producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       const uint32_t sq = base + C::OFF_Q;
-      // Q: hi plane, then (after the softmax warps moved it to TMEM) lo plane through the same staging buffer
-      if (elect_one()) {
-        mbar_expect_tx(bar_q_full, C::Q_STAGE);
-        for (int kb = 0; kb < KB2; ++kb) tma_load_4d(sq + kb * AQ * 128, &mapQh, kb * KW, h, q0, b, bar_q_full);
-      }
-      mbar_wait(bar_q_free, 0);
-      if (elect_one()) {
-        mbar_expect_tx(bar_q_full, C::Q_STAGE);
-        for (int kb = 0; kb < KB2; ++kb) tma_load_4d(sq + kb * AQ * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
+      mbar_expect_tx(bar_q_full, 2 * C::Q_PLANE);
+      for (int kb = 0; kb < KB2; ++kb) {
+        tma_load_4d(sq + kb * AQ * 128, &mapQh, kb * KW, h, q0, b, bar_q_full);
+        tma_load_4d(sq + C::Q_PLANE + kb * AQ * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
       }
       for (int j = 0; j < nb; ++j) {
-        const int s = j % KS, it = j / KS;
         // K block j: [64 keys x d] hi + lo
-        if (j == KS - 1) mbar_wait(bar_q_ready, 0);            // the last K stage doubles as the Q staging buffer
-        mbar_wait(bar_k_empty(s), (it & 1) ^ 1);
+        const int s = j % KS;
+        mbar_wait(bar_k_empty(s), ((j / KS) & 1) ^ 1);
         const uint32_t sk = base + C::OFF_K + s * C::K_STAGE;
-        if (elect_one()) {
-          mbar_expect_tx(bar_k_full(s), C::K_STAGE);
-          for (int kb = 0; kb < KB2; ++kb) {
-            tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, b, bar_k_full(s));
-            tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, b, bar_k_full(s));
-          }
+        mbar_expect_tx(bar_k_full(s), C::K_STAGE);
+        for (int kb = 0; kb < KB2; ++kb) {
+          tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, b, bar_k_full(s));
+          tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, b, bar_k_full(s));
         }
-        // V^T block j: [NV channel rows x 64 keys] as two 32-key tiles, hi + lo
-        const int sv_ = j % VS, itv = j / VS;
-        mbar_wait(bar_v_empty(sv_), (itv & 1) ^ 1);
+        // V^T block j: [NV channel rows x 64 keys] (TF32: two 32-key tiles), hi + lo
+        const int sv_ = j % VS;
+        mbar_wait(bar_v_empty(sv_), ((j / VS) & 1) ^ 1);
         const uint32_t sv = base + C::OFF_V + sv_ * C::V_STAGE;
-        if (elect_one()) {
-          mbar_expect_tx(bar_v_full(sv_), C::V_STAGE);
-          if (F16) {
-            tma_load_4d(sv, &mapVh, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
-            tma_load_4d(sv + C::VTILE, &mapVl, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
-          } else {
-            for (int kk = 0; kk < 2; ++kk) {
-              tma_load_4d(sv + kk * C::VTILE, &mapVh, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
-              tma_load_4d(sv + (2 + kk) * C::VTILE, &mapVl, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // =========================================================================== MMA issuer of the Q.K^T stream (whole warp, elected issue)
-    {
-      const uint32_t idesc_qk = (1u << 4) | (F16 ? 0u : ((2u << 7) | (2u << 10))) | ((uint32_t)(AKV >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-      const uint32_t q_hi = tmem_base + C::COL_QH, q_lo = tmem_base + C::COL_QL;
-
-      auto issue_qk = [&](int j) {
-        const int sb = j % SB, ks = j % KS;
-        const uint32_t sk = base + C::OFF_K + ks * C::K_STAGE;
-        const uint32_t s_acc = tmem_base + C::COL_S + sb * AKV;
-        if (!elect_one()) return;
-#pragma unroll
-        for (int c = 0; c < C::NG; ++c) {      // K steps along the head dim: 8 floats, or 16 halves (= 8 TMEM columns of Q, 32 B of a K row)
-          const int kb = c >> 2;
-          const uint64_t adv = (uint64_t)(((c & 3) * 32) >> 4);
-          const uint64_t k_hi = make_desc(sk + kb * C::KTILE) + adv;
-          const uint64_t k_lo = make_desc(sk + (KB2 + kb) * C::KTILE) + adv;
-          if (F16) {
-            umma_ts_f16(s_acc, q_lo + c * 8, k_hi, idesc_qk, c > 0 ? 1u : 0u);
-            umma_ts_f16(s_acc, q_hi + c * 8, k_lo, idesc_qk, 1u);
-            umma_ts_f16(s_acc, q_hi + c * 8, k_hi, idesc_qk, 1u);
-          } else {
-            umma_ts(s_acc, q_lo + c * 8, k_hi, idesc_qk, c > 0 ? 1u : 0u);
-            umma_ts(s_acc, q_hi + c * 8, k_lo, idesc_qk, 1u);
-            umma_ts(s_acc, q_hi + c * 8, k_hi, idesc_qk, 1u);
-          }
-        }
-        umma_commit(bar_s_full(sb));
-        umma_commit(bar_k_empty(ks));
-      };
-
-      // QK stream: S_j = Q K_j^T as soon as K_j has landed and the softmax warps have taken S_{j-SB} out of the buffer
-      mbar_wait(bar_q_ready, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      for (int j = 0; j < nb; ++j) {
-        mbar_wait(bar_k_full(j % KS), (j / KS) & 1);
-        if (j >= SB) mbar_wait(bar_s_empty(j % SB), ((j / SB) - 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        issue_qk(j);
-      }
-    }
-  } else if (warp == 2 || warp == 3) {
-    // =========================================================================== MMA issuers of the P.V stream
-    // (a profile of the single-issuer version showed the issuing thread itself -- ~40 cycles per tcgen05.mma through the
-    // uniform datapath, 39 MMAs per key block -- as the bottleneck: tensor pipe 49 % active, softmax warps waiting on S).
-    // With two P/O buffers the even and the odd key blocks are independent streams: one issuer warp each.
-    constexpr int NPV = (PB == 2) ? 2 : 1;
-    if (warp - 2 < NPV) {
-      const uint32_t idesc_pv = (1u << 4) | (F16 ? 0u : ((2u << 7) | (2u << 10))) | ((uint32_t)(NV >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-      for (int j = warp - 2; j < nb; j += NPV) {
-        const int vs = j % VS, pb = j % PB;
-        mbar_wait(bar_v_full(vs), (j / VS) & 1);
-        mbar_wait(bar_p_full(pb), (j / PB) & 1);
-        if (j >= PB) mbar_wait(bar_o_empty(pb), ((j / PB) - 1) & 1);                  // O buffer of block j-PB has been accumulated
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sv = base + C::OFF_V + vs * C::V_STAGE;
-        const uint32_t p_hi = tmem_base + C::COL_P + pb * 2 * PW, p_lo = p_hi + PW;
-        const uint32_t o_acc = tmem_base + C::COL_O + pb * NV;
-        if (!elect_one()) continue;
+        mbar_expect_tx(bar_v_full(sv_), C::V_STAGE);
         if (F16) {
-#pragma unroll
-          for (int c = 0; c < AKV / 16; ++c) {   // K steps of 16 keys: 8 TMEM columns of P, 32 B of a V^T row
-            const uint64_t adv = (uint64_t)((c * 32) >> 4);
-            const uint64_t v_hi = make_desc(sv) + adv;
-            const uint64_t v_lo = make_desc(sv + C::VTILE) + adv;
-            umma_ts_f16(o_acc, p_lo + c * 8, v_hi, idesc_pv, c > 0 ? 1u : 0u);
-            umma_ts_f16(o_acc, p_hi + c * 8, v_lo, idesc_pv, 1u);
-            umma_ts_f16(o_acc, p_hi + c * 8, v_hi, idesc_pv, 1u);
-          }
+          tma_load_4d(sv, &mapVh, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
+          tma_load_4d(sv + C::VTILE, &mapVl, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
         } else {
-#pragma unroll
-        for (int c = 0; c < AKV / 8; ++c) {    // K chunks of 8 keys
-          const int kk = c >> 2;
-          const uint64_t adv = (uint64_t)(((c & 3) * 32) >> 4);
-          const uint64_t v_hi = make_desc(sv + kk * C::VTILE) + adv;
-          const uint64_t v_lo = make_desc(sv + (2 + kk) * C::VTILE) + adv;
-          umma_ts(o_acc, p_lo + c * 8, v_hi, idesc_pv, c > 0 ? 1u : 0u);
-          umma_ts(o_acc, p_hi + c * 8, v_lo, idesc_pv, 1u);
-          umma_ts(o_acc, p_hi + c * 8, v_hi, idesc_pv, 1u);
+          for (int kk = 0; kk < 2; ++kk) {
+            tma_load_4d(sv + kk * C::VTILE, &mapVh, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
+            tma_load_4d(sv + (2 + kk) * C::VTILE, &mapVl, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
+          }
         }
-        }
-        umma_commit(bar_pv_done(pb));
-        umma_commit(bar_v_empty(vs));
       }
     }
-  } else {
-    // =========================================================================== softmax + accumulation warps
-    const int qd = warp & 3;                       // TMEM lane quadrant (warps 4.. -> 0,1,2,3,...)
-    const int hf = (warp - 4) >> 2;                // 0..NSUB-1: which AKV/NSUB key columns and NV/NSUB O columns of the row
-    const int row = qd * 32 + lane;                // query row of this thread
-    const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
-    const uint32_t rbase = (uint32_t)row * 128u, rx = (uint32_t)(row & 7);
-    constexpr int HC = AKV / NSUB;                 // 16 score columns per thread
-    constexpr int HO = NV / NSUB;                  // O columns per thread (4, 8, 12, 16, 20)
-    const uint32_t xchg = base + C::OFF_XCHG;      // [buffer][half][row] floats
+    return;
+  }
 
-    // ---- Q planes: staging smem -> TMEM (this thread's row); done by the first four warps
-    if (hf == 0) {
-#pragma unroll 1
-      for (int plane = 0; plane < 2; ++plane) {
-        mbar_wait(bar_q_full, plane);
-        const uint32_t col = tmem_base + lane_base + (plane == 0 ? C::COL_QH : C::COL_QL);
+  // ============================================================================= consumer warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = (warp >> 2) - 1;                  // rows [64 wg, 64 wg + 64) of the CTA's queries
+  const int wi = warp & 3, g = lane >> 2, qd = lane & 3;
+  // F16: the planes carry 2^eq q, 2^ek k, 2^ev v -> scores rescaled by the exact 2^-(eq+ek), output by 2^-ev; P is handed to the
+  // tensor core as p * 2^10 (folded into the exponent; the row sum carries the same factor, so O / l is unchanged)
+  float scale_l2 = p.scale_log2e, oscale = 1.f;
+  if (F16) {
+    scale_l2 = scale_l2 * exp2i(-h16_exp_of(*p.q_amax)) * exp2i(-h16_exp_of(*p.k_amax));
+    oscale = exp2i(-h16_exp_of(*p.v_amax));
+  }
+  constexpr float PEXP = F16 ? 10.f : 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: this thread's share of the row sum
+  float o[NO], ob[NO], sc[32];
 #pragma unroll
-        for (int c8 = 0; c8 < C::NG; ++c8) {         // 8 TMEM columns = two 16-byte chunks of the row
-          const int kb = c8 >> 2, ch = (c8 & 3) * 2;
-          const uint32_t a = base + C::OFF_Q + kb * AQ * 128 + rbase;
-          uint32_t v[8];
-          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(a + (((uint32_t)ch ^ rx) << 4)));
-          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "r"(a + (((uint32_t)(ch + 1) ^ rx) << 4)));
-          tmem_st8(col + c8 * 8, v);
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(plane == 0 ? bar_q_free : bar_q_ready);
-      }
-    }
-
-    // F16: the planes carry 2^eq q, 2^ek k, 2^ev v -> scores rescaled by the exact 2^-(eq+ek), output by 2^-ev; P is handed to the
-    // tensor core as p * 2^10 (folded into the exponent; the row sum carries the same factor, so O / l is unchanged)
-    float scale_l2 = p.scale_log2e, oscale = 1.f;
-    if (F16) {
-      scale_l2 = scale_l2 * exp2i(-h16_exp_of(*p.q_amax)) * exp2i(-h16_exp_of(*p.k_amax));
-      oscale = exp2i(-h16_exp_of(*p.v_amax));
-    }
-    constexpr float PEXP = F16 ? 10.f : 0.f;
-    float m_run = -INFINITY, l_run = 0.f, corr_prev = 1.f;
-    float o[HO];
-#pragma unroll
-    for (int c = 0; c < HO; ++c) o[c] = 0.f;
-
-    auto accumulate_o = [&](int jdone, float corr_j) {   // O_total = O_total * corr_j + O_blk_j, this thread's columns
-      const int pb = jdone % PB;
-      mbar_wait(bar_pv_done(pb), (jdone / PB) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t v[HO];
-#pragma unroll
-      for (int part = 0; part < HO / 4; ++part) tmem_ld4(tmem_base + lane_base + C::COL_O + pb * NV + hf * HO + part * 4, v + part * 4);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int c = 0; c < HO; ++c) o[c] = o[c] * corr_j + __uint_as_float(v[c]);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_o_empty(pb));
-    };
+  for (int c = 0; c < NO; ++c) o[c] = 0.f;
+  const uint32_t qh_base = base + C::OFF_Q + (uint32_t)wg * 64u * 128u, ql_base = qh_base + C::Q_PLANE;
+  mbar_wait(bar_q_full, 0);
 
 #pragma unroll 1
-    for (int j = 0; j < nb; ++j) {
-      const int s = j % SB;
-      mbar_wait(bar_s_full(s), (j / SB) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      float sc[HC];
-      {
-        uint32_t v[HC];
-        if constexpr (HC == 32) tmem_ld32(tmem_base + lane_base + C::COL_S + s * AKV + hf * HC, v);
-        else tmem_ld16(tmem_base + lane_base + C::COL_S + s * AKV + hf * HC, v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  for (int j = 0; j < nb; ++j) {
+    // ---- S = Q K_j^T
+    const int ks = j % KS;
+    mbar_wait(bar_k_full(ks), (j / KS) & 1);
+    const uint32_t sk = base + C::OFF_K + ks * C::K_STAGE;
 #pragma unroll
-        for (int c = 0; c < HC; ++c) sc[c] = __uint_as_float(v[c]);
+    for (int c = 0; c < 32; ++c) sc[c] = 0.f;
+    wgmma_pin(sc);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < C::NG; ++c) {
+      const int kb = c >> 2;
+      const uint64_t adv = (uint64_t)((c & 3) * 2);
+      const uint64_t q_hi = make_desc(qh_base + kb * AQ * 128) + adv, q_lo = make_desc(ql_base + kb * AQ * 128) + adv;
+      const uint64_t k_hi = make_desc(sk + kb * C::KTILE) + adv, k_lo = make_desc(sk + (KB2 + kb) * C::KTILE) + adv;
+      if (F16) {
+        Wgmma<64>::f16_ss(sc, q_lo, k_hi);
+        Wgmma<64>::f16_ss(sc, q_hi, k_lo);
+        Wgmma<64>::f16_ss(sc, q_hi, k_hi);
+      } else {
+        Wgmma<64>::tf32_ss(sc, q_lo, k_hi);
+        Wgmma<64>::tf32_ss(sc, q_hi, k_lo);
+        Wgmma<64>::tf32_ss(sc, q_hi, k_hi);
       }
-      if (j == nb - 1 && nb * AKV != p.Nk) {           // ragged last key block (TMA zero-filled the missing keys): mask
-        const int k0 = j * AKV + hf * HC;
+    }
+    wgmma_commit();
+    wgmma_wait0();
+    wgmma_pin(sc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_k_empty(ks));
+    // element j8*4 + i*2 + c: query row 16 wi + g + 8 i, key j*64 + 8 j8 + 2 qd + c
+    if (j == nb - 1 && nb * AKV != p.Nk) {           // ragged last key block (TMA zero-filled the missing keys): mask
 #pragma unroll
-        for (int c = 0; c < HC; ++c)
-          if (k0 + c >= p.Nk) sc[c] = -INFINITY;
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_s_empty(s));
-
-      // row max over both halves (raw scores; the positive scale commutes with max)
-      float mx = sc[0];
+      for (int c = 0; c < 32; ++c)
+        if (j * AKV + 8 * (c >> 2) + 2 * qd + (c & 1) >= p.Nk) sc[c] = -INFINITY;
+    }
+    // ---- online softmax (rows g, g + 8: the four lanes of a quad share a row)
+    float corr[2];
 #pragma unroll
-      for (int c = 1; c < HC; ++c) mx = fmaxf(mx, sc[c]);
-      const uint32_t xa = xchg + (uint32_t)(((j & 1) * NSUB) * 128 + row) * 4u;
-      asm volatile("st.shared.f32 [%0], %1;" ::"r"(xa + (uint32_t)hf * 512u), "f"(mx) : "memory");
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + qd), "n"(NSUB * 32) : "memory");
+    for (int i = 0; i < 2; ++i) {
+      float mx = -INFINITY;
 #pragma unroll
-      for (int o2 = 1; o2 < NSUB; ++o2) {
-        float other;
-        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(other) : "r"(xa + (uint32_t)((hf + o2) % NSUB) * 512u) : "memory");
-        mx = fmaxf(mx, other);
-      }
-      mx *= scale_l2;
-      const float m_new = fmaxf(m_run, mx);
-      const float corr = ex2_approx(m_run - m_new);      // 0 on the first block (m_run = -inf)
+      for (int j8 = 0; j8 < 8; ++j8) mx = fmaxf(mx, fmaxf(sc[j8 * 4 + i * 2], sc[j8 * 4 + i * 2 + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      mx *= scale_l2;                                // (raw scores; the positive scale commutes with max)
+      const float m_new = fmaxf(m_run[i], mx);
+      corr[i] = ex2_approx(m_run[i] - m_new);        // 0 on the first block (m_run = -inf)
       const float nm = PEXP - m_new;
       float psum = 0.f;
 #pragma unroll
-      for (int c = 0; c < HC; ++c) {
-        sc[c] = ex2_approx(fmaf(sc[c], scale_l2, nm));
-        psum += sc[c];
-      }
-      l_run = l_run * corr + psum;
-      m_run = m_new;
-
-      // corr_prev = corr_{j-1}: the rescale that belongs to adding O_blk_{j-1}
-      if (PB == 1 && j >= 1) accumulate_o(j - 1, corr_prev);     // single P buffer: PV_{j-1} must be done before P_j is written
-
-      // P -> hi / lo planes in TMEM (hi rounded to nearest; lo is left to the tensor core's own truncation: |lo| <= 2^-12 p)
-      if (F16) {
-        // fp16 hi / lo, two keys per TMEM column (even key in the low half), both rounded to nearest
+      for (int j8 = 0; j8 < 8; ++j8)
 #pragma unroll
-        for (int c8 = 0; c8 < HC / 16; ++c8) {
-          uint32_t hi[8], lo[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float x0 = sc[c8 * 16 + 2 * e], x1 = sc[c8 * 16 + 2 * e + 1];
-            const __half2 hh = __floats2half2_rn(x0, x1);
-            const float2 hf2 = __half22float2(hh);
-            const __half2 ll = __floats2half2_rn(x0 - hf2.x, x1 - hf2.y);
-            hi[e] = *reinterpret_cast<const uint32_t*>(&hh);
-            lo[e] = *reinterpret_cast<const uint32_t*>(&ll);
-          }
-          const uint32_t pcol = tmem_base + lane_base + C::COL_P + (j % PB) * 2 * PW + (hf * HC) / 2 + c8 * 8;
-          tmem_st8(pcol, hi);
-          tmem_st8(pcol + PW, lo);
+        for (int c = 0; c < 2; ++c) {
+          float& x = sc[j8 * 4 + i * 2 + c];
+          x = ex2_approx(fmaf(x, scale_l2, nm));
+          psum += x;
         }
-      } else {
+      l_run[i] = l_run[i] * corr[i] + psum;
+      m_run[i] = m_new;
+    }
+    // ---- O_j = P V_j, P hi / lo as register A fragments
+    const int vs = j % VS;
+    mbar_wait(bar_v_full(vs), (j / VS) & 1);
+    const uint32_t sv = base + C::OFF_V + vs * C::V_STAGE;
 #pragma unroll
-      for (int c8 = 0; c8 < HC / 8; ++c8) {
-        uint32_t hi[8], lo[8];
+    for (int c = 0; c < NO; ++c) ob[c] = 0.f;
+    if (F16) {
+      uint32_t ph[4][4], pl[4][4];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          hi[e] = rn_tf32(__float_as_uint(sc[c8 * 8 + e]));
-          lo[e] = __float_as_uint(sc[c8 * 8 + e] - __uint_as_float(hi[e]));
+      for (int kk = 0; kk < 4; ++kk)               // keys 16 kk .. 16 kk + 15: accumulator groups 2 kk, 2 kk + 1
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int e = (2 * kk + (r >> 1)) * 4 + (r & 1) * 2;
+          split_h16_pair(sc[e], sc[e + 1], ph[kk][r], pl[kk][r]);
         }
-        const uint32_t pcol = tmem_base + lane_base + C::COL_P + (j % PB) * 2 * AKV + hf * HC + c8 * 8;
-        tmem_st8(pcol, hi);
-        tmem_st8(pcol + AKV, lo);
-      }
-      }
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p_full(j % PB));
-      // two P/O buffers: P_j went into the other buffer (free since accumulate_o(j-2) below), so the accumulation of
-      // block j-1 happens AFTER handing P_j to the tensor core and is off the critical path
-      if (PB == 2 && j >= 1) accumulate_o(j - 1, corr_prev);
-      corr_prev = (j == 0) ? 1.f : corr;                 // corr_j rescales what was accumulated before block j
-    }
-    accumulate_o(nb - 1, corr_prev);
-
-    // total row sum = both halves; exchange through smem (buffer 0 of the max exchange is free again: nb >= 2 or resynced below)
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + qd), "n"(NSUB * 32) : "memory");
-    const uint32_t xl = xchg + (uint32_t)row * 4u;
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(xl + (uint32_t)hf * 512u), "f"(l_run) : "memory");
-    asm volatile("bar.sync %0, %1;" ::"r"(1 + qd), "n"(NSUB * 32) : "memory");
-    float l_tot = 0.f;
+      wgmma_pin(ob);
+      wgmma_fence();
 #pragma unroll
-    for (int o2 = 0; o2 < NSUB; ++o2) {               // fixed order 0..NSUB-1: every thread of the row gets the same sum
-      float lv;
-      asm volatile("ld.shared.f32 %0, [%1];" : "=f"(lv) : "r"(xl + (uint32_t)o2 * 512u) : "memory");
-      l_tot += lv;
-    }
-    const float inv_l = oscale / l_tot;
-    float* dst = p.out + ((long long)b * p.N + q0 + row) * p.ldo + h * p.d + hf * HO;
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t adv = (uint64_t)(kk * 2);
+        const uint64_t v_hi = make_desc(sv) + adv, v_lo = make_desc(sv + C::VTILE) + adv;
+        Wgmma<NV>::f16_rs(ob, pl[kk], v_hi);
+        Wgmma<NV>::f16_rs(ob, ph[kk], v_lo);
+        Wgmma<NV>::f16_rs(ob, ph[kk], v_hi);
+      }
+    } else {
+      // TF32 A fragment of keys 8 kk .. 8 kk + 7: (row, key qd) and (row, key qd + 4); this thread holds keys 2 qd, 2 qd + 1
+      uint32_t ph[8][4], pl[8][4];
+      const int src1 = (lane & ~3) | (qd >> 1), src2 = src1 + 2;
 #pragma unroll
-    for (int c = 0; c < HO; c += 4) {
-      if (hf * HO + c < D) {
-        float4 v;
-        v.x = o[c] * inv_l; v.y = o[c + 1] * inv_l; v.z = o[c + 2] * inv_l; v.w = o[c + 3] * inv_l;
-        *reinterpret_cast<float4*>(dst + c) = v;
+      for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float a0 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2], src1), a1 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2 + 1], src1);
+          const float b0 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2], src2), b1 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2 + 1], src2);
+          const float xa = (qd & 1) ? a1 : a0, xb = (qd & 1) ? b1 : b0;
+          ph[kk][i] = rn_tf32(__float_as_uint(xa));
+          pl[kk][i] = __float_as_uint(xa - __uint_as_float(ph[kk][i]));   // lo left to the tensor core's own truncation
+          ph[kk][2 + i] = rn_tf32(__float_as_uint(xb));
+          pl[kk][2 + i] = __float_as_uint(xb - __uint_as_float(ph[kk][2 + i]));
+        }
+      wgmma_pin(ob);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint64_t adv = (uint64_t)((kk & 3) * 2);
+        const uint64_t v_hi = make_desc(sv + (kk >> 2) * C::VTILE) + adv, v_lo = make_desc(sv + (2 + (kk >> 2)) * C::VTILE) + adv;
+        Wgmma<NV>::tf32_rs(ob, pl[kk], v_hi);
+        Wgmma<NV>::tf32_rs(ob, ph[kk], v_lo);
+        Wgmma<NV>::tf32_rs(ob, ph[kk], v_hi);
       }
     }
+    wgmma_commit();
+    wgmma_wait0();
+    wgmma_pin(ob);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_v_empty(vs));
+#pragma unroll
+    for (int c = 0; c < NO; ++c) o[c] = o[c] * corr[(c >> 1) & 1] + ob[c];
   }
 
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  // total row sums over the quad, fixed order: every thread of the row gets the same sum
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const float l0 = __shfl_sync(0xffffffffu, l_run[i], lane & ~3), l1 = __shfl_sync(0xffffffffu, l_run[i], (lane & ~3) | 1);
+    const float l2 = __shfl_sync(0xffffffffu, l_run[i], (lane & ~3) | 2), l3 = __shfl_sync(0xffffffffu, l_run[i], (lane & ~3) | 3);
+    const float inv_l = oscale / (((l0 + l1) + l2) + l3);
+    const int row = wg * 64 + wi * 16 + g + 8 * i;
+    float* dst = p.out + ((long long)b * p.N + q0 + row) * p.ldo + h * p.d;
+#pragma unroll
+    for (int j8 = 0; j8 < NV / 8; ++j8) {
+      const int col = 8 * j8 + 2 * qd;
+      if (col < D) *reinterpret_cast<float2*>(dst + col) = make_float2(o[j8 * 4 + i * 2] * inv_l, o[j8 * 4 + i * 2 + 1] * inv_l);
+    }
   }
 }
 
@@ -518,14 +316,13 @@ void launch_flash(const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMa
     CDX_CUDA(cudaFuncSetAttribute(flash_attn_kernel<D, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, ACfg<D, F16>::SMEM_BYTES));
     attr[dev & 63] = true;
   }
-  launch_ex(flash_attn_kernel<D, F16>, dim3(p.N / AQ, p.heads, p.B), dim3(ACfg<D, F16>::THREADS), ACfg<D, F16>::SMEM_BYTES, s, 1, qh, ql, kh, kl, vh, vl, p);
+  launch_ex(flash_attn_kernel<D, F16>, dim3(p.N / AQ, p.heads, p.B), dim3(ATHREADS), ACfg<D, F16>::SMEM_BYTES, s, 1, qh, ql, kh, kl, vh, vl, p);
 }
-
 
 // x * 2^e -> fp16 hi / lo planes, e = h16_exp_of(*amax) (the exponent the attention kernel derives from the same slot).
 // src [rows, ld] (cols % 4 == 0) -> hi / lo [rows, ldh]
-__global__ void split_rows_h16_kernel(const float* __restrict__ src, long long rows, int cols, long long ld, __half* __restrict__ hi,
-                                      __half* __restrict__ lo, long long ldh, const float* __restrict__ amax) {
+__global__ void split_rows_h16_kernel(const float* src, long long rows, int cols, long long ld, __half* hi,
+                                      __half* lo, long long ldh, const float* amax) {
   pdl_trigger();
   pdl_wait();
   const float sc = exp2i(h16_exp_of(*amax));
@@ -547,10 +344,10 @@ __global__ void split_rows_h16_kernel(const float* __restrict__ src, long long r
   }
 }
 
-// the same split, transposed: src [R, ld] columns 0..C-1 -> hi / lo [C, R] (V^T: both P.V operands K-major for tcgen05).
+// the same split, transposed: src [R, ld] columns 0..C-1 -> hi / lo [C, R] (V^T: both P.V operands K-major for wgmma).
 // 64 (rows) x 32 (columns) tiles through shared memory; R % 2 == 0
-__global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* __restrict__ src, int R, int Cc, long long ld, __half* __restrict__ hi,
-                                                                   __half* __restrict__ lo, const float* __restrict__ amax) {
+__global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* src, int R, int Cc, long long ld, __half* hi,
+                                                                   __half* lo, const float* amax) {
   __shared__ float tile[64][33];
   pdl_trigger();
   pdl_wait();

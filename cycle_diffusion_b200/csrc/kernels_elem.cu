@@ -580,7 +580,7 @@ void pixel_step_with_eps(Engine& e, const float* xt, const float* et, const floa
 }
 
 // softmax(q k^T * scale) v through two batched contractions and a row softmax.  Scores live in the arena
-// ([B*heads, Nq, ldS]); the fused tcgen05 flash kernel supersedes this when eligible.
+// ([B*heads, Nq, ldS]); the fused wgmma flash kernel supersedes this when eligible.
 void attention(Engine& e, const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo, int B, int Nq,
                int Nk, int heads, int d, int head_stride, float scale, cudaStream_t s, bool causal) {
   Scope sc(e.arena);

@@ -7,7 +7,7 @@
 //   * batched Q.K^T and P.V                  -- attention score / value contractions (ATT:180-191, IU:351-361, AEM:187-197)
 // Layout: activations NHWC (= token-major [M, C]), weights [N][K] with K = tap*Cin + c.  128x128x16 or 64x64x16
 // CTA tiles, 256 threads, 8x8 / 4x4 register micro-tiles, double-buffered shared memory, 128-bit global loads.
-// The tcgen05 back end (kernels_tc.cu) replaces this for TMA-eligible shapes; this one is always correct.
+// The wgmma back end (kernels_tc.cu) replaces this for TMA-eligible shapes; this one is always correct.
 #include "common.cuh"
 
 namespace cdx {

@@ -5,7 +5,7 @@
 // so that the concat is never materialised before the norm.
 //
 // Statistics are per-(image, channel) fp64 sums  stats[(b*C + c)*2 + {sum, sum of squares}]  attached to the TENSOR, not to the
-// norm: the tcgen05 GEMM that produces an activation adds them from its epilogue registers (kernels_tc.cu), so a GroupNorm
+// norm: the tensor-core GEMM that produces an activation adds them from its epilogue registers (kernels_tc.cu), so a GroupNorm
 // over it -- or over the concat of two such tensors, channel sums being additive -- costs no statistics pass at all; tensors
 // from other producers get them from gn_stats_kernel (one read).  The apply kernel then is the algorithmic one read + one write:
 // every block folds the channel sums of its image into the 32 group means / rstds (fp64), y = x * sc + sh per channel (the form
@@ -84,12 +84,12 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
 
 // grid (row chunks, B); thread (tr, tc) owns channel vectors tc, tc+ncol, ... (so group / affine coefficients are hoisted out
 // of the row loop) and walks the chunk's rows 4 at a time.  Dynamic smem: float2 (sc, sh) per channel.
-__global__ void __launch_bounds__(256) gn_apply_kernel(const float* __restrict__ x1, int C1, const float* __restrict__ x2, int C2,
-                                                       const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                       const double* __restrict__ st1, const double* __restrict__ st2, double inv_count,
+__global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, const float* x2, int C2,
+                                                       const float* gamma, const float* beta,
+                                                       const double* st1, const double* st2, double inv_count,
                                                        float eps, int silu,
-                                                       const float* __restrict__ scale, const float* __restrict__ shift,
-                                                       int ld_ss, float* __restrict__ y, int HW, int rows_per_chunk, float* __restrict__ amax) {
+                                                       const float* scale, const float* shift,
+                                                       int ld_ss, float* y, int HW, int rows_per_chunk, float* amax) {
   tc::pdl_trigger();
   tc::pdl_wait();
   const int C = C1 + C2;
@@ -217,9 +217,9 @@ __global__ void __launch_bounds__(256) gn_affine_kernel(int C1, int C2, const fl
 // one warp per row, the row held in registers (NV float4 per lane: C <= 128 NV): one read, one write.  Persistent warps walk the
 // rows two at a time (both rows' loads in flight before either reduction).
 template <int NV>
-__global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
-                                                        const float* __restrict__ beta, float* __restrict__ y, int M, int C,
-                                                        float eps, float* __restrict__ amax) {
+__global__ void __launch_bounds__(256) layernorm_kernel(const float* x, const float* gamma,
+                                                        const float* beta, float* y, int M, int C,
+                                                        float eps, float* amax) {
   tc::pdl_trigger();
   tc::pdl_wait();
   const int lane = threadIdx.x & 31;

@@ -8,7 +8,7 @@
 //   KL-f8 VAE                    Encoder / Decoder      ref ldm/modules/diffusionmodules/model.py:434-459, 535-568
 //                                ResnetBlock / AttnBlock / Downsample / Upsample   ref model.py:42-202
 //
-// B200-first design decisions (DESIGN.md has the full rationale):
+// Design decisions (DESIGN.md has the full rationale):
 //   * activations are NHWC, so a [B,H,W,C] feature map *is* the [B*HW, C] token matrix: the reference's
 //     'b c h w -> b (h w) c' rearranges disappear and every conv / Linear is one implicit-GEMM family;
 //   * skip-connection concatenation (th.cat, OAI:736) is never materialised: GroupNorm and the 1x1 skip conv read
@@ -482,7 +482,7 @@ void net_finalize(Net& n) {
     CDX_CUDA(cudaMemcpy(n.freqs_dev, n.freqs_host.data(), n.freqs_host.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
   if (!n.planes_valid) {
-    // TF32 hi / lo planes of every weight for the tcgen05 TS kernel (3x the weight memory: 10.3 GB for SD v1-4 of 180 GB)
+    // TF32 hi / lo planes of every weight for the TF32-plane kernel (3x the weight memory: 10.3 GB for SD v1-4 of the H100's 80 GB)
     if (!n.blob_hi) CDX_CUDA(cudaMalloc(&n.blob_hi, n.blob_floats * sizeof(float)));
     if (!n.blob_lo) CDX_CUDA(cudaMalloc(&n.blob_lo, n.blob_floats * sizeof(float)));
     split_planes(*n.eng, n.blob, n.blob_hi, n.blob_lo, n.blob_floats, 0);
@@ -557,7 +557,7 @@ struct Exec {
     }
     const int Cin = x.C;
     if (up == 2 && e.mma_mode == 1 && (Cin % 32) == 0 && !out_nchw) {
-      // tcgen05 path: the TMA box gather cannot express the >>1 source index, so materialise the nearest-2x upsample
+      // tensor-core path: the TMA box gather cannot express the >>1 source index, so materialise the nearest-2x upsample
       // (one extra write+read of the activation, <2% of the conv's time) and run the plain tensor-core conv on it
       Tensor xu = alloc(x.B, x.H * 2, x.W * 2, x.C);
       upsample2(e, x.p, xu.p, x.B, x.H, x.W, x.C, s);
@@ -816,7 +816,7 @@ struct UNetExec : Exec {
       const bool flash_ok = e.mma_mode == 1 && e.flash_attn && (HW % 128) == 0 && (d == 16 || d == 32 || d == 40 || d == 64 || d == 80);
       if (flash_ok && e.tc_kind >= 1 && (C % 8) == 0) {
         // fp16-split fused attention: ONE plain fp32 q|k|v projection (its range tracked by the epilogue), then one pass that
-        // writes the fp16 hi / lo planes of q|k and of V^T (both P.V operands K-major for tcgen05) with the tensor's exponent
+        // writes the fp16 hi / lo planes of q|k and of V^T (both P.V operands K-major for wgmma) with the tensor's exponent
         Scope sa(e.arena);
         float* qkv = (float*)e.arena.alloc((size_t)M * 3 * C * sizeof(float));
         linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_q.weight"), 3 * C, nullptr, nullptr, 0, qkv, 3 * C, nullptr, n1.amax, nullptr,
@@ -832,7 +832,7 @@ struct UNetExec : Exec {
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands
-        // are K-major for tcgen05) are written by their GEMM epilogues directly as TF32 hi / lo planes
+        // are K-major for wgmma) are written by their GEMM epilogues directly as TF32 hi / lo planes
         Scope sa(e.arena);
         const size_t nqk = (size_t)M * 2 * C, nvt = (size_t)C * M;
         float* qk_hi = (float*)e.arena.alloc(nqk * sizeof(float));

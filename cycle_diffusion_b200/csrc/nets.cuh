@@ -33,7 +33,7 @@ struct Net {
   std::vector<Param> params;
   std::unordered_map<std::string, int> index;
   float* blob = nullptr;
-  float* blob_hi = nullptr;     // rn_tf32(blob)            } pre-split planes for the tcgen05 TS kernel,
+  float* blob_hi = nullptr;     // rn_tf32(blob)            } pre-split planes for the TF32-plane (KIND_TS) kernel,
   float* blob_lo = nullptr;     // rn_tf32(blob - blob_hi)  } same offsets as `blob`, derived at finalize
   bool planes_valid = false;
   // fp16-split planes (MODE_H16): hi = fp16(w * 2^w_exp), lo = fp16(w * 2^w_exp - hi), element index = float index into `blob`;

@@ -1,7 +1,7 @@
 """Python handles over the libcdx C ABI: Engine (per device), UNet / VAE networks, per-step kernels, loop drivers.
 
 PyTorch is used only as plumbing: device memory (``torch.empty(..., device='cuda')``), streams and
-``torch.distributed``.  Every compute call goes through ctypes into hand-written sm_100a kernels; there is no
+``torch.distributed``.  Every compute call goes through ctypes into hand-written sm_90a kernels; there is no
 torch.nn / CPU fallback anywhere on this path.
 """
 import ctypes as C

@@ -1,5 +1,5 @@
 /*
- * cdx.h -- C ABI of libcdx.so, the B200-native CycleDiffusion sampling engine.
+ * cdx.h -- C ABI of libcdx.so, the H100-native CycleDiffusion sampling engine.
  *
  * This is the drop-in boundary for the one hot path of ChenWu98/cycle-diffusion: the DPM-Encoder
  * inversion + decode-with-recovered-noise loops including the U-Net / VAE forwards.  Every entry
@@ -55,8 +55,8 @@ size_t cdx_engine_workspace_bytes(const cdx_engine* e);
 /* number of kernels this engine has launched since creation (bench.py's gpu_launches) */
 uint64_t cdx_engine_launch_count(const cdx_engine* e);
 /* Per-kernel-family timing with CUDA events on the launching stream (off by default; bench.py turns it on for a
- * separate, untimed pass).  Tags: 0 conv3x3 FFMA, 1 dense FFMA, 2 batched (attention) FFMA, 3 conv3x3 tcgen05,
- * 4 dense tcgen05, 5 batched tcgen05, 6 GroupNorm, 7 LayerNorm, 8 softmax, 9 other.  profile_read synchronises the
+ * separate, untimed pass).  Tags: 0 conv3x3 FFMA, 1 dense FFMA, 2 batched (attention) FFMA, 3 conv3x3 tensor-core,
+ * 4 dense tensor-core, 5 batched tensor-core, 6 GroupNorm, 7 LayerNorm, 8 softmax, 9 other.  profile_read synchronises the
  * device, sums the records of `tag` (ms, algorithmic flops / bytes, launches) and keeps them until profile(e, 1/0)
  * is called again. */
 #define CDX_PROF_NTAGS 10
@@ -64,10 +64,10 @@ int cdx_engine_profile(cdx_engine* e, int enable);
 int cdx_engine_profile_read(cdx_engine* e, int tag, double* ms, double* flops, double* bytes, uint64_t* launches);
 /* select the dense-contraction path:
  *   0 = SIMT fp32 FFMA tiles (exact fp32)
- *   1 = tcgen05, fp32-faithful split products (default): weight GEMMs / convs as 3 x kind::f16 over an fp16 hi/lo split of
- *       power-of-two-scaled operands, attention and activation x activation contractions as 3 x kind::tf32
+ *   1 = tensor cores (wgmma), fp32-faithful split products (default): weight GEMMs / convs as 3 x wgmma .f16 over an fp16 hi/lo split of
+ *       power-of-two-scaled operands, attention and activation x activation contractions as 3 x wgmma .tf32
  *   2 = as 1 but attention unfused (A/B comparisons)
- *   3 = as 1 with every contraction as 3 x kind::tf32 (the round-1 scheme)
+ *   3 = as 1 with every contraction as 3 x wgmma .tf32 (the round-1 scheme)
  *   4 = FAST PATH, not fp32-faithful: weight GEMMs / convs with the hi*hi term only (plain fp16 inputs, fp32 accumulate);
  *       reported separately by bench.py together with its measured |delta pixel| */
 int cdx_engine_set_mma_mode(cdx_engine* e, int mode);

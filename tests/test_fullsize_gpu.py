@@ -67,7 +67,7 @@ def test_sd_v14_unet_full_size(eng, sd_unet):
         ref = unet_openai.unet_forward(sd, cfg, x, t.long(), ctx)
     r = relmax(y, ref)
     print(f'SD v1-4 U-Net 64x64 B2: rel max err vs oracle {r:.3e}  (|ref|max {float(ref.abs().max()):.3f}) families {sorted(fam)}')
-    assert 'conv3x3_tc' in fam and 'dense_tc' in fam, f'tcgen05 path not taken: {fam}'
+    assert 'conv3x3_tc' in fam and 'dense_tc' in fam, f'tensor-core path not taken: {fam}'
     assert not [k for k in fam if k.endswith('ffma') and fam[k]['flops'] > 0.02 * fam['conv3x3_tc']['flops']], f'large FFMA share: {fam}'
     assert r < TOL
 

@@ -1,8 +1,8 @@
-"""tcgen05 back end: per-op and network-level parity against fp32 references, for both fp32-faithful product schemes --
-mma_mode 1 (default): weight GEMMs / convs as 3 x kind::f16 over an fp16 hi/lo split of power-of-two-scaled operands;
-mma_mode 3: everything as 3 x kind::tf32.
+"""Tensor-core (wgmma) back end: per-op and network-level parity against fp32 references, for both fp32-faithful product schemes --
+mma_mode 1 (default): weight GEMMs / convs as 3 x wgmma .f16 over an fp16 hi/lo split of power-of-two-scaled operands;
+mma_mode 3: everything as 3 x wgmma .tf32.
 
-Both keep ~2^-21 relative error per product (hi*hi + lo*hi + hi*lo with fp32 TMEM accumulation drained every 256 K elements),
+Both keep ~2^-21 relative error per product (hi*hi + lo*hi + hi*lo with fp32 accumulation in registers, chunked every 256 K elements),
 so the same fp32 round-off budgets as the FFMA path apply (2e-5 relative per op, 2e-4 through a whole U-Net)."""
 import math
 
@@ -47,7 +47,7 @@ def test_linear_tc(eng, M, K, N):
     y = eng.op_linear(x.cuda(), w.cuda(), b.cuda()).cpu()
     fam = eng.profile_read()
     eng.profile(False)
-    assert 'dense_tc' in fam, f'tcgen05 path was not taken: {fam}'
+    assert 'dense_tc' in fam, f'tensor-core path was not taken: {fam}'
     r = rel(y, F.linear(x, w, b))
     print(f'linear_tc {M}x{K}x{N}: rel {r:.2e}')
     assert r < 2e-5
@@ -55,10 +55,10 @@ def test_linear_tc(eng, M, K, N):
 
 @pytest.mark.parametrize('B,Cin,Cout,H', [(1, 32, 128, 16), (2, 64, 64, 16), (1, 320, 320, 32), (4, 128, 256, 64), (3, 96, 160, 8), (8, 64, 32, 4),
                                            (2, 1280, 1280, 8),
-                                           # halo schedule (Cin % 64 == 0, W >= 16): split-K items that start / end inside a channel
+                                           # Cin % 64 == 0, W >= 16: split-K items that start / end inside a channel
                                            # block, ragged batch, ragged N tile, many channel blocks
                                            (1, 1280, 640, 16), (8, 640, 640, 32), (3, 192, 96, 32), (1, 1920, 320, 64), (5, 64, 48, 16),
-                                           # 8 x 8 level on CTA pairs: two images per 128-row tile, 200-pixel halo plane; ragged batch / N
+                                           # 8 x 8 level: two images per 128-row tile; ragged batch / N
                                            (8, 1280, 1280, 8), (4, 128, 64, 8), (12, 192, 80, 8), (7, 64, 48, 8)])
 def test_conv3x3_tc(eng, B, Cin, Cout, H):
     g = torch.Generator().manual_seed(Cin * 1000 + Cout + H)
@@ -69,7 +69,7 @@ def test_conv3x3_tc(eng, B, Cin, Cout, H):
     y = nchw(eng.op_conv3x3(nhwc(x).cuda(), w.cuda(), b.cuda(), 1, 1, 1).cpu())
     fam = eng.profile_read()
     eng.profile(False)
-    assert 'conv3x3_tc' in fam, f'tcgen05 path was not taken: {fam}'
+    assert 'conv3x3_tc' in fam, f'tensor-core path was not taken: {fam}'
     r = rel(y, F.conv2d(x, w, b, padding=1))
     print(f'conv_tc B{B} {Cin}->{Cout} @{H}: rel {r:.2e}')
     assert r < 2e-5
@@ -86,7 +86,7 @@ def test_unet_tc_vs_reference_fixture(eng, name, cfg):
     fam = eng.profile_read()
     eng.profile(False)
     r = float((y.double() - g['y'].double()).abs().max() / max(1.0, float(g['y'].abs().max())))
-    print(f'{name} (tcgen05): rel max err {r:.3e}; families {{k: v["launches"] for k, v in fam.items()}}')
+    print(f'{name} (tensor cores): rel max err {r:.3e}; families {{k: v["launches"] for k, v in fam.items()}}')
     assert 'conv3x3_tc' in fam or 'dense_tc' in fam
     assert r < 2e-4
 
@@ -112,14 +112,14 @@ def test_cycle_tc_vs_reference_fixture(eng):
     rz = maxdiff(z.cpu(), zref) / float(zref.abs().max())
     tgt = unet.latent_decode(zref, g['c_tgt'], g['uc'], dec_scale, sched).cpu()
     own = unet.latent_decode(z, g['c_src'], g['uc'], enc_scale, sched).cpu()
-    print(f'cycle (tcgen05): rel|dz| {rz:.2e} |d tgt| {maxdiff(tgt, g["tgt_a"]):.2e} own-cycle {maxdiff(own, g["x0"]):.2e}')
+    print(f'cycle (tensor cores): rel|dz| {rz:.2e} |d tgt| {maxdiff(tgt, g["tgt_a"]):.2e} own-cycle {maxdiff(own, g["x0"]):.2e}')
     assert rz < 2e-4 and maxdiff(tgt, g['tgt_a']) < 1e-3 and maxdiff(own, g['x0']) < 1e-3
 
 
 @pytest.mark.parametrize('mode', [1, 2, 3])
 @pytest.mark.parametrize('B,N,heads,d', [(1, 4096, 8, 40), (2, 1024, 8, 80), (2, 256, 2, 16), (1, 128, 4, 64), (1, 256, 3, 32), (3, 384, 2, 40)])
 def test_attention_tc(B, N, heads, d, mode):
-    """mode 1: fused flash kernel on fp16-split operands (tcgen05 kind::f16, S/P never leave the SM); mode 2: unfused tcgen05
+    """mode 1: fused flash kernel on fp16-split operands (wgmma .f16, S/P never leave the SM); mode 2: unfused tensor-core
     QK^T / softmax / PV^T; mode 3: the fused kernel on TF32 planes (round-1 scheme, kept for --mma 3)."""
     from cycle_diffusion_b200.engine import Engine
     e = Engine(0)
@@ -144,7 +144,7 @@ def test_attention_tc(B, N, heads, d, mode):
 
 def test_attention_tc_vae_shape():
     """The KL-f8 mid-block attention at 512x512 (AEM:178-202): one head, d = 512, 4096 tokens.  It is outside the fused kernel's
-    head dims, so it must take the unfused tcgen05 route (two batched contractions around the row softmax), not the FFMA tiles."""
+    head dims, so it must take the unfused tensor-core route (two batched contractions around the row softmax), not the FFMA tiles."""
     from cycle_diffusion_b200.engine import Engine
     e = Engine(0)
     e.set_mma_mode(1)
@@ -250,8 +250,7 @@ def test_fast_path_is_reduced_precision_and_marked():
 
 
 def test_gn_fusion_opt_in_keeps_parity():
-    """The opt-in experiment CDX_GN_FUSION=1 (GroupNorm + SiLU applied inside the conv3x3 halo conversion, two-source halo; measured slower,
-    profiles/r02_gn_fusion_negative.txt) stays correct: the 320-channel U-Net fixture in a fresh process with the switch on."""
+    """The opt-in experiment CDX_GN_FUSION=1 (GroupNorm + SiLU applied while the conv3x3 splits its A operand, two-source input; opt-in) stays correct: the 320-channel U-Net fixture in a fresh process with the switch on."""
     import os
     import subprocess
     import sys

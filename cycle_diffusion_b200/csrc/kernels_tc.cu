@@ -21,8 +21,9 @@
 //                 materialised; or (batched mode) 4D maps over (k, head, row, batch) for the attention contractions.  B: pre-split
 //                 weight planes (fp16 or TF32), or raw fp32 (KIND_SS).  128B-swizzled smem, STAGES-deep ring.
 //   warpgroups 1-2  64 rows each: raw fp32 A from smem -> hi / lo split in registers (the wgmma A fragment layout) -> three wgmmas
-//                 per K step against the B tiles in smem -> chunk accumulator -> total; then the epilogue straight from registers:
-//                 alpha / rescale, +bias, +per-sample row vector (timestep embedding), GEGLU, +residual, range / GroupNorm side outputs.
+//                 per K step against the B tiles in smem -> chunk accumulator -> total, software-pipelined (the next stage's A
+//                 is split into a second fragment set while the current stage's wgmmas run, one batch per stage); then the
+//                 epilogue straight from registers: alpha / rescale, +bias, +per-sample row vector (timestep embedding), GEGLU, +residual, range / GroupNorm side outputs.
 #include <algorithm>
 
 #include <mutex>
@@ -48,11 +49,13 @@ constexpr int TILE_BYTES = TBM * TBK * 4;          // 16 KB: one 32-float A sub-
 constexpr int TC_THREADS = 384;                     // producer warpgroup + two consumer warpgroups (setmaxnreg is per warpgroup)
 constexpr int STAGES = 3;
 
-enum { KIND_SS = 0, KIND_TS = 1, KIND_H16 = 2 };
+// KIND_H16_FAST: the separately reported reduced-precision path (hi*hi term only), a compile-time variant of KIND_H16 so that no
+// runtime branch sits inside a batch of wgmmas
+enum { KIND_SS = 0, KIND_TS = 1, KIND_H16 = 2, KIND_H16_FAST = 3 };
 
 template <int KIND, int BN>
 struct Cfg {
-  static constexpr bool H16 = KIND == KIND_H16;
+  static constexpr bool H16 = KIND == KIND_H16 || KIND == KIND_H16_FAST;
   static constexpr int BK = H16 ? 64 : 32;           // K elements per pipeline stage
   static constexpr int KCHUNK = 256 / BK;            // stages per accumulation chunk (256 K elements)
   static constexpr int A_BYTES = (H16 ? 2 : 1) * TILE_BYTES;
@@ -88,18 +91,16 @@ struct TcParams {
   int a_code[4], b_code[4];   // per map dim: 0 -> k0, 1 -> row0, 2 -> zh, 3 -> zb, 4 -> 0
   int a_rowoff_h, b_rowoff_h; // row0 += zh * rowoff (heads packed along the row dimension)
   long long sC_b, sC_h;       // output offsets per zb / zh
-  // work item t (= blockIdx.x) -> (split = t % splits, tm, tn, z) with t / splits = tm + tiles_m * (tn + tiles_n * z)
+  // work item t (= blockIdx.x) -> (split = t % splits, tm, tn, z): see tile_coord
   int tiles_m, tiles_n, total_tiles;
   int tn_w;                 // tile width along N (== the kernel's BN)
   // split-K (small-M layers that cannot fill the GPU): split s covers k-blocks [s*kb_per_split, min(num_kb, (s+1)*kb_per_split)) and
   // writes its raw partial tile to ws[s][M][N]; splitk_reduce_kernel then sums the partials in fixed order and applies the epilogue
   int splits, kb_per_split;
   float* ws;
-  // KIND_H16: tracked max |A| (device scalars written by the producers of A / A2), exponent of the pre-scaled fp16 weight
-  // planes, `fast` = hi*hi term only (the separately reported reduced-precision path)
+  // KIND_H16: tracked max |A| (device scalars written by the producers of A / A2), exponent of the pre-scaled fp16 weight planes
   const float* a_amax; const float* a2_amax;
   int b_exp;
-  int fast;
   float* c_amax;            // optional: atomic max of |C| over everything this launch stores (operand range for the consumer GEMM)
   double* c_stats;          // optional: per-(image, channel) fp64 {sum, sum sq} of C, for the GroupNorm that consumes it; requires
                             // every 32-row quadrant of a tile to lie inside one image (checked on the host)
@@ -114,15 +115,25 @@ __device__ __forceinline__ int h16_a_exp(const TcParams& p) {
 
 struct TileCoord { int n0, nend, m0, x0, y0, b0, zb, zh, kb0, kb1, split; };
 
+// Raster of the tiles of one z: bands of RASTER_M tiles along M, walked band by band; inside a band M varies fastest, then N.  A wave
+// of CTAs then covers a few M tiles x many N tiles instead of ~num_sms M tiles x one N tile, so every A row band is fetched from HBM
+// about once per launch rather than once per N tile (an A tile and a B tile of a k-block are both 32 KB: the wave's footprint is
+// smallest when it spans similar numbers of M and N tiles).
+constexpr int RASTER_M = 8;
+
 __device__ __forceinline__ TileCoord tile_coord(const TcParams& p, int t, int num_kb) {
   TileCoord c;
   c.split = t % p.splits;
   t /= p.splits;
   c.kb0 = c.split * p.kb_per_split;
   c.kb1 = min(num_kb, c.kb0 + p.kb_per_split);
-  const int tm = t % p.tiles_m;
-  const int r = t / p.tiles_m;
-  const int tn = r % p.tiles_n, z = r / p.tiles_n;
+  const int per_z = p.tiles_m * p.tiles_n;
+  const int z = t / per_z;
+  int u = t - z * per_z;
+  const int m_lo = u / (RASTER_M * p.tiles_n) * RASTER_M;       // first M tile of the band
+  const int bm = min(RASTER_M, p.tiles_m - m_lo);                 // M tiles of the band (the last one may be short)
+  u -= m_lo * p.tiles_n;
+  const int tm = m_lo + u % bm, tn = u / bm;
   c.n0 = tn * p.tn_w;
   c.nend = min(p.N, c.n0 + p.tn_w);
   c.m0 = 0; c.x0 = 0; c.y0 = 0; c.b0 = 0; c.zb = 0; c.zh = 0;
@@ -146,7 +157,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2,
                const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapBlo, const TcParams p) {
   using CF = Cfg<KIND, BN>;
-  constexpr bool H16 = CF::H16;
+  constexpr bool H16 = CF::H16, FAST = KIND == KIND_H16_FAST;
   constexpr int BK = CF::BK, A_BYTES = CF::A_BYTES, B_PLANE = CF::B_PLANE, STAGE_BYTES = CF::STAGE_BYTES;
   constexpr int NACC = BN / 2;                     // fp32 accumulators per thread of an m64nBN tile
   pdl_trigger();
@@ -226,7 +237,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const int r0 = wg * 64 + wi * 16 + g;            // tile rows r0 and r0 + 8 of this thread
   const int ea = H16 ? h16_a_exp(p) : 0;
   const float asc = exp2i(ea);
-  const bool fast = H16 && p.fast == 1;
   const int kchunk = (tc_.kb1 - tc_.kb0) <= 2 * CF::KCHUNK ? 2 * CF::KCHUNK : CF::KCHUNK;
   const int cblocks = p.mode == 1 ? p.Cin / TBK : 1;
   // conv + fused GroupNorm: pixel of each of this thread's two rows
@@ -243,15 +253,21 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 #pragma unroll
   for (int j = 0; j < NACC; ++j) { acc[j] = 0.f; tot[j] = 0.f; }
 
-  int it = 0, kin = 0;
-#pragma unroll 1
-  for (int kb = tc_.kb0; kb < tc_.kb1; ++kb, ++it) {
+  // Software pipeline over the stages of the work item: while the wgmmas of stage it run, stage it + 1's A is split into the
+  // other fragment set; wgmma.wait_group 1 then retires stage it - 1, whose smem slot goes back to the producer.
+  struct Frag { uint32_t h[4][4], l[4][4]; };     // A fragments of one stage's K steps (rows r0 / r0 + 8), hi / lo
+  const int nst = tc_.kb1 - tc_.kb0;               // stages of this work item (>= 1)
+  // H16: a stage whose second 32-element sub-block lies beyond K (odd K tail, only the last stage of the K range) has 2 K steps
+  auto tail = [&](int it) { return H16 && (tc_.kb0 + it) * BK + TBK >= p.K; };
+
+  // wait for stage it to land, then split its A into f
+  auto load_split = [&](int it, Frag& f) {
     const int s = it % STAGES;
     mbar_wait(bar_full(s), (it / STAGES) & 1);
     const uint32_t st = base + s * STAGE_BYTES;
-    const uint32_t sb = st + A_BYTES;
     if (KIND == KIND_SS) {
       // raw fp32 B tile -> TF32 hi in place, lo into the second plane (both consumer warpgroups, then a named barrier)
+      const uint32_t sb = st + A_BYTES;
       const int ct = threadIdx.x - 128;
 #pragma unroll 4
       for (int i = ct; i < B_PLANE / 16; i += 256) {
@@ -266,11 +282,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
       asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    const uint64_t bhi = make_desc(sb), blo = make_desc(sb + B_PLANE);
-    const int k0 = kb * BK;
-    const int nsl = (k0 + TBK < p.K || !H16) ? 4 : 2;             // K steps of this stage (H16 odd tail: one sub-block = 2 steps)
-    // A fragments of all K steps of the stage (rows r0 / r0 + 8), split into hi / lo
-    uint32_t ah[4][4], al[4][4];
+    const int k0 = (tc_.kb0 + it) * BK;
+    const int nsl = tail(it) ? 2 : 4;
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       if (kk >= nsl) break;
@@ -307,10 +320,12 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             }
             if (ea != 0) { x.x *= asc; x.y *= asc; }
             const __half2 h = __floats2half2_rn(x.x, x.y);       // .x (low half) = even k
-            const float2 hf = __half22float2(h);
-            const __half2 l = __floats2half2_rn(x.x - hf.x, x.y - hf.y);
-            ah[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&h);
-            al[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&l);
+            f.h[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&h);
+            if (!FAST) {
+              const float2 hf = __half22float2(h);
+              const __half2 l = __floats2half2_rn(x.x - hf.x, x.y - hf.y);
+              f.l[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&l);
+            }
           }
         }
       } else {
@@ -324,41 +339,67 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
                          : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
             const uint32_t h = rn_tf32(__float_as_uint(x));
-            ah[kk][hk * 2 + i] = h;
-            al[kk][hk * 2 + i] = tf32_lo(x, h);
+            f.h[kk][hk * 2 + i] = h;
+            f.l[kk][hk * 2 + i] = tf32_lo(x, h);
           }
         }
       }
     }
+  };
+
+  // the wgmmas of stage it (NSL K steps) from f: one straight-line batch, small terms first
+  auto mma = [&](auto nsl_c, int it, const Frag& f) {
+    constexpr int NSL = decltype(nsl_c)::value;
+    const uint32_t sb = base + (it % STAGES) * STAGE_BYTES + A_BYTES;
+    const uint64_t bhi = make_desc(sb), blo = make_desc(sb + B_PLANE);
     wgmma_pin(acc);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      if (kk >= nsl) break;
+    for (int kk = 0; kk < NSL; ++kk) {
       const uint64_t adv = (uint64_t)kk * 2u;       // 32 bytes per K step along the 128-byte row
       if (H16) {
-        if (!fast) {
-          Wgmma<BN>::f16_rs(acc, al[kk], bhi + adv);      // small terms first
-          Wgmma<BN>::f16_rs(acc, ah[kk], blo + adv);
+        if (!FAST) {
+          Wgmma<BN>::f16_rs(acc, f.l[kk], bhi + adv);
+          Wgmma<BN>::f16_rs(acc, f.h[kk], blo + adv);
         }
-        Wgmma<BN>::f16_rs(acc, ah[kk], bhi + adv);
+        Wgmma<BN>::f16_rs(acc, f.h[kk], bhi + adv);
       } else {
-        Wgmma<BN>::tf32_rs(acc, al[kk], bhi + adv);
-        Wgmma<BN>::tf32_rs(acc, ah[kk], blo + adv);
-        Wgmma<BN>::tf32_rs(acc, ah[kk], bhi + adv);
+        Wgmma<BN>::tf32_rs(acc, f.l[kk], bhi + adv);
+        Wgmma<BN>::tf32_rs(acc, f.h[kk], blo + adv);
+        Wgmma<BN>::tf32_rs(acc, f.h[kk], bhi + adv);
       }
     }
     wgmma_commit();
-    wgmma_wait0();
-    wgmma_pin(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_empty(s));
-    if (++kin == kchunk || kb == tc_.kb1 - 1) {     // chunk complete: round-to-nearest fp32 add into the total
+  };
+
+  // stage it: its fragments are in cur; nxt held stage it - 1's
+  int kin = 0;
+  auto step = [&](int it, const Frag& cur, Frag& nxt) {
+    if (tail(it)) mma(std::integral_constant<int, 2>(), it, cur);
+    else mma(std::integral_constant<int, 4>(), it, cur);
+    wgmma_wait1();                                  // stage it - 1 has retired: its slot and its fragment set are free
+    if (it > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty((it - 1) % STAGES));
+    }
+    if (it + 1 < nst) load_split(it + 1, nxt);
+    if (++kin == kchunk || it == nst - 1) {        // chunk complete: retire it, round-to-nearest fp32 add into the total
+      wgmma_wait0();
+      wgmma_pin(acc);
 #pragma unroll
       for (int j = 0; j < NACC; ++j) { tot[j] += acc[j]; acc[j] = 0.f; }
       kin = 0;
     }
+  };
+
+  Frag fa, fb;
+  load_split(0, fa);
+#pragma unroll 1
+  for (int it = 0; it < nst; it += 2) {
+    step(it, fa, fb);
+    if (it + 1 < nst) step(it + 1, fb, fa);
   }
+  // (the last stage's slot is not handed back: the producer has loaded everything)
 
   // ============================================================================= epilogue (straight from registers)
   // accumulator element j*4 + i*2 + c: tile row r0 + 8 i, column n0 + 8 j + 2 qd + c
@@ -602,6 +643,8 @@ void ensure_attr(int device) {
     set_smem_attr<KIND_TS, 64>();
     set_smem_attr<KIND_H16, 128>();
     set_smem_attr<KIND_H16, 64>();
+    set_smem_attr<KIND_H16_FAST, 128>();
+    set_smem_attr<KIND_H16_FAST, 64>();
     attr_set[d] = true;
   }
 }
@@ -887,8 +930,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
       p.a2_amax = slot;
     }
     p.b_exp = a.b_exp;
-    p.fast = e.tc_kind == 2 ? 1 : 0;
   }
+  const bool fast = h16 && e.tc_kind == 2;
   // side outputs fused into the epilogue: range of C always (the split-K reduce kernel covers the split case); GroupNorm
   // statistics when every 32-row quadrant of a tile lies inside one image and the epilogue is the final one
   p.c_amax = a.out_nchw ? nullptr : a.c_amax;
@@ -910,9 +953,11 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   ensure_attr(e.device);
   ProfScope ps(e, s, a.mode == 1 ? PROF_CONV_TC : PROF_DENSE_TC, 2.0 * a.M * a.N * a.K,
                4.0 * ((double)a.M * a.K / (a.mode == 1 ? 9 : 1) + (double)a.N * a.K + (double)a.M * a.N), 1);
-  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s%s", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (p.fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
+  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s%s", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
           p.gn_ab ? " gn" : "", a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "");
-  if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, s);
+  if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, s);
+  else if (fast) launch_gemm<KIND_H16_FAST, 64>(p, *mA, *mA2, *mB, *mBlo, s);
+  else if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (h16) launch_gemm<KIND_H16, 64>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (ts && p.tn_w == 128) launch_gemm<KIND_TS, 128>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (ts) launch_gemm<KIND_TS, 64>(p, *mA, *mA2, *mB, *mBlo, s);

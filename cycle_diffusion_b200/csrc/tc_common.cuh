@@ -38,11 +38,14 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity)
       : "memory");
   return ok;
 }
+// Not inlined: a trap instruction inside a kernel makes ptxas hold the whole kernel to its launch register count, which ignores
+// the setmaxnreg budget of the consumer warpgroups (the 128-wide wgmma consumers then spill); behind a call it does not.
+static __device__ __noinline__ void mbar_wait_timeout() { __trap(); }
 // bounded wait: a protocol bug traps (error returned to the host) instead of hanging the GPU
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) __trap();
+    if (++spins > (1u << 26)) mbar_wait_timeout();
   }
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {

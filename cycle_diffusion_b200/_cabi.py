@@ -74,6 +74,8 @@ SIGNATURES = {
     'cdx_vae_encode': (_I, [_P, _P, _P, _I, _I, _P]),
     'cdx_text_encode': (_I, [_P, _P, _I, _I, _P, _P]),
     'cdx_vae_decode': (_I, [_P, _P, _P, _I, _I, _P]),
+    'cdx_vae_encode_hw': (_I, [_P, _P, _P, _I, _I, _I, _P]),
+    'cdx_vae_decode_hw': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_affine': (_I, [_P, _P, _F, _F, _P, _S, _P]),
     'cdx_shift_scale': (_I, [_P, _P, _F, _F, _P, _S, _P]),
     'cdx_q_sample': (_I, [_P, _P, _P, _F, _F, _P, _S, _P]),

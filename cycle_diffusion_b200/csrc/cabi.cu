@@ -387,11 +387,14 @@ int cdx_unet_forward(cdx_net* n, const float* x, const float* t_dev, const float
     with_arena(n->owner->e, S(stream), [&] { unet_forward(*n->n, x, t_dev, ctx, ctx_len, out, B, H, W, S(stream)); });
   });
 }
-int cdx_vae_encode(cdx_net* n, const float* img, float* moments, int B, int R, void* stream) {
+int cdx_vae_encode_hw(cdx_net* n, const float* img, float* moments, int B, int H, int W, void* stream) {
   return guard([&] {
     CDX_CHECK(n && n->owner && img && moments && B > 0, "vae_encode: bad arguments");
-    with_arena(n->owner->e, S(stream), [&] { vae_encode(*n->n, img, moments, B, R, S(stream)); });
+    with_arena(n->owner->e, S(stream), [&] { vae_encode(*n->n, img, moments, B, H, W, S(stream)); });
   });
+}
+int cdx_vae_encode(cdx_net* n, const float* img, float* moments, int B, int R, void* stream) {
+  return cdx_vae_encode_hw(n, img, moments, B, R, R, stream);
 }
 int cdx_text_encode(cdx_net* n, const int* ids, int B, int L, float* out, void* stream) {
   return guard([&] {
@@ -431,11 +434,14 @@ int cdx_image_metrics(cdx_engine* eh, const float* a, const float* b, int B, int
     with_arena(eh->e, S(stream), [&] { image_metrics(eh->e, a, b, B, H, W, out, S(stream)); });
   });
 }
-int cdx_vae_decode(cdx_net* n, const float* z, float* img, int B, int h, void* stream) {
+int cdx_vae_decode_hw(cdx_net* n, const float* z, float* img, int B, int h, int w, void* stream) {
   return guard([&] {
     CDX_CHECK(n && n->owner && z && img && B > 0, "vae_decode: bad arguments");
-    with_arena(n->owner->e, S(stream), [&] { vae_decode(*n->n, z, img, B, h, S(stream)); });
+    with_arena(n->owner->e, S(stream), [&] { vae_decode(*n->n, z, img, B, h, w, S(stream)); });
   });
+}
+int cdx_vae_decode(cdx_net* n, const float* z, float* img, int B, int h, void* stream) {
+  return cdx_vae_decode_hw(n, z, img, B, h, h, stream);
 }
 
 // ---------------------------------------------------------------- per-step kernels

@@ -72,7 +72,7 @@ struct TcParams {
   int Cin;                  // conv: input channels (multiple of 32)
   int H, W, B;              // conv: spatial size of the output and batch
   int bw, bh, bn;           // conv: pixel box of one M tile (bw*bh*bn == 128)
-  int tiles_x, tiles_y;     // conv: tiles per row / column
+  int tiles_x, tiles_y;     // conv: tiles per row / column (cdiv: a tile may overhang the map; its outside rows are masked)
   int cstride, cpad;        // conv: stride (1 or 2: TMA element traversal stride) and low-side padding
   // conv3x3, optional: the A operand is silu?(x * a + o), (a, o) = gn_ab[b * Cin + c] (GroupNorm of the input applied while A is
   // split; out-of-image pixels stay 0, as the reference pads the normalised tensor).  C1 < Cin: channels >= C1 come from mapA2
@@ -414,7 +414,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       mrow[i] = (long long)tc_.m0 + r;
       rok[i] = mrow[i] < p.M;
     } else {
-      rok[i] = pb[i] < p.B;
+      // rows of a tile that overhangs the map's right / bottom edge (or the batch) are not pixels: nothing is stored for them
+      rok[i] = pb[i] < p.B && px[i] < p.W && py[i] < p.H;
       mrow[i] = ((long long)pb[i] * p.H + py[i]) * p.W + px[i];
     }
   }
@@ -777,6 +778,26 @@ bool conv_halo_eligible(const Engine& e, int B, int H, int W, int C1, int C2, in
   return true;
 }
 
+// Pixel box of a conv3x3 M tile for an output map whose sides are not both powers of two: bw x bh pixels of bn images, bw*bh*bn == 128,
+// so every factor is a power of two and the box generally overhangs the map.  The box that covers [B, H, W] with the fewest tiles
+// wins (fewest masked rows); ties go to the smallest halo per tile, bn * (bw + 2) * (bh + 2) pixels fetched (then the wider box: longer
+// contiguous TMA rows).  Tiles past the map's edge read TMA's zero fill and their rows are masked in the epilogue.
+static void conv_ragged_tile(int W, int H, int B, int stride, int* bw_out, int* bh_out, int* bn_out) {
+  long long best_tiles = -1, best_halo = 0;
+  for (int bw = TBM; bw >= 1; bw >>= 1) {
+    for (int bh = TBM / bw; bh >= 1; bh >>= 1) {
+      const int bn = TBM / (bw * bh);
+      if (bw * stride > 256 || bh * stride > 256) continue;
+      const long long tiles = (long long)cdiv(W, bw) * cdiv(H, bh) * cdiv(B, bn);
+      const long long halo = (long long)bn * (bw + 2) * (bh + 2);
+      if (best_tiles < 0 || tiles < best_tiles || (tiles == best_tiles && halo < best_halo)) {
+        best_tiles = tiles; best_halo = halo;
+        *bw_out = bw; *bh_out = bh; *bn_out = bn;
+      }
+    }
+  }
+}
+
 bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   // ---- eligibility (everything else takes the FFMA tiles)
   if (a.batch * a.heads != 1 || a.b_kn) return false;
@@ -834,16 +855,22 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
     const bool fused_in = a.A2 != nullptr || a.gn_ab != nullptr;
     CDX_CHECK(!a.A2 || a.gn_ab, "conv3x3: a channel-concat input is only supported together with the fused GroupNorm");
     CDX_CHECK(!fused_in || (a.stride == 1 && a.pad == 1 && (a.C1 % TBK) == 0), "conv3x3: concat / fused GroupNorm input needs stride 1, pad 1, C1 %% 32 == 0");
-    if (a.Hin != a.Hout * a.stride || a.Win != a.Wout * a.stride || !pow2(a.Hout) || !pow2(a.Wout)) return false;
+    if (a.Hin != a.Hout * a.stride || a.Win != a.Wout * a.stride) return false;
     const int B = a.M / (a.Hout * a.Wout);
-    int bw = a.Wout < 16 ? a.Wout : 16;
-    int bh = a.Hout < TBM / bw ? a.Hout : TBM / bw;
-    int bn = TBM / (bw * bh);
+    int bw, bh, bn;
+    if (pow2(a.Hout) && pow2(a.Wout)) {
+      bw = a.Wout < 16 ? a.Wout : 16;
+      bh = a.Hout < TBM / bw ? a.Hout : TBM / bw;
+      bn = TBM / (bw * bh);
+    } else {
+      CDX_CHECK(!fused_in, "conv3x3: fused GroupNorm / concat input on a %dx%d map (power-of-two maps only)", a.Hout, a.Wout);
+      conv_ragged_tile(a.Wout, a.Hout, B, a.stride, &bw, &bh, &bn);
+    }
     if (bn > 256 || bw * a.stride > 256 || bh * a.stride > 256) return false;
     p.mode = 1; p.Cin = Cin; p.H = a.Hout; p.W = a.Wout; p.B = B;      // H, W: OUTPUT grid (tile -> row mapping)
     p.bw = bw; p.bh = bh; p.bn = bn;
     p.cstride = a.stride; p.cpad = a.pad;
-    p.tiles_x = a.Wout / bw; p.tiles_y = a.Hout / bh;
+    p.tiles_x = cdiv(a.Wout, bw); p.tiles_y = cdiv(a.Hout, bh);
     uint64_t d[4] = {(uint64_t)a.C1, (uint64_t)a.Win, (uint64_t)a.Hin, (uint64_t)B};
     uint64_t st[3] = {(uint64_t)a.lda * 4, (uint64_t)a.lda * 4 * a.Win, (uint64_t)a.lda * 4 * a.Win * a.Hin};
     // stride 2 (Downsample convs): TMA traverses every 2nd pixel; box = 2x the number of pixels wanted
@@ -935,7 +962,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   // side outputs fused into the epilogue: range of C always (the split-K reduce kernel covers the split case); GroupNorm
   // statistics when every 32-row quadrant of a tile lies inside one image and the epilogue is the final one
   p.c_amax = a.out_nchw ? nullptr : a.c_amax;
-  const bool quad_ok = a.mode == 1 ? ((p.bw * p.bh) % 32 == 0) : (a.rows_per_batch % 32 == 0);
+  // (a tile that overhangs its map may start a warp on a masked row: its statistics are left to the standalone pass)
+  const bool quad_ok = a.mode == 1 ? ((p.bw * p.bh) % 32 == 0 && p.tiles_x * p.bw == p.W && p.tiles_y * p.bh == p.H) : (a.rows_per_batch % 32 == 0);
   p.c_stats = (a.c_stats && quad_ok && p.splits == 1 && !a.out_nchw && !a.geglu && !a.Ct_hi && !a.Cout_lo && a.ldc == a.N) ? a.c_stats : nullptr;
   if (side_done) *side_done = (p.c_amax ? 1 : 0) | (p.c_stats ? 2 : 0);
   if (e.dry()) return true;
@@ -953,8 +981,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   ensure_attr(e.device);
   ProfScope ps(e, s, a.mode == 1 ? PROF_CONV_TC : PROF_DENSE_TC, 2.0 * a.M * a.N * a.K,
                4.0 * ((double)a.M * a.K / (a.mode == 1 ? 9 : 1) + (double)a.N * a.K + (double)a.M * a.N), 1);
-  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s%s", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
-          p.gn_ab ? " gn" : "", a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "");
+  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s%s box%dx%dx%d", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
+          p.gn_ab ? " gn" : "", a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "", p.bw, p.bh, p.bn);
   if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (fast) launch_gemm<KIND_H16_FAST, 64>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, s);

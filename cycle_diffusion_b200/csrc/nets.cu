@@ -1200,13 +1200,13 @@ struct VaeExec : Exec {
     return out;
   }
 
-  void encode(const float* img_nchw, float* moments_nchw, int B, int R) {
+  void encode(const float* img_nchw, float* moments_nchw, int B, int H, int W) {
     const cdx_vae_config& c = n.vcfg;
     Scope top(e.arena);
     e.pools_reset(s);
     const std::string E = "encoder.";
-    Tensor xin = alloc(B, R, R, c.in_channels);
-    nchw_to_nhwc(e, img_nchw, xin.p, B, c.in_channels, R * R, s);
+    Tensor xin = alloc(B, H, W, c.in_channels);
+    nchw_to_nhwc(e, img_nchw, xin.p, B, c.in_channels, H * W, s);
     Tensor h = conv3(xin, E + "conv_in");
     for (int lvl = 0; lvl < c.n_mult; ++lvl) {
       for (int b = 0; b < c.num_res_blocks; ++b) h = resnet(h, E + "down." + std::to_string(lvl) + ".block." + std::to_string(b));
@@ -1220,16 +1220,16 @@ struct VaeExec : Exec {
     nhwc_to_nchw(e, q.p, moments_nchw, B, q.C, q.H * q.W, s);
   }
 
-  void decode(const float* z_nchw, float* img_nchw, int B, int hsz) {
+  void decode(const float* z_nchw, float* img_nchw, int B, int hsz, int wsz) {
     const cdx_vae_config& c = n.vcfg;
     Scope top(e.arena);
     e.pools_reset(s);
     const std::string D = "decoder.";
-    Tensor zin = alloc(B, hsz, hsz, c.embed_dim);
-    nchw_to_nhwc(e, z_nchw, zin.p, B, c.embed_dim, hsz * hsz, s);
+    Tensor zin = alloc(B, hsz, wsz, c.embed_dim);
+    nchw_to_nhwc(e, z_nchw, zin.p, B, c.embed_dim, hsz * wsz, s);
     if (c.vq) {       // VQModelInterface.decode: quantise first (autoencoder.py:272-281)
-      Tensor zq = alloc(B, hsz, hsz, c.embed_dim);
-      vq_quantize(e, zin.p, n.P("quantize.embedding.weight"), zq.p, (size_t)B * hsz * hsz, c.embed_dim, c.n_embed, s);
+      Tensor zq = alloc(B, hsz, wsz, c.embed_dim);
+      vq_quantize(e, zin.p, n.P("quantize.embedding.weight"), zq.p, (size_t)B * hsz * wsz, c.embed_dim, c.n_embed, s);
       zin = zq;
     }
     Tensor h = linear(zin, "post_quant_conv", true);
@@ -1390,17 +1390,19 @@ void clip_image_features(Net& n, const float* pixels, float* out, int B, cudaStr
   ex.linear_into(pooled.p, W, W, nullptr, 0, 0, B, n.P("visual_projection.weight"), c.proj_dim, nullptr, nullptr, 0, out, c.proj_dim, nullptr, pooled.amax);
 }
 
-void vae_encode(Net& n, const float* img, float* moments, int B, int R, cudaStream_t s) {
+void vae_encode(Net& n, const float* img, float* moments, int B, int H, int W, cudaStream_t s) {
   CDX_CHECK(n.kind == NET_VAE && n.finalized, "vae_encode: not a finalized VAE");
-  CDX_CHECK(R % (1 << (n.vcfg.n_mult - 1)) == 0, "vae_encode: resolution %d", R);
+  const int down = 1 << (n.vcfg.n_mult - 1);
+  CDX_CHECK(H > 0 && W > 0 && H % down == 0 && W % down == 0, "vae_encode: image %dx%d, both sides must be multiples of %d", H, W, down);
   VaeExec ex(n, s);
-  ex.encode(img, moments, B, R);
+  ex.encode(img, moments, B, H, W);
 }
 
-void vae_decode(Net& n, const float* z, float* img, int B, int h, cudaStream_t s) {
+void vae_decode(Net& n, const float* z, float* img, int B, int h, int w, cudaStream_t s) {
   CDX_CHECK(n.kind == NET_VAE && n.finalized, "vae_decode: not a finalized VAE");
+  CDX_CHECK(h > 0 && w > 0, "vae_decode: latent %dx%d", h, w);
   VaeExec ex(n, s);
-  ex.decode(z, img, B, h);
+  ex.decode(z, img, B, h, w);
 }
 
 }  // namespace cdx

@@ -77,8 +77,8 @@ void net_ensure_blob(Net& n);
 // at the start of the loop) -> context K / V projections are taken from n.ctxkv instead of being recomputed
 void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* ctx, int ctx_len, float* out_nchw, int B, int H,
                   int W, cudaStream_t s, bool reuse_ctx = false);
-void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int R, cudaStream_t s);
-void vae_decode(Net& n, const float* z_nchw, float* img_nchw, int B, int h, cudaStream_t s);
+void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int H, int W, cudaStream_t s);
+void vae_decode(Net& n, const float* z_nchw, float* img_nchw, int B, int h, int w, cudaStream_t s);
 void text_encode(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);
 void text_features(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);                // CLIP.encode_text   -> [B, proj_dim]
 void clip_image_features(Net& n, const float* pixels, float* out, int B, cudaStream_t s);            // CLIP.encode_image  -> [B, proj_dim]

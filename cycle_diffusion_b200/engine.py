@@ -494,21 +494,21 @@ class VAE(Net):
         self.down = 2 ** (len(cfg['ch_mult']) - 1)
 
     def encode_moments(self, img):
+        """img [B,3,H,W] in [-1,1], H and W multiples of ``self.down`` -> moments [B, 2*embed_dim, H/down, W/down]."""
         e = self.engine
         img = _f32c(img, e.device)
-        B, _, R, R2 = img.shape
-        assert R == R2
-        out = e.empty(B, (1 if self.cfg.get('vq') else 2) * self.cfg['embed_dim'], R // self.down, R // self.down)      # vq: h itself
-        check(lib.cdx_vae_encode(self.h, _ptr(img), _ptr(out), B, R, e.stream))
+        B, _, H, W = img.shape
+        out = e.empty(B, (1 if self.cfg.get('vq') else 2) * self.cfg['embed_dim'], H // self.down, W // self.down)      # vq: h itself
+        check(lib.cdx_vae_encode_hw(self.h, _ptr(img), _ptr(out), B, H, W, e.stream))
         return out
 
     def decode(self, z):
+        """z [B,embed_dim,h,w] -> img [B, out_ch, h*down, w*down]."""
         e = self.engine
         z = _f32c(z, e.device)
-        B, _, h, h2 = z.shape
-        assert h == h2
-        out = e.empty(B, self.cfg['out_ch'], h * self.down, h * self.down)
-        check(lib.cdx_vae_decode(self.h, _ptr(z), _ptr(out), B, h, e.stream))
+        B, _, h, w = z.shape
+        out = e.empty(B, self.cfg['out_ch'], h * self.down, w * self.down)
+        check(lib.cdx_vae_decode_hw(self.h, _ptr(z), _ptr(out), B, h, w, e.stream))
         return out
 
 

@@ -46,6 +46,11 @@ class CycleDiffusionPipeline:
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
         sources = [source_prompt] if isinstance(source_prompt, str) else list(source_prompt)
         assert torch.is_tensor(image) and image.dim() == 4, 'image: float tensor [B,3,H,W] in [0,1] (PIL preprocessing is host glue)'
+        # any H x W the first stage and the U-Net can both halve all the way down: no silent resize
+        side = g.vae.down * 2 ** (len(g.unet.cfg['channel_mult']) - 1)
+        if image.shape[2] % side or image.shape[3] % side:
+            raise ValueError(f'image height and width must both be multiples of {side} (the first stage\'s factor {g.vae.down} x '
+                             f'2^(len(channel_mult) - 1)), got {image.shape[2]}x{image.shape[3]}')
         B = image.shape[0] * num_images_per_prompt
         if num_images_per_prompt > 1:
             image = image.repeat_interleave(num_images_per_prompt, dim=0)

@@ -162,6 +162,9 @@ int cdx_unet_forward(cdx_net* n, const float* x_dev, const float* t_dev, const f
 /* AutoencoderKL.encode (autoencoder.py:324-328 + AEM:434-459): img [B,3,R,R] in [-1,1] ->
  * moments [B, 2*embed_dim, R/8, R/8] (mean | logvar), both NCHW dev. */
 int cdx_vae_encode(cdx_net* n, const float* img_dev, float* moments_dev, int B, int R, void* stream);
+/* The same for any image shape: img [B,3,H,W] -> moments [B, 2*embed_dim, H/f, W/f], f = 2^(len(ch_mult)-1).
+ * H and W must be multiples of f (CDX_E_INVALID otherwise).  cdx_vae_encode(..., R, ...) is this call with H = W = R. */
+int cdx_vae_encode_hw(cdx_net* n, const float* img_dev, float* moments_dev, int B, int H, int W, void* stream);
 /* FrozenCLIPEmbedder.forward after tokenisation (ldm/modules/encoders/modules.py:140-158 -> transformer(input_ids=tokens)
  * .last_hidden_state; HF modeling_clip.py CLIPTextTransformer.forward, transformers==4.19.2 pinned by environment.yml:466):
  * token + position embedding, `layers` pre-LN blocks with causal self-attention and quick-GELU MLP, final LayerNorm.
@@ -172,6 +175,9 @@ int cdx_text_encode(cdx_net* n, const int* ids_dev, int B, int L, float* out_dev
 /* AutoencoderKL.decode (autoencoder.py:330-333 + AEM:535-568): z [B,embed_dim,h,h] (already
  * divided by scale_factor) -> img [B, out_ch, 8h, 8h]. */
 int cdx_vae_decode(cdx_net* n, const float* z_dev, float* img_dev, int B, int h, void* stream);
+/* The same for any latent shape: z [B,embed_dim,h,w] -> img [B, out_ch, f*h, f*w], f = 2^(len(ch_mult)-1).
+ * cdx_vae_decode(..., h, ...) is this call with w = h. */
+int cdx_vae_decode_hw(cdx_net* n, const float* z_dev, float* img_dev, int B, int h, int w, void* stream);
 
 /* ---------------------------------------------------------------- per-step kernels ---------- */
 /* All element counts `n` are B*C*H*W of one NCHW tensor; scalars are the batch-uniform fp32

@@ -35,26 +35,62 @@ int guard(F&& f) {
 // The arena, the context K/V cache and the weight planes are reused from call to call with no synchronisation of their own,
 // which is only safe in stream order.  A caller that switches streams between calls is handed over explicitly: every call
 // records an event at its end, and a call arriving on a different stream first waits for it.
+// `e2`: the engine of a second net taking part in the same call (two-model loops); both arenas are sized by the one dry pass, and
+// both engines are handed over on `s`.
 template <class F>
-void with_arena(Engine& e, cudaStream_t s, F&& f) {
+void with_arena(Engine& e, cudaStream_t s, F&& f, Engine* e2 = nullptr) {
+  Engine* const engs[2] = {&e, e2 == &e ? nullptr : e2};
+  if (engs[1]) CDX_CHECK(engs[1]->device == e.device, "the two nets of a call live on devices %d and %d", e.device, engs[1]->device);
   CDX_CUDA(cudaSetDevice(e.device));
-  e.arena.begin_dry();
+  for (Engine* x : engs) if (x) x->arena.begin_dry();
   try {
     f();
   } catch (...) {
-    e.arena.dry = false;
-    e.arena.off = 0;
+    for (Engine* x : engs) if (x) { x->arena.dry = false; x->arena.off = 0; }
     throw;
   }
-  e.arena.end_dry();
-  if (!e.done_ev) CDX_CUDA(cudaEventCreateWithFlags(&e.done_ev, cudaEventDisableTiming));
-  if (e.ev_recorded && e.last_stream != s) CDX_CUDA(cudaStreamWaitEvent(s, e.done_ev, 0));
+  for (Engine* x : engs) {
+    if (!x) continue;
+    x->arena.end_dry();
+    if (!x->done_ev) CDX_CUDA(cudaEventCreateWithFlags(&x->done_ev, cudaEventDisableTiming));
+    if (x->ev_recorded && x->last_stream != s) CDX_CUDA(cudaStreamWaitEvent(s, x->done_ev, 0));
+  }
   f();
-  e.arena.off = 0;
-  CDX_CUDA(cudaEventRecord(e.done_ev, s));
-  e.ev_recorded = true;
-  e.last_stream = s;
+  for (Engine* x : engs) {
+    if (!x) continue;
+    x->arena.off = 0;
+    CDX_CUDA(cudaEventRecord(x->done_ev, s));
+    x->ev_recorded = true;
+    x->last_stream = s;
+  }
 }
+
+// Streams of the two U-Net calls of one two-model step.  The calls are independent (each reads its own chain's x_t); only the
+// elementwise step after them joins the chains.  Nets of different engines share no arena, pools or caches, so the target's call
+// runs on the target engine's side stream, forked from and joined back into `s` once per step.  Nets of one engine run in order
+// on `s`.
+struct PairStreams {
+  Engine& tgt;
+  cudaStream_t s;
+  bool two;
+  PairStreams(Engine& src_eng, Engine& tgt_eng, cudaStream_t st) : tgt(tgt_eng), s(st), two(&src_eng != &tgt_eng) {
+    if (!two || tgt.dry() || tgt.side) return;
+    CDX_CUDA(cudaStreamCreateWithFlags(&tgt.side, cudaStreamNonBlocking));     // overlaps a caller on the legacy default stream
+    CDX_CUDA(cudaEventCreateWithFlags(&tgt.fork_ev, cudaEventDisableTiming));
+    CDX_CUDA(cudaEventCreateWithFlags(&tgt.join_ev, cudaEventDisableTiming));
+  }
+  cudaStream_t target_stream() const { return two ? tgt.side : s; }
+  void fork() {
+    if (!two || tgt.dry()) return;
+    CDX_CUDA(cudaEventRecord(tgt.fork_ev, s));
+    CDX_CUDA(cudaStreamWaitEvent(tgt.side, tgt.fork_ev, 0));
+  }
+  void join() {
+    if (!two || tgt.dry()) return;
+    CDX_CUDA(cudaEventRecord(tgt.join_ev, tgt.side));
+    CDX_CUDA(cudaStreamWaitEvent(s, tgt.join_ev, 0));
+  }
+};
 
 inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
@@ -123,7 +159,10 @@ struct LatentLoopArgs {
   int B = 0, C = 0, h = 0, w = 0;
 };
 
-void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s) {
+// `tgt_net`: the target chain runs under its own net (two-model translation, LOCK mode, context-free): the step's U-Net call is split
+// into a source call and a target call over the two halves of `xin` / `eout`.  With n_rec < n_steps the target chain continues
+// alone after the last recovered step, with `extra` noise (ddim.py:640).
+void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s, Net* tgt_net = nullptr) {
   Engine& e = *unet.eng;
   const int B = a.B, chw = a.C * a.h * a.w;
   const size_t n = (size_t)B * chw;
@@ -183,11 +222,22 @@ void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s) {
     for (int sg = 0; sg < nseg_tgt; ++sg) copy_dd(e, yb[0], xin + (size_t)sg * n, n, s);
   }
   const int iters = e.dry() ? std::min(loop_steps, 1) : loop_steps;
+  PairStreams ps(e, tgt_net ? *tgt_net->eng : e, s);
   for (int i = 0; i < iters; ++i) {
-    unet_forward(unet, xin, tdev + (size_t)i * nb, ctx_in, a.L, eout, nb, a.h, a.w, s, true);
+    const bool enc_i = enc && i < a.n_rec;
+    if (!tgt_net) {
+      unet_forward(unet, xin, tdev + (size_t)i * nb, ctx_in, a.L, eout, nb, a.h, a.w, s, true);
+    } else {
+      const size_t ns = (size_t)nseg_src * B;
+      ps.fork();
+      if (enc_i) unet_forward(unet, xin, tdev + (size_t)i * nb, nullptr, 0, eout, (int)ns, a.h, a.w, s);
+      unet_forward(*tgt_net, xin + ns * chw, tdev + (size_t)i * nb + ns, nullptr, 0, eout + ns * chw, nb - (int)ns, a.h, a.w,
+                   ps.target_stream());
+      ps.join();
+    }
     LatentStep st;
     st.n = n; st.chw = chw;
-    if (enc) {
+    if (enc_i) {
       st.enc = 1;
       st.x0 = a.x0; st.xt = xb[0]; st.xn = xb[1];
       st.es_c = es_c; st.es_uc = es_uc; st.s_scale = a.s_scale; st.s_scale_v = a.s_scale_v; st.cs = a.coef[i];
@@ -202,12 +252,14 @@ void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s) {
       if (!enc) {
         if (i < a.n_eps) { st.eps_in = a.z_in + (size_t)(1 + i) * chw; st.eps_stride = (long long)(a.n_eps + 1) * chw; }
         else { st.eps_in = a.extra + (size_t)(i - a.n_eps) * n; st.eps_stride = chw; }
+      } else if (!enc_i) {
+        st.eps_in = a.extra + (size_t)(i - a.n_rec) * n; st.eps_stride = chw;
       }
       st.y_out = (i == loop_steps - 1) ? a.x_out : yb[1];
     }
     st.xin = xin; st.nseg_src = nseg_src; st.nseg_tgt = nseg_tgt;
     latent_step(e, st, s);
-    if (enc) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
+    if (enc_i) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
     if (dec) std::swap(yb[0], yb[1]);
   }
 }
@@ -250,6 +302,9 @@ void cdx_engine_destroy(cdx_engine* e) {
   cudaDeviceSynchronize();
   e->e.arena.destroy();
   if (e->e.done_ev) cudaEventDestroy(e->e.done_ev);
+  if (e->e.side) cudaStreamDestroy(e->e.side);
+  if (e->e.fork_ev) cudaEventDestroy(e->e.fork_ev);
+  if (e->e.join_ev) cudaEventDestroy(e->e.join_ev);
   if (e->e.amax_pool) cudaFree(e->e.amax_pool);
   delete e;
 }
@@ -628,6 +683,61 @@ int cdx_pixel_decode(cdx_net* un, const float* z, int n_eps, const cdx_pixel_coe
         std::swap(xa, xb);
       }
     });
+  });
+}
+
+int cdx_pixel_cycle_lockstep(cdx_net* src, cdx_net* tgt, const float* x0, const cdx_pixel_coef* coef, const float* t_host, int i0, int i1,
+                             const float* noise, float sqrt_a_T, float sqrt_1ma_T, float* state, int B, int C, int R, void* stream) {
+  return guard([&] {
+    CDX_CHECK(src && src->owner && tgt && tgt->owner && x0 && noise && state && B > 0, "pixel_cycle_lockstep: null argument");
+    CDX_CHECK(i0 >= 0 && i1 >= i0 && (i1 == i0 || (coef && t_host)), "pixel_cycle_lockstep: steps [%d, %d)", i0, i1);
+    Engine& es = src->owner->e;
+    Engine& et = tgt->owner->e;
+    cudaStream_t s = S(stream);
+    const int chw = C * R * R, steps = i1 - i0;
+    const int net_chw_s = src->n->ucfg.out_channels * R * R, net_chw_t = tgt->n->ucfg.out_channels * R * R;
+    const size_t n = (size_t)B * chw;
+    float* xs = state;
+    float* ys = state + n;
+    with_arena(es, s, [&] {
+      Scope sc_s(es.arena), sc_t(et.arena);
+      float* e_src = (float*)es.arena.alloc((size_t)B * net_chw_s * sizeof(float));
+      float* e_tgt = (float*)et.arena.alloc((size_t)B * net_chw_t * sizeof(float));
+      float* tdev = (float*)es.arena.alloc((size_t)std::max(steps, 1) * B * sizeof(float));
+      if (steps) upload_timesteps(es, t_host + i0, steps, B, tdev, s);
+      const float* nz = noise;
+      if (i0 == 0) {                                                                      // sample_xt, DW:310-314 (incl. the DW:483 index quirk)
+        q_sample(es, x0, nz, sqrt_a_T, sqrt_1ma_T, xs, n, s);
+        copy_dd(es, xs, ys, n, s);
+        nz += n;
+      }
+      PairStreams ps(es, et, s);
+      const int iters = es.dry() ? std::min(steps, 1) : steps;
+      for (int k = 0; k < iters; ++k) {
+        ps.fork();
+        unet_forward(*src->n, xs, tdev + (size_t)k * B, nullptr, 0, e_src, B, R, R, s);
+        unet_forward(*tgt->n, ys, tdev + (size_t)k * B, nullptr, 0, e_tgt, B, R, R, ps.target_stream());
+        ps.join();
+        pixel_lockstep_step(es, x0, xs, ys, e_src, e_tgt, nz + (size_t)k * n, coef[i0 + k], B, chw, net_chw_s, net_chw_t, s);
+      }
+    }, &et);
+  });
+}
+
+int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx_ddim_coef* coef, const float* t_host, int n_steps, int n_rec,
+                          const float* noise, float sqrt_a_T, float sqrt_1ma_T, const float* extra_noise, float* x_out, int B, int C, int h,
+                          int w, void* stream) {
+  return guard([&] {
+    CDX_CHECK(src && src->owner && tgt && tgt->owner && x0 && coef && t_host && noise && x_out, "latent_cycle_pair: null argument");
+    CDX_CHECK(n_steps >= 1 && n_rec >= 0 && n_rec <= n_steps, "latent_cycle_pair: n_steps=%d n_rec=%d", n_steps, n_rec);
+    CDX_CHECK(n_rec == n_steps || extra_noise, "latent_cycle_pair: %d steps, %d recovered noises and no extra noise", n_steps, n_rec);
+    CDX_CHECK(src->n->ucfg.context_dim == 0 && tgt->n->ucfg.context_dim == 0, "latent_cycle_pair: unconditional U-Nets only");
+    for (int i = 0; i < n_rec; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_cycle_pair: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
+    LatentLoopArgs a;
+    a.mode = LOOP_LOCK;
+    a.x0 = x0; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_rec; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
+    a.extra = extra_noise; a.x_out = x_out; a.B = B; a.C = C; a.h = h; a.w = w;
+    with_arena(src->owner->e, S(stream), [&] { run_latent_loop(*src->n, a, S(stream), tgt->n); }, &tgt->owner->e);
   });
 }
 

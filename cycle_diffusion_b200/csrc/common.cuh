@@ -89,6 +89,10 @@ struct Engine {
   cudaStream_t last_stream = nullptr;   // stream of the previous arena-using call and the event recorded at its end
   cudaEvent_t done_ev = nullptr;
   bool ev_recorded = false;
+  // second stream (non-blocking, created on first use) on which the two-model loops run this engine's U-Net calls when the other
+  // chain's net lives in another engine; fork / join events order it against the caller's stream once per step
+  cudaStream_t side = nullptr;
+  cudaEvent_t fork_ev = nullptr, join_ev = nullptr;
   uint64_t launches = 0;
   bool dry() const { return arena.dry; }
 };
@@ -294,6 +298,10 @@ void pixel_compute_eps(Engine& e, const float* xt, const float* xt_next, const f
                        int B, int chw, int net_chw, cudaStream_t s);
 void pixel_step_with_eps(Engine& e, const float* xt, const float* et, const float* eps, const cdx_pixel_coef& c, float* out,
                          int B, int chw, int net_chw, cudaStream_t s);
+// one step of the two-model pixel loop (identical schedules): x_{t-1} = sample_xt_next(x0, xs, noise), eps = compute_eps(xs, x_{t-1},
+// et_src), ys <- denoising_step_with_eps(ys, et_tgt, eps), xs <- x_{t-1}; bit-identical to the three kernels above
+void pixel_lockstep_step(Engine& e, const float* x0, float* xs, float* ys, const float* et_src, const float* et_tgt, const float* noise,
+                         const cdx_pixel_coef& c, int B, int chw, int net_chw_src, int net_chw_tgt, cudaStream_t s);
 
 inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 

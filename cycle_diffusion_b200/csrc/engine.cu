@@ -66,11 +66,20 @@ ProfScope::~ProfScope() {
   if (idx >= 0) cudaEventRecord(e.prof.recs[idx].b, s);
 }
 
+// A pool is created by the first network call that needs it, in the middle of enqueueing that call.  cudaMemset runs on the legacy
+// default stream, which a non-blocking stream does not wait for: the target U-Net of a two-engine lock-step loop runs on such a
+// stream (PairStreams), and its kernels would accumulate into the pool while the memset clears it.  Wait for the zeroing once.
+static void wait_pool_zeroed() {
+  const cudaError_t err = cudaDeviceSynchronize();
+  if (err != cudaSuccess) throw Error(CDX_E_CUDA, std::string("pool zeroing: ") + cudaGetErrorString(err));
+}
+
 float* Engine::amax_slot() {
   if (dry()) return reinterpret_cast<float*>((uintptr_t)0x100);   // never dereferenced
   if (!amax_pool) {
     if (cudaMalloc(&amax_pool, (size_t)amax_cap * sizeof(float)) != cudaSuccess) throw Error(CDX_E_NOMEM, "amax pool allocation failed");
     if (cudaMemset(amax_pool, 0, (size_t)amax_cap * sizeof(float)) != cudaSuccess) throw Error(CDX_E_CUDA, "amax pool memset failed");
+    wait_pool_zeroed();
   }
   if (amax_used >= amax_cap) throw Error(CDX_E_NOMEM, "amax pool exhausted (engine bug: amax_reset not called per network call)");
   return amax_pool + amax_used++;
@@ -81,6 +90,7 @@ double* Engine::stat_alloc(size_t n) {
   if (!stat_pool) {
     if (cudaMalloc(&stat_pool, stat_cap * sizeof(double)) != cudaSuccess) throw Error(CDX_E_NOMEM, "statistics pool allocation failed");
     if (cudaMemset(stat_pool, 0, stat_cap * sizeof(double)) != cudaSuccess) throw Error(CDX_E_CUDA, "statistics pool memset failed");
+    wait_pool_zeroed();
   }
   if (stat_used + n > stat_cap) throw Error(CDX_E_NOMEM, "statistics pool exhausted");
   double* p = stat_pool + stat_used;

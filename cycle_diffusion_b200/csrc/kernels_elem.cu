@@ -330,6 +330,35 @@ __global__ void pixel_step_kernel(const float* __restrict__ xt, const float* __r
     }
   }
 }
+// One step of the two-model pixel loop: the three kernels above in one launch, same op order, x_{t-1} of the source chain and the
+// recovered noise held in registers.  xs / ys (source x_t, target x_t) are advanced in place.  Every input but x0 and the noise
+// slice was written by the launches just before this one, so all loads take the coherent path.
+__global__ void pixel_lockstep_kernel(const float* x0, float* xs, float* ys, const float* es_, const float* et_, const float* nz,
+                                      cdx_pixel_coef c, int B, int chw, int net_chw_s, int net_chw_t) {
+  const size_t n = (size_t)B * chw;
+  GRID_STRIDE(i, n) {
+    const size_t b = i / chw, r = i - b * chw;
+    const float x0v = __ldcg(x0 + i), xt = __ldcg(xs + i), yt = __ldcg(ys + i), z = __ldcg(nz + i);
+    const float es = __ldcg(es_ + b * net_chw_s + r), et = __ldcg(et_ + b * net_chw_t + r);
+    float yn, xn;
+    if (c.ddpm) {
+      xn = ADD(ADD(MUL(c.w0, x0v), MUL(c.wt, xt)), MUL(c.post_std, z));                     // DW:293, 297
+      const float mean_s = MUL(c.inv_sqrt_1m_bt, SUB(xt, MUL(c.weight, es)));               // DW:266
+      const float eps = DIV(SUB(xn, mean_s), c.std_model);                                  // DW:268
+      const float mean_t = MUL(c.inv_sqrt_1m_bt, SUB(yt, MUL(c.weight, et)));               // DW:204
+      yn = ADD(mean_t, MUL(MUL(c.mask, c.std_model), eps));                                 // DW:208
+    } else {
+      const float e_post = DIV(SUB(xt, MUL(c.sqrt_at, x0v)), c.sqrt_1m_at);                 // DW:299
+      xn = ADD(ADD(MUL(c.sqrt_at_next, x0v), MUL(c.c2, e_post)), MUL(c.c1, z));            // DW:302
+      const float x0_s = DIV(SUB(xt, MUL(es, c.sqrt_1m_at)), c.sqrt_at);                    // DW:271
+      const float eps = DIV(SUB(SUB(xn, MUL(c.sqrt_at_next, x0_s)), MUL(c.c2, es)), c.c1);  // DW:275
+      const float x0_t = DIV(SUB(yt, MUL(et, c.sqrt_1m_at)), c.sqrt_at);                    // DW:213
+      yn = ADD(ADD(MUL(c.sqrt_at_next, x0_t), MUL(c.c2, et)), MUL(c.c1, eps));              // DW:222
+    }
+    xs[i] = xn;
+    ys[i] = yn;
+  }
+}
 
 }  // namespace
 
@@ -577,6 +606,10 @@ void pixel_compute_eps(Engine& e, const float* xt, const float* xn, const float*
 void pixel_step_with_eps(Engine& e, const float* xt, const float* et, const float* eps, const cdx_pixel_coef& c, float* out, int B, int chw,
                          int net_chw, cudaStream_t s) {
   LAUNCH1(pixel_step_kernel, (size_t)B * chw, xt, et, eps, c, out, B, chw, net_chw);
+}
+void pixel_lockstep_step(Engine& e, const float* x0, float* xs, float* ys, const float* et_src, const float* et_tgt, const float* noise,
+                         const cdx_pixel_coef& c, int B, int chw, int net_chw_src, int net_chw_tgt, cudaStream_t s) {
+  LAUNCH1(pixel_lockstep_kernel, (size_t)B * chw, x0, xs, ys, et_src, et_tgt, noise, c, B, chw, net_chw_src, net_chw_tgt);
 }
 
 // softmax(q k^T * scale) v through two batched contractions and a row softmax.  Scores live in the arena

@@ -462,6 +462,36 @@ class UNet(Net):
                                    sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(z), B, Cc, R, e.stream))
         return z
 
+    def pixel_cycle_lockstep(self, target, x0, sched, state, noise, i0, i1):
+        """Steps [i0, i1) of the two-model pixel loop (cdx_pixel_cycle_lockstep): this net runs the source chain's DPM-Encoder,
+        ``target`` (a UNet) the target chain's decode, both on ``sched``.  state [2, B, C, R, R] (source x_t, target x_t) is
+        advanced in place; noise [i1 - i0, B, C, R, R], preceded by the x_T draw when i0 == 0 (which initialises state)."""
+        e = self.engine
+        x0, noise = _f32c(x0, e.device), _f32c(noise, e.device)
+        B, Cc, R, _ = x0.shape
+        n_rec = sched.es_steps - 1
+        assert 0 <= i0 <= i1 <= n_rec, f'steps [{i0}, {i1}) of {n_rec}'
+        assert state.shape == (2, B, Cc, R, R) and state.dtype == torch.float32 and state.is_contiguous() and state.device == e.device
+        assert noise.shape == (i1 - i0 + (i0 == 0), B, Cc, R, R), f'noise shape {tuple(noise.shape)}'
+        coef = sched.coef_array(sched.coef[:n_rec]) if n_rec else None
+        t = (C.c_float * max(n_rec, 1))(*sched.t_loop[:n_rec])
+        check(lib.cdx_pixel_cycle_lockstep(self.h, target.h, _ptr(x0), coef, t, i0, i1, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T,
+                                           _ptr(state), B, Cc, R, e.stream))
+
+    def latent_cycle_pair(self, target, x0, sched, n_rec, noise, extra_noise=None):
+        """latent_encode under this net followed by latent_decode under ``target`` (a UNet), both context-free at scale 1, in one
+        lock-step loop (cdx_latent_cycle_pair): x0 [B,C,h,w] -> decoded latent [B,C,h,w].  noise as for latent_encode; extra_noise
+        [refine_steps - n_rec, B,C,h,w] for the steps the target chain runs alone."""
+        e = self.engine
+        x0, noise = _f32c(x0, e.device), _f32c(noise, e.device)
+        extra_noise = _f32c(extra_noise, e.device) if extra_noise is not None else None
+        B, Cc, h, w = x0.shape
+        assert noise.shape == (n_rec + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
+        out = e.empty(B, Cc, h, w)
+        check(lib.cdx_latent_cycle_pair(self.h, target.h, _ptr(x0), sched.coef_array(), sched.t_array(), sched.refine_steps, n_rec, _ptr(noise),
+                                        sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(extra_noise), _ptr(out), B, Cc, h, w, e.stream))
+        return out
+
     def pixel_decode(self, z, sched, coefs=None, t_loop=None, last_noise=None):
         e = self.engine
         z = _f32c(z, e.device)

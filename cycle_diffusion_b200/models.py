@@ -8,7 +8,7 @@ Extra keyword arguments (engine, state_dict, cond_stage, ...) are forwarded to t
 import torch
 import torch.nn as nn
 
-from .wrappers import get_gan_wrapper
+from .wrappers import get_gan_wrapper, lockstep_compatible
 
 
 def _gan_args(args):
@@ -59,8 +59,12 @@ class UnsupervisedTranslation(nn.Module):
             img = self.target_gan_wrapper(z=z, class_label=class_label)
         else:
             assert class_label is None
-            z = self.source_gan_wrapper.encode(image=original_image)
-            img = self.target_gan_wrapper(z=z)
+            if lockstep_compatible(self.source_gan_wrapper, self.target_gan_wrapper):
+                # the reference's encode -> z -> target(z) (unsupervised_translation.py:44-49) as one lock-step loop of both models
+                img = self.source_gan_wrapper.cycle(original_image, self.target_gan_wrapper)
+            else:
+                z = self.source_gan_wrapper.encode(image=original_image)
+                img = self.target_gan_wrapper(z=z)
         losses = dict()
         weighted_loss = torch.zeros_like(sample_id).float()
         return (original_image, img), weighted_loss, losses

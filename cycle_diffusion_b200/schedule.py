@@ -65,6 +65,14 @@ class DDIMSchedule:
         return (ctypes.c_float * len(self.t_loop))(*self.t_loop)
 
 
+def same_schedule(a, b):
+    """Do two schedules drive identical loops: same kind and length, bit-identical coefficient tables, timesteps and x_T scalars?
+    (Two models may then run their chains in lock-step.)"""
+    return (type(a) is type(b) and getattr(a, 'es_steps', None) == getattr(b, 'es_steps', None) and a.t_loop == b.t_loop
+            and (a.sqrt_a_T, a.sqrt_1ma_T) == (b.sqrt_a_T, b.sqrt_1ma_T) and len(a.coef) == len(b.coef)
+            and all(bytes(x) == bytes(y) for x, y in zip(a.coef, b.coef)))
+
+
 # ------------------------------------------------------------------------------------------ pixel models
 class PixelSchedule:
     """Per-step scalars of DDPMDDIMWrapper.encode / generate (ddpm_ddim_wrapper.py:392-523)."""

@@ -26,7 +26,11 @@ import torch
 
 from . import specs
 from .engine import Engine, UNet, VAE
-from .schedule import DDIMSchedule, PixelSchedule
+from .schedule import DDIMSchedule, PixelSchedule, same_schedule
+
+# Recovery steps per chunk of the lock-step pixel loop (DDPMDDIMWrapper.cycle): device memory holds one chunk of noise, not
+# es_steps of it.  At 256^2 and batch 8 a chunk is 32 x 8 x 3 x 256^2 x 4 B = 0.2 GB (the two-phase path: 1.3 GB per image at 850 steps).
+LOCKSTEP_CHUNK = 32
 
 
 class ClipTextCondStage:
@@ -439,10 +443,22 @@ class LatentDiffStochasticWrapper(torch.nn.Module):
         n_extra = sched.refine_steps - (eps_list.shape[1] - 1)
         extra = torch.stack([torch.randn(eps_list[:, 0].shape) for _ in range(n_extra)]) if n_extra > 0 else None      # ddim.py:640
         sample = g.unet.latent_decode(eps_list, None, None, 1.0, sched, extra)
+        return self._refine_and_decode(sample)
+
+    def _refine_and_decode(self, sample):
+        g = self.generator
         if self.refine_steps > 0:                                     # refine_eta = 1 (latentdiff_stochastic_wrapper.py:68-77)
             noise = torch.stack([torch.randn(sample.shape) for _ in range(self.refine_steps + 1)])
             sample = g.unet.latent_refine(sample, None, None, 1.0, self.custom_steps, self.refine_steps, noise, g.alphas_cumprod)
         return g.decode_first_stage(sample)
+
+    def _encode_noise(self, sched, n_rec, shape):
+        noise = torch.zeros((n_rec + 1,) + tuple(shape))
+        noise[0] = torch.randn(shape)
+        for i in range(n_rec):
+            if sched.refine_steps - 1 - i != 0:                        # ddim.py:583-584: the last step returns x0 without a draw
+                noise[1 + i] = torch.randn(shape)
+        return noise
 
     def encode(self, image, class_label=None):
         g, e = self.generator, self.engine
@@ -453,14 +469,29 @@ class LatentDiffStochasticWrapper(torch.nn.Module):
         assert self.eta > 0
         sched = self._sched()
         n_rec = max(0, min(sched.refine_steps, self.white_box_steps - 1))
-        noise = torch.zeros((n_rec + 1,) + tuple(x0.shape))
-        noise[0] = torch.randn(x0.shape)
-        for i in range(n_rec):
-            if sched.refine_steps - 1 - i != 0:                        # ddim.py:583-584: the last step returns x0 without a draw
-                noise[1 + i] = torch.randn(x0.shape)
+        noise = self._encode_noise(sched, n_rec, x0.shape)
         z = g.unet.latent_encode(x0, None, None, 1.0, sched, n_rec, noise).view(bsz, -1)
         assert z.shape[1] == self.latent_dim
         return z
+
+    def cycle(self, image, target):
+        """``target(self.encode(image))`` for a target wrapper with the same schedule (see lockstep_compatible), as one lock-step
+        loop (cdx_latent_cycle_pair): the source chain runs under this wrapper's U-Net, the target chain under the target's, and
+        the noise recovered at a step is consumed by the target chain at once, so ``z`` is never written.  Same random draws in
+        the same order, same result bit for bit.  Then the target's own refine pass and first-stage decode."""
+        g, e = self.generator, self.engine
+        image = e.shift_scale(image, -0.5, 2.0)
+        assert image.shape[2] == image.shape[3] == self.resolution
+        x0 = g.get_first_stage_encoding(g.encode_first_stage(image))
+        assert self.eta > 0
+        sched = self._sched()
+        n_rec = max(0, min(sched.refine_steps, self.white_box_steps - 1))
+        assert n_rec + 1 == self.white_box_steps, 'white_box_steps - 1 > custom_steps (encode() would fail the latent_dim check)'
+        noise = self._encode_noise(sched, n_rec, x0.shape)
+        n_extra = sched.refine_steps - n_rec
+        extra = torch.stack([torch.randn(x0.shape) for _ in range(n_extra)]) if n_extra > 0 else None      # ddim.py:640
+        sample = g.unet.latent_cycle_pair(target.generator.unet, x0, sched, n_rec, noise, extra)
+        return target.engine.shift_scale(target._refine_and_decode(sample), 1.0, 0.5)
 
     def forward(self, z, class_label=None):
         return self.engine.shift_scale(self.generate(z, class_label), 1.0, 0.5)
@@ -532,6 +563,10 @@ class DDPMDDIMWrapper(torch.nn.Module):
         shape = eps_list[:, 0].shape
         last = self._randn(shape).unsqueeze(0)       # denoising_step draws once more; the draw is multiplied by 0 (DU:115,131)
         x = self.generator.pixel_decode(eps_list, self.sched, last_noise=last)
+        return self._refine(x, shape)
+
+    def _refine(self, x, shape):
+        bsz = shape[0]
         if self.refine_steps != 0:
             assert self.refine_steps < self.custom_steps
             ref = PixelSchedule(self.sample_type, self.custom_steps, self.es_steps, 1 if self.sample_type == 'ddim' else None, self.t_0)
@@ -566,9 +601,82 @@ class DDPMDDIMWrapper(torch.nn.Module):
         img = self.generate(z, class_label)
         return self.engine.shift_scale(img, 1.0, 0.5)
 
+    def cycle(self, image, target):
+        """``target(self.encode(image))`` for a target wrapper with the same schedule (see lockstep_compatible), as one lock-step
+        loop (cdx_pixel_cycle_lockstep): per step the source U-Net call on the source chain and the target U-Net call on the target
+        chain, then one fused kernel that recovers the step's noise and advances the target chain with it, so ``z`` is never
+        written.  The loop walks the es_steps - 1 recovery steps in chunks of LOCKSTEP_CHUNK, so device memory holds one chunk of
+        noise.  Then the target's own last step and refine pass, as target.generate does.
+
+        rng='cpu': the same draws in the same order as the two calls (x_T, one per recovery step, then the target's ``last`` and
+        refine draws), so the result is bit-identical.  They are drawn chunk by chunk into two pinned buffers used in turn, so the
+        host draws chunk k+1 while the device runs chunk k.  rng='cuda': drawn on the device per chunk, which matches the two-phase
+        path in distribution only (bit for bit when one chunk covers every step)."""
+        e = self.engine
+        x = e.shift_scale(image, -0.5, 2.0)
+        assert x.shape[2] == x.shape[3] == self.resolution
+        shape = tuple(x.shape)
+        n_rec = self.es_steps - 1
+        chunk = max(1, int(LOCKSTEP_CHUNK))
+        state = e.empty(2, *shape)
+        if self.rng == 'cuda':
+            for i0, i1 in _chunk_ranges(n_rec, chunk):
+                noise = torch.randn((i1 - i0 + (i0 == 0),) + shape, device=e.device)
+                self.generator.pixel_cycle_lockstep(target.generator, x, self.sched, state, noise, i0, i1)
+        else:
+            bufs = [torch.empty((min(chunk, n_rec) + 1,) + shape, pin_memory=True) for _ in range(2 if n_rec > chunk else 1)]
+            copied = [None] * len(bufs)
+            for j, (i0, i1, host) in enumerate(lockstep_noise_chunks(shape, n_rec, chunk, bufs)):
+                noise = torch.empty(host.shape, device=e.device)
+                noise.copy_(host, non_blocking=True)
+                copied[j % len(bufs)] = torch.cuda.Event()
+                copied[j % len(bufs)].record()
+                self.generator.pixel_cycle_lockstep(target.generator, x, self.sched, state, noise, i0, i1)
+                nxt = copied[(j + 1) % len(bufs)]
+                if nxt is not None:
+                    nxt.synchronize()          # the next chunk is drawn into the buffer this upload read
+        last = target._randn(shape).unsqueeze(0)      # target.generate's last step: t = 0 with the `last` draw (DU:115,131)
+        y = target.generator.pixel_decode(state[1].unsqueeze(1), target.sched, coefs=target.sched.coef[n_rec:],
+                                          t_loop=target.sched.t_loop[n_rec:], last_noise=last)
+        return target.engine.shift_scale(target._refine(y, shape), 1.0, 0.5)
+
     @property
     def device(self):
         return self.engine.device
+
+
+def _chunk_ranges(n_rec, chunk):
+    """[i0, i1) ranges of the lock-step pixel loop: [0, n_rec) in pieces of `chunk` steps; one empty range when n_rec == 0
+    (the call that only draws x_T)."""
+    return [(i0, min(n_rec, i0 + chunk)) for i0 in range(0, max(n_rec, 1), chunk)]
+
+
+def lockstep_noise_chunks(shape, n_rec, chunk, buffers=None):
+    """The CPU draws of DDPMDDIMWrapper.encode (x_T, then one per recovery step; torch.randn(shape) each, in that order) in the
+    chunks the lock-step loop consumes them: yields (i0, i1, noise) with noise [i1 - i0, *shape], preceded by the x_T draw when
+    i0 == 0.  ``buffers``: host tensors of at least min(chunk, n_rec) + 1 draws, filled in turn (pinned buffers for asynchronous
+    uploads); without them each chunk is a new tensor."""
+    for j, (i0, i1) in enumerate(_chunk_ranges(n_rec, chunk)):
+        k = i1 - i0 + (i0 == 0)
+        noise = buffers[j % len(buffers)][:k] if buffers else torch.empty((k,) + tuple(shape))
+        for d in range(k):
+            noise[d].normal_()                 # what torch.randn(shape) draws
+        yield i0, i1, noise
+
+
+def lockstep_compatible(source, target):
+    """Can UnsupervisedTranslation run source.cycle(image, target) instead of target(source.encode(image))?  Both wrappers of
+    the same kind with a lock-step loop, no class input, and identical schedules (coefficient tables, timesteps, x_T scalars,
+    number of recovered steps)."""
+    if type(source) is not type(target) or not isinstance(source, (DDPMDDIMWrapper, LatentDiffStochasticWrapper)):
+        return False
+    if source.enforce_class_input or target.enforce_class_input:
+        return False
+    if isinstance(source, DDPMDDIMWrapper):
+        return source.es_steps == target.es_steps and same_schedule(source.sched, target.sched)
+    g, h = source.generator, target.generator
+    return (source.white_box_steps == target.white_box_steps and (g.channels, g.image_size) == (h.channels, h.image_size)
+            and same_schedule(source._sched(), target._sched()))
 
 
 def get_gan_wrapper(args, target=False, **extra):

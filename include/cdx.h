@@ -317,6 +317,31 @@ int cdx_pixel_decode(cdx_net* unet, const float* z, int n_eps, const cdx_pixel_c
                      const float* t_host, int n_steps, const float* last_noise, float* x_out, int B,
                      int C, int R, void* stream);
 
+/* ---- Unpaired translation in lock-step: the source model's DPM-Encoder chain and the target model's decode chain advance
+ * together, so z is never written.  Replaces source.encode(image) -> z -> target(z) of UnsupervisedTranslation.forward
+ * (unsupervised_translation.py:44-49).  The two schedules must be identical.  The two U-Net calls of a step are independent: when
+ * the nets belong to different engines the target's call runs on the target engine's own non-blocking stream, forked from and
+ * joined into `stream` once per step; nets of one engine run in order on `stream`.  Results are bit-identical to the two-phase
+ * calls either way.
+ *
+ * cdx_pixel_cycle_lockstep: DDPMDDIMWrapper.encode (DW:472-523) under `src` with the first es_steps - 1 steps of .generate
+ * (DW:392-429) under `tgt`, steps [i0, i1) of that loop.  Per step: both U-Net calls, then one fused kernel that draws the source
+ * chain's x_{t-1} (DW:291-303), recovers the step's noise (DW:264-276) and advances the target chain with it (DW:202-222).
+ * state [2, B,C,R,R] = (source x_t, target x_t), caller-owned, carried from call to call; coef / t_host: the loop's n_rec = es_steps-1
+ * steps (loop order, indexed by i).  noise: this range's draws [i1 - i0, B,C,R,R], preceded by the x_T draw when i0 == 0 (which
+ * also initialises state).  Walking [0, n_rec) in chunks keeps device memory at one chunk of noise.  The final target-only step
+ * (t = 0, with the `last` draw) is cdx_pixel_decode on state[1] with n_eps = 0. */
+int cdx_pixel_cycle_lockstep(cdx_net* src, cdx_net* tgt, const float* x0, const cdx_pixel_coef* coef, const float* t_host,
+                             int i0, int i1, const float* noise, float sqrt_a_T, float sqrt_1ma_T, float* state, int B,
+                             int C, int R, void* stream);
+/* cdx_latent_cycle_pair: LatentDiffStochasticWrapper.encode under `src` and .generate's sampler under `tgt`
+ * (latentdiff_stochastic_wrapper.py:253-311), unconditional U-Nets, scale 1.  noise [n_rec+1, B,C,h,w] as for cdx_latent_encode;
+ * with n_rec < n_steps the target chain continues alone for the last n_steps - n_rec steps with extra_noise [n_steps-n_rec,
+ * B,C,h,w] (ddim.py:640).  x_out [B,C,h,w]: the decoded latent, before any refine pass. */
+int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx_ddim_coef* coef, const float* t_host,
+                          int n_steps, int n_rec, const float* noise, float sqrt_a_T, float sqrt_1ma_T,
+                          const float* extra_noise, float* x_out, int B, int C, int h, int w, void* stream);
+
 /* ---------------------------------------------------------------- unit-test hooks ----------- */
 /* Individual ops exported for per-op parity tests (tests/test_ops_gpu.py).  NHWC = [B,H,W,C]. */
 int cdx_op_conv3x3(cdx_engine* e, const float* x_nhwc, const float* w_oihw, const float* bias,

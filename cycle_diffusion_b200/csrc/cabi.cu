@@ -315,7 +315,8 @@ int cdx_engine_set_mma_mode(cdx_engine* e, int mode) {
     CDX_CHECK(e != nullptr && mode >= 0 && mode <= 5, "set_mma_mode: bad arguments");
     e->e.mma_mode = mode == 0 ? 0 : 1;       // 2 = tensor-core contractions but unfused attention (A/B comparisons)
     e->e.flash_attn = mode != 2 && mode != 0;
-    e->e.tc_kind = mode == 3 ? 0 : mode == 4 ? 2 : 1;    // 3 = 3xTF32 contractions, 4 = single-term fp16 (fast path), else fp16 split
+    e->e.tc_kind = mode == 3 ? 0 : mode >= 4 ? 2 : 1;    // 3 = 3xTF32 contractions, 4 / 5 = single-term fp16, else fp16 split
+    e->e.attn_one = mode == 5;                            // 5 = as 4, plus one-term fused attention ("autocast")
   });
 }
 
@@ -839,12 +840,13 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
           }
           kp = kb; vp = vb;
         }
+        const bool lo = !e.attn_one;                 // mode 5: hi planes only
         void* qh = e.arena.alloc((size_t)M * C * 2);
-        void* ql = e.arena.alloc((size_t)M * C * 2);
+        void* ql = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
         void* kh = e.arena.alloc((size_t)Mk * C * 2);
-        void* kl = e.arena.alloc((size_t)Mk * C * 2);
+        void* kl = lo ? e.arena.alloc((size_t)Mk * C * 2) : nullptr;
         void* vh = e.arena.alloc((size_t)Mk * C * 2);
-        void* vl = e.arena.alloc((size_t)Mk * C * 2);
+        void* vl = lo ? e.arena.alloc((size_t)Mk * C * 2) : nullptr;
         split_rows_h16(e, q, M, C, C, qh, ql, C, qa, s);
         split_rows_h16(e, kp, Mk, C, C, kh, kl, C, ka, s);
         split_transpose_h16(e, vp, Mk, C, C, vh, vl, va, s);

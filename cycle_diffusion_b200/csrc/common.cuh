@@ -75,6 +75,7 @@ struct Engine {
   bool flash_attn = true;        // fused wgmma attention kernel (kernels_attn.cu); false -> unfused QK^T / softmax / PV
   int mma_mode = 1;              // 0 SIMT FFMA (exact fp32), 1 tensor cores (wgmma)
   int tc_kind = 1;               // tensor-core product scheme: 0 3xTF32, 1 3x fp16-split at the f16 rate (default), 2 1x fp16 (fast, not fp32-faithful)
+  bool attn_one = false;         // mode 5 ("autocast"): fused fp16 attention with one product term on hi planes only (no lo planes written)
   // tracked |max| scalars of activation tensors (operand range of the fp16-split GEMMs): a pool of device floats, handed out
   // per tensor by the graph executors and zeroed at the start of every network call
   float* amax_pool = nullptr;
@@ -178,7 +179,8 @@ bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq
                         const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int heads, int d,
                         float scale, cudaStream_t s);
 // fp16-split operands (the default scheme): planes made by split_rows_h16 / split_transpose_h16 from fp32 q | k and v with the
-// tensors' tracked ranges (device slots); halves the tensor-pipe time and the operand bytes of the TF32-plane version
+// tensors' tracked ranges (device slots); halves the tensor-pipe time and the operand bytes of the TF32-plane version.
+// q_lo, k_lo and vt_lo all null: one-term products on the hi planes (mode 5); the split functions then write hi only.
 bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
                          const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
                          int Nk, int Nks, int heads, int d, float scale, cudaStream_t s);

@@ -7,7 +7,9 @@
 // Inputs are hi / lo planes of q, k [rows, ld] and of the transposed values V^T [C, B*N] (see nets.cu), so every operand tile arrives
 // by TMA ready for the tensor core.  Default (F16): fp16 planes of x * 2^e, e from the tensor's tracked range (split_rows_h16 /
 // split_transpose_h16 at the end of this file), three wgmma .f16 per 16-wide K step; F16 = false: TF32 planes (rn_tf32(x),
-// rn_tf32(x - hi)) written by the projection's epilogue, three wgmma .tf32 per 8-wide step (--mma 3).
+// rn_tf32(x - hi)) written by the projection's epilogue, three wgmma .tf32 per 8-wide step (--mma 3).  ONE (mma mode 5,
+// "autocast"): fp16 hi planes only and a single wgmma .f16 per step (S = Q_hi K_hi^T, O_j = P_hi V_hi): fp16 inputs with fp32
+// accumulation, the precision of torch.autocast's matmuls, at a third of the tensor-pipe time and half the K / V bytes.
 //
 // One CTA = 128 queries of one (batch, head); keys are walked in blocks of 64.  384 threads = 3 warpgroups:
 //   warpgroup 0     TMA producer (one thread): Q planes once, then K and V^T hi+lo tiles into KS / VS deep rings.
@@ -32,28 +34,36 @@ constexpr int ATHREADS = 384;
 // F16: operands are fp16 hi / lo planes (x * 2^e split as in kernels_tc.cu's KIND_H16) and the three product terms run as
 // wgmma .f16 (K = 16 per instruction): half the tensor-pipe time and half the operand bytes of the TF32 planes.  P is split as
 // fp16(p * 2^10): the scale keeps the lo term out of fp16's subnormal range and cancels in O / l.
-template <int D, bool F16>
+// ONE (F16 only): hi planes alone, one product term; P rounded once as fp16(p * 2^10) (the scale keeps small probabilities out of
+// the subnormals).  The stages are half the size, so the ring is as deep as shared memory allows (up to 4; the three-term
+// variants keep depth 2).
+template <int D, bool F16, bool ONE = false>
 struct ACfg {
+  static_assert(!ONE || F16, "the one-term variant is fp16 only");
+  static constexpr int NPL = ONE ? 1 : 2;                   // operand planes per tensor (hi, or hi + lo)
   static constexpr int KD = F16 ? (D + 15) / 16 * 16 : D;    // head dim as the QK products see it (F16: zero-padded to K = 16 steps by the TMA fill)
   static constexpr int KW = F16 ? 64 : 32;                  // elements per 128-byte k-block row
   static constexpr int KB2 = (D + KW - 1) / KW;             // 128-byte k-blocks covering the head dim
   static constexpr int NG = F16 ? KD / 16 : D / 8;          // K steps of Q.K^T (4 per 128-byte k-block)
   static constexpr int NV = (D + 15) / 16 * 16;             // PV N (rows of the V^T tile)
   static constexpr int KTILE = AKV * 128;                   // one k-block tile of K: 64 rows x 128 B
-  static constexpr int K_STAGE = 2 * KB2 * KTILE;           // hi + lo
+  static constexpr int K_STAGE = NPL * KB2 * KTILE;         // hi (+ lo)
   static constexpr int VTILE = NV * 128;                    // one 128-byte block of V^T (32 keys; F16: 64 keys): NV rows x 128 B
-  static constexpr int V_STAGE = (F16 ? 1 : 2) * 2 * VTILE; // (key sub-blocks) x (hi + lo)
+  static constexpr int V_STAGE = (F16 ? 1 : 2) * NPL * VTILE; // (key sub-blocks) x (hi (+ lo))
   static constexpr int Q_PLANE = KB2 * AQ * 128;            // one plane of Q
-  // ring depth 2 where shared memory allows (TF32 at d = 80 has room for one K and one V stage only)
-  static constexpr int RING = (2 * Q_PLANE + 2 * (K_STAGE + V_STAGE) + 2048 <= 232448) ? 2 : 1;
+  // ring depth: the deepest up to RING_MAX that fits (TF32 at d = 80 has room for one K and one V stage only)
+  static constexpr int RING_MAX = ONE ? 4 : 2;
+  static constexpr int RING_FIT = (232448 - 2048 - NPL * Q_PLANE) / (K_STAGE + V_STAGE);
+  static constexpr int RING = RING_FIT < 1 ? 1 : RING_FIT < RING_MAX ? RING_FIT : RING_MAX;
   static constexpr int KS = RING, VS = RING;
   static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = 2 * Q_PLANE;
+  static constexpr int OFF_K = NPL * Q_PLANE;
   static constexpr int OFF_V = OFF_K + KS * K_STAGE;
   static constexpr int OFF_BAR = OFF_V + VS * V_STAGE;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;   // 1 KB slack: the tiles are placed at the next 1024-byte boundary
   static_assert(D % 8 == 0 && D >= 16 && D <= 80, "head dim must be a multiple of 8 in [16, 80]");
   static_assert(SMEM_BYTES <= 232448, "smem overflow");
+  static_assert(8 + 32 * RING <= 256, "barrier area");
   static_assert(NV % 16 == 0, "NV");
 };
 
@@ -78,12 +88,12 @@ __device__ __forceinline__ void split_h16_pair(float x0, float x1, uint32_t& hi,
   lo = *reinterpret_cast<const uint32_t*>(&ll);
 }
 
-template <int D, bool F16>
+template <int D, bool F16, bool ONE>
 __global__ void __launch_bounds__(ATHREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_constant__ CUtensorMap mapQl,
                   const __grid_constant__ CUtensorMap mapKh, const __grid_constant__ CUtensorMap mapKl,
                   const __grid_constant__ CUtensorMap mapVh, const __grid_constant__ CUtensorMap mapVl, const AttnParams p) {
-  using C = ACfg<D, F16>;
+  using C = ACfg<D, F16, ONE>;
   constexpr int KB2 = C::KB2, NV = C::NV, KW = C::KW, KS = C::KS, VS = C::VS;
   constexpr int NO = NV / 2;                       // O accumulators per thread (m64nNV)
   pdl_trigger();
@@ -92,9 +102,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   const uint32_t bars = base + C::OFF_BAR;
   const uint32_t bar_q_full = bars;
   auto bar_k_full = [&](int s) { return bars + 8u + 8u * s; };
-  auto bar_k_empty = [&](int s) { return bars + 24u + 8u * s; };
-  auto bar_v_full = [&](int s) { return bars + 40u + 8u * s; };
-  auto bar_v_empty = [&](int s) { return bars + 56u + 8u * s; };
+  auto bar_k_empty = [&](int s) { return bars + 8u + 8u * (KS + s); };
+  auto bar_v_full = [&](int s) { return bars + 8u + 8u * (2 * KS + s); };
+  auto bar_v_empty = [&](int s) { return bars + 8u + 8u * (2 * KS + VS + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AQ, h = blockIdx.y, b = blockIdx.z;
@@ -114,10 +124,10 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
       const uint32_t sq = base + C::OFF_Q;
-      mbar_expect_tx(bar_q_full, 2 * C::Q_PLANE);
+      mbar_expect_tx(bar_q_full, C::NPL * C::Q_PLANE);
       for (int kb = 0; kb < KB2; ++kb) {
         tma_load_4d(sq + kb * AQ * 128, &mapQh, kb * KW, h, q0, b, bar_q_full);
-        tma_load_4d(sq + C::Q_PLANE + kb * AQ * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
+        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * AQ * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
       }
       for (int j = 0; j < nb; ++j) {
         // K block j: [64 keys x d] hi + lo
@@ -127,7 +137,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
         mbar_expect_tx(bar_k_full(s), C::K_STAGE);
         for (int kb = 0; kb < KB2; ++kb) {
           tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, b, bar_k_full(s));
-          tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, b, bar_k_full(s));
+          if (!ONE) tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, b, bar_k_full(s));
         }
         // V^T block j: [NV channel rows x 64 keys] (TF32: two 32-key tiles), hi + lo
         const int sv_ = j % VS;
@@ -136,7 +146,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
         mbar_expect_tx(bar_v_full(sv_), C::V_STAGE);
         if (F16) {
           tma_load_4d(sv, &mapVh, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
-          tma_load_4d(sv + C::VTILE, &mapVl, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
+          if (!ONE) tma_load_4d(sv + C::VTILE, &mapVl, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
         } else {
           for (int kk = 0; kk < 2; ++kk) {
             tma_load_4d(sv + kk * C::VTILE, &mapVh, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
@@ -183,7 +193,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
       const uint64_t adv = (uint64_t)((c & 3) * 2);
       const uint64_t q_hi = make_desc(qh_base + kb * AQ * 128) + adv, q_lo = make_desc(ql_base + kb * AQ * 128) + adv;
       const uint64_t k_hi = make_desc(sk + kb * C::KTILE) + adv, k_lo = make_desc(sk + (KB2 + kb) * C::KTILE) + adv;
-      if (F16) {
+      if (ONE) {
+        Wgmma<64>::f16_ss(sc, q_hi, k_hi);
+      } else if (F16) {
         Wgmma<64>::f16_ss(sc, q_lo, k_hi);
         Wgmma<64>::f16_ss(sc, q_hi, k_lo);
         Wgmma<64>::f16_ss(sc, q_hi, k_hi);
@@ -235,7 +247,21 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     const uint32_t sv = base + C::OFF_V + vs * C::V_STAGE;
 #pragma unroll
     for (int c = 0; c < NO; ++c) ob[c] = 0.f;
-    if (F16) {
+    if (ONE) {
+      uint32_t ph[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int e = (2 * kk + (r >> 1)) * 4 + (r & 1) * 2;
+          const __half2 hh = __floats2half2_rn(sc[e], sc[e + 1]);
+          ph[kk][r] = *reinterpret_cast<const uint32_t*>(&hh);
+        }
+      wgmma_pin(ob);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) Wgmma<NV>::f16_rs(ob, ph[kk], make_desc(sv) + (uint64_t)(kk * 2));
+    } else if (F16) {
       uint32_t ph[4][4], pl[4][4];
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)               // keys 16 kk .. 16 kk + 15: accumulator groups 2 kk, 2 kk + 1
@@ -306,21 +332,23 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   }
 }
 
-template <int D, bool F16>
+template <int D, bool F16, bool ONE = false>
 void launch_flash(const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMap& kh, const CUtensorMap& kl, const CUtensorMap& vh,
                   const CUtensorMap& vl, const AttnParams& p, cudaStream_t s) {
   static bool attr[64] = {};          // per device (cudaFuncSetAttribute is device state); engines are single-threaded per device
   int dev = 0;
   CDX_CUDA(cudaGetDevice(&dev));
   if (!attr[dev & 63]) {
-    CDX_CUDA(cudaFuncSetAttribute(flash_attn_kernel<D, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, ACfg<D, F16>::SMEM_BYTES));
+    CDX_CUDA(cudaFuncSetAttribute(flash_attn_kernel<D, F16, ONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, ACfg<D, F16, ONE>::SMEM_BYTES));
     attr[dev & 63] = true;
   }
-  launch_ex(flash_attn_kernel<D, F16>, dim3(p.N / AQ, p.heads, p.B), dim3(ATHREADS), ACfg<D, F16>::SMEM_BYTES, s, 1, qh, ql, kh, kl, vh, vl, p);
+  launch_ex(flash_attn_kernel<D, F16, ONE>, dim3(p.N / AQ, p.heads, p.B), dim3(ATHREADS), ACfg<D, F16, ONE>::SMEM_BYTES, s, 1, qh, ql, kh, kl, vh,
+            vl, p);
 }
 
 // x * 2^e -> fp16 hi / lo planes, e = h16_exp_of(*amax) (the exponent the attention kernel derives from the same slot).
-// src [rows, ld] (cols % 4 == 0) -> hi / lo [rows, ldh]
+// src [rows, ld] (cols % 4 == 0) -> hi / lo [rows, ldh].  LO = false: the hi plane only (one-term attention)
+template <bool LO>
 __global__ void split_rows_h16_kernel(const float* src, long long rows, int cols, long long ld, __half* hi,
                                       __half* lo, long long ldh, const float* amax) {
   pdl_trigger();
@@ -334,18 +362,22 @@ __global__ void split_rows_h16_kernel(const float* src, long long rows, int cols
     float4 v = *reinterpret_cast<const float4*>(src + r * ld + c);
     v.x *= sc; v.y *= sc; v.z *= sc; v.w *= sc;
     const __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
-    const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-    const __half2 l0 = __floats2half2_rn(v.x - f0.x, v.y - f0.y), l1 = __floats2half2_rn(v.z - f1.x, v.w - f1.y);
-    uint2 ph, pl;
+    uint2 ph;
     ph.x = *reinterpret_cast<const uint32_t*>(&h0); ph.y = *reinterpret_cast<const uint32_t*>(&h1);
-    pl.x = *reinterpret_cast<const uint32_t*>(&l0); pl.y = *reinterpret_cast<const uint32_t*>(&l1);
     *reinterpret_cast<uint2*>(hi + r * ldh + c) = ph;
-    *reinterpret_cast<uint2*>(lo + r * ldh + c) = pl;
+    if (LO) {
+      const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
+      const __half2 l0 = __floats2half2_rn(v.x - f0.x, v.y - f0.y), l1 = __floats2half2_rn(v.z - f1.x, v.w - f1.y);
+      uint2 pl;
+      pl.x = *reinterpret_cast<const uint32_t*>(&l0); pl.y = *reinterpret_cast<const uint32_t*>(&l1);
+      *reinterpret_cast<uint2*>(lo + r * ldh + c) = pl;
+    }
   }
 }
 
 // the same split, transposed: src [R, ld] columns 0..C-1 -> hi / lo [C, R] (V^T: both P.V operands K-major for wgmma).
 // 64 (rows) x 32 (columns) tiles through shared memory; R % 2 == 0
+template <bool LO>
 __global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* src, int R, int Cc, long long ld, __half* hi,
                                                                    __half* lo, const float* amax) {
   __shared__ float tile[64][33];
@@ -366,10 +398,11 @@ __global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* s
     if (c < Cc && r < R) {
       const float x0 = tile[2 * tx][ty + 8 * k], x1 = tile[2 * tx + 1][ty + 8 * k];
       const __half2 h = __floats2half2_rn(x0, x1);
-      const float2 f = __half22float2(h);
-      const __half2 l = __floats2half2_rn(x0 - f.x, x1 - f.y);
       *reinterpret_cast<__half2*>(hi + (long long)c * R + r) = h;
-      *reinterpret_cast<__half2*>(lo + (long long)c * R + r) = l;
+      if (LO) {
+        const float2 f = __half22float2(h);
+        *reinterpret_cast<__half2*>(lo + (long long)c * R + r) = __floats2half2_rn(x0 - f.x, x1 - f.y);
+      }
     }
   }
 }
@@ -422,31 +455,38 @@ bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq
 
 void split_rows_h16(Engine& e, const float* src, long long rows, int cols, long long ld, void* hi, void* lo, long long ldh, const float* amax,
                     cudaStream_t s) {
-  CDX_CHECK((cols & 3) == 0 && (ld & 3) == 0 && (ldh & 3) == 0 && a16(src) && a16(hi) && a16(lo), "split_rows_h16: cols / strides must be multiples of 4");
+  CDX_CHECK((cols & 3) == 0 && (ld & 3) == 0 && (ldh & 3) == 0 && a16(src) && a16(hi) && (!lo || a16(lo)),
+            "split_rows_h16: cols / strides must be multiples of 4");
   if (e.dry()) return;
   const long long total = rows * (long long)(cols >> 2);
   const int blocks = (int)std::min<long long>((total + 255) / 256, (long long)e.num_sms * 16);
-  launch_ex(split_rows_h16_kernel, dim3((unsigned)(blocks > 0 ? blocks : 1)), dim3(256), 0, s, 1, src, rows, cols, ld, (__half*)hi, (__half*)lo, ldh, amax);
+  launch_ex(lo ? split_rows_h16_kernel<true> : split_rows_h16_kernel<false>, dim3((unsigned)(blocks > 0 ? blocks : 1)), dim3(256), 0, s, 1, src, rows,
+            cols, ld, (__half*)hi, (__half*)lo, ldh, amax);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
 }
 
 void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long ld, void* hi, void* lo, const float* amax, cudaStream_t s) {
-  CDX_CHECK((R & 1) == 0 && a16(hi) && a16(lo), "split_transpose_h16: even row count");
+  CDX_CHECK((R & 1) == 0 && a16(hi) && (!lo || a16(lo)), "split_transpose_h16: even row count");
   if (e.dry()) return;
-  launch_ex(split_transpose_h16_kernel, dim3((unsigned)((R + 63) / 64), (unsigned)((Cc + 31) / 32)), dim3(256), 0, s, 1, src, R, Cc, ld, (__half*)hi, (__half*)lo, amax);
+  launch_ex(lo ? split_transpose_h16_kernel<true> : split_transpose_h16_kernel<false>, dim3((unsigned)((R + 63) / 64), (unsigned)((Cc + 31) / 32)),
+            dim3(256), 0, s, 1, src, R, Cc, ld, (__half*)hi, (__half*)lo, amax);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
 }
 
 // fp16-split variant: q / k planes [rows, ld] halves (head h at column h*d), V^T planes [heads*d, B*Nks] halves, each tensor's
 // planes scaled by 2^h16_exp_of(*amax) of its slot (split_rows_h16 / split_transpose_h16 above).  ld and Nks multiples of 8.
+// All three lo planes null: the one-term kernel (hi * hi products only, mma mode 5).
 bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
                          const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
                          int Nk, int Nks, int heads, int d, float scale, cudaStream_t s) {
   if ((N % AQ) || (ldq & 7) || (ldk & 7) || (ldo & 3) || (Nks & 7) || Nk < 1 || Nk > Nks) return false;
   if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) return false;
-  if (!a16(q_hi) || !a16(q_lo) || !a16(k_hi) || !a16(k_lo) || !a16(vt_hi) || !a16(vt_lo) || !a16(out)) return false;
+  const bool one = q_lo == nullptr;
+  if (one ? (k_lo || vt_lo) : (!k_lo || !vt_lo)) return false;
+  if (!a16(q_hi) || !a16(k_hi) || !a16(vt_hi) || !a16(out)) return false;
+  if (!one && (!a16(q_lo) || !a16(k_lo) || !a16(vt_lo))) return false;
   if (e.dry()) return true;
   const int NV = (d + 15) / 16 * 16;
   uint64_t dq[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)N, (uint64_t)B};
@@ -458,17 +498,32 @@ bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq,
   uint64_t sv[3] = {(uint64_t)Nks * 2, (uint64_t)B * Nks * 2, (uint64_t)B * Nks * 2 * heads * d};
   uint32_t bv[4] = {64, 1, (uint32_t)NV, 1};
   const CUtensorMap& qh = get_map(q_hi, 4, dq, sq, bq, nullptr, 2);
-  const CUtensorMap& ql = get_map(q_lo, 4, dq, sq, bq, nullptr, 2);
   const CUtensorMap& kh = get_map(k_hi, 4, dk, sk, bk, nullptr, 2);
-  const CUtensorMap& kl = get_map(k_lo, 4, dk, sk, bk, nullptr, 2);
   const CUtensorMap& vh = get_map(vt_hi, 4, dv, sv, bv, nullptr, 2);
-  const CUtensorMap& vl = get_map(vt_lo, 4, dv, sv, bv, nullptr, 2);
+  // (one-term: the lo maps are never read; the hi maps stand in for them)
+  const CUtensorMap& ql = one ? qh : get_map(q_lo, 4, dq, sq, bq, nullptr, 2);
+  const CUtensorMap& kl = one ? kh : get_map(k_lo, 4, dk, sk, bk, nullptr, 2);
+  const CUtensorMap& vl = one ? vh : get_map(vt_lo, 4, dv, sv, bv, nullptr, 2);
   AttnParams p;
   p.N = N; p.Nk = Nk; p.heads = heads; p.d = d; p.B = B;
   p.scale_log2e = scale * 1.4426950408889634f;
   p.out = out; p.ldo = ldo;
   p.q_amax = q_amax; p.k_amax = k_amax; p.v_amax = v_amax;
-  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * B * heads, 2.0 * B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + 4.0 * B * heads * (double)N * d, 1);
+  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * B * heads,
+               (one ? 1.0 : 2.0) * B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + 4.0 * B * heads * (double)N * d, 1);
+  if (one) {
+    switch (d) {
+      case 16: launch_flash<16, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+      case 32: launch_flash<32, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+      case 40: launch_flash<40, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+      case 64: launch_flash<64, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+      case 80: launch_flash<80, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+      default: return false;
+    }
+    CDX_CUDA(cudaGetLastError());
+    e.launches++;
+    return true;
+  }
   switch (d) {
     case 16: launch_flash<16, true>(qh, ql, kh, kl, vh, vl, p, s); break;
     case 32: launch_flash<32, true>(qh, ql, kh, kl, vh, vl, p, s); break;

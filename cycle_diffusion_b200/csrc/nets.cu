@@ -821,14 +821,16 @@ struct UNetExec : Exec {
         float* qkv = (float*)e.arena.alloc((size_t)M * 3 * C * sizeof(float));
         linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_q.weight"), 3 * C, nullptr, nullptr, 0, qkv, 3 * C, nullptr, n1.amax, nullptr,
                     a.amax);                    // range of q | k | v (v bounds the attention output: a convex combination of V rows)
+        // (mode 5: hi planes only, one-term kernel)
+        const bool lo = !e.attn_one;
         void* qk_hi = e.arena.alloc((size_t)M * 2 * C * 2);
-        void* qk_lo = e.arena.alloc((size_t)M * 2 * C * 2);
+        void* qk_lo = lo ? e.arena.alloc((size_t)M * 2 * C * 2) : nullptr;
         void* vt_hi = e.arena.alloc((size_t)C * M * 2);
-        void* vt_lo = e.arena.alloc((size_t)C * M * 2);
+        void* vt_lo = lo ? e.arena.alloc((size_t)C * M * 2) : nullptr;
         split_rows_h16(e, qkv, M, 2 * C, 3 * C, qk_hi, qk_lo, 2 * C, a.amax, s);
         split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s);
-        done = flash_attention_h16(e, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, (const char*)qk_lo + (size_t)C * 2, 2 * C, vt_hi, vt_lo,
-                                   a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, heads, d, scale, s);
+        done = flash_attention_h16(e, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr, 2 * C,
+                                   vt_hi, vt_lo, a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, heads, d, scale, s);
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands
@@ -898,17 +900,19 @@ struct UNetExec : Exec {
       if (ctx_pad && e.tc_kind >= 1 && (C % 8) == 0 && (HW % 128) == 0 && (d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) {
         // fp16-split fused attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the kernel):
         // q projected as plain fp32 (range tracked), K | V from one fused projection of the context; fp16 planes by the split pass.
-        // K and V share the layer's slot (one exponent for both); in loop mode planes and slot are computed by the first call only
+        // K and V share the layer's slot (one exponent for both); in loop mode planes and slot are computed by the first call only.
+        // Mode 5: hi planes only (the cache then holds no lo planes; it lives for one loop, which runs in one mode)
         Scope sa(e.arena);
+        const bool lo = !e.attn_one;
         const int Mk = B * ctx_lp;
         const size_t nk = (size_t)Mk * C;
         float* k_hi = kv_take(nk / 2);
-        float* k_lo = kv_take(nk / 2);
+        float* k_lo = lo ? kv_take(nk / 2) : nullptr;
         float* vt_hi = kv_take(nk / 2);
-        float* vt_lo = kv_take(nk / 2);
+        float* vt_lo = lo ? kv_take(nk / 2) : nullptr;
         Tensor qf = linear(n2, t + ".attn2.to_q", false, nullptr, true);
         void* q_hi = e.arena.alloc((size_t)M * C * 2);
-        void* q_lo = e.arena.alloc((size_t)M * C * 2);
+        void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
         split_rows_h16(e, qf.p, M, C, C, q_hi, q_lo, C, qf.amax, s);
         if (!kv_hit) {
           Scope sk(e.arena);

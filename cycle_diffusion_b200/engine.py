@@ -4,6 +4,7 @@ PyTorch is used only as plumbing: device memory (``torch.empty(..., device='cuda
 ``torch.distributed``.  Every compute call goes through ctypes into hand-written sm_90a kernels; there is no
 torch.nn / CPU fallback anywhere on this path.
 """
+import contextlib
 import ctypes as C
 import math
 
@@ -35,6 +36,7 @@ class Engine:
         h = C.c_void_p()
         check(lib.cdx_engine_create(self.device.index, C.byref(h)))
         self.h = h
+        self.mma_mode = 1                # what cdx_engine_create selects
 
     def close(self):
         if getattr(self, 'h', None):
@@ -61,6 +63,28 @@ class Engine:
 
     def set_mma_mode(self, mode):
         check(lib.cdx_engine_set_mma_mode(self.h, int(mode)))
+        self.mma_mode = int(mode)
+
+    # the reference wrappers' `precision` values (SDW:117, txt2img.py --precision {full,autocast}) and the mma mode each selects;
+    # None: the engine keeps its current mode
+    PRECISIONS = {'full': None, 'autocast': 5}
+
+    @contextlib.contextmanager
+    def precision(self, precision):
+        """``with engine.precision('autocast'):`` runs the enclosed calls in mma mode 5 (single-term fp16 weight GEMMs, convs and
+        fused attention, fp32 activations and accumulation) and restores the previous mode on exit, also on an exception.
+        ``'full'`` leaves the current mode as it is.  Any other value raises ValueError."""
+        if precision not in self.PRECISIONS:
+            raise ValueError(f'precision must be one of {sorted(self.PRECISIONS)}, got {precision!r}')
+        mode, prev = self.PRECISIONS[precision], self.mma_mode
+        if mode is None:
+            yield self
+            return
+        self.set_mma_mode(mode)
+        try:
+            yield self
+        finally:
+            self.set_mma_mode(prev)
 
     PROF_TAGS = ['conv3x3_ffma', 'dense_ffma', 'batched_ffma', 'conv3x3_tc', 'dense_tc', 'batched_tc', 'groupnorm', 'layernorm',
                  'softmax', 'other']

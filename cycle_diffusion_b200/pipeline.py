@@ -24,14 +24,18 @@ class CycleDiffusionPipelineOutput:
 
 
 class CycleDiffusionPipeline:
-    def __init__(self, generator):
-        """generator: wrappers._LatentGenerator (engine + U-Net + VAE + text encoder callable)."""
+    def __init__(self, generator, precision='full'):
+        """generator: wrappers._LatentGenerator (engine + U-Net + VAE + text encoder callable).  precision: 'full' or 'autocast'
+        (txt2img.py --precision): conditioning, first stage and sampling loop run inside ``engine.precision(precision)``."""
+        if precision not in generator.engine.PRECISIONS:
+            raise ValueError(f'precision must be one of {sorted(generator.engine.PRECISIONS)}, got {precision!r}')
         self.g = generator
         self.engine = generator.engine
+        self.precision = precision
 
     @classmethod
     def from_wrapper(cls, wrapper):
-        return cls(wrapper.generator)
+        return cls(wrapper.generator, precision=wrapper.precision)
 
     @torch.no_grad()
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
@@ -58,31 +62,32 @@ class CycleDiffusionPipeline:
             sources = [p for p in sources for _ in range(num_images_per_prompt)]
         if len(prompts) == 1 and B > 1:
             prompts, sources = prompts * B, sources * B
-        rnd = lambda shape: torch.randn(shape, generator=generator)
-        c_tgt = prompt_embeds if prompt_embeds is not None else g.get_learned_conditioning(prompts)
-        c_src = g.get_learned_conditioning(sources)
-        uc = g.get_learned_conditioning(B * [''])
-        S = num_inference_steps
-        skip = S - min(int(S * strength), S)
-        sched = DDIMSchedule(S, eta, skip, g.alphas_cumprod)
-        x = e.shift_scale(image, -0.5, 2.0)
-        moments = g.encode_first_stage(x)
-        lat_shape = (B, moments.shape[1] // 2, moments.shape[2], moments.shape[3])
-        x0 = e.vae_posterior(moments, rnd(lat_shape) if g.sample_posterior else None, g.scale_factor)
-        n_rec = sched.refine_steps
-        noise = torch.zeros((n_rec + 1,) + lat_shape)
-        noise[0] = rnd(lat_shape)
-        for i in range(n_rec):
-            if sched.refine_steps - 1 - i != 0:
-                noise[1 + i] = rnd(lat_shape)
-        if two_phase:
-            z = g.unet.latent_encode(x0, c_src, uc, source_guidance_scale, sched, n_rec, noise)
-            latents = g.unet.latent_decode(z, c_tgt, uc, guidance_scale, sched)
-        else:
-            latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise)
-        if callback is not None:
-            callback(n_rec - 1, sched.t_loop[-1], latents)
-        img = e.shift_scale(g.decode_first_stage(latents), 1.0, 0.5).clamp(0, 1)
+        with e.precision(self.precision):
+            rnd = lambda shape: torch.randn(shape, generator=generator)
+            c_tgt = prompt_embeds if prompt_embeds is not None else g.get_learned_conditioning(prompts)
+            c_src = g.get_learned_conditioning(sources)
+            uc = g.get_learned_conditioning(B * [''])
+            S = num_inference_steps
+            skip = S - min(int(S * strength), S)
+            sched = DDIMSchedule(S, eta, skip, g.alphas_cumprod)
+            x = e.shift_scale(image, -0.5, 2.0)
+            moments = g.encode_first_stage(x)
+            lat_shape = (B, moments.shape[1] // 2, moments.shape[2], moments.shape[3])
+            x0 = e.vae_posterior(moments, rnd(lat_shape) if g.sample_posterior else None, g.scale_factor)
+            n_rec = sched.refine_steps
+            noise = torch.zeros((n_rec + 1,) + lat_shape)
+            noise[0] = rnd(lat_shape)
+            for i in range(n_rec):
+                if sched.refine_steps - 1 - i != 0:
+                    noise[1 + i] = rnd(lat_shape)
+            if two_phase:
+                z = g.unet.latent_encode(x0, c_src, uc, source_guidance_scale, sched, n_rec, noise)
+                latents = g.unet.latent_decode(z, c_tgt, uc, guidance_scale, sched)
+            else:
+                latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise)
+            if callback is not None:
+                callback(n_rec - 1, sched.t_loop[-1], latents)
+            img = e.shift_scale(g.decode_first_stage(latents), 1.0, 0.5).clamp(0, 1)
         if output_type == 'np':
             img = img.permute(0, 2, 3, 1).float().cpu().numpy()
         elif output_type == 'pil':

@@ -151,6 +151,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         self.n_trials = n_trials
         self.eta, self.custom_steps, self.white_box_steps, self.skip_steps = eta, custom_steps, white_box_steps, skip_steps
         self.resolution = resolution or self.RESOLUTION
+        # SDW:117: "full" or "autocast" (txt2img.py --precision).  encode / generate / cycle run inside _precision_scope; a value
+        # other than these two raises ValueError when the wrapper is called (the reference treats a typo as "full")
         self.precision = "full"
         self.directional_clip = ranker
         if generator is not None:
@@ -187,6 +189,11 @@ class _StochasticTextWrapperBase(torch.nn.Module):
             self.generator = _LatentGenerator(self.engine, unet, vae, cond, ucfg['in_channels'], latent_size or self.LATENT, 0.18215,
                                               self.SAMPLE_POSTERIOR)
         self._dummy = torch.nn.Parameter(torch.zeros(1, device=self.engine.device), requires_grad=False)
+
+    def _precision_scope(self):
+        """SDW:143-144, 173: ``autocast("cuda")`` when precision == "autocast", else a null context -- here the engine's mma
+        mode 5 (single-term fp16 tensor-core products, fp32 activations), the previous mode restored on exit."""
+        return self.engine.precision(self.precision)
 
     # -- helpers mirroring the module-level functions of the reference wrapper
     def _get_condition(self, text, bs):
@@ -269,6 +276,10 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         return z_ensemble
 
     def generate(self, z_ensemble, decode_text):
+        with self._precision_scope():
+            return self._generate(z_ensemble, decode_text)
+
+    def _generate(self, z_ensemble, decode_text):
         g = self.generator
         if self.ensemble_batch and len(z_ensemble) * len(self.decoder_unconditional_guidance_scales) > 1:
             return self._generate_batched(z_ensemble, decode_text)
@@ -292,6 +303,10 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         return img_ensemble
 
     def encode(self, image, encode_text):
+        with self._precision_scope():                  # SDW:173-186: the first stage and the ensemble loops
+            return self._encode(image, encode_text)
+
+    def _encode(self, image, encode_text):
         g, e = self.generator, self.engine
         image = e.shift_scale(image, -0.5, 2.0)                                   # (image - 0.5) * 2.0
         assert image.shape[2] == image.shape[3] == self.resolution
@@ -325,8 +340,13 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         engine's lock-step driver (cdx_cycle_lockstep): both chains advance together, one U-Net call per step on the batch
         [source | target uncond | target cond], and the noise recovered at a step is consumed by the target chain at once -- the
         ``z`` tensor of SDW:169-206 is never materialised.  Same random draws in the same order as encode(); same result per sample
-        as the two calls (tests/test_cycle_gpu.py).  Called by TextUnsupervisedTranslation.forward when single_member()."""
+        as the two calls (tests/test_cycle_gpu.py).  Called by TextUnsupervisedTranslation.forward when single_member().  The whole
+        cycle runs in the wrapper's precision scope, as encode() and generate() do."""
         assert self.single_member(), 'cycle(): single-member ensembles only (use encode() + forward())'
+        with self._precision_scope():
+            return self._cycle(image, encode_text, decode_text)
+
+    def _cycle(self, image, encode_text, decode_text):
         g, e = self.generator, self.engine
         x = e.shift_scale(image, -0.5, 2.0)
         assert x.shape[2] == x.shape[3] == self.resolution

@@ -69,7 +69,12 @@ int cdx_engine_profile_read(cdx_engine* e, int tag, double* ms, double* flops, d
  *   2 = as 1 but attention unfused (A/B comparisons)
  *   3 = as 1 with every contraction as 3 x wgmma .tf32 (the round-1 scheme)
  *   4 = FAST PATH, not fp32-faithful: weight GEMMs / convs with the hi*hi term only (plain fp16 inputs, fp32 accumulate);
- *       reported separately by bench.py together with its measured |delta pixel| */
+ *       reported separately by bench.py together with its measured |delta pixel|
+ *   5 = "autocast" (the reference wrappers' precision="autocast", txt2img.py --precision autocast): as 4, and the fused self- /
+ *       cross-attention of the SD U-Net also single-term (S = Q_hi K_hi^T, O = P_hi V_hi over fp16 hi planes, P = fp16(p * 2^10)).
+ *       Activations stay fp32 in memory and every accumulation is fp32; GroupNorm / LayerNorm / softmax, the sampler kernels and
+ *       the paths that use 3xTF32 or FFMA in mode 1 (d = 160 attention, the VAE mid-block, M < 64, the text towers) are
+ *       unchanged.  Not bit-compatible with torch.autocast, which rounds every op's output to fp16; at least as accurate. */
 int cdx_engine_set_mma_mode(cdx_engine* e, int mode);
 
 /* ---------------------------------------------------------------- networks ----------------- */

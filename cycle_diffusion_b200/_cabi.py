@@ -103,6 +103,9 @@ SIGNATURES = {
     'cdx_pixel_decode': (_I, [_P, _P, _I, C.POINTER(PixelCoef), C.POINTER(_F), _I, _P, _P, _I, _I, _I, _P]),
     'cdx_pixel_cycle_lockstep': (_I, [_P, _P, _P, C.POINTER(PixelCoef), C.POINTER(_F), _I, _I, _P, _F, _F, _P, _I, _I, _I, _P]),
     'cdx_latent_cycle_pair': (_I, [_P, _P, _P, C.POINTER(DdimCoef), C.POINTER(_F), _I, _I, _P, _F, _F, _P, _P, _I, _I, _I, _I, _P]),
+    'cdx_latent_cycle_fan': (_I, [_P, _I, _I, _P, _P, _P, _P, _I, C.POINTER(_F), C.POINTER(_F), C.POINTER(DdimCoef), C.POINTER(_F), _I, _P,
+                                  _F, _F, _P, _P, _I, _I, _I, _P]),
+    'cdx_ensemble_select': (_I, [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_op_conv3x3': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     'cdx_op_linear': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_groupnorm': (_I, [_P, _P, _P, _P, _F, _I, _P, _I, _I, _I, _P]),

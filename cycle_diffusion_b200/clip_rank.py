@@ -75,9 +75,25 @@ class DirectionalCLIP:
         return self.engine.dclip_scores(self.encode_image(img), self.encode_image(original_img), self.encode_text(encode_text),
                                         self.encode_text(decode_text))
 
+    @torch.no_grad()
+    def reference(self, original_img, encode_text, decode_text):
+        """What every candidate of one forward is scored against, computed once: (original-image features, source-text features,
+        target-text features), each [B, D]."""
+        assert len(encode_text) == original_img.shape[0] == len(decode_text)
+        return self.encode_image(original_img), self.encode_text(encode_text), self.encode_text(decode_text)
+
+    @torch.no_grad()
+    def scores(self, img, ref, sel=None):
+        """D-CLIP scores [n] of a candidate batch img [n,3,R,R] against ``ref`` (from reference()); candidate c belongs to sample
+        sel[c] (None: candidate b is sample b)."""
+        orig_f, enc_f, dec_f = ref if sel is None else (f[sel] for f in ref)
+        assert orig_f.shape[0] == img.shape[0]
+        return self.engine.dclip_scores(self.encode_image(img), orig_f, enc_f, dec_f)[1]
+
     def rank(self, img_ensemble, original_img, encode_text, decode_text):
         """SDW:233-249: D-CLIP score of every candidate, per-sample argmax, gather -- all on the device."""
-        scores = torch.stack([self(img, original_img, encode_text, decode_text)[1] for img in img_ensemble], dim=1)      # [B, members]
+        ref = self.reference(original_img, encode_text, decode_text)
+        scores = torch.stack([self.scores(img, ref) for img in img_ensemble], dim=1)                                    # [B, members]
         best = scores.argmax(dim=1)
         stack = torch.stack(list(img_ensemble), dim=1)                                                                  # [B, members, 3, R, R]
         return stack[torch.arange(stack.shape[0], device=stack.device), best], best, scores

@@ -264,6 +264,100 @@ void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s, Net* tg
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The ensemble search in lock-step (SDW:189-204 encode, :146-165 generate): n_src source chains, each (member, sample) pair's
+// DPM-Encoder chain, drive K decoder-scale chains each with the noise they recover.  Per step: one U-Net call over exactly the rows
+// the chains need (a chain at scale 0 or 1 has one row, any other scale a cond and an uncond row) and one latent_fan_step launch.
+// The row layout follows from the host scales, so nothing is read back from the device.
+// ---------------------------------------------------------------------------------------------------------------------
+struct LatentFanArgs {
+  int n_src = 0, K = 0;
+  const float* x0 = nullptr; const float* c_src = nullptr; const float* c_tgt = nullptr; const float* uc = nullptr; int L = 0;
+  const float* src_scales = nullptr; const float* tgt_scales = nullptr;          // host [n_src], [n_src*K]
+  const cdx_ddim_coef* coef = nullptr; const float* t_host = nullptr; int n_steps = 0;
+  const float* noise = nullptr; float sa = 0.f, s1 = 0.f;                         // noise [n_steps+1, n_src, chw]
+  float* x_out = nullptr; float* z_out = nullptr;
+  int C = 0, h = 0, w = 0;
+};
+
+// the rows of every chain: source chain j first, then its K targets; returns the row count
+int fan_rows(const LatentFanArgs& a, std::vector<FanChain>& ch) {
+  ch.assign((size_t)a.n_src * (1 + a.K), FanChain{});
+  int rows = 0;
+  auto place = [&](FanChain& c, float scale) {
+    c.scale = scale;
+    c.row = rows++;
+    c.row2 = (scale != 0.0f && scale != 1.0f) ? rows++ : -1;
+  };
+  for (int j = 0; j < a.n_src; ++j) {
+    place(ch[j], a.src_scales[j]);
+    for (int k = 0; k < a.K; ++k) place(ch[a.n_src + (size_t)j * a.K + k], a.tgt_scales[(size_t)j * a.K + k]);
+  }
+  return rows;
+}
+
+void run_latent_fan(Net& unet, const LatentFanArgs& a, cudaStream_t s) {
+  Engine& e = *unet.eng;
+  const int chw = a.C * a.h * a.w;
+  const size_t n = (size_t)a.n_src * chw, n_tgt = (size_t)a.n_src * a.K * chw;
+  std::vector<FanChain> ch;
+  const int rows = fan_rows(a, ch);
+  const size_t ctx_n = (size_t)a.L * unet.ucfg.context_dim;
+  Scope sc(e.arena);
+  unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
+  struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
+  float* xin = (float*)e.arena.alloc((size_t)rows * chw * sizeof(float));
+  float* eout = (float*)e.arena.alloc((size_t)rows * chw * sizeof(float));
+  float* ctx_in = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
+  float* xb[3];
+  for (float*& p : xb) p = (float*)e.arena.alloc(n * sizeof(float));
+  float* yb[2];
+  for (float*& p : yb) p = (float*)e.arena.alloc(n_tgt * sizeof(float));
+  float* tdev = (float*)e.arena.alloc((size_t)a.n_steps * rows * sizeof(float));
+  FanChain* chd = (FanChain*)e.arena.alloc(ch.size() * sizeof(FanChain));
+  upload_timesteps(e, a.t_host, a.n_steps, rows, tdev, s);
+  if (!e.dry())   // pageable source: staged before the call returns
+    CDX_CUDA(cudaMemcpyAsync(chd, ch.data(), ch.size() * sizeof(FanChain), cudaMemcpyHostToDevice, s));
+  // one context per row: the chain's condition on its cond row, uc on its uncond row (ddim.py:555-557)
+  auto ctx_rows = [&](const FanChain& c, const float* cond, int j) {
+    copy_dd(e, c.scale == 0.0f ? a.uc + j * ctx_n : cond + j * ctx_n, ctx_in + (size_t)c.row * ctx_n, ctx_n, s);
+    if (c.row2 >= 0) copy_dd(e, a.uc + j * ctx_n, ctx_in + (size_t)c.row2 * ctx_n, ctx_n, s);
+  };
+  for (int j = 0; j < a.n_src; ++j) {
+    ctx_rows(ch[j], a.c_src, j);
+    for (int k = 0; k < a.K; ++k) ctx_rows(ch[a.n_src + (size_t)j * a.K + k], a.c_tgt, j);
+  }
+  auto next_kind = [&](int i_next) {             // as in run_latent_loop with every step recovered
+    if (i_next >= a.n_steps) return 0;
+    return (a.n_steps - 1 - i_next) == 0 ? 2 : 1;                               // ddim.py:583-584
+  };
+  LatentFan f;
+  f.n = n; f.chw = chw; f.n_src = a.n_src; f.K = a.K; f.chains = chd; f.x0 = a.x0; f.xin = xin;
+  {
+    LatentFan in = f;
+    in.noise0 = a.noise; in.sa = a.sa; in.s1 = a.s1;
+    in.z_out = a.z_out; in.z_stride = (long long)(a.n_steps + 1) * chw;
+    in.xt = xb[0]; in.xn = xb[1]; in.yt = yb[0];
+    in.next = next_kind(0);
+    if (in.next) { in.noise_next = a.noise + n; in.cnext = a.coef[0]; }
+    latent_fan_init(e, in, s);
+  }
+  const int iters = e.dry() ? std::min(a.n_steps, 1) : a.n_steps;
+  for (int i = 0; i < iters; ++i) {
+    unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true);
+    LatentFan st = f;
+    st.eout = eout; st.c = a.coef[i];
+    st.xt = xb[0]; st.xn = xb[1]; st.xn2 = xb[2];
+    if (a.z_out) { st.z_out = a.z_out + (size_t)(1 + i) * chw; st.z_stride = (long long)(a.n_steps + 1) * chw; }
+    st.next = next_kind(i + 1);
+    if (st.next) { st.noise_next = a.noise + (size_t)(2 + i) * n; st.cnext = a.coef[i + 1]; }
+    st.yt = yb[0]; st.y_out = (i == a.n_steps - 1) ? a.x_out : yb[1];
+    latent_fan_step(e, st, s);
+    float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0;
+    std::swap(yb[0], yb[1]);
+  }
+}
+
 }  // namespace
 }  // namespace cdx
 
@@ -740,6 +834,33 @@ int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx
     a.extra = extra_noise; a.x_out = x_out; a.B = B; a.C = C; a.h = h; a.w = w;
     with_arena(src->owner->e, S(stream), [&] { run_latent_loop(*src->n, a, S(stream), tgt->n); }, &tgt->owner->e);
   });
+}
+
+int cdx_latent_cycle_fan(cdx_net* un, int n_src, int K, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
+                         const float* src_scales, const float* tgt_scales, const cdx_ddim_coef* coef, const float* t_host, int n_steps,
+                         const float* noise, float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int C, int h, int w, void* stream) {
+  return guard([&] {
+    CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && uc && src_scales && tgt_scales && coef && t_host && noise && x_out,
+              "latent_cycle_fan: null argument");
+    CDX_CHECK(n_src >= 1 && K >= 1 && n_steps >= 1 && L >= 1 && C >= 1 && h >= 1 && w >= 1, "latent_cycle_fan: n_src=%d K=%d n_steps=%d L=%d",
+              n_src, K, n_steps, L);
+    CDX_CHECK(un->n->ucfg.context_dim > 0, "latent_cycle_fan: the U-Net takes no context");
+    for (int i = 0; i < n_steps; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_cycle_fan: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
+    LatentFanArgs a;
+    a.n_src = n_src; a.K = K; a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L;
+    a.src_scales = src_scales; a.tgt_scales = tgt_scales; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps;
+    a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T; a.x_out = x_out; a.z_out = z_out; a.C = C; a.h = h; a.w = w;
+    with_arena(un->owner->e, S(stream), [&] { run_latent_fan(*un->n, a, S(stream)); });
+  });
+}
+
+int cdx_ensemble_select(cdx_engine* eh, int n, const float* scores, const int64_t* cand_idx, const int* sample_idx, const float* images,
+                        float* best_score, int64_t* best_idx, float* best_img, float* score_mat, int B, int n_total, int H, int W, void* stream) {
+  ENG_CALL(eh, CDX_CHECK(n >= 0 && B >= 1 && n_total >= 1 && H >= 1 && W >= 1, "ensemble_select: n=%d B=%d n_total=%d %dx%d", n, B, n_total, H, W);
+           CDX_CHECK(n == 0 || (scores && cand_idx && sample_idx && images), "ensemble_select: null candidate array");
+           CDX_CHECK(best_score && best_idx && best_img && score_mat, "ensemble_select: null state");
+           ensemble_select(eh->e, n, scores, reinterpret_cast<const long long*>(cand_idx), sample_idx, images, best_score,
+                           reinterpret_cast<long long*>(best_idx), best_img, score_mat, B, n_total, (size_t)3 * H * W, S(stream)));
 }
 
 // ---------------------------------------------------------------- unit-test hooks

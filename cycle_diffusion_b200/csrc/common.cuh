@@ -294,6 +294,33 @@ struct LatentInit {
   float* xin = nullptr; int nseg_src = 0, nseg_tgt = 0;
 };
 void latent_init(Engine& e, const LatentInit& a, cudaStream_t s);
+// Fan-out lock-step loop of the ensemble search: n_src source chains (one (member, sample) pair each), each driving K target chains
+// (chain j*K + k) with the noise it recovers.  A chain's U-Net rows are found through its FanChain entry instead of a fixed segment
+// layout: `row` is the cond row (the uncond row when scale == 0), `row2` the uncond row when scale is neither 0 nor 1, else -1, so
+// eps-hat is cfg_combine_v of the two and each chain computes what latent_step computes for it.
+struct FanChain { int row, row2; float scale; };
+struct LatentFan {
+  size_t n = 0; int chw = 0, n_src = 0, K = 0;   // n = n_src*chw elements; one thread element carries its source and K targets
+  const FanChain* chains = nullptr;              // [n_src] source chains, then [n_src*K] target chains
+  const float* x0 = nullptr;
+  const float* eout = nullptr;                   // step: U-Net output [rows, chw]
+  cdx_ddim_coef c{};                             // step: coefficients of this step (both chains share the schedule)
+  const float* noise0 = nullptr; float sa = 0.f, s1 = 0.f;     // init: x_T draw and its scalars
+  float* xt = nullptr; float* xn = nullptr;      // source x_t, x_{t-1} (init writes both, step reads them)
+  int next = 0; const float* noise_next = nullptr; cdx_ddim_coef cnext{};   // as in LatentStep
+  float* xn2 = nullptr;                          // step: next x_{t-1} of the source chains
+  float* z_out = nullptr; long long z_stride = 0;     // optional: x_T (init) / recovered noise (step) -> z_out[j*z_stride + r]
+  float* yt = nullptr; float* y_out = nullptr;   // target chains [n_src*K, chw]: init writes yt = x_T; step reads yt, writes y_out
+  float* xin = nullptr;                          // next U-Net input [rows, chw]
+};
+void latent_fan_init(Engine& e, const LatentFan& a, cudaStream_t s);
+void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s);
+// Running per-sample best of the ensemble search over candidates that arrive in chunks, in any order: candidate c of the chunk
+// (image images[c], score scores[c], reference candidate index cand[c], sample sample[c]) replaces the best of its sample when it
+// wins under torch.argmax's rule over the [B, n_total] score matrix (larger score; NaN beats any number; ties and NaNs: lower
+// index).  best_idx < 0: no candidate yet.  Scores are also written to score_mat[sample, cand].
+void ensemble_select(Engine& e, int n, const float* scores, const long long* cand, const int* sample, const float* images, float* best_score,
+                     long long* best_idx, float* best_img, float* score_mat, int B, int n_total, size_t img_n, cudaStream_t s);
 
 void pixel_posterior_sample(Engine& e, const float* x0, const float* xt, const float* noise, const cdx_pixel_coef& c, float* out, size_t n, cudaStream_t s);
 void pixel_compute_eps(Engine& e, const float* xt, const float* xt_next, const float* et, const cdx_pixel_coef& c, float* out,

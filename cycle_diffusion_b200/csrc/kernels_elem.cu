@@ -287,6 +287,114 @@ __global__ void latent_init_kernel(const LatentInit a) {
   }
 }
 
+// eps-hat of one fan chain: cfg_combine_v with the chain's own rows (a chain at scale 0 or 1 has one row, which is then the uncond or
+// the cond row, and cfg_combine_v returns that row's output unchanged)
+__device__ __forceinline__ float fan_eps_hat(const float* eout, const FanChain& ch, size_t r, int chw) {
+  const float ec = __ldcg(eout + (size_t)ch.row * chw + r);
+  if (ch.row2 < 0) return ec;
+  const float eu = __ldcg(eout + (size_t)ch.row2 * chw + r);
+  return ADD(eu, MUL(ch.scale, SUB(ec, eu)));                  // ddim.py:559
+}
+__device__ __forceinline__ void fan_put(float* xin, const FanChain& ch, size_t r, int chw, float v) {
+  xin[(size_t)ch.row * chw + r] = v;
+  if (ch.row2 >= 0) xin[(size_t)ch.row2 * chw + r] = v;
+}
+// x_T of every source chain (ddim.py:477-479), shared by its K target chains, and the first U-Net input.  Every input was written by
+// the copies and launches just before, so all loads take the coherent path.
+__global__ void latent_fan_init_kernel(const LatentFan a) {
+  GRID_STRIDE(i, a.n) {
+    const size_t j = i / a.chw, r = i - j * a.chw;
+    const float x0 = __ldcg(a.x0 + i);
+    const float xT = ADD(MUL(a.sa, x0), MUL(a.s1, __ldcg(a.noise0 + i)));                      // ddim.py:477-479
+    if (a.z_out) a.z_out[j * a.z_stride + r] = xT;
+    a.xt[i] = xT;
+    if (a.next == 1) a.xn[i] = ddim_posterior_f(x0, xT, __ldcg(a.noise_next + i), a.cnext);
+    else if (a.next == 2) a.xn[i] = x0;
+    fan_put(a.xin, a.chains[j], r, a.chw, xT);
+    for (int k = 0; k < a.K; ++k) {
+      const size_t t = j * a.K + k;
+      a.yt[t * a.chw + r] = xT;
+      fan_put(a.xin, a.chains[a.n_src + t], r, a.chw, xT);
+    }
+  }
+}
+// One step of the fan-out loop: latent_step_kernel's source half once per source chain, its target half once per target chain with
+// the recovered noise held in a register; same op order and intrinsics.
+__global__ void latent_fan_step_kernel(const LatentFan a) {
+  GRID_STRIDE(i, a.n) {
+    const size_t j = i / a.chw, r = i - j * a.chw;
+    const FanChain src = a.chains[j];
+    const float e_t = fan_eps_hat(a.eout, src, r, a.chw);
+    const float xt = __ldcg(a.xt + i), xn = __ldcg(a.xn + i);
+    const float pred_x0 = DIV(SUB(xt, MUL(a.c.sqrt_1m_at_tab, e_t)), a.c.sqrt_at);              // ddim.py:576
+    const float dir = MUL(a.c.dir_coef, e_t);                                                    // :578
+    const float eps = DIV(DIV(SUB(SUB(xn, MUL(a.c.sqrt_aprev, pred_x0)), dir), a.c.sigma), 1.0f);     // :579 (temperature 1)
+    if (a.z_out) a.z_out[j * a.z_stride + r] = eps;
+    if (a.next == 1) a.xn2[i] = ddim_posterior_f(__ldcg(a.x0 + i), xn, __ldcg(a.noise_next + i), a.cnext);
+    else if (a.next == 2) a.xn2[i] = __ldcg(a.x0 + i);                                          // ddim.py:583-584
+    fan_put(a.xin, src, r, a.chw, xn);
+    for (int k = 0; k < a.K; ++k) {
+      const size_t t = j * a.K + k, ti = t * a.chw + r;
+      const FanChain tc = a.chains[a.n_src + t];
+      const float et = fan_eps_hat(a.eout, tc, r, a.chw);
+      const float y = __ldcg(a.yt + ti);
+      const float px0 = DIV(SUB(y, MUL(a.c.sqrt_1m_at_tab, et)), a.c.sqrt_at);                 // ddim.py:634
+      const float tdir = MUL(a.c.dir_coef, et);                                                 // :638
+      const float noise = MUL(MUL(a.c.sigma, eps), 1.0f);                                       // :642
+      const float yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                         // :645
+      a.y_out[ti] = yn;
+      fan_put(a.xin, tc, r, a.chw, yn);
+    }
+  }
+}
+
+// does candidate (sa, ia) beat (sb, ib) under torch.argmax?  larger wins, NaN beats any number, ties and NaN pairs go to the lower
+// index; an index < 0 is an empty slot
+__device__ __forceinline__ bool select_better(float sa, long long ia, float sb, long long ib) {
+  if (ia < 0) return false;
+  if (ib < 0) return true;
+  const bool na = sa != sa, nb = sb != sb;
+  if (na || nb) return na && (!nb || ia < ib);
+  return sa > sb || (sa == sb && ia < ib);
+}
+// one block per sample: the chunk's best candidate of sample b (a block reduction under select_better, so the result does not depend
+// on the order candidates arrive in), then the running best; the winner's image is copied only when it replaces the best
+__global__ void ensemble_select_kernel(int n, const float* scores, const long long* cand, const int* sample, const float* images,
+                                       float* best_score, long long* best_idx, float* best_img, float* score_mat, int n_total, size_t img_n) {
+  __shared__ float ss[256];
+  __shared__ long long si[256];
+  __shared__ int sr[256];
+  __shared__ int win;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  float bs = 0.f;
+  long long bi = -1;
+  int br = -1;
+  for (int c = tid; c < n; c += blockDim.x) {
+    const long long ci = __ldcg(cand + c);
+    if (__ldcg(sample + c) != b || ci < 0 || ci >= n_total) continue;
+    const float v = __ldcg(scores + c);
+    score_mat[(size_t)b * n_total + ci] = v;
+    if (select_better(v, ci, bs, bi)) { bs = v; bi = ci; br = c; }
+  }
+  ss[tid] = bs; si[tid] = bi; sr[tid] = br;
+  __syncthreads();
+  for (int o = blockDim.x / 2; o > 0; o >>= 1) {
+    if (tid < o && select_better(ss[tid + o], si[tid + o], ss[tid], si[tid])) { ss[tid] = ss[tid + o]; si[tid] = si[tid + o]; sr[tid] = sr[tid + o]; }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    win = -1;
+    if (select_better(ss[0], si[0], __ldcg(best_score + b), __ldcg(best_idx + b))) {
+      best_score[b] = ss[0]; best_idx[b] = si[0]; win = sr[0];
+    }
+  }
+  __syncthreads();
+  if (win < 0) return;
+  const float* src = images + (size_t)win * img_n;
+  float* dst = best_img + (size_t)b * img_n;
+  for (size_t p = tid; p < img_n; p += blockDim.x) dst[p] = __ldcg(src + p);
+}
+
 __global__ void pixel_posterior_kernel(const float* __restrict__ x0, const float* __restrict__ xt, const float* __restrict__ nz,
                                        cdx_pixel_coef c, float* __restrict__ out, size_t n) {
   GRID_STRIDE(i, n) {
@@ -531,6 +639,15 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
 
 void latent_step(Engine& e, const LatentStep& a, cudaStream_t s) { LAUNCH1(latent_step_kernel, a.n, a); }
 void latent_init(Engine& e, const LatentInit& a, cudaStream_t s) { LAUNCH1(latent_init_kernel, a.n, a); }
+void latent_fan_init(Engine& e, const LatentFan& a, cudaStream_t s) { LAUNCH1(latent_fan_init_kernel, a.n, a); }
+void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s) { LAUNCH1(latent_fan_step_kernel, a.n, a); }
+void ensemble_select(Engine& e, int n, const float* scores, const long long* cand, const int* sample, const float* images, float* best_score,
+                     long long* best_idx, float* best_img, float* score_mat, int B, int n_total, size_t img_n, cudaStream_t s) {
+  if (e.dry() || n <= 0 || B <= 0) return;
+  ensemble_select_kernel<<<B, 256, 0, s>>>(n, scores, cand, sample, images, best_score, best_idx, best_img, score_mat, n_total, img_n);
+  CDX_CUDA(cudaGetLastError());
+  e.launches++;
+}
 void affine(Engine& e, const float* x, float a, float b, float* out, size_t n, cudaStream_t s) { LAUNCH1(affine_kernel, n, x, a, b, out, n); }
 void shift_scale(Engine& e, const float* x, float b, float a, float* out, size_t n, cudaStream_t s) { LAUNCH1(shift_scale_kernel, n, x, b, a, out, n); }
 void q_sample(Engine& e, const float* x0, const float* nz, float sa, float s1, float* out, size_t n, cudaStream_t s) { LAUNCH1(q_sample_kernel, n, x0, nz, sa, s1, out, n); }

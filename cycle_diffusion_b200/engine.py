@@ -226,6 +226,12 @@ class Engine:
         check(lib.cdx_image_metrics(self.h, _ptr(a), _ptr(b), B, H, W, _ptr(out), self.stream))
         return out
 
+    def ensemble_select(self, B, n_candidates, H, W):
+        """Running per-sample best of an ensemble whose candidates arrive in chunks (cdx_ensemble_select): returns an
+        EnsembleSelection holding best_img [B,3,H,W], best_idx [B] (int64), best_score [B] and the score matrix
+        scores [B, n_candidates] on this engine's device."""
+        return EnsembleSelection(self, B, n_candidates, H, W)
+
     def op_groupnorm(self, x_nhwc, gamma, beta, eps, silu):
         x, gamma, beta = (_f32c(t, self.device) for t in (x_nhwc, gamma, beta))
         B, H, W, Cc = x.shape
@@ -261,6 +267,32 @@ class Engine:
         y = self.empty(B, Cc, H, W)
         check(lib.cdx_op_nhwc_to_nchw(self.h, _ptr(x), _ptr(y), B, Cc, H * W, self.stream))
         return y
+
+
+class EnsembleSelection:
+    """State of Engine.ensemble_select.  ``add(scores, cand_idx, sample_idx, images)`` folds in one chunk: scores [n], cand_idx [n]
+    (column of the score matrix, the reference's candidate order), sample_idx [n], images [n,3,H,W].  After every candidate has
+    arrived, best_idx equals torch.argmax(scores, dim=1) and best_img[b] is candidate best_idx[b]'s image of sample b, whatever the
+    arrival order.  Columns not yet supplied hold NaN."""
+
+    def __init__(self, engine, B, n_candidates, H, W):
+        self.engine, self.B, self.n_candidates, self.H, self.W = engine, B, n_candidates, H, W
+        dev = engine.device
+        self.best_img = engine.empty(B, 3, H, W)
+        self.best_idx = torch.full((B,), -1, dtype=torch.int64, device=dev)
+        self.best_score = engine.empty(B)
+        self.scores = torch.full((B, n_candidates), float('nan'), dtype=torch.float32, device=dev)
+
+    def add(self, scores, cand_idx, sample_idx, images):
+        e = self.engine
+        scores, images = _f32c(scores, e.device), _f32c(images, e.device)
+        cand = torch.as_tensor(cand_idx).to(device=e.device, dtype=torch.int64).contiguous()
+        samp = torch.as_tensor(sample_idx).to(device=e.device, dtype=torch.int32).contiguous()
+        n = scores.numel()
+        assert cand.shape == samp.shape == (n,) and images.shape == (n, 3, self.H, self.W), \
+            f'chunk shapes {tuple(scores.shape)} {tuple(cand.shape)} {tuple(samp.shape)} {tuple(images.shape)}'
+        check(lib.cdx_ensemble_select(e.h, n, _ptr(scores), _ptr(cand), _ptr(samp), _ptr(images), _ptr(self.best_score), _ptr(self.best_idx),
+                                      _ptr(self.best_img), _ptr(self.scores), self.B, self.n_candidates, self.H, self.W, e.stream))
 
 
 def _int_arr8(vals):
@@ -472,6 +504,30 @@ class UNet(Net):
         check(lib.cdx_cycle_lockstep(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale), float(tgt_scale),
                                      sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out), _ptr(z),
                                      B, Cc, h, w, e.stream))
+        return (out, z) if return_z else out
+
+    def cycle_fan(self, x0, c_src, c_tgt, uc, src_scales, tgt_scales, sched, noise, return_z=False):
+        """The ensemble search's lock-step loop (cdx_latent_cycle_fan): source chain j (x0[j], c_src[j] at src_scales[j]) drives K
+        target chains (c_tgt[j] at tgt_scales[j][k]) with the noise it recovers; one U-Net call per step over only the rows the
+        scales need.  x0 [n_src,C,h,w]; c_src, c_tgt, uc [n_src,L,D]; src_scales [n_src] and tgt_scales [n_src][K] host numbers;
+        noise [n+1, n_src,C,h,w] as for latent_encode with n_rec == sched.refine_steps -> latents [n_src*K,C,h,w] (row j*K + k)
+        and, when return_z, z [n_src, n+1, C,h,w]."""
+        e = self.engine
+        x0, c_src, c_tgt, uc, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, uc, noise))
+        n_src, Cc, h, w = x0.shape
+        src = [float(s) for s in src_scales]
+        tgt = [[float(s) for s in row] for row in tgt_scales]
+        K = len(tgt[0]) if tgt else 0
+        assert len(src) == len(tgt) == n_src and all(len(r) == K for r in tgt), 'src_scales [n_src], tgt_scales [n_src][K]'
+        n = sched.refine_steps
+        assert noise.shape == (n + 1, n_src, Cc, h, w), f'noise shape {tuple(noise.shape)}'
+        assert c_src.shape == c_tgt.shape == uc.shape and c_src.shape[0] == n_src
+        out = e.empty(n_src * K, Cc, h, w)
+        z = e.empty(n_src, n + 1, Cc, h, w) if return_z else None
+        check(lib.cdx_latent_cycle_fan(self.h, n_src, K, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1],
+                                       (C.c_float * n_src)(*src), (C.c_float * (n_src * K))(*[s for r in tgt for s in r]),
+                                       sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out),
+                                       _ptr(z), Cc, h, w, e.stream))
         return (out, z) if return_z else out
 
     def pixel_encode(self, x0, sched, noise):

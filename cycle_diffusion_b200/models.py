@@ -28,7 +28,12 @@ class TextUnsupervisedTranslation(nn.Module):
         if getattr(w, 'single_member', None) is not None and w.single_member():
             # one ensemble member: the reference's encode -> z -> generate (text_unsupervised_translation.py:33-36) as one lock-step loop
             img = w.cycle(original_image, encode_text, decode_text)
+        elif getattr(w, 'lockstep_ensemble', None) is not None and w.lockstep_ensemble():
+            # the ensemble search (SDW:169-249) with every member's chains in lock-step and the candidates ranked as they finish
+            img = w.cycle_ensemble(original_image, encode_text, decode_text)[0]
         else:
+            if getattr(w, 'require_ranker', None) is not None:
+                w.require_ranker()                 # before any sampling
             z_ensemble = w.encode(image=original_image, encode_text=encode_text)
             img = w(z_ensemble=z_ensemble, original_img=original_image, encode_text=encode_text, decode_text=decode_text)
         losses = dict()

@@ -26,11 +26,17 @@ import torch
 
 from . import specs
 from .engine import Engine, UNet, VAE
+from .ensemble import EnsemblePlan, MemberNoise
 from .schedule import DDIMSchedule, PixelSchedule, same_schedule
 
 # Recovery steps per chunk of the lock-step pixel loop (DDPMDDIMWrapper.cycle): device memory holds one chunk of noise, not
 # es_steps of it.  At 256^2 and batch 8 a chunk is 32 x 8 x 3 x 256^2 x 4 B = 0.2 GB (the two-phase path: 1.3 GB per image at 850 steps).
 LOCKSTEP_CHUNK = 32
+
+# U-Net rows per call of the lock-step ensemble search (the text wrappers' ensemble_rows default).  The row-budget sweep of
+# tools/bench_ensemble.py (DESIGN.md section 8; SD v1-4, H100) found the time per sample-forward falling only slightly from 12 to
+# 48 rows (11.70 -> 11.28 ms), and a 96-row SD call exceeds the engine's GroupNorm statistics pool, so 48 it is.
+ENSEMBLE_ROWS = 48
 
 
 class ClipTextCondStage:
@@ -141,11 +147,13 @@ class _StochasticTextWrapperBase(torch.nn.Module):
     def __init__(self, source_model_type, custom_steps, eta, white_box_steps, skip_steps,
                  encoder_unconditional_guidance_scales=None, decoder_unconditional_guidance_scales=None, n_trials=None, *,
                  engine=None, device=0, state_dict=None, cond_stage=None, ranker=None, unet_config=None, vae_config=None,
-                 latent_size=None, resolution=None, generator=None, seed=1234, tokenizer=None, ensemble_batch=16):
+                 latent_size=None, resolution=None, generator=None, seed=1234, tokenizer=None, ensemble_batch=16, ensemble_rows=ENSEMBLE_ROWS):
         super().__init__()
         # ensemble members that share a schedule are batched along the batch dimension, up to this many samples per sampling loop
         # (cdx_latent_loop_ens); None / 0 = one member at a time, the reference's loop shape
         self.ensemble_batch = ensemble_batch
+        # lock-step ensemble search (cycle_ensemble): U-Net rows per call a chunk of source chains may fill (at least one chain)
+        self.ensemble_rows = ensemble_rows
         self.encoder_unconditional_guidance_scales = encoder_unconditional_guidance_scales
         self.decoder_unconditional_guidance_scales = decoder_unconditional_guidance_scales
         self.n_trials = n_trials
@@ -368,9 +376,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         img_ensemble = [self.engine.shift_scale(img, 1.0, 0.5) for img in img_ensemble]     # Normalize(mean=-1, std=2)
         if len(img_ensemble) == 1:
             return img_ensemble[0]
-        if self.directional_clip is None:
-            raise NotImplementedError('ranking an ensemble needs ranker=<callable(img, original_img, encode_text, decode_text) -> (_, score[B])>, '
-                                      'e.g. cycle_diffusion_b200.clip_rank.DirectionalCLIP(engine, clip_state_dict, tokenizer) (SURVEY.md 8f-3)')
+        self.require_ranker()
         if hasattr(self.directional_clip, 'rank'):        # in-engine DirectionalCLIP (clip_rank.py): scores, argmax and gather stay on the device
             return self.directional_clip.rank(img_ensemble, original_img, encode_text, decode_text)[0]
         scores = []
@@ -380,6 +386,75 @@ class _StochasticTextWrapperBase(torch.nn.Module):
             scores.append(s)
         best_idx = torch.argmax(torch.stack(scores, dim=1), dim=1)
         return torch.stack([img_ensemble[best_idx[b].item()][b] for b in range(best_idx.shape[0])], dim=0)
+
+    def n_candidates(self):
+        return (self.n_trials * len(self.encoder_unconditional_guidance_scales) * len(self.skip_steps)
+                * len(self.decoder_unconditional_guidance_scales))
+
+    def require_ranker(self):
+        """An ensemble of more than one candidate is ranked by ``ranker``: raise when there is none."""
+        if self.n_candidates() > 1 and self.directional_clip is None:
+            raise NotImplementedError('ranking an ensemble needs ranker=<callable(img, original_img, encode_text, decode_text) -> (_, score[B])>, '
+                                      'e.g. cycle_diffusion_b200.clip_rank.DirectionalCLIP(engine, clip_state_dict, tokenizer) (SURVEY.md 8f-3)')
+
+    def _schedules(self):
+        return {skip: DDIMSchedule(self.custom_steps, self.eta, skip, self.generator.alphas_cumprod) for skip in dict.fromkeys(self.skip_steps)}
+
+    def lockstep_ensemble(self):
+        """True when cycle_ensemble can run the ensemble search: more than one candidate, eta > 0, every step of every skip
+        recovered (white_box_steps - skip - 1 >= refine_steps, as in all published configurations) and a ranker."""
+        if self.n_candidates() <= 1 or not self.eta > 0 or self.white_box_steps == -1 or self.directional_clip is None:
+            return False
+        return all(self.white_box_steps - skip - 1 >= s.refine_steps for skip, s in self._schedules().items())
+
+    def ensemble_plan(self, bsz):
+        scheds = self._schedules()
+        return EnsemblePlan(self.n_trials, self.encoder_unconditional_guidance_scales, self.skip_steps, self.decoder_unconditional_guidance_scales,
+                            bsz, {k: s.refine_steps for k, s in scheds.items()}, self.ensemble_rows), scheds
+
+    def cycle_ensemble(self, image, encode_text, decode_text):
+        """encode(image, encode_text) followed by forward(z, image, encode_text, decode_text) for an ensemble (lockstep_ensemble()),
+        in lock-step and streamed: each (member, sample) pair's DPM-Encoder chain drives its decoder-scale chains with the noise it
+        recovers (cdx_latent_cycle_fan), a chain runs a CFG row only when its scale needs one, and each chunk's candidates are
+        decoded, scored and folded into a per-sample best (cdx_ensemble_select) as soon as the chunk finishes.  No z and no list of
+        candidate images is kept.  Same random draws in the same order as encode().
+
+        -> (img [B,3,R,R] in [0,1], unclamped; best_idx [B] int64 in the reference's candidate order, member * n_dec + k;
+        scores [B, candidates]).  Loops and VAE run in the wrapper's precision scope, ranking outside it, as in encode + forward."""
+        assert self.lockstep_ensemble(), 'cycle_ensemble(): needs an ensemble with every step recovered, eta > 0 and a ranker'
+        g, e, rank = self.generator, self.engine, self.directional_clip
+        with self._precision_scope():
+            x = e.shift_scale(image, -0.5, 2.0)
+            assert x.shape[2] == x.shape[3] == self.resolution
+            x0 = g.get_first_stage_encoding(g.encode_first_stage(x))
+            bsz = x.shape[0]
+            c_src, uc = self._get_condition(encode_text, bsz)
+            c_tgt, _ = self._get_condition(decode_text, bsz)
+        plan, scheds = self.ensemble_plan(bsz)
+        noise = MemberNoise(plan, lambda skip: self._encode_noise(scheds[skip], scheds[skip].refine_steps, x0.shape))
+        R = self.resolution
+        sel = e.ensemble_select(bsz, plan.n_candidates, R, R)
+        ref = rank.reference(image, encode_text, decode_text) if hasattr(rank, 'reference') else None
+        eb = max(1, self.ensemble_batch or 1)
+        K = plan.n_dec
+        for chunk in plan.chunks:
+            samples = torch.tensor([b for _, b in chunk.chains], device=e.device)
+            pick = lambda t: t[samples.to(t.device)]
+            with self._precision_scope():
+                lat = g.unet.cycle_fan(pick(x0), pick(c_src), pick(c_tgt), pick(uc), [plan.members[m][1] for m, _ in chunk.chains],
+                                       [plan.dec_scales] * len(chunk.chains), scheds[chunk.skip], noise.chunk(chunk))
+                imgs = torch.cat([g.decode_first_stage(lat[i:i + eb]) for i in range(0, lat.shape[0], eb)])
+            imgs = e.shift_scale(imgs, 1.0, 0.5)                                            # Normalize(mean=-1, std=2)
+            cand = [plan.candidate(m, k) for m, _ in chunk.chains for k in range(K)]
+            samp = samples.repeat_interleave(K)
+            if ref is not None:
+                s = rank.scores(imgs, ref, samp)
+            else:                                                                           # a plain callable: per-sample slices
+                rows = samp.tolist()
+                _, s = rank(imgs, image[samp.to(image.device)], [encode_text[b] for b in rows], [decode_text[b] for b in rows])
+                assert s.shape == (imgs.shape[0],)
+            sel.add(s, cand, samp, imgs)
+        return sel.best_img, sel.best_idx, sel.scores
 
     @property
     def device(self):

@@ -347,6 +347,32 @@ int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx
                           int n_steps, int n_rec, const float* noise, float sqrt_a_T, float sqrt_1ma_T,
                           const float* extra_noise, float* x_out, int B, int C, int h, int w, void* stream);
 
+/* ---- The ensemble search of the text wrappers in lock-step (SURVEY 8f-2).  Replaces encode's loop over trial x encoder scale x
+ * skip (SDW:189-204), generate's loop over each z x decoder scale (SDW:146-165) and the Directional-CLIP argmax (SDW:219-249).
+ *
+ * cdx_latent_cycle_fan: n_src source chains -- _ddpm_ddim_encoding (ddim.py:450-501) of one (member, sample) pair under c_src[j] at
+ * src_scales[j] -- each driving K target chains -- ddim_sampling_with_eps (ddim.py:395-448) under c_tgt[j] at tgt_scales[j*K + k] --
+ * with the noise it recovers at each step (ddim.py:575-579, consumed at :603-646 in registers).  Every step is ONE U-Net call over
+ * exactly the rows the chains need (a chain at scale 1 runs its cond row only, at scale 0 its uncond row only, else both,
+ * ddim.py:550-559) and one fused elementwise launch.  The scales are host arrays: the row layout is derived from them, with no
+ * device read.  Each chain computes what cdx_latent_encode / cdx_latent_decode compute for it, up to the summation order of
+ * split-K GEMMs at a different batch size.  All steps recovered (eta > 0, white_box_steps > custom_steps - skip).
+ *   x0 [n_src,C,h,w]; c_src, c_tgt, uc [n_src,L,D]; noise [n_steps+1, n_src,C,h,w] as for cdx_latent_encode;
+ *   x_out [n_src*K, C,h,w]: target chain j*K + k's final latent; z_out optional [n_src, n_steps+1, C,h,w] (test hook).
+ *
+ * cdx_ensemble_select: running per-sample best over candidates that arrive in chunks, in any order.  Chunk entry c: score scores[c],
+ * image images[c] [3,H,W], index cand_idx[c] in the reference's candidate order (column of the [B, n_total] score matrix of
+ * SDW:225), sample sample_idx[c] in [0, B).  The state best_score [B], best_idx [B] (int64; < 0 = empty), best_img [B,3,H,W]
+ * reproduces torch.argmax over the score matrix (larger wins; NaN beats any number; ties and NaNs go to the lower index); an
+ * image is copied only when it becomes its sample's best.  score_mat [B, n_total] receives the chunk's scores. */
+int cdx_latent_cycle_fan(cdx_net* unet, int n_src, int K, const float* x0, const float* c_src, const float* c_tgt,
+                         const float* uc, int ctx_len, const float* src_scales_host, const float* tgt_scales_host,
+                         const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                         float sqrt_1ma_T, float* x_out, float* z_out, int C, int h, int w, void* stream);
+int cdx_ensemble_select(cdx_engine* e, int n, const float* scores, const int64_t* cand_idx, const int* sample_idx,
+                        const float* images, float* best_score, int64_t* best_idx, float* best_img, float* score_mat, int B,
+                        int n_total, int H, int W, void* stream);
+
 /* ---------------------------------------------------------------- unit-test hooks ----------- */
 /* Individual ops exported for per-op parity tests (tests/test_ops_gpu.py).  NHWC = [B,H,W,C]. */
 int cdx_op_conv3x3(cdx_engine* e, const float* x_nhwc, const float* w_oihw, const float* bias,

@@ -12,6 +12,9 @@ LIB_PATH = os.path.join(HERE, 'libcdx.so')
 CDX_UNET_OPENAI = 1
 CDX_UNET_IDDPM = 2
 CDX_UNET_DDPM = 3
+CDX_TEXT_OPENCLIP = 4
+CDX_PRED_EPS = 0
+CDX_PRED_V = 1
 
 
 class UnetConfig(C.Structure):
@@ -70,6 +73,7 @@ SIGNATURES = {
     'cdx_net_weight_blob': (_I, [_P, C.POINTER(_P), C.POINTER(_S)]),
     'cdx_net_adopt_blob': (_I, [_P]),
     'cdx_unet_set_time_freqs': (_I, [_P, C.POINTER(_F), _I]),
+    'cdx_unet_set_prediction': (_I, [_P, _I, C.POINTER(_F), C.POINTER(_F), _I]),
     'cdx_unet_forward': (_I, [_P, _P, _P, _P, _I, _P, _I, _I, _I, _P]),
     'cdx_vae_encode': (_I, [_P, _P, _P, _I, _I, _P]),
     'cdx_text_encode': (_I, [_P, _P, _I, _I, _P, _P]),

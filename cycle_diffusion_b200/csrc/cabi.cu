@@ -159,6 +159,21 @@ struct LatentLoopArgs {
   int B = 0, C = 0, h = 0, w = 0;
 };
 
+// v-prediction nets (cdx_unet_set_prediction): every U-Net timestep of the loop must index the net's sqrt(abar) tables
+void check_v_steps(const Net& u, const float* t_host, int n) {
+  if (!u.pred) return;
+  for (int i = 0; i < n; ++i) {
+    const int t = (int)t_host[i];
+    CDX_CHECK((float)t == t_host[i] && t >= 0 && t < (int)u.sa_v.size(), "v-prediction: timestep %g outside the %d-entry table", t_host[i],
+              (int)u.sa_v.size());
+  }
+}
+template <class Step>
+void set_v(const Net& u, float t, Step& st) {
+  if (!u.pred) return;
+  st.pred = 1; st.vsa = u.sa_v[(int)t]; st.vs1 = u.s1_v[(int)t];
+}
+
 // `tgt_net`: the target chain runs under its own net (two-model translation, LOCK mode, context-free): the step's U-Net call is split
 // into a source call and a target call over the two halves of `xin` / `eout`.  With n_rec < n_steps the target chain continues
 // alone after the last recovered step, with `extra` noise (ddim.py:640).
@@ -185,6 +200,8 @@ void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s, Net* tg
   if (enc) for (int k = 0; k < 3; ++k) xb[k] = (float*)e.arena.alloc(n * sizeof(float));
   if (dec) for (int k = 0; k < 2; ++k) yb[k] = (float*)e.arena.alloc(n * sizeof(float));
   const int loop_steps = enc && !dec ? a.n_rec : a.n_steps;
+  CDX_CHECK(!tgt_net || (!unet.pred && !tgt_net->pred), "two-model latent loop: eps-prediction U-Nets only");
+  check_v_steps(unet, a.t_host, loop_steps);
   float* tdev = (float*)e.arena.alloc((size_t)std::max(loop_steps, 1) * nb * sizeof(float));
   upload_timesteps(e, a.t_host, loop_steps, nb, tdev, s);
   if (ctx_n) {   // cat([uc, c]) per chain: uncond first (ddim.py:555-557); unconditional models (L == 0) carry no context
@@ -258,6 +275,7 @@ void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s, Net* tg
       st.y_out = (i == loop_steps - 1) ? a.x_out : yb[1];
     }
     st.xin = xin; st.nseg_src = nseg_src; st.nseg_tgt = nseg_tgt;
+    set_v(unet, a.t_host[i], st);
     latent_step(e, st, s);
     if (enc_i) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
     if (dec) std::swap(yb[0], yb[1]);
@@ -303,6 +321,7 @@ void run_latent_fan(Net& unet, const LatentFanArgs& a, cudaStream_t s) {
   std::vector<FanChain> ch;
   const int rows = fan_rows(a, ch);
   const size_t ctx_n = (size_t)a.L * unet.ucfg.context_dim;
+  check_v_steps(unet, a.t_host, a.n_steps);
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
   struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
@@ -352,6 +371,7 @@ void run_latent_fan(Net& unet, const LatentFanArgs& a, cudaStream_t s) {
     st.next = next_kind(i + 1);
     if (st.next) { st.noise_next = a.noise + (size_t)(2 + i) * n; st.cnext = a.coef[i + 1]; }
     st.yt = yb[0]; st.y_out = (i == a.n_steps - 1) ? a.x_out : yb[1];
+    set_v(unet, a.t_host[i], st);
     latent_fan_step(e, st, s);
     float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0;
     std::swap(yb[0], yb[1]);
@@ -527,6 +547,22 @@ int cdx_unet_set_time_freqs(cdx_net* n, const float* freqs, int half) {
     CDX_CHECK(half == n->n->ucfg.model_channels / 2, "set_time_freqs: half=%d, expected %d", half, n->n->ucfg.model_channels / 2);
     n->n->freqs_host.assign(freqs, freqs + half);
     if (n->n->finalized) net_finalize(*n->n);
+  });
+}
+
+int cdx_unet_set_prediction(cdx_net* n, int prediction, const float* sa_v, const float* s1_v, int T) {
+  return guard([&] {
+    CDX_CHECK(n && n->n, "set_prediction: null net");
+    CDX_CHECK(n->n->kind == NET_UNET_OPENAI, "set_prediction: SD / LDM U-Nets only");
+    CDX_CHECK(prediction == CDX_PRED_EPS || prediction == CDX_PRED_V, "set_prediction: prediction %d", prediction);
+    if (prediction == CDX_PRED_EPS) {
+      n->n->pred = 0; n->n->sa_v.clear(); n->n->s1_v.clear();
+      return;
+    }
+    CDX_CHECK(sa_v && s1_v && T > 0, "set_prediction: v needs both tables");
+    n->n->sa_v.assign(sa_v, sa_v + T);
+    n->n->s1_v.assign(s1_v, s1_v + T);
+    n->n->pred = 1;
   });
 }
 
@@ -827,6 +863,7 @@ int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx
     CDX_CHECK(n_steps >= 1 && n_rec >= 0 && n_rec <= n_steps, "latent_cycle_pair: n_steps=%d n_rec=%d", n_steps, n_rec);
     CDX_CHECK(n_rec == n_steps || extra_noise, "latent_cycle_pair: %d steps, %d recovered noises and no extra noise", n_steps, n_rec);
     CDX_CHECK(src->n->ucfg.context_dim == 0 && tgt->n->ucfg.context_dim == 0, "latent_cycle_pair: unconditional U-Nets only");
+    CDX_CHECK(!src->n->pred && !tgt->n->pred, "latent_cycle_pair: eps-prediction U-Nets only");
     for (int i = 0; i < n_rec; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_cycle_pair: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
     LatentLoopArgs a;
     a.mode = LOOP_LOCK;

@@ -281,6 +281,9 @@ struct LatentStep {
   float* y_out = nullptr;
   // --- next U-Net input batch [nseg, B, chw]: segments [0, nseg_src) <- x_{t-1}, [nseg_src, nseg_src + nseg_tgt) <- y_{t-1}
   float* xin = nullptr; int nseg_src = 0, nseg_tgt = 0;
+  // --- v-prediction (SD 2.x "-v" models): the U-Net output is v; after the guidance combine, e_t = vsa*v + vs1*x_t and
+  // pred_x0 = vsa*x_t - vs1*v with vsa = sqrt(abar_t), vs1 = sqrt(1 - abar_t) of the step's timestep (both chains share the step)
+  int pred = 0; float vsa = 0.f, vs1 = 0.f;
 };
 void latent_step(Engine& e, const LatentStep& a, cudaStream_t s);
 // x_T = sqrt(a_T) x0 + sqrt(1 - a_T) noise0 (ddim.py:477-479) -> z slot 0 (optional), x_T buffer, y_T buffer (optional), first
@@ -312,6 +315,7 @@ struct LatentFan {
   float* z_out = nullptr; long long z_stride = 0;     // optional: x_T (init) / recovered noise (step) -> z_out[j*z_stride + r]
   float* yt = nullptr; float* y_out = nullptr;   // target chains [n_src*K, chw]: init writes yt = x_T; step reads yt, writes y_out
   float* xin = nullptr;                          // next U-Net input [rows, chw]
+  int pred = 0; float vsa = 0.f, vs1 = 0.f;      // step: v-prediction, as in LatentStep
 };
 void latent_fan_init(Engine& e, const LatentFan& a, cudaStream_t s);
 void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s);

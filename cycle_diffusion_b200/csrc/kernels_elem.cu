@@ -241,15 +241,30 @@ __device__ __forceinline__ float ddim_posterior_f(float x0, float xt, float nz, 
   return ADD(ADD(MUL(c.sqrt_aprev, x0), dir), noise);                     // :600
 }
 
+// e_t and pred_x0 of one chain from the guidance-combined U-Net output `o` at x_t = `x`: eps-prediction as ddim.py:576 / :634;
+// v-prediction (SD 2 LatentDiffusion.predict_eps_from_z_and_v / predict_start_from_z_and_v), each product rounded before the add
+template <int PRED>
+__device__ __forceinline__ void eps_x0(float o, float x, const cdx_ddim_coef& c, float vsa, float vs1, float& e_t, float& pred_x0) {
+  if constexpr (PRED == 0) {
+    e_t = o;
+    pred_x0 = DIV(SUB(x, MUL(c.sqrt_1m_at_tab, e_t)), c.sqrt_at);
+  } else {
+    e_t = ADD(MUL(vsa, o), MUL(vs1, x));
+    pred_x0 = SUB(MUL(vsa, x), MUL(vs1, o));
+  }
+}
+
+template <int PRED>
 __global__ void latent_step_kernel(const LatentStep a) {
   const size_t seg = a.n;
   GRID_STRIDE(i, a.n) {
     const size_t b = i / a.chw, r = i - b * a.chw;
     float eps = 0.f;
     if (a.enc) {
-      const float e_t = a.s_scale_v ? cfg_combine_v(a.es_c, a.es_uc, a.s_scale_v[b], i) : cfg_combine(a.es_c, a.es_uc, a.s_scale, i);
+      const float o = a.s_scale_v ? cfg_combine_v(a.es_c, a.es_uc, a.s_scale_v[b], i) : cfg_combine(a.es_c, a.es_uc, a.s_scale, i);
       const float xt = a.xt[i], xn = a.xn[i];
-      const float pred_x0 = DIV(SUB(xt, MUL(a.cs.sqrt_1m_at_tab, e_t)), a.cs.sqrt_at);          // ddim.py:576
+      float e_t, pred_x0;
+      eps_x0<PRED>(o, xt, a.cs, a.vsa, a.vs1, e_t, pred_x0);                                    // ddim.py:576
       const float dir = MUL(a.cs.dir_coef, e_t);                                                // :578
       eps = DIV(DIV(SUB(SUB(xn, MUL(a.cs.sqrt_aprev, pred_x0)), dir), a.cs.sigma), 1.0f);       // :579 (temperature 1)
       if (a.z_out) a.z_out[b * a.z_stride + r] = eps;
@@ -260,9 +275,10 @@ __global__ void latent_step_kernel(const LatentStep a) {
       eps = a.eps_in[b * a.eps_stride + r];
     }
     if (a.dec) {
-      const float e_t = a.t_scale_v ? cfg_combine_v(a.et_c, a.et_uc, a.t_scale_v[b], i) : cfg_combine(a.et_c, a.et_uc, a.t_scale, i);
+      const float o = a.t_scale_v ? cfg_combine_v(a.et_c, a.et_uc, a.t_scale_v[b], i) : cfg_combine(a.et_c, a.et_uc, a.t_scale, i);
       const float y = a.yt[i];
-      const float pred_x0 = DIV(SUB(y, MUL(a.ct.sqrt_1m_at_tab, e_t)), a.ct.sqrt_at);           // ddim.py:634
+      float e_t, pred_x0;
+      eps_x0<PRED>(o, y, a.ct, a.vsa, a.vs1, e_t, pred_x0);                                     // ddim.py:634
       const float dir = MUL(a.ct.dir_coef, e_t);                                                // :638
       const float noise = MUL(MUL(a.ct.sigma, eps), 1.0f);                                      // :642
       const float yn = ADD(ADD(MUL(a.ct.sqrt_aprev, pred_x0), dir), noise);                     // :645
@@ -319,14 +335,17 @@ __global__ void latent_fan_init_kernel(const LatentFan a) {
   }
 }
 // One step of the fan-out loop: latent_step_kernel's source half once per source chain, its target half once per target chain with
-// the recovered noise held in a register; same op order and intrinsics.
+// the recovered noise held in a register; same op order and intrinsics.  Under v-prediction each target chain forms e_t and pred_x0
+// from its own x_t and v.
+template <int PRED>
 __global__ void latent_fan_step_kernel(const LatentFan a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
     const FanChain src = a.chains[j];
-    const float e_t = fan_eps_hat(a.eout, src, r, a.chw);
+    const float o = fan_eps_hat(a.eout, src, r, a.chw);
     const float xt = __ldcg(a.xt + i), xn = __ldcg(a.xn + i);
-    const float pred_x0 = DIV(SUB(xt, MUL(a.c.sqrt_1m_at_tab, e_t)), a.c.sqrt_at);              // ddim.py:576
+    float e_t, pred_x0;
+    eps_x0<PRED>(o, xt, a.c, a.vsa, a.vs1, e_t, pred_x0);                                       // ddim.py:576
     const float dir = MUL(a.c.dir_coef, e_t);                                                    // :578
     const float eps = DIV(DIV(SUB(SUB(xn, MUL(a.c.sqrt_aprev, pred_x0)), dir), a.c.sigma), 1.0f);     // :579 (temperature 1)
     if (a.z_out) a.z_out[j * a.z_stride + r] = eps;
@@ -336,9 +355,10 @@ __global__ void latent_fan_step_kernel(const LatentFan a) {
     for (int k = 0; k < a.K; ++k) {
       const size_t t = j * a.K + k, ti = t * a.chw + r;
       const FanChain tc = a.chains[a.n_src + t];
-      const float et = fan_eps_hat(a.eout, tc, r, a.chw);
+      const float ot = fan_eps_hat(a.eout, tc, r, a.chw);
       const float y = __ldcg(a.yt + ti);
-      const float px0 = DIV(SUB(y, MUL(a.c.sqrt_1m_at_tab, et)), a.c.sqrt_at);                 // ddim.py:634
+      float et, px0;
+      eps_x0<PRED>(ot, y, a.c, a.vsa, a.vs1, et, px0);                                          // ddim.py:634
       const float tdir = MUL(a.c.dir_coef, et);                                                 // :638
       const float noise = MUL(MUL(a.c.sigma, eps), 1.0f);                                       // :642
       const float yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                         // :645
@@ -637,10 +657,16 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
   }
 }
 
-void latent_step(Engine& e, const LatentStep& a, cudaStream_t s) { LAUNCH1(latent_step_kernel, a.n, a); }
+void latent_step(Engine& e, const LatentStep& a, cudaStream_t s) {
+  if (a.pred) LAUNCH1(latent_step_kernel<1>, a.n, a);
+  else LAUNCH1(latent_step_kernel<0>, a.n, a);
+}
 void latent_init(Engine& e, const LatentInit& a, cudaStream_t s) { LAUNCH1(latent_init_kernel, a.n, a); }
 void latent_fan_init(Engine& e, const LatentFan& a, cudaStream_t s) { LAUNCH1(latent_fan_init_kernel, a.n, a); }
-void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s) { LAUNCH1(latent_fan_step_kernel, a.n, a); }
+void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s) {
+  if (a.pred) LAUNCH1(latent_fan_step_kernel<1>, a.n, a);
+  else LAUNCH1(latent_fan_step_kernel<0>, a.n, a);
+}
 void ensemble_select(Engine& e, int n, const float* scores, const long long* cand, const int* sample, const float* images, float* best_score,
                      long long* best_idx, float* best_img, float* score_mat, int B, int n_total, size_t img_n, cudaStream_t s) {
   if (e.dry() || n <= 0 || B <= 0) return;

@@ -318,7 +318,14 @@ Net* make_unet(Engine* e, const cdx_unet_config& cfg) {
   CDX_CHECK(cfg.kind == CDX_UNET_OPENAI || cfg.kind == CDX_UNET_IDDPM || cfg.kind == CDX_UNET_DDPM, "unet: bad kind %d", cfg.kind);
   CDX_CHECK(cfg.n_mult >= 1 && cfg.n_mult <= 8 && cfg.n_attn >= 0 && cfg.n_attn <= 8, "unet: bad level counts");
   CDX_CHECK(cfg.model_channels % 32 == 0, "unet: model_channels must be a multiple of 32 (GroupNorm32)");
-  if (cfg.kind == CDX_UNET_OPENAI && cfg.context_dim > 0) CDX_CHECK(cfg.num_heads > 0, "unet: heads");
+  if (cfg.kind == CDX_UNET_OPENAI && cfg.context_dim > 0) {
+    // SD v1 fixes the head count (num_heads), SD 2.x the head width (num_head_channels = 64, OAI:542-549): heads = C / width per level
+    CDX_CHECK(cfg.num_heads > 0 || cfg.num_head_channels > 0, "unet: num_heads / num_head_channels");
+    if (cfg.num_head_channels > 0)
+      for (int l = 0; l < cfg.n_mult; ++l)
+        CDX_CHECK((cfg.channel_mult[l] * cfg.model_channels) % cfg.num_head_channels == 0, "unet: %d channels are not whole heads of %d",
+                  cfg.channel_mult[l] * cfg.model_channels, cfg.num_head_channels);
+  }
   else if (cfg.kind != CDX_UNET_DDPM) CDX_CHECK(cfg.num_head_channels > 0 || cfg.num_heads > 0, "unet: num_head_channels / num_heads");
   Net* n = new Net();
   n->eng = e;
@@ -798,7 +805,7 @@ struct UNetExec : Exec {
 
   // SpatialTransformer (ATT:250-261) with one BasicTransformerBlock (ATT:211-215)
   Tensor spatial_transformer(const Tensor& x, const std::string& p) {
-    const int C = x.C, heads = n.ucfg.num_heads, d = C / heads;
+    const int C = x.C, heads = n.ucfg.num_head_channels > 0 ? C / n.ucfg.num_head_channels : n.ucfg.num_heads, d = C / heads;
     const int M = x.rows(), HW = x.H * x.W, B = x.B;
     Tensor out = alloc(B, x.H, x.W, C);
     Scope sc(e.arena);
@@ -1269,9 +1276,9 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
 }
 
 // CLIPEncoderLayer stack (HF modeling_clip.py; OpenAI clip ResidualAttentionBlock): pre-LN, self-attention (q scaled by d^-1/2; causal
-// for the text tower), quick-GELU MLP.  x [B, L, W] -> returns the last layer's output tensor.
+// for the text tower), quick-GELU MLP (exact-erf GELU for the OpenCLIP tower).  x [B, L, W] -> returns the last layer's output tensor.
 static Tensor clip_layers(Exec& ex, Net& n, const std::string& prefix, Tensor x, int B, int L, int W, int heads, int layers, int mlp_width,
-                          bool causal, cudaStream_t s) {
+                          bool causal, cudaStream_t s, bool erf_gelu = false) {
   Engine& e = *n.eng;
   const int d = W / heads;
   const float scale = (float)pow((double)d, -0.5);
@@ -1290,7 +1297,8 @@ static Tensor clip_layers(Exec& ex, Net& n, const std::string& prefix, Tensor x,
       Tensor h = ex.linear(a, p + ".self_attn.out_proj", true, x.p);                 // + residual
       Tensor n2 = ex.ln(h, p + ".layer_norm2");
       Tensor f = ex.linear(n2, p + ".mlp.fc1", true, nullptr, true);
-      quick_gelu(e, f.p, f.p, f.numel(), s);           // |x sigmoid(1.702 x)| <= |x|
+      if (erf_gelu) gelu(e, f.p, f.p, f.numel(), s);    // |gelu(x)| <= |x|
+      else quick_gelu(e, f.p, f.p, f.numel(), s);      // |x sigmoid(1.702 x)| <= |x|
       const Param& w2 = n.param(p + ".mlp.fc2.weight");
       ex.linear_into(f.p, mlp_width, mlp_width, nullptr, 0, 0, B * L, n.blob + w2.off, W, n.P(p + ".mlp.fc2.bias"), h.p, W, y.p, W, nullptr, f.amax);
     }
@@ -1346,7 +1354,7 @@ void text_encode(Net& n, const int* ids, float* out, int B, int L, cudaStream_t 
   Scope top(e.arena);
   Tensor x = ex.alloc(B, L, 1, W);
   embed_tokens(e, ids, n.P(T + "embeddings.token_embedding.weight"), n.P(T + "embeddings.position_embedding.weight"), x.p, B, L, W, c.vocab_size, s);
-  x = clip_layers(ex, n, T, x, B, L, W, c.heads, c.layers, c.mlp_width, true, s);
+  x = clip_layers(ex, n, T, x, B, L, W, c.heads, c.layers, c.mlp_width, true, s, c.kind == CDX_TEXT_OPENCLIP);
   // final LayerNorm straight into the caller's buffer
   layernorm(e, x.p, n.P(T + "final_layer_norm.weight"), n.P(T + "final_layer_norm.bias"), out, B * L, W, s);
 }

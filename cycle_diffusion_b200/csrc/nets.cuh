@@ -43,6 +43,9 @@ struct Net {
   int w_exp = 0;
   size_t blob_floats = 0;
   bool finalized = false;
+  // output parameterisation of an SD U-Net (cdx_unet_set_prediction): 0 eps, 1 v with sqrt(abar_t) / sqrt(1 - abar_t) per timestep t
+  int pred = 0;
+  std::vector<float> sa_v, s1_v;
   // timestep embedding
   std::vector<float> freqs_host;
   float* freqs_dev = nullptr;

@@ -323,6 +323,10 @@ class Net:
 
     def inventory(self):
         """[(name, shape)] in the reference checkpoint's key names."""
+        return self._engine_inventory()
+
+    def _engine_inventory(self):
+        """[(name, shape)] as the engine stores the parameters (cdx_net_param_shape)."""
         out = []
         dims = (C.c_int64 * 4)()
         for i in range(lib.cdx_net_num_params(self.h)):
@@ -338,14 +342,14 @@ class Net:
         if strict:
             extra = [k[len(prefix):] for k in sd if k.startswith(prefix) and k[len(prefix):] not in names]
             assert not extra, f'unexpected keys in state_dict: {extra[:5]}...'
-        for name, shape in inv:
+        for (name, shape), (_, eshape) in zip(inv, self._engine_inventory()):
             key = prefix + name
             assert key in sd, f'missing key in state_dict: {key}'
             t = sd[key]
             assert tuple(t.shape) == shape, f'{key}: shape {tuple(t.shape)} != {shape}'
-            t = t.detach().to(torch.float32).contiguous()
-            dims = (C.c_int64 * 4)(*(list(shape) + [1] * (4 - len(shape))))
-            check(lib.cdx_net_load_param(self.h, name.encode(), _ptr(t), 1 if t.is_cuda else 0, dims, len(shape)))
+            t = t.detach().to(torch.float32).reshape(eshape).contiguous()        # a checkpoint's own layout viewed as the engine's
+            dims = (C.c_int64 * 4)(*(list(eshape) + [1] * (4 - len(eshape))))
+            check(lib.cdx_net_load_param(self.h, name.encode(), _ptr(t), 1 if t.is_cuda else 0, dims, len(eshape)))
         self.finalize()
         return self
 
@@ -373,11 +377,12 @@ class Net:
 
 
 class UNet(Net):
-    """SD/LDM (kind='openai') or improved-DDPM (kind='iddpm') eps-prediction U-Net."""
+    """SD/LDM (kind='openai') or improved-DDPM (kind='iddpm') U-Net; eps-prediction unless set_prediction('v') (SD 2.x "-v")."""
 
     def __init__(self, engine, cfg, kind='openai'):
         self.cfg = dict(cfg)
         self.kind = kind
+        self.prediction = 'eps'
         c = UnetConfig()
         c.kind = {'openai': _cabi.CDX_UNET_OPENAI, 'iddpm': _cabi.CDX_UNET_IDDPM, 'ddpm': _cabi.CDX_UNET_DDPM}[kind]
         c.in_channels, c.out_channels = cfg['in_channels'], cfg['out_channels']
@@ -402,6 +407,32 @@ class UNet(Net):
                 freqs = torch.exp(-math.log(10000) * torch.arange(start=0, end=half, dtype=torch.float32) / half)
             arr = (C.c_float * half)(*freqs.tolist())
             check(lib.cdx_unet_set_time_freqs(self.h, arr, half))
+
+    def inventory(self):
+        """As Net.inventory, except that an SD 2.x config (``use_linear_in_transformer``) lists the spatial transformers'
+        proj_in / proj_out weights as the checkpoint stores them, [C, C] Linear weights; the engine holds them as the equivalent
+        [C, C, 1, 1] 1x1 convolutions and load_state_dict views one as the other."""
+        inv = self._engine_inventory()
+        if self.kind == 'openai' and self.cfg.get('use_linear_in_transformer') and self.cfg.get('context_dim'):
+            inv = [(n, s[:2] if n.endswith(('.proj_in.weight', '.proj_out.weight')) and len(s) == 4 else s) for n, s in inv]
+        return inv
+
+    def set_prediction(self, prediction, alphas_cumprod_f64=None):
+        """What the U-Net predicts: 'eps' (default) or 'v' (SD 2.x parameterization: "v").  Under 'v' the latent loop drivers
+        convert the guidance-combined output at timestep t as e_t = sqrt(abar_t) v + sqrt(1 - abar_t) x_t and
+        pred_x0 = sqrt(abar_t) x_t - sqrt(1 - abar_t) v inside their fused step kernels.  alphas_cumprod_f64: the float64
+        abar table (register_schedule's, before the fp32 cast); default the LDM linear schedule."""
+        from .schedule import v_tables
+        if prediction not in ('eps', 'v'):
+            raise ValueError(f"prediction must be 'eps' or 'v', got {prediction!r}")
+        if prediction == 'eps':
+            check(lib.cdx_unet_set_prediction(self.h, _cabi.CDX_PRED_EPS, None, None, 0))
+        else:
+            sa, s1 = v_tables(alphas_cumprod_f64)
+            T = len(sa)
+            check(lib.cdx_unet_set_prediction(self.h, _cabi.CDX_PRED_V, (C.c_float * T)(*sa.tolist()), (C.c_float * T)(*s1.tolist()), T))
+        self.prediction = prediction
+        return self
 
     def forward(self, x, timesteps, context=None):
         e = self.engine
@@ -632,7 +663,7 @@ class TextEncoder(Net):
         c = TextConfig()
         c.vocab_size, c.width, c.layers = cfg['vocab_size'], cfg['width'], cfg['layers']
         c.heads, c.max_len, c.mlp_width = cfg['heads'], cfg['max_len'], cfg['mlp_width']
-        c.kind = {'clip': 1, 'xtransformer': 2, 'clip_vision': 3}[cfg.get('kind', 'clip')]
+        c.kind = {'clip': 1, 'xtransformer': 2, 'clip_vision': 3, 'openclip': 4}[cfg.get('kind', 'clip')]
         c.dim_head = cfg.get('dim_head', cfg['width'] // cfg['heads'])
         c.proj_dim, c.patch, c.image_size = cfg.get('proj_dim', 0), cfg.get('patch', 0), cfg.get('image_size', 0)
         h = C.c_void_p()

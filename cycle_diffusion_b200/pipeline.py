@@ -32,6 +32,10 @@ class CycleDiffusionPipeline:
         self.g = generator
         self.engine = generator.engine
         self.precision = precision
+        # the U-Net's output parameterisation is the generator's (SD 2.x "-v": 'v'); the loop drivers convert v inside the step
+        pred = getattr(generator, 'parameterization', 'eps')
+        if generator.unet.prediction != pred:
+            generator.unet.set_prediction(pred)
 
     @classmethod
     def from_wrapper(cls, wrapper):

@@ -19,6 +19,19 @@ def ldm_alphas_cumprod(n_timestep=1000, linear_start=0.00085, linear_end=0.012):
     return torch.tensor(np.cumprod(1.0 - betas, axis=0), dtype=torch.float32)
 
 
+def ldm_alphas_cumprod_f64(n_timestep=1000, linear_start=0.00085, linear_end=0.012):
+    """The same schedule before the fp32 cast: register_schedule's float64 alphas_cumprod (numpy)."""
+    betas = (torch.linspace(linear_start ** 0.5, linear_end ** 0.5, n_timestep, dtype=torch.float64) ** 2).numpy()
+    return np.cumprod(1.0 - betas, axis=0)
+
+
+def v_tables(alphas_cumprod_f64=None):
+    """The v-prediction tables of an SD 2 model, indexed by the U-Net timestep t: fp32(sqrt(abar_t)) and fp32(sqrt(1 - abar_t))
+    of the float64 abar (register_schedule's sqrt_alphas_cumprod / sqrt_one_minus_alphas_cumprod buffers)."""
+    ac = ldm_alphas_cumprod_f64() if alphas_cumprod_f64 is None else np.asarray(alphas_cumprod_f64, dtype=np.float64)
+    return np.sqrt(ac).astype(np.float32), np.sqrt(1.0 - ac).astype(np.float32)
+
+
 class DDIMSchedule:
     """DDIMSampler.make_schedule for (S, eta) plus the loop geometry of _ddpm_ddim_encoding / ddim_sampling_with_eps."""
 

@@ -25,6 +25,13 @@ def sd_unet_config(context_dim=768):
                 num_res_blocks=2, channel_mult=(1, 2, 4, 4), num_heads=8, context_dim=context_dim)
 
 
+def sd2_unet_config():
+    """v2-inference.yaml / v2-inference-v.yaml unet_config (SD 2.x base and -v): SD v1's topology with a fixed head WIDTH of 64
+    (5 / 10 / 20 heads), the OpenCLIP-H context width 1024 and Linear proj_in / proj_out (use_linear_in_transformer)."""
+    return dict(in_channels=4, out_channels=4, model_channels=320, attention_resolutions=(4, 2, 1),
+                num_res_blocks=2, channel_mult=(1, 2, 4, 4), num_head_channels=64, context_dim=1024, use_linear_in_transformer=True)
+
+
 def kl_f8_config():
     """v1-inference.yaml:51-65."""
     return dict(ch=128, ch_mult=(1, 2, 4, 4), num_res_blocks=2, in_channels=3, out_ch=3, z_channels=4, embed_dim=4)
@@ -78,8 +85,9 @@ def openai_unet_params(cfg, prefix=''):
             out.append((p + '.proj_out.weight', (c, c, 1), 'w'))
             out.append((p + '.proj_out.bias', (c,), 'b'))
             return
+        lin = cfg.get('use_linear_in_transformer', False)     # SD 2.x: Linear [C, C] projections instead of 1x1 convolutions
         _norm(out, p + '.norm', c)
-        _conv(out, p + '.proj_in', c, c, 1)
+        _lin(out, p + '.proj_in', c, c) if lin else _conv(out, p + '.proj_in', c, c, 1)
         t = p + '.transformer_blocks.0'
         for a, kd in (('attn1', c), ('attn2', ctx)):
             _lin(out, f'{t}.{a}.to_q', c, c, bias=False)
@@ -90,7 +98,7 @@ def openai_unet_params(cfg, prefix=''):
         _lin(out, t + '.ff.net.2', 4 * c, c)
         for n in ('norm1', 'norm2', 'norm3'):
             _norm(out, f'{t}.{n}', c)
-        _conv(out, p + '.proj_out', c, c, 1)
+        _lin(out, p + '.proj_out', c, c) if lin else _conv(out, p + '.proj_out', c, c, 1)
 
     P = prefix
     _lin(out, P + 'time_embed.0', mc, ted)
@@ -278,6 +286,70 @@ def clip_text_params(cfg, prefix=''):
         out += [(f'{p}.mlp.fc2.weight', (W, M), 'w'), (f'{p}.mlp.fc2.bias', (W,), 'b')]
         out += [(f'{p}.layer_norm2.weight', (W,), 'nw'), (f'{p}.layer_norm2.bias', (W,), 'nb')]
     out += [(T + 'final_layer_norm.weight', (W,), 'nw'), (T + 'final_layer_norm.bias', (W,), 'nb')]
+    return out
+
+
+def openclip_h14_text_config(layers=23, total_layers=24, vocab_size=49408, width=1024, heads=16, max_len=77, mlp_width=4096):
+    """SD 2.x conditioning model: FrozenOpenCLIPEmbedder(arch="ViT-H-14", layer="penultimate") -- 24 pre-LN blocks of width 1024,
+    16 heads, exact-erf GELU; `layers` = 23 blocks run (the penultimate output), then ln_final.  `total_layers` is what the
+    checkpoint holds (block 23 is loaded by nobody)."""
+    return dict(kind='openclip', vocab_size=vocab_size, width=width, layers=layers, total_layers=total_layers, heads=heads,
+                max_len=max_len, mlp_width=mlp_width)
+
+
+def openclip_text_params(cfg, prefix=''):
+    """Ordered (name, shape, kind) list of the OpenCLIP text transformer as the SD 2 checkpoint stores it under
+    ``cond_stage_model.model.`` (open_clip CLIP without `visual`): all `total_layers` blocks, text_projection and logit_scale."""
+    W, M, V = cfg['width'], cfg['mlp_width'], cfg['vocab_size']
+    P = prefix
+    out = [(P + 'positional_embedding', (cfg['max_len'], W), 'w'), (P + 'text_projection', (W, W), 'w'),
+           (P + 'logit_scale', (), 'b'), (P + 'token_embedding.weight', (V, W), 'w')]
+    for l in range(cfg.get('total_layers', cfg['layers'])):
+        p = f'{P}transformer.resblocks.{l}'
+        out += [(p + '.ln_1.weight', (W,), 'nw'), (p + '.ln_1.bias', (W,), 'nb'),
+                (p + '.attn.in_proj_weight', (3 * W, W), 'w'), (p + '.attn.in_proj_bias', (3 * W,), 'b'),
+                (p + '.attn.out_proj.weight', (W, W), 'w'), (p + '.attn.out_proj.bias', (W,), 'b'),
+                (p + '.ln_2.weight', (W,), 'nw'), (p + '.ln_2.bias', (W,), 'nb'),
+                (p + '.mlp.c_fc.weight', (M, W), 'w'), (p + '.mlp.c_fc.bias', (M,), 'b'),
+                (p + '.mlp.c_proj.weight', (W, M), 'w'), (p + '.mlp.c_proj.bias', (W,), 'b')]
+    out += [(P + 'ln_final.weight', (W,), 'nw'), (P + 'ln_final.bias', (W,), 'nb')]
+    return out
+
+
+def openclip_to_hf(sd, layers, prefix=''):
+    """OpenCLIP text-transformer keys (under `prefix`) -> the HF CLIPTextModel keys of the engine's OpenCLIP tower, blocks
+    0 .. layers-1 only: in_proj split into q / k / v (stacked [q; k; v] along dim 0), positional_embedding ->
+    position_embedding.weight, ln_1 / ln_2 / mlp.c_fc / mlp.c_proj / ln_final -> layer_norm1 / layer_norm2 / mlp.fc1 / mlp.fc2 /
+    final_layer_norm.  text_projection, logit_scale and the blocks past `layers` are not used for conditioning."""
+    T = 'text_model.'
+    out = {T + 'embeddings.token_embedding.weight': sd[prefix + 'token_embedding.weight'],
+           T + 'embeddings.position_embedding.weight': sd[prefix + 'positional_embedding']}
+    for l in range(layers):
+        o, h = f'{prefix}transformer.resblocks.{l}.', f'{T}encoder.layers.{l}.'
+        q, k, v = sd[o + 'attn.in_proj_weight'].chunk(3, dim=0)
+        qb, kb, vb = sd[o + 'attn.in_proj_bias'].chunk(3, dim=0)
+        for nm, w, b in (('q_proj', q, qb), ('k_proj', k, kb), ('v_proj', v, vb)):
+            out[h + f'self_attn.{nm}.weight'], out[h + f'self_attn.{nm}.bias'] = w, b
+        for src, dst in (('attn.out_proj', 'self_attn.out_proj'), ('ln_1', 'layer_norm1'), ('ln_2', 'layer_norm2'),
+                         ('mlp.c_fc', 'mlp.fc1'), ('mlp.c_proj', 'mlp.fc2')):
+            out[h + dst + '.weight'], out[h + dst + '.bias'] = sd[o + src + '.weight'], sd[o + src + '.bias']
+    out[T + 'final_layer_norm.weight'], out[T + 'final_layer_norm.bias'] = sd[prefix + 'ln_final.weight'], sd[prefix + 'ln_final.bias']
+    return out
+
+
+def hf_to_openclip(sd, layers, prefix=''):
+    """The inverse of openclip_to_hf for blocks 0 .. layers-1 (no text_projection / logit_scale)."""
+    T = 'text_model.'
+    out = {prefix + 'token_embedding.weight': sd[T + 'embeddings.token_embedding.weight'],
+           prefix + 'positional_embedding': sd[T + 'embeddings.position_embedding.weight']}
+    for l in range(layers):
+        o, h = f'{prefix}transformer.resblocks.{l}.', f'{T}encoder.layers.{l}.'
+        out[o + 'attn.in_proj_weight'] = torch.cat([sd[h + f'self_attn.{n}.weight'] for n in ('q_proj', 'k_proj', 'v_proj')])
+        out[o + 'attn.in_proj_bias'] = torch.cat([sd[h + f'self_attn.{n}.bias'] for n in ('q_proj', 'k_proj', 'v_proj')])
+        for src, dst in (('attn.out_proj', 'self_attn.out_proj'), ('ln_1', 'layer_norm1'), ('ln_2', 'layer_norm2'),
+                         ('mlp.c_fc', 'mlp.fc1'), ('mlp.c_proj', 'mlp.fc2')):
+            out[o + src + '.weight'], out[o + src + '.bias'] = sd[h + dst + '.weight'], sd[h + dst + '.bias']
+    out[prefix + 'ln_final.weight'], out[prefix + 'ln_final.bias'] = sd[T + 'final_layer_norm.weight'], sd[T + 'final_layer_norm.bias']
     return out
 
 

@@ -2,6 +2,7 @@
 
 Mirrors (same constructor kwargs, method names, argument meaning, return layouts and precondition checks):
   SDStochasticTextWrapper            ref model/gan_wrapper/stable_diffusion_stochastic_text_wrapper.py:100-253
+  SD2StochasticTextWrapper           the same wrapper for the SD 2.x checkpoints (v2-1_512 eps, v2-1_768 v-prediction)
   LatentDiffStochasticTextWrapper    ref model/gan_wrapper/latentdiff_stochastic_text_wrapper.py:102-252
   DDPMDDIMWrapper                    ref model/gan_wrapper/ddpm_ddim_wrapper.py:317-538
   get_gan_wrapper                    ref model/gan_wrapper/get_gan_wrapper.py:3-31
@@ -70,6 +71,21 @@ class BertTextCondStage(ClipTextCondStage):
         super().__init__(engine, state_dict, tokenizer, cfg or specs.bert_text_config(), prefix)
 
 
+class OpenClipTextCondStage(ClipTextCondStage):
+    """SD 2.x conditioning model: FrozenOpenCLIPEmbedder(arch="ViT-H-14", layer="penultimate").encode_with_transformer after
+    tokenisation -- token + positional embedding, the first 23 of the 24 pre-LN blocks (causal attention, exact-erf GELU MLP),
+    ln_final -> [B, 77, 1024].  ``state_dict``: the checkpoint's OpenCLIP keys under ``prefix`` (``cond_stage_model.model.``),
+    mapped to the engine's HF-named CDX_TEXT_OPENCLIP tower by specs.openclip_to_hf.  ``tokenizer``: a host callable
+    ``list[str] -> LongTensor [B, 77]`` (open_clip.tokenize: start / end tokens, zero padding)."""
+
+    def __init__(self, engine, state_dict, tokenizer, cfg=None, prefix='cond_stage_model.model.'):
+        from .engine import TextEncoder
+        self.cfg = cfg or specs.openclip_h14_text_config()
+        self.tokenizer = tokenizer
+        self.encoder = TextEncoder(engine, self.cfg)
+        self.encoder.load_state_dict(specs.openclip_to_hf(state_dict, self.cfg['layers'], prefix))
+
+
 class SyntheticTextEncoder:
     """Deterministic stand-in for FrozenCLIPEmbedder / BERTEmbedder: prompt string -> N(0,1) tokens [77, dim].
 
@@ -110,6 +126,7 @@ class _LatentGenerator:
         self.channels, self.image_size, self.scale_factor = channels, image_size, scale_factor
         self.sample_posterior = sample_posterior
         self.alphas_cumprod = None      # default LDM linear schedule (v1-inference.yaml:5-9)
+        self.parameterization = unet.prediction     # what the U-Net predicts: 'eps', or 'v' for the SD 2.x "-v" models
 
     def get_learned_conditioning(self, c):
         return self.cond_stage(c)
@@ -170,7 +187,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
             self.engine = engine or Engine(device)
             ucfg = unet_config or specs.sd_unet_config(self.CONTEXT_DIM)
             vcfg = vae_config or specs.kl_f8_config()
-            unet, vae = UNet(self.engine, ucfg, 'openai'), VAE(self.engine, vcfg)
+            unet, vae = self._build_unet(ucfg), VAE(self.engine, vcfg)
             ckpt = self.default_checkpoint(source_model_type)
             cond = cond_stage
             if state_dict == 'synthetic':
@@ -197,6 +214,9 @@ class _StochasticTextWrapperBase(torch.nn.Module):
             self.generator = _LatentGenerator(self.engine, unet, vae, cond, ucfg['in_channels'], latent_size or self.LATENT, 0.18215,
                                               self.SAMPLE_POSTERIOR)
         self._dummy = torch.nn.Parameter(torch.zeros(1, device=self.engine.device), requires_grad=False)
+
+    def _build_unet(self, ucfg):
+        return UNet(self.engine, ucfg, 'openai')
 
     def _precision_scope(self):
         """SDW:143-144, 173: ``autocast("cuda")`` when precision == "autocast", else a null context -- here the engine's mma
@@ -463,6 +483,31 @@ class _StochasticTextWrapperBase(torch.nn.Module):
 
 class SDStochasticTextWrapper(_StochasticTextWrapperBase):
     """Stable Diffusion v1 (512 px, latent 64, CLIP context 768, posterior *sample*)."""
+
+
+class SD2StochasticTextWrapper(_StochasticTextWrapperBase):
+    """Stable Diffusion 2.x: ``parameterization='eps'`` is v2-1_512 ("base", 512 px, latent 64), ``'v'`` is v2-1_768 ("-v",
+    768 px, latent 96, v-prediction), the ldm yaml key of the same name.  OpenCLIP-H context 1024 (OpenClipTextCondStage from the
+    checkpoint's ``cond_stage_model.model.*`` keys), 64-channel heads, Linear transformer projections, posterior *sample*.
+    Everything else -- precision, encode / forward, cycle, cycle_ensemble -- is SDStochasticTextWrapper's."""
+    CONTEXT_DIM = 1024
+    COND_PREFIX = 'cond_stage_model.model.'           # FrozenOpenCLIPEmbedder.model (open_clip CLIP without `visual`)
+    COND_CLASS = OpenClipTextCondStage
+    RESOLUTIONS = {'eps': 512, 'v': 768}
+
+    def __init__(self, *args, parameterization='eps', resolution=None, latent_size=None, unet_config=None, **kwargs):
+        if parameterization not in self.RESOLUTIONS:
+            raise ValueError(f"parameterization must be 'eps' or 'v', got {parameterization!r}")
+        self.parameterization = parameterization
+        resolution = resolution or self.RESOLUTIONS[parameterization]
+        super().__init__(*args, resolution=resolution, latent_size=latent_size or resolution // 8,
+                         unet_config=unet_config or specs.sd2_unet_config(), **kwargs)
+        if self.generator.unet.prediction != parameterization:      # a generator passed in is switched to this wrapper's yaml key
+            self.generator.unet.set_prediction(parameterization)
+        self.generator.parameterization = parameterization
+
+    def _build_unet(self, ucfg):
+        return UNet(self.engine, ucfg, 'openai').set_prediction(self.parameterization)
 
 
 class LatentDiffStochasticTextWrapper(_StochasticTextWrapperBase):
@@ -798,5 +843,7 @@ def get_gan_wrapper(args, target=False, **extra):
         return LatentDiffStochasticTextWrapper(**kwargs)
     elif gan_type == "SDStochasticText":
         return SDStochasticTextWrapper(**kwargs)
+    elif gan_type == "SD2StochasticText":
+        return SD2StochasticTextWrapper(**kwargs)
     else:
         raise ValueError()

@@ -127,6 +127,10 @@ typedef struct cdx_text_config { /* CLIP ViT-L/14 text tower as FrozenCLIPEmbedd
 #define CDX_TEXT_CLIP 1
 #define CDX_TEXT_XTRANSFORMER 2
 #define CDX_CLIP_VISION 3
+/* OpenCLIP ViT-H/14 text tower of SD 2.x (FrozenOpenCLIPEmbedder, layer="penultimate"): the parameter names and order of
+   CDX_TEXT_CLIP, exact-erf GELU in the MLP instead of quick-GELU.  `layers` is the number of blocks that run (23 of 24 for the
+   penultimate output); the final LayerNorm follows the last of them. */
+#define CDX_TEXT_OPENCLIP 4
 
 /* Build the host-side execution plan and parameter inventory (no GPU work). */
 int cdx_unet_create(cdx_engine* e, const cdx_unet_config* cfg, cdx_net** out);
@@ -156,6 +160,16 @@ int cdx_net_adopt_blob(cdx_net* n); /* mark a blob filled externally (broadcast)
  * passes the table computed with the reference expression so that CPU oracle and engine agree
  * bit-for-bit on the frequencies; `half` must equal model_channels/2. */
 int cdx_unet_set_time_freqs(cdx_net* n, const float* freqs_host, int half);
+
+/* Output parameterisation of a CDX_UNET_OPENAI net (CDX_E_INVALID for any other kind).  CDX_PRED_EPS (the default): the U-Net
+ * predicts the noise.  CDX_PRED_V (SD 2.x "-v" checkpoints, parameterization: "v"): it predicts v, and the latent loop drivers
+ * (cdx_latent_encode / _decode, cdx_cycle_lockstep, cdx_latent_loop_ens, cdx_latent_cycle_fan) convert the guidance-combined output
+ * of a step at timestep t as e_t = sa_v[t] v + s1_v[t] x_t, pred_x0 = sa_v[t] x_t - s1_v[t] v inside their fused step kernels.
+ * sa_v / s1_v: host [T], fp32(sqrt(abar_t)) and fp32(sqrt(1 - abar_t)) of the float64 schedule; every loop timestep must be < T.
+ * cdx_latent_cycle_pair rejects v nets; the single-op cdx_ddim_* kernels are eps-only. */
+#define CDX_PRED_EPS 0
+#define CDX_PRED_V 1
+int cdx_unet_set_prediction(cdx_net* unet, int prediction, const float* sa_v_host, const float* s1_v_host, int T);
 
 /* UNetModel.forward (OAI:710-742 via LatentDiffusion.apply_model ddpm.py:882-983 / IU:639-668).
  * x, out: [B, C, H, W] NCHW dev; t_dev: [B] float timesteps on device (the reference's int64

@@ -137,26 +137,32 @@ void hook_h16_planes(Engine& e, const float* w, size_t n, GemmArgs& g, cudaStrea
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// The latent sampling loops (DDIMSampler._ddpm_ddim_encoding ddim.py:450-501, ddim_sampling_with_eps ddim.py:395-448) as ONE
-// driver with three modes: DPM-Encoder only, decode only, or both chains in lock-step (the source chain under the source
-// condition and the target chain under the target condition share one U-Net call per step; the noise recovered at step i is
-// consumed by the target chain in registers, so no z buffer is needed -- the Diffusers CycleDiffusionPipeline loop shape).
-// Per step: one U-Net call on the batch [src segments | tgt segments] (a chain contributes [uncond, cond] when it runs with
-// classifier-free guidance, ddim.py:550-559, else one segment) and ONE fused elementwise launch (latent_step).
+// The latent sampling loops (DDIMSampler._ddpm_ddim_encoding ddim.py:450-501, ddim_sampling_with_eps ddim.py:395-448, and the
+// ensemble search SDW:189-204 / :146-165) as ONE driver over chains.  Each of the n_src element groups has at most one source chain
+// (the DPM-Encoder under the source condition) and K target chains (decoders under the target condition); the noise the source
+// recovers at step i is consumed by its targets in registers, so lock-step needs no z buffer -- the Diffusers
+// CycleDiffusionPipeline loop shape.  K == 0 is the DPM-Encoder alone, no source chain the decoder alone (noise read from z_in /
+// extra), K == 1 the single-image cycle, K > 1 one recovered chain driving several decoder scales.
+// Per step: one U-Net call over exactly the rows the chains need (a chain contributes [uncond, cond] when it runs with
+// classifier-free guidance, ddim.py:550-559, else one row) and ONE fused elementwise launch (latent_chains_step).
 // ---------------------------------------------------------------------------------------------------------------------
-enum { LOOP_ENC = 1, LOOP_DEC = 2, LOOP_LOCK = 3 };
-struct LatentLoopArgs {
-  int mode = 0;
-  const float* x0 = nullptr;                       // ENC / LOCK
+struct ChainLoopArgs {
+  int n_src = 0, K = 0;                            // element groups; target chains per group
+  bool src = false;                                // a source chain per group
+  const float* x0 = nullptr;                       // src
+  // contexts [n_src, L, D]: every chain of group j runs under c_src[j] / c_tgt[j], its uncond row under uc[j]
   const float* c_src = nullptr; const float* c_tgt = nullptr; const float* uc = nullptr; int L = 0;
-  float s_scale = 1.f, t_scale = 1.f;
-  const float* s_scale_v = nullptr; const float* t_scale_v = nullptr;     // per-sample scales (device, [B]): ensemble members along B
+  // guidance scales [n_src] / [n_src*K], from the host or on the device.  Host scales decide the rows: with `uc`, a chain at a
+  // scale other than 0 and 1 has a cond and an uncond row, else one.  Device scales cannot (nothing is read back), so with `uc`
+  // every chain has both rows and the step kernel picks the row of a chain at scale 0 or 1.
+  const float* s_scales = nullptr; const float* t_scales = nullptr; bool scales_on_device = false;
   const cdx_ddim_coef* coef = nullptr; const float* t_host = nullptr; int n_steps = 0;
-  int n_rec = 0; const float* noise = nullptr; float sa = 0.f, s1 = 0.f;      // ENC / LOCK: noise [n_rec+1, B, chw]
-  float* z_out = nullptr;                           // ENC: [B, n_rec+1, chw]; LOCK: optional
-  const float* z_in = nullptr; int n_eps = 0; const float* extra = nullptr;   // DEC
-  float* x_out = nullptr;                           // DEC / LOCK
-  int B = 0, C = 0, h = 0, w = 0;
+  int n_rec = 0; const float* noise = nullptr; float sa = 0.f, s1 = 0.f;      // src: steps the source runs; noise [n_rec+1, n_src, chw]
+  float* z_out = nullptr;                           // src: [n_src, n_rec+1, chw], optional when K > 0
+  const float* z_in = nullptr; int n_eps = 0;       // no src: [n_src, n_eps+1, chw], x_T then the recovered noises
+  const float* extra = nullptr;                     // noise of the steps past n_eps (no src) / past n_rec (src)
+  float* x_out = nullptr;                           // K > 0: [n_src*K, chw]
+  int C = 0, h = 0, w = 0;
 };
 
 // v-prediction nets (cdx_unet_set_prediction): every U-Net timestep of the loop must index the net's sqrt(abar) tables
@@ -168,212 +174,116 @@ void check_v_steps(const Net& u, const float* t_host, int n) {
               (int)u.sa_v.size());
   }
 }
-template <class Step>
-void set_v(const Net& u, float t, Step& st) {
+void set_v(const Net& u, float t, LatentChains& st) {
   if (!u.pred) return;
   st.pred = 1; st.vsa = u.sa_v[(int)t]; st.vs1 = u.s1_v[(int)t];
 }
 
-// `tgt_net`: the target chain runs under its own net (two-model translation, LOCK mode, context-free): the step's U-Net call is split
-// into a source call and a target call over the two halves of `xin` / `eout`.  With n_rec < n_steps the target chain continues
-// alone after the last recovered step, with `extra` noise (ddim.py:640).
-void run_latent_loop(Net& unet, const LatentLoopArgs& a, cudaStream_t s, Net* tgt_net = nullptr) {
+// `tgt_net`: the target chains run under their own net (two-model translation, context-free): the step's U-Net call is split into a
+// source call and a target call over the source rows and the target rows of `xin` / `eout`.  With n_rec < n_steps the target chains
+// continue alone after the last recovered step, with `extra` noise (ddim.py:640).
+void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* tgt_net = nullptr) {
   Engine& e = *unet.eng;
-  const int B = a.B, chw = a.C * a.h * a.w;
-  const size_t n = (size_t)B * chw;
-  const bool enc = a.mode & LOOP_ENC, dec = a.mode & LOOP_DEC;
-  // (with per-sample scales both segments always run; samples whose scale is 0 / 1 pick their segment's output unchanged)
-  const bool cfg_s = enc && a.uc && (a.s_scale_v || (a.s_scale != 1.0f && a.s_scale != 0.0f));
-  const bool cfg_t = dec && a.uc && (a.t_scale_v || (a.t_scale != 1.0f && a.t_scale != 0.0f));
-  const int nseg_src = enc ? (cfg_s ? 2 : 1) : 0, nseg_tgt = dec ? (cfg_t ? 2 : 1) : 0, nseg = nseg_src + nseg_tgt;
-  const int nb = nseg * B;
-  const int D = unet.ucfg.context_dim;
-  const size_t ctx_n = (size_t)B * a.L * D;
-  Scope sc(e.arena);
-  unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
-  struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
-  float* xin = (float*)e.arena.alloc((size_t)nseg * n * sizeof(float));
-  float* eout = (float*)e.arena.alloc((size_t)nseg * n * sizeof(float));
-  float* ctx_in = (float*)e.arena.alloc((size_t)nseg * ctx_n * sizeof(float));
-  float* xb[3] = {nullptr, nullptr, nullptr};
-  float* yb[2] = {nullptr, nullptr};
-  if (enc) for (int k = 0; k < 3; ++k) xb[k] = (float*)e.arena.alloc(n * sizeof(float));
-  if (dec) for (int k = 0; k < 2; ++k) yb[k] = (float*)e.arena.alloc(n * sizeof(float));
-  const int loop_steps = enc && !dec ? a.n_rec : a.n_steps;
+  const int chw = a.C * a.h * a.w, n_tgt_chains = a.n_src * a.K;
+  const size_t n = (size_t)a.n_src * chw;
+  const size_t ctx_n = (size_t)a.L * unet.ucfg.context_dim;
+  // the chain table: all source-chain rows first, then all target-chain rows (the two-model loop runs the two blocks under two
+  // nets); inside a block the uncond rows come first, cat([uc, c]) as ddim.py:555-557
+  std::vector<Chain> ch((size_t)a.n_src + n_tgt_chains, Chain{-1, -1, 1.f});
+  int rows = 0;
+  auto place = [&](Chain* c, int count, const float* scales) {
+    for (int k = 0; k < count; ++k) {
+      if (!a.scales_on_device && scales) c[k].scale = scales[k];
+      if (a.uc && (a.scales_on_device || (c[k].scale != 0.0f && c[k].scale != 1.0f))) c[k].row2 = rows++;
+    }
+    for (int k = 0; k < count; ++k) c[k].row = rows++;
+  };
+  if (a.src) place(ch.data(), a.n_src, a.s_scales);
+  const int rows_src = rows;
+  place(ch.data() + a.n_src, n_tgt_chains, a.t_scales);
+  const int loop_steps = a.K ? a.n_steps : a.n_rec;
   CDX_CHECK(!tgt_net || (!unet.pred && !tgt_net->pred), "two-model latent loop: eps-prediction U-Nets only");
   check_v_steps(unet, a.t_host, loop_steps);
-  float* tdev = (float*)e.arena.alloc((size_t)std::max(loop_steps, 1) * nb * sizeof(float));
-  upload_timesteps(e, a.t_host, loop_steps, nb, tdev, s);
-  if (ctx_n) {   // cat([uc, c]) per chain: uncond first (ddim.py:555-557); unconditional models (L == 0) carry no context
-    int sg = 0;
-    if (enc) {
-      if (cfg_s) copy_dd(e, a.uc, ctx_in + (size_t)(sg++) * ctx_n, ctx_n, s);
-      copy_dd(e, (a.uc && !a.s_scale_v && a.s_scale == 0.0f) ? a.uc : a.c_src, ctx_in + (size_t)(sg++) * ctx_n, ctx_n, s);
-    }
-    if (dec) {
-      if (cfg_t) copy_dd(e, a.uc, ctx_in + (size_t)(sg++) * ctx_n, ctx_n, s);
-      copy_dd(e, (a.uc && !a.t_scale_v && a.t_scale == 0.0f) ? a.uc : a.c_tgt, ctx_in + (size_t)(sg++) * ctx_n, ctx_n, s);
-    }
-  }
-  const float* es_uc = cfg_s ? eout : nullptr;
-  const float* es_c = eout + (cfg_s ? n : 0);
-  const float* et_uc = cfg_t ? eout + (size_t)nseg_src * n : nullptr;
-  const float* et_c = eout + (size_t)nseg_src * n + (cfg_t ? n : 0);
-  auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
-    if (i_next >= a.n_rec) return 0;
-    return (a.n_steps - 1 - i_next) == 0 ? 2 : 1;                               // ddim.py:583-584
-  };
-  if (enc) {
-    LatentInit in;
-    in.n = n; in.chw = chw;
-    in.x0 = a.x0; in.noise0 = a.noise; in.sa = a.sa; in.s1 = a.s1;
-    in.z_out = a.z_out; in.z_stride = (long long)(a.n_rec + 1) * chw;
-    in.xt = xb[0]; in.yt = dec ? yb[0] : nullptr;
-    in.next = next_kind(0);
-    if (in.next) { in.noise_next = a.noise + n; in.cnext = a.coef[0]; }
-    in.xn = xb[1];
-    in.xin = xin; in.nseg_src = nseg_src; in.nseg_tgt = nseg_tgt;
-    latent_init(e, in, s);
-  } else {
-    gather_slot(e, a.z_in, yb[0], B, chw, a.n_eps + 1, 0, s);                   // x_T = eps_list[:, 0], SDW:153
-    for (int sg = 0; sg < nseg_tgt; ++sg) copy_dd(e, yb[0], xin + (size_t)sg * n, n, s);
-  }
-  const int iters = e.dry() ? std::min(loop_steps, 1) : loop_steps;
-  PairStreams ps(e, tgt_net ? *tgt_net->eng : e, s);
-  for (int i = 0; i < iters; ++i) {
-    const bool enc_i = enc && i < a.n_rec;
-    if (!tgt_net) {
-      unet_forward(unet, xin, tdev + (size_t)i * nb, ctx_in, a.L, eout, nb, a.h, a.w, s, true);
-    } else {
-      const size_t ns = (size_t)nseg_src * B;
-      ps.fork();
-      if (enc_i) unet_forward(unet, xin, tdev + (size_t)i * nb, nullptr, 0, eout, (int)ns, a.h, a.w, s);
-      unet_forward(*tgt_net, xin + ns * chw, tdev + (size_t)i * nb + ns, nullptr, 0, eout + ns * chw, nb - (int)ns, a.h, a.w,
-                   ps.target_stream());
-      ps.join();
-    }
-    LatentStep st;
-    st.n = n; st.chw = chw;
-    if (enc_i) {
-      st.enc = 1;
-      st.x0 = a.x0; st.xt = xb[0]; st.xn = xb[1];
-      st.es_c = es_c; st.es_uc = es_uc; st.s_scale = a.s_scale; st.s_scale_v = a.s_scale_v; st.cs = a.coef[i];
-      if (a.z_out) { st.z_out = a.z_out + (size_t)(1 + i) * chw; st.z_stride = (long long)(a.n_rec + 1) * chw; }
-      st.next = next_kind(i + 1);
-      if (st.next) { st.noise_next = a.noise + (size_t)(2 + i) * n; st.cnext = a.coef[i + 1]; }
-      st.xn2 = xb[2];
-    }
-    if (dec) {
-      st.dec = 1;
-      st.yt = yb[0]; st.et_c = et_c; st.et_uc = et_uc; st.t_scale = a.t_scale; st.t_scale_v = a.t_scale_v; st.ct = a.coef[i];
-      if (!enc) {
-        if (i < a.n_eps) { st.eps_in = a.z_in + (size_t)(1 + i) * chw; st.eps_stride = (long long)(a.n_eps + 1) * chw; }
-        else { st.eps_in = a.extra + (size_t)(i - a.n_eps) * n; st.eps_stride = chw; }
-      } else if (!enc_i) {
-        st.eps_in = a.extra + (size_t)(i - a.n_rec) * n; st.eps_stride = chw;
-      }
-      st.y_out = (i == loop_steps - 1) ? a.x_out : yb[1];
-    }
-    st.xin = xin; st.nseg_src = nseg_src; st.nseg_tgt = nseg_tgt;
-    set_v(unet, a.t_host[i], st);
-    latent_step(e, st, s);
-    if (enc_i) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
-    if (dec) std::swap(yb[0], yb[1]);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// The ensemble search in lock-step (SDW:189-204 encode, :146-165 generate): n_src source chains, each (member, sample) pair's
-// DPM-Encoder chain, drive K decoder-scale chains each with the noise they recover.  Per step: one U-Net call over exactly the rows
-// the chains need (a chain at scale 0 or 1 has one row, any other scale a cond and an uncond row) and one latent_fan_step launch.
-// The row layout follows from the host scales, so nothing is read back from the device.
-// ---------------------------------------------------------------------------------------------------------------------
-struct LatentFanArgs {
-  int n_src = 0, K = 0;
-  const float* x0 = nullptr; const float* c_src = nullptr; const float* c_tgt = nullptr; const float* uc = nullptr; int L = 0;
-  const float* src_scales = nullptr; const float* tgt_scales = nullptr;          // host [n_src], [n_src*K]
-  const cdx_ddim_coef* coef = nullptr; const float* t_host = nullptr; int n_steps = 0;
-  const float* noise = nullptr; float sa = 0.f, s1 = 0.f;                         // noise [n_steps+1, n_src, chw]
-  float* x_out = nullptr; float* z_out = nullptr;
-  int C = 0, h = 0, w = 0;
-};
-
-// the rows of every chain: source chain j first, then its K targets; returns the row count
-int fan_rows(const LatentFanArgs& a, std::vector<FanChain>& ch) {
-  ch.assign((size_t)a.n_src * (1 + a.K), FanChain{});
-  int rows = 0;
-  auto place = [&](FanChain& c, float scale) {
-    c.scale = scale;
-    c.row = rows++;
-    c.row2 = (scale != 0.0f && scale != 1.0f) ? rows++ : -1;
-  };
-  for (int j = 0; j < a.n_src; ++j) {
-    place(ch[j], a.src_scales[j]);
-    for (int k = 0; k < a.K; ++k) place(ch[a.n_src + (size_t)j * a.K + k], a.tgt_scales[(size_t)j * a.K + k]);
-  }
-  return rows;
-}
-
-void run_latent_fan(Net& unet, const LatentFanArgs& a, cudaStream_t s) {
-  Engine& e = *unet.eng;
-  const int chw = a.C * a.h * a.w;
-  const size_t n = (size_t)a.n_src * chw, n_tgt = (size_t)a.n_src * a.K * chw;
-  std::vector<FanChain> ch;
-  const int rows = fan_rows(a, ch);
-  const size_t ctx_n = (size_t)a.L * unet.ucfg.context_dim;
-  check_v_steps(unet, a.t_host, a.n_steps);
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
   struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
   float* xin = (float*)e.arena.alloc((size_t)rows * chw * sizeof(float));
   float* eout = (float*)e.arena.alloc((size_t)rows * chw * sizeof(float));
   float* ctx_in = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
-  float* xb[3];
-  for (float*& p : xb) p = (float*)e.arena.alloc(n * sizeof(float));
-  float* yb[2];
-  for (float*& p : yb) p = (float*)e.arena.alloc(n_tgt * sizeof(float));
-  float* tdev = (float*)e.arena.alloc((size_t)a.n_steps * rows * sizeof(float));
-  FanChain* chd = (FanChain*)e.arena.alloc(ch.size() * sizeof(FanChain));
-  upload_timesteps(e, a.t_host, a.n_steps, rows, tdev, s);
-  if (!e.dry())   // pageable source: staged before the call returns
-    CDX_CUDA(cudaMemcpyAsync(chd, ch.data(), ch.size() * sizeof(FanChain), cudaMemcpyHostToDevice, s));
-  // one context per row: the chain's condition on its cond row, uc on its uncond row (ddim.py:555-557)
-  auto ctx_rows = [&](const FanChain& c, const float* cond, int j) {
-    copy_dd(e, c.scale == 0.0f ? a.uc + j * ctx_n : cond + j * ctx_n, ctx_in + (size_t)c.row * ctx_n, ctx_n, s);
-    if (c.row2 >= 0) copy_dd(e, a.uc + j * ctx_n, ctx_in + (size_t)c.row2 * ctx_n, ctx_n, s);
-  };
-  for (int j = 0; j < a.n_src; ++j) {
-    ctx_rows(ch[j], a.c_src, j);
-    for (int k = 0; k < a.K; ++k) ctx_rows(ch[a.n_src + (size_t)j * a.K + k], a.c_tgt, j);
+  float* xb[3] = {nullptr, nullptr, nullptr};
+  float* yb[2] = {nullptr, nullptr};
+  if (a.src) for (float*& p : xb) p = (float*)e.arena.alloc(n * sizeof(float));
+  if (a.K) for (float*& p : yb) p = (float*)e.arena.alloc((size_t)n_tgt_chains * chw * sizeof(float));
+  float* tdev = (float*)e.arena.alloc((size_t)std::max(loop_steps, 1) * rows * sizeof(float));
+  Chain* chd = (Chain*)e.arena.alloc(ch.size() * sizeof(Chain));
+  upload_timesteps(e, a.t_host, loop_steps, rows, tdev, s);
+  if (!e.dry()) {   // pageable source: staged before the call returns
+    CDX_CUDA(cudaMemcpyAsync(chd, ch.data(), ch.size() * sizeof(Chain), cudaMemcpyHostToDevice, s));
+    auto scales_to = [&](Chain* c, const float* scales, int count) {
+      CDX_CUDA(cudaMemcpy2DAsync(&c->scale, sizeof(Chain), scales, sizeof(float), sizeof(float), count, cudaMemcpyDeviceToDevice, s));
+    };
+    if (a.scales_on_device && a.src) scales_to(chd, a.s_scales, a.n_src);
+    if (a.scales_on_device && a.K) scales_to(chd + a.n_src, a.t_scales, n_tgt_chains);
   }
-  auto next_kind = [&](int i_next) {             // as in run_latent_loop with every step recovered
-    if (i_next >= a.n_steps) return 0;
+  if (ctx_n) {   // one context per row: the chain's condition on its cond row, uc on its uncond row; unconditional models carry none
+    auto ctx_rows = [&](const Chain& c, const float* cond, int j) {
+      const bool uncond_only = a.uc && !a.scales_on_device && c.scale == 0.0f;
+      copy_dd(e, (uncond_only ? a.uc : cond) + j * ctx_n, ctx_in + (size_t)c.row * ctx_n, ctx_n, s);
+      if (c.row2 >= 0) copy_dd(e, a.uc + j * ctx_n, ctx_in + (size_t)c.row2 * ctx_n, ctx_n, s);
+    };
+    for (int j = 0; j < a.n_src; ++j) {
+      if (a.src) ctx_rows(ch[j], a.c_src, j);
+      for (int k = 0; k < a.K; ++k) ctx_rows(ch[a.n_src + (size_t)j * a.K + k], a.c_tgt, j);
+    }
+  }
+  auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
+    if (i_next >= a.n_rec) return 0;
     return (a.n_steps - 1 - i_next) == 0 ? 2 : 1;                               // ddim.py:583-584
   };
-  LatentFan f;
+  // the noise of a step no source chain recovers: the z_in slots while they last, then `extra`
+  const int n_given = a.src ? a.n_rec : a.n_eps;
+  LatentChains f;
   f.n = n; f.chw = chw; f.n_src = a.n_src; f.K = a.K; f.chains = chd; f.x0 = a.x0; f.xin = xin;
+  f.z_stride = (long long)(a.n_rec + 1) * chw;
   {
-    LatentFan in = f;
-    in.noise0 = a.noise; in.sa = a.sa; in.s1 = a.s1;
-    in.z_out = a.z_out; in.z_stride = (long long)(a.n_steps + 1) * chw;
+    LatentChains in = f;
+    in.src = a.src;
+    in.noise0 = a.noise; in.sa = a.sa; in.s1 = a.s1; in.z_out = a.z_out;
+    in.eps_in = a.z_in; in.eps_stride = (long long)(a.n_eps + 1) * chw;                // x_T = eps_list[:, 0], SDW:153
     in.xt = xb[0]; in.xn = xb[1]; in.yt = yb[0];
-    in.next = next_kind(0);
+    in.next = a.src ? next_kind(0) : 0;
     if (in.next) { in.noise_next = a.noise + n; in.cnext = a.coef[0]; }
-    latent_fan_init(e, in, s);
+    latent_chains_init(e, in, s);
   }
-  const int iters = e.dry() ? std::min(a.n_steps, 1) : a.n_steps;
+  const int iters = e.dry() ? std::min(loop_steps, 1) : loop_steps;
+  PairStreams ps(e, tgt_net ? *tgt_net->eng : e, s);
   for (int i = 0; i < iters; ++i) {
-    unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true);
-    LatentFan st = f;
-    st.eout = eout; st.c = a.coef[i];
-    st.xt = xb[0]; st.xn = xb[1]; st.xn2 = xb[2];
-    if (a.z_out) { st.z_out = a.z_out + (size_t)(1 + i) * chw; st.z_stride = (long long)(a.n_steps + 1) * chw; }
-    st.next = next_kind(i + 1);
-    if (st.next) { st.noise_next = a.noise + (size_t)(2 + i) * n; st.cnext = a.coef[i + 1]; }
-    st.yt = yb[0]; st.y_out = (i == a.n_steps - 1) ? a.x_out : yb[1];
+    const bool src_i = a.src && i < a.n_rec;
+    if (!tgt_net) {
+      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true);
+    } else {
+      ps.fork();
+      if (src_i) unet_forward(unet, xin, tdev + (size_t)i * rows, nullptr, 0, eout, rows_src, a.h, a.w, s);
+      unet_forward(*tgt_net, xin + (size_t)rows_src * chw, tdev + (size_t)i * rows + rows_src, nullptr, 0, eout + (size_t)rows_src * chw,
+                   rows - rows_src, a.h, a.w, ps.target_stream());
+      ps.join();
+    }
+    LatentChains st = f;
+    st.src = src_i; st.eout = eout; st.c = a.coef[i];
+    if (src_i) {
+      st.xt = xb[0]; st.xn = xb[1]; st.xn2 = xb[2];
+      if (a.z_out) st.z_out = a.z_out + (size_t)(1 + i) * chw;
+      st.next = next_kind(i + 1);
+      if (st.next) { st.noise_next = a.noise + (size_t)(2 + i) * n; st.cnext = a.coef[i + 1]; }
+    } else if (i < n_given) {
+      st.eps_in = a.z_in + (size_t)(1 + i) * chw; st.eps_stride = (long long)(a.n_eps + 1) * chw;
+    } else {
+      st.eps_in = a.extra + (size_t)(i - n_given) * n; st.eps_stride = chw;
+    }
+    st.yt = yb[0]; st.y_out = (i == loop_steps - 1) ? a.x_out : yb[1];
     set_v(unet, a.t_host[i], st);
-    latent_fan_step(e, st, s);
-    float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0;
+    latent_chains_step(e, st, s);
+    if (src_i) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
     std::swap(yb[0], yb[1]);
   }
 }
@@ -677,12 +587,13 @@ int cdx_latent_encode(cdx_net* un, const float* x0, const float* c, const float*
     CDX_CHECK(un && un->owner && x0 && (c || L == 0) && coef && t_host && noise && z_out, "latent_encode: null argument");
     CDX_CHECK(n_steps >= 1 && n_rec >= 0 && n_rec <= n_steps, "latent_encode: n_steps=%d n_rec=%d", n_steps, n_rec);
     for (int i = 0; i < n_rec; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_encode: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
-    LatentLoopArgs a;
-    a.mode = LOOP_ENC;
-    a.x0 = x0; a.c_src = c; a.uc = uc; a.L = L; a.s_scale = scale;
+    const std::vector<float> scales((size_t)std::max(B, 0), scale);
+    ChainLoopArgs a;
+    a.n_src = B; a.src = true;
+    a.x0 = x0; a.c_src = c; a.uc = uc; a.L = L; a.s_scales = scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_rec; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
-    a.z_out = z_out; a.B = B; a.C = C; a.h = h; a.w = w;
-    with_arena(un->owner->e, S(stream), [&] { run_latent_loop(*un->n, a, S(stream)); });
+    a.z_out = z_out; a.C = C; a.h = h; a.w = w;
+    with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
 
@@ -692,13 +603,14 @@ int cdx_latent_decode(cdx_net* un, const float* z, int n_eps, const float* c, co
     CDX_CHECK(un && un->owner && z && (c || L == 0) && coef && t_host && x_out, "latent_decode: null argument");
     CDX_CHECK(n_steps >= 1 && n_eps >= 0, "latent_decode: n_steps=%d n_eps=%d", n_steps, n_eps);
     CDX_CHECK(n_eps >= n_steps || extra_noise != nullptr, "latent_decode: %d steps but only %d recovered noises and no extra noise", n_steps, n_eps);
-    LatentLoopArgs a;
-    a.mode = LOOP_DEC;
-    a.c_tgt = c; a.uc = uc; a.L = L; a.t_scale = scale;
+    const std::vector<float> scales((size_t)std::max(B, 0), scale);
+    ChainLoopArgs a;
+    a.n_src = B; a.K = 1;
+    a.c_tgt = c; a.uc = uc; a.L = L; a.t_scales = scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps;
     a.z_in = z; a.n_eps = n_eps; a.extra = extra_noise; a.x_out = x_out;
-    a.B = B; a.C = C; a.h = h; a.w = w;
-    with_arena(un->owner->e, S(stream), [&] { run_latent_loop(*un->n, a, S(stream)); });
+    a.C = C; a.h = h; a.w = w;
+    with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
 
@@ -709,12 +621,13 @@ int cdx_cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, const f
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
     for (int i = 0; i < n_steps; ++i) CDX_CHECK(coef[i].sigma > 0.f, "cycle_lockstep: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
-    LatentLoopArgs a;
-    a.mode = LOOP_LOCK;
-    a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scale = src_scale; a.t_scale = tgt_scale;
+    const std::vector<float> s_scales((size_t)std::max(B, 0), src_scale), t_scales((size_t)std::max(B, 0), tgt_scale);
+    ChainLoopArgs a;
+    a.n_src = B; a.K = 1; a.src = true;
+    a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scales = s_scales.data(); a.t_scales = t_scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
-    a.z_out = z_out; a.x_out = x_out; a.B = B; a.C = C; a.h = h; a.w = w;
-    with_arena(un->owner->e, S(stream), [&] { run_latent_loop(*un->n, a, S(stream)); });
+    a.z_out = z_out; a.x_out = x_out; a.C = C; a.h = h; a.w = w;
+    with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
 
@@ -723,30 +636,30 @@ int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_s
                         const float* noise, float sqrt_a_T, float sqrt_1ma_T, const float* z_in, int n_eps, const float* extra_noise,
                         float* z_out, float* x_out, int B, int C, int h, int w, void* stream) {
   return guard([&] {
-    CDX_CHECK(un && un->owner && coef && t_host && mode >= LOOP_ENC && mode <= LOOP_LOCK, "latent_loop_ens: bad arguments (mode %d)", mode);
-    const bool enc = mode & LOOP_ENC, dec = mode & LOOP_DEC;
+    CDX_CHECK(un && un->owner && coef && t_host && mode >= 1 && mode <= 3, "latent_loop_ens: bad arguments (mode %d)", mode);
+    const bool enc = mode & 1, dec = mode & 2;            // 1 encode, 2 decode, 3 both in lock-step
     CDX_CHECK(n_steps >= 1, "latent_loop_ens: n_steps=%d", n_steps);
-    LatentLoopArgs a;
-    a.mode = mode;
+    ChainLoopArgs a;
+    a.n_src = B; a.K = dec; a.src = enc; a.scales_on_device = true;
     a.uc = uc; a.L = L; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps;
-    a.B = B; a.C = C; a.h = h; a.w = w;
+    a.C = C; a.h = h; a.w = w;
     if (enc) {
       CDX_CHECK(x0 && c_src && noise && src_scales && uc, "latent_loop_ens: the encode chain needs x0, c_src, uc, noise and per-sample scales");
-      if (mode == LOOP_LOCK) n_rec = n_steps;
+      if (dec) n_rec = n_steps;
       CDX_CHECK(n_rec >= 0 && n_rec <= n_steps, "latent_loop_ens: n_rec=%d", n_rec);
       for (int i = 0; i < n_rec; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_loop_ens: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
-      CDX_CHECK(mode == LOOP_LOCK || z_out, "latent_loop_ens: encode needs z_out");
-      a.x0 = x0; a.c_src = c_src; a.s_scale_v = src_scales; a.n_rec = n_rec; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T; a.z_out = z_out;
+      CDX_CHECK(dec || z_out, "latent_loop_ens: encode needs z_out");
+      a.x0 = x0; a.c_src = c_src; a.s_scales = src_scales; a.n_rec = n_rec; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T; a.z_out = z_out;
     }
     if (dec) {
       CDX_CHECK(c_tgt && tgt_scales && uc && x_out, "latent_loop_ens: the decode chain needs c_tgt, uc, per-sample scales and x_out");
-      a.c_tgt = c_tgt; a.t_scale_v = tgt_scales; a.x_out = x_out;
+      a.c_tgt = c_tgt; a.t_scales = tgt_scales; a.x_out = x_out;
       if (!enc) {
         CDX_CHECK(z_in && n_eps >= 0 && (n_eps >= n_steps || extra_noise), "latent_loop_ens: decode needs z (%d noises for %d steps) or extra noise", n_eps, n_steps);
         a.z_in = z_in; a.n_eps = n_eps; a.extra = extra_noise;
       }
     }
-    with_arena(un->owner->e, S(stream), [&] { run_latent_loop(*un->n, a, S(stream)); });
+    with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
 
@@ -865,11 +778,11 @@ int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx
     CDX_CHECK(src->n->ucfg.context_dim == 0 && tgt->n->ucfg.context_dim == 0, "latent_cycle_pair: unconditional U-Nets only");
     CDX_CHECK(!src->n->pred && !tgt->n->pred, "latent_cycle_pair: eps-prediction U-Nets only");
     for (int i = 0; i < n_rec; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_cycle_pair: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
-    LatentLoopArgs a;
-    a.mode = LOOP_LOCK;
+    ChainLoopArgs a;
+    a.n_src = B; a.K = 1; a.src = true;
     a.x0 = x0; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_rec; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
-    a.extra = extra_noise; a.x_out = x_out; a.B = B; a.C = C; a.h = h; a.w = w;
-    with_arena(src->owner->e, S(stream), [&] { run_latent_loop(*src->n, a, S(stream), tgt->n); }, &tgt->owner->e);
+    a.extra = extra_noise; a.x_out = x_out; a.C = C; a.h = h; a.w = w;
+    with_arena(src->owner->e, S(stream), [&] { run_latent_chains(*src->n, a, S(stream), tgt->n); }, &tgt->owner->e);
   });
 }
 
@@ -883,11 +796,11 @@ int cdx_latent_cycle_fan(cdx_net* un, int n_src, int K, const float* x0, const f
               n_src, K, n_steps, L);
     CDX_CHECK(un->n->ucfg.context_dim > 0, "latent_cycle_fan: the U-Net takes no context");
     for (int i = 0; i < n_steps; ++i) CDX_CHECK(coef[i].sigma > 0.f, "latent_cycle_fan: eta must be > 0 (sigma[%d] == 0), ddim.py:268", i);
-    LatentFanArgs a;
-    a.n_src = n_src; a.K = K; a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L;
-    a.src_scales = src_scales; a.tgt_scales = tgt_scales; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps;
+    ChainLoopArgs a;
+    a.n_src = n_src; a.K = K; a.src = true; a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L;
+    a.s_scales = src_scales; a.t_scales = tgt_scales; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps;
     a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T; a.x_out = x_out; a.z_out = z_out; a.C = C; a.h = h; a.w = w;
-    with_arena(un->owner->e, S(stream), [&] { run_latent_fan(*un->n, a, S(stream)); });
+    with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
 

@@ -255,70 +255,38 @@ void ddim_compute_eps(Engine& e, const float* xt, const float* xt_next, const fl
                       const cdx_ddim_coef& c, float* out, size_t n, cudaStream_t s);
 void ddim_step_with_eps(Engine& e, const float* x, const float* e_c, const float* e_uc, float scale, const float* eps,
                         const cdx_ddim_coef& c, float* out, size_t n, cudaStream_t s);
-// One fused elementwise launch per sampling step of the latent loops (DPM-Encoder, decode, or both in lock-step): recovers the
-// noise of step i from the U-Net output (compute_eps), draws the next posterior sample of the source chain (sample_xt_next),
-// advances the target chain with the recovered noise (p_sample_ddim_with_eps) and writes the next U-Net input batch.  Op order
-// inside is that of the three single-purpose kernels above (bit-exact against the reference formulas).
-struct LatentStep {
-  size_t n = 0; int chw = 0;                 // B*chw elements
-  // --- source chain (enc != 0)
-  int enc = 0;
-  const float* x0 = nullptr; const float* xt = nullptr; const float* xn = nullptr;    // x_t and x_{t-1} (already drawn)
-  const float* es_c = nullptr; const float* es_uc = nullptr; float s_scale = 1.f;     // eps-hat under the source condition
-  const float* s_scale_v = nullptr; const float* t_scale_v = nullptr;   // optional per-sample guidance scales [B] (ensemble members batched
-                                                                        // along B); scale 1 -> eps-hat(c) and 0 -> eps-hat(uc) EXACTLY,
-                                                                        // as the reference's single-forward branches (ddim.py:550-551)
-  cdx_ddim_coef cs{};
-  float* z_out = nullptr; long long z_stride = 0;   // optional: eps -> z_out[b*z_stride + r]
-  int next = 0;                              // 0 none, 1 posterior sample x_{t-2} from (x0, xn, noise_next), 2 x_{t-2} = x0 (index 0)
-  const float* noise_next = nullptr; cdx_ddim_coef cnext{};
-  float* xn2 = nullptr;
-  // --- target chain (dec != 0)
-  int dec = 0;
-  const float* yt = nullptr; const float* et_c = nullptr; const float* et_uc = nullptr; float t_scale = 1.f;
-  cdx_ddim_coef ct{};
-  const float* eps_in = nullptr; long long eps_stride = 0;    // dec without enc: recovered noise read from z (or extra noise, stride chw)
-  float* y_out = nullptr;
-  // --- next U-Net input batch [nseg, B, chw]: segments [0, nseg_src) <- x_{t-1}, [nseg_src, nseg_src + nseg_tgt) <- y_{t-1}
-  float* xin = nullptr; int nseg_src = 0, nseg_tgt = 0;
-  // --- v-prediction (SD 2.x "-v" models): the U-Net output is v; after the guidance combine, e_t = vsa*v + vs1*x_t and
-  // pred_x0 = vsa*x_t - vs1*v with vsa = sqrt(abar_t), vs1 = sqrt(1 - abar_t) of the step's timestep (both chains share the step)
-  int pred = 0; float vsa = 0.f, vs1 = 0.f;
-};
-void latent_step(Engine& e, const LatentStep& a, cudaStream_t s);
-// x_T = sqrt(a_T) x0 + sqrt(1 - a_T) noise0 (ddim.py:477-479) -> z slot 0 (optional), x_T buffer, y_T buffer (optional), first
-// posterior sample x_{T-1} (next as in LatentStep) and the first U-Net input batch
-struct LatentInit {
-  size_t n = 0; int chw = 0;
-  const float* x0 = nullptr; const float* noise0 = nullptr; float sa = 0.f, s1 = 0.f;
-  float* z_out = nullptr; long long z_stride = 0;
-  float* xt = nullptr; float* yt = nullptr;
-  int next = 0; const float* noise_next = nullptr; cdx_ddim_coef cnext{}; float* xn = nullptr;
-  float* xin = nullptr; int nseg_src = 0, nseg_tgt = 0;
-};
-void latent_init(Engine& e, const LatentInit& a, cudaStream_t s);
-// Fan-out lock-step loop of the ensemble search: n_src source chains (one (member, sample) pair each), each driving K target chains
-// (chain j*K + k) with the noise it recovers.  A chain's U-Net rows are found through its FanChain entry instead of a fixed segment
-// layout: `row` is the cond row (the uncond row when scale == 0), `row2` the uncond row when scale is neither 0 nor 1, else -1, so
-// eps-hat is cfg_combine_v of the two and each chain computes what latent_step computes for it.
-struct FanChain { int row, row2; float scale; };
-struct LatentFan {
+// The latent sampling loops (DPM-Encoder, decode, or both in lock-step) run n_src element groups: one source chain per group (when the
+// loop has one) drives the group's K target chains (chain j*K + k) with the noise it recovers.  One fused elementwise launch per step
+// recovers the noise of step i from the U-Net output (compute_eps), draws the next posterior sample of the source chain
+// (sample_xt_next), advances every target chain with the recovered noise (p_sample_ddim_with_eps) and writes the next U-Net input
+// batch.  Op order inside is that of the three single-purpose kernels above (bit-exact against the reference formulas).
+// A chain finds its U-Net rows through its Chain entry: `row` is the cond row (the uncond row when the chain runs at scale 0 on one
+// row), `row2` the uncond row of a chain under classifier-free guidance, else -1.  eps-hat is e(row) when row2 < 0 or scale == 1,
+// e(row2) when scale == 0 -- EXACTLY, as the reference's single-forward branches (ddim.py:550-551) -- else
+// e(row2) + scale * (e(row) - e(row2)) (ddim.py:559).
+struct Chain { int row, row2; float scale; };
+struct LatentChains {
   size_t n = 0; int chw = 0, n_src = 0, K = 0;   // n = n_src*chw elements; one thread element carries its source and K targets
-  const FanChain* chains = nullptr;              // [n_src] source chains, then [n_src*K] target chains
+  const Chain* chains = nullptr;                 // [n_src] source chains, then [n_src*K] target chains
+  int src = 0;                                   // a source chain runs this step; else the recovered noise is read from eps_in
   const float* x0 = nullptr;
   const float* eout = nullptr;                   // step: U-Net output [rows, chw]
   cdx_ddim_coef c{};                             // step: coefficients of this step (both chains share the schedule)
-  const float* noise0 = nullptr; float sa = 0.f, s1 = 0.f;     // init: x_T draw and its scalars
+  const float* noise0 = nullptr; float sa = 0.f, s1 = 0.f;     // init with a source: x_T = sa*x0 + s1*noise0 (ddim.py:477-479)
   float* xt = nullptr; float* xn = nullptr;      // source x_t, x_{t-1} (init writes both, step reads them)
-  int next = 0; const float* noise_next = nullptr; cdx_ddim_coef cnext{};   // as in LatentStep
+  int next = 0;                                  // 0 none, 1 posterior sample x_{t-2} from (x0, xn, noise_next), 2 x_{t-2} = x0 (index 0)
+  const float* noise_next = nullptr; cdx_ddim_coef cnext{};
   float* xn2 = nullptr;                          // step: next x_{t-1} of the source chains
   float* z_out = nullptr; long long z_stride = 0;     // optional: x_T (init) / recovered noise (step) -> z_out[j*z_stride + r]
+  const float* eps_in = nullptr; long long eps_stride = 0;    // no source: x_T (init) / the step's noise <- eps_in[j*eps_stride + r]
   float* yt = nullptr; float* y_out = nullptr;   // target chains [n_src*K, chw]: init writes yt = x_T; step reads yt, writes y_out
   float* xin = nullptr;                          // next U-Net input [rows, chw]
-  int pred = 0; float vsa = 0.f, vs1 = 0.f;      // step: v-prediction, as in LatentStep
+  // v-prediction (SD 2.x "-v" models): the U-Net output is v; after the guidance combine, e_t = vsa*v + vs1*x_t and
+  // pred_x0 = vsa*x_t - vs1*v with vsa = sqrt(abar_t), vs1 = sqrt(1 - abar_t) of the step's timestep (both chains share the step)
+  int pred = 0; float vsa = 0.f, vs1 = 0.f;
 };
-void latent_fan_init(Engine& e, const LatentFan& a, cudaStream_t s);
-void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s);
+void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s);
+void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s);
 // Running per-sample best of the ensemble search over candidates that arrive in chunks, in any order: candidate c of the chunk
 // (image images[c], score scores[c], reference candidate index cand[c], sample sample[c]) replaces the best of its sample when it
 // wins under torch.argmax's rule over the [B, n_total] score matrix (larger score; NaN beats any number; ties and NaNs: lower

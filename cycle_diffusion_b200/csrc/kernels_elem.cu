@@ -196,15 +196,6 @@ __device__ __forceinline__ float cfg_combine(const float* e_c, const float* e_uc
   return ADD(eu, MUL(scale, SUB(ec, eu)));      // e_t_uncond + s * (e_t - e_t_uncond), ddim.py:559
 }
 
-// per-sample scale (ensemble batching): members whose scale is 1 or 0 take the reference's single-forward value bit for bit
-__device__ __forceinline__ float cfg_combine_v(const float* e_c, const float* e_uc, float scale, size_t i) {
-  const float ec = e_c[i];
-  if (e_uc == nullptr || scale == 1.0f) return ec;
-  const float eu = e_uc[i];
-  if (scale == 0.0f) return eu;
-  return ADD(eu, MUL(scale, SUB(ec, eu)));
-}
-
 __global__ void ddim_posterior_kernel(const float* __restrict__ x0, const float* __restrict__ xt, const float* __restrict__ nz,
                                       cdx_ddim_coef c, float* __restrict__ out, size_t n) {
   GRID_STRIDE(i, n) {
@@ -254,108 +245,70 @@ __device__ __forceinline__ void eps_x0(float o, float x, const cdx_ddim_coef& c,
   }
 }
 
-template <int PRED>
-__global__ void latent_step_kernel(const LatentStep a) {
-  const size_t seg = a.n;
-  GRID_STRIDE(i, a.n) {
-    const size_t b = i / a.chw, r = i - b * a.chw;
-    float eps = 0.f;
-    if (a.enc) {
-      const float o = a.s_scale_v ? cfg_combine_v(a.es_c, a.es_uc, a.s_scale_v[b], i) : cfg_combine(a.es_c, a.es_uc, a.s_scale, i);
-      const float xt = a.xt[i], xn = a.xn[i];
-      float e_t, pred_x0;
-      eps_x0<PRED>(o, xt, a.cs, a.vsa, a.vs1, e_t, pred_x0);                                    // ddim.py:576
-      const float dir = MUL(a.cs.dir_coef, e_t);                                                // :578
-      eps = DIV(DIV(SUB(SUB(xn, MUL(a.cs.sqrt_aprev, pred_x0)), dir), a.cs.sigma), 1.0f);       // :579 (temperature 1)
-      if (a.z_out) a.z_out[b * a.z_stride + r] = eps;
-      if (a.next == 1) a.xn2[i] = ddim_posterior_f(a.x0[i], xn, a.noise_next[i], a.cnext);
-      else if (a.next == 2) a.xn2[i] = a.x0[i];                                                 // ddim.py:583-584
-      for (int sg = 0; sg < a.nseg_src; ++sg) a.xin[sg * seg + i] = xn;
-    } else if (a.dec) {
-      eps = a.eps_in[b * a.eps_stride + r];
-    }
-    if (a.dec) {
-      const float o = a.t_scale_v ? cfg_combine_v(a.et_c, a.et_uc, a.t_scale_v[b], i) : cfg_combine(a.et_c, a.et_uc, a.t_scale, i);
-      const float y = a.yt[i];
-      float e_t, pred_x0;
-      eps_x0<PRED>(o, y, a.ct, a.vsa, a.vs1, e_t, pred_x0);                                     // ddim.py:634
-      const float dir = MUL(a.ct.dir_coef, e_t);                                                // :638
-      const float noise = MUL(MUL(a.ct.sigma, eps), 1.0f);                                      // :642
-      const float yn = ADD(ADD(MUL(a.ct.sqrt_aprev, pred_x0), dir), noise);                     // :645
-      a.y_out[i] = yn;
-      for (int sg = 0; sg < a.nseg_tgt; ++sg) a.xin[(a.nseg_src + sg) * seg + i] = yn;
-    }
-  }
-}
-
-__global__ void latent_init_kernel(const LatentInit a) {
-  const size_t seg = a.n;
-  GRID_STRIDE(i, a.n) {
-    const size_t b = i / a.chw, r = i - b * a.chw;
-    const float x0 = a.x0[i];
-    const float xT = ADD(MUL(a.sa, x0), MUL(a.s1, a.noise0[i]));                                // ddim.py:477-479
-    if (a.z_out) a.z_out[b * a.z_stride + r] = xT;
-    a.xt[i] = xT;
-    if (a.yt) a.yt[i] = xT;
-    if (a.next == 1) a.xn[i] = ddim_posterior_f(x0, xT, a.noise_next[i], a.cnext);
-    else if (a.next == 2) a.xn[i] = x0;
-    for (int sg = 0; sg < a.nseg_src + a.nseg_tgt; ++sg) a.xin[sg * seg + i] = xT;
-  }
-}
-
-// eps-hat of one fan chain: cfg_combine_v with the chain's own rows (a chain at scale 0 or 1 has one row, which is then the uncond or
-// the cond row, and cfg_combine_v returns that row's output unchanged)
-__device__ __forceinline__ float fan_eps_hat(const float* eout, const FanChain& ch, size_t r, int chw) {
+// eps-hat of one chain from its own U-Net rows.  A chain on one row takes that row's output unchanged; a chain on two rows at scale
+// 1 or 0 takes its cond or uncond row unchanged (the reference's single-forward value bit for bit), else ddim.py:559.
+__device__ __forceinline__ float chain_eps_hat(const float* eout, const Chain& ch, size_t r, int chw) {
   const float ec = __ldcg(eout + (size_t)ch.row * chw + r);
-  if (ch.row2 < 0) return ec;
+  if (ch.row2 < 0 || ch.scale == 1.0f) return ec;
   const float eu = __ldcg(eout + (size_t)ch.row2 * chw + r);
+  if (ch.scale == 0.0f) return eu;
   return ADD(eu, MUL(ch.scale, SUB(ec, eu)));                  // ddim.py:559
 }
-__device__ __forceinline__ void fan_put(float* xin, const FanChain& ch, size_t r, int chw, float v) {
+__device__ __forceinline__ void chain_put(float* xin, const Chain& ch, size_t r, int chw, float v) {
   xin[(size_t)ch.row * chw + r] = v;
   if (ch.row2 >= 0) xin[(size_t)ch.row2 * chw + r] = v;
 }
-// x_T of every source chain (ddim.py:477-479), shared by its K target chains, and the first U-Net input.  Every input was written by
-// the copies and launches just before, so all loads take the coherent path.
-__global__ void latent_fan_init_kernel(const LatentFan a) {
+// x_T of every element group, shared by its source chain and its K target chains, and the first U-Net input: drawn from x0
+// (ddim.py:477-479) when the loop has a source chain, else slot 0 of the recovered noises (SDW:153).  Every input was written by the
+// copies and launches just before, so all loads take the coherent path.
+__global__ void latent_chains_init_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
-    const float x0 = __ldcg(a.x0 + i);
-    const float xT = ADD(MUL(a.sa, x0), MUL(a.s1, __ldcg(a.noise0 + i)));                      // ddim.py:477-479
-    if (a.z_out) a.z_out[j * a.z_stride + r] = xT;
-    a.xt[i] = xT;
-    if (a.next == 1) a.xn[i] = ddim_posterior_f(x0, xT, __ldcg(a.noise_next + i), a.cnext);
-    else if (a.next == 2) a.xn[i] = x0;
-    fan_put(a.xin, a.chains[j], r, a.chw, xT);
+    float xT;
+    if (a.src) {
+      const float x0 = __ldcg(a.x0 + i);
+      xT = ADD(MUL(a.sa, x0), MUL(a.s1, __ldcg(a.noise0 + i)));                                // ddim.py:477-479
+      if (a.z_out) a.z_out[j * a.z_stride + r] = xT;
+      a.xt[i] = xT;
+      if (a.next == 1) a.xn[i] = ddim_posterior_f(x0, xT, __ldcg(a.noise_next + i), a.cnext);
+      else if (a.next == 2) a.xn[i] = x0;
+      chain_put(a.xin, a.chains[j], r, a.chw, xT);
+    } else {
+      xT = __ldcg(a.eps_in + j * a.eps_stride + r);
+    }
     for (int k = 0; k < a.K; ++k) {
       const size_t t = j * a.K + k;
       a.yt[t * a.chw + r] = xT;
-      fan_put(a.xin, a.chains[a.n_src + t], r, a.chw, xT);
+      chain_put(a.xin, a.chains[a.n_src + t], r, a.chw, xT);
     }
   }
 }
-// One step of the fan-out loop: latent_step_kernel's source half once per source chain, its target half once per target chain with
-// the recovered noise held in a register; same op order and intrinsics.  Under v-prediction each target chain forms e_t and pred_x0
-// from its own x_t and v.
+// One step of the loop: the source half once per source chain, the target half once per target chain with the recovered noise held
+// in a register.  Under v-prediction each target chain forms e_t and pred_x0 from its own x_t and v.
 template <int PRED>
-__global__ void latent_fan_step_kernel(const LatentFan a) {
+__global__ void latent_chains_step_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
-    const FanChain src = a.chains[j];
-    const float o = fan_eps_hat(a.eout, src, r, a.chw);
-    const float xt = __ldcg(a.xt + i), xn = __ldcg(a.xn + i);
-    float e_t, pred_x0;
-    eps_x0<PRED>(o, xt, a.c, a.vsa, a.vs1, e_t, pred_x0);                                       // ddim.py:576
-    const float dir = MUL(a.c.dir_coef, e_t);                                                    // :578
-    const float eps = DIV(DIV(SUB(SUB(xn, MUL(a.c.sqrt_aprev, pred_x0)), dir), a.c.sigma), 1.0f);     // :579 (temperature 1)
-    if (a.z_out) a.z_out[j * a.z_stride + r] = eps;
-    if (a.next == 1) a.xn2[i] = ddim_posterior_f(__ldcg(a.x0 + i), xn, __ldcg(a.noise_next + i), a.cnext);
-    else if (a.next == 2) a.xn2[i] = __ldcg(a.x0 + i);                                          // ddim.py:583-584
-    fan_put(a.xin, src, r, a.chw, xn);
+    float eps;
+    if (a.src) {
+      const Chain src = a.chains[j];
+      const float o = chain_eps_hat(a.eout, src, r, a.chw);
+      const float xt = __ldcg(a.xt + i), xn = __ldcg(a.xn + i);
+      float e_t, pred_x0;
+      eps_x0<PRED>(o, xt, a.c, a.vsa, a.vs1, e_t, pred_x0);                                     // ddim.py:576
+      const float dir = MUL(a.c.dir_coef, e_t);                                                  // :578
+      eps = DIV(DIV(SUB(SUB(xn, MUL(a.c.sqrt_aprev, pred_x0)), dir), a.c.sigma), 1.0f);         // :579 (temperature 1)
+      if (a.z_out) a.z_out[j * a.z_stride + r] = eps;
+      if (a.next == 1) a.xn2[i] = ddim_posterior_f(__ldcg(a.x0 + i), xn, __ldcg(a.noise_next + i), a.cnext);
+      else if (a.next == 2) a.xn2[i] = __ldcg(a.x0 + i);                                        // ddim.py:583-584
+      chain_put(a.xin, src, r, a.chw, xn);
+    } else {
+      eps = __ldcg(a.eps_in + j * a.eps_stride + r);
+    }
     for (int k = 0; k < a.K; ++k) {
       const size_t t = j * a.K + k, ti = t * a.chw + r;
-      const FanChain tc = a.chains[a.n_src + t];
-      const float ot = fan_eps_hat(a.eout, tc, r, a.chw);
+      const Chain tc = a.chains[a.n_src + t];
+      const float ot = chain_eps_hat(a.eout, tc, r, a.chw);
       const float y = __ldcg(a.yt + ti);
       float et, px0;
       eps_x0<PRED>(ot, y, a.c, a.vsa, a.vs1, et, px0);                                          // ddim.py:634
@@ -363,7 +316,7 @@ __global__ void latent_fan_step_kernel(const LatentFan a) {
       const float noise = MUL(MUL(a.c.sigma, eps), 1.0f);                                       // :642
       const float yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                         // :645
       a.y_out[ti] = yn;
-      fan_put(a.xin, tc, r, a.chw, yn);
+      chain_put(a.xin, tc, r, a.chw, yn);
     }
   }
 }
@@ -657,15 +610,10 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
   }
 }
 
-void latent_step(Engine& e, const LatentStep& a, cudaStream_t s) {
-  if (a.pred) LAUNCH1(latent_step_kernel<1>, a.n, a);
-  else LAUNCH1(latent_step_kernel<0>, a.n, a);
-}
-void latent_init(Engine& e, const LatentInit& a, cudaStream_t s) { LAUNCH1(latent_init_kernel, a.n, a); }
-void latent_fan_init(Engine& e, const LatentFan& a, cudaStream_t s) { LAUNCH1(latent_fan_init_kernel, a.n, a); }
-void latent_fan_step(Engine& e, const LatentFan& a, cudaStream_t s) {
-  if (a.pred) LAUNCH1(latent_fan_step_kernel<1>, a.n, a);
-  else LAUNCH1(latent_fan_step_kernel<0>, a.n, a);
+void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s) { LAUNCH1(latent_chains_init_kernel, a.n, a); }
+void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
+  if (a.pred) LAUNCH1(latent_chains_step_kernel<1>, a.n, a);
+  else LAUNCH1(latent_chains_step_kernel<0>, a.n, a);
 }
 void ensemble_select(Engine& e, int n, const float* scores, const long long* cand, const int* sample, const float* images, float* best_score,
                      long long* best_idx, float* best_img, float* score_mat, int B, int n_total, size_t img_n, cudaStream_t s) {

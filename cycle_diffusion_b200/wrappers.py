@@ -118,6 +118,17 @@ def _load_sd(state_dict, ckpt_default, synth_params, seed):
     return sd['state_dict'] if 'state_dict' in sd else sd       # txt2img.py:27-32 / DW:378-379
 
 
+def encode_noise(sched, n_rec, shape):
+    """Draws of _ddpm_ddim_encoding in order: x_T (ddim.py:479), then one per step except index==0 (ddim.py:583-584, 599: the last
+    step returns x0 without a draw)."""
+    noise = torch.zeros((n_rec + 1,) + tuple(shape))
+    noise[0] = torch.randn(shape)
+    for i in range(n_rec):
+        if sched.refine_steps - 1 - i != 0:
+            noise[1 + i] = torch.randn(shape)
+    return noise
+
+
 class _LatentGenerator:
     """What the text wrappers call ``self.generator`` (LatentDiffusion): U-Net + first stage + cond stage."""
 
@@ -142,6 +153,13 @@ class _LatentGenerator:
             B, C2, h, w = moments.shape
             noise = torch.randn(B, C2 // 2, h, w)
         return self.engine.vae_posterior(moments, noise, self.scale_factor)
+
+    def encode_image(self, image, resolution):
+        """image [B,3,R,R] in [0,1] -> x0: (image - 0.5) * 2.0, then the first stage and its encoding (whose posterior draw comes
+        before any noise of the sampling loop)."""
+        image = self.engine.shift_scale(image, -0.5, 2.0)
+        assert image.shape[2] == image.shape[3] == resolution
+        return self.get_first_stage_encoding(self.encode_first_stage(image))
 
     def decode_first_stage(self, z):
         return self.vae.decode(self.engine.affine(z, 1. / self.scale_factor, 0.0))     # ddpm.py:705
@@ -232,13 +250,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         return c, uc
 
     def _encode_noise(self, sched, n_rec, shape):
-        """Draws of _ddpm_ddim_encoding in order: x_T (ddim.py:479), then one per step except index==0 (ddim.py:583-584, 599)."""
-        noise = torch.zeros((n_rec + 1,) + tuple(shape))
-        noise[0] = torch.randn(shape)
-        for i in range(n_rec):
-            if sched.refine_steps - 1 - i != 0:
-                noise[1 + i] = torch.randn(shape)
-        return noise
+        return encode_noise(sched, n_rec, shape)
 
     def _chunks(self, members, bsz):
         per = max(1, (self.ensemble_batch or 1) // max(1, bsz))
@@ -335,10 +347,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
             return self._encode(image, encode_text)
 
     def _encode(self, image, encode_text):
-        g, e = self.generator, self.engine
-        image = e.shift_scale(image, -0.5, 2.0)                                   # (image - 0.5) * 2.0
-        assert image.shape[2] == image.shape[3] == self.resolution
-        x0 = g.get_first_stage_encoding(g.encode_first_stage(image))
+        g = self.generator
+        x0 = g.encode_image(image, self.resolution)
         bsz = image.shape[0]
         if self.ensemble_batch and self.n_trials * len(self.encoder_unconditional_guidance_scales) * len(self.skip_steps) > 1:
             return self._encode_batched(x0, encode_text)
@@ -376,10 +386,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
 
     def _cycle(self, image, encode_text, decode_text):
         g, e = self.generator, self.engine
-        x = e.shift_scale(image, -0.5, 2.0)
-        assert x.shape[2] == x.shape[3] == self.resolution
-        x0 = g.get_first_stage_encoding(g.encode_first_stage(x))
-        bsz = x.shape[0]
+        x0 = g.encode_image(image, self.resolution)
+        bsz = image.shape[0]
         c_src, uc = self._get_condition(encode_text, bsz)
         c_tgt, _ = self._get_condition(decode_text, bsz)
         assert self.eta > 0
@@ -444,10 +452,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         assert self.lockstep_ensemble(), 'cycle_ensemble(): needs an ensemble with every step recovered, eta > 0 and a ranker'
         g, e, rank = self.generator, self.engine, self.directional_clip
         with self._precision_scope():
-            x = e.shift_scale(image, -0.5, 2.0)
-            assert x.shape[2] == x.shape[3] == self.resolution
-            x0 = g.get_first_stage_encoding(g.encode_first_stage(x))
-            bsz = x.shape[0]
+            x0 = g.encode_image(image, self.resolution)
+            bsz = image.shape[0]
             c_src, uc = self._get_condition(encode_text, bsz)
             c_tgt, _ = self._get_condition(decode_text, bsz)
         plan, scheds = self.ensemble_plan(bsz)
@@ -592,24 +598,14 @@ class LatentDiffStochasticWrapper(torch.nn.Module):
             sample = g.unet.latent_refine(sample, None, None, 1.0, self.custom_steps, self.refine_steps, noise, g.alphas_cumprod)
         return g.decode_first_stage(sample)
 
-    def _encode_noise(self, sched, n_rec, shape):
-        noise = torch.zeros((n_rec + 1,) + tuple(shape))
-        noise[0] = torch.randn(shape)
-        for i in range(n_rec):
-            if sched.refine_steps - 1 - i != 0:                        # ddim.py:583-584: the last step returns x0 without a draw
-                noise[1 + i] = torch.randn(shape)
-        return noise
-
     def encode(self, image, class_label=None):
-        g, e = self.generator, self.engine
+        g = self.generator
         bsz = image.shape[0]
-        image = e.shift_scale(image, -0.5, 2.0)
-        assert image.shape[2] == image.shape[3] == self.resolution
-        x0 = g.get_first_stage_encoding(g.encode_first_stage(image))
+        x0 = g.encode_image(image, self.resolution)
         assert self.eta > 0
         sched = self._sched()
         n_rec = max(0, min(sched.refine_steps, self.white_box_steps - 1))
-        noise = self._encode_noise(sched, n_rec, x0.shape)
+        noise = encode_noise(sched, n_rec, x0.shape)
         z = g.unet.latent_encode(x0, None, None, 1.0, sched, n_rec, noise).view(bsz, -1)
         assert z.shape[1] == self.latent_dim
         return z
@@ -619,15 +615,13 @@ class LatentDiffStochasticWrapper(torch.nn.Module):
         loop (cdx_latent_cycle_pair): the source chain runs under this wrapper's U-Net, the target chain under the target's, and
         the noise recovered at a step is consumed by the target chain at once, so ``z`` is never written.  Same random draws in
         the same order, same result bit for bit.  Then the target's own refine pass and first-stage decode."""
-        g, e = self.generator, self.engine
-        image = e.shift_scale(image, -0.5, 2.0)
-        assert image.shape[2] == image.shape[3] == self.resolution
-        x0 = g.get_first_stage_encoding(g.encode_first_stage(image))
+        g = self.generator
+        x0 = g.encode_image(image, self.resolution)
         assert self.eta > 0
         sched = self._sched()
         n_rec = max(0, min(sched.refine_steps, self.white_box_steps - 1))
         assert n_rec + 1 == self.white_box_steps, 'white_box_steps - 1 > custom_steps (encode() would fail the latent_dim check)'
-        noise = self._encode_noise(sched, n_rec, x0.shape)
+        noise = encode_noise(sched, n_rec, x0.shape)
         n_extra = sched.refine_steps - n_rec
         extra = torch.stack([torch.randn(x0.shape) for _ in range(n_extra)]) if n_extra > 0 else None      # ddim.py:640
         sample = g.unet.latent_cycle_pair(target.generator.unet, x0, sched, n_rec, noise, extra)

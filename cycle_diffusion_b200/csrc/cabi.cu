@@ -891,7 +891,8 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
     with_arena(e, s, [&] {
       Scope sc(e.arena);
       bool done = false;
-      if (e.mma_mode == 1 && e.flash_attn && e.tc_kind >= 1 && (Nq % 128) == 0 && (C % 8) == 0 && (d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) {
+      const bool fused = flash_eligible(e, Nq, Nk, d, C);
+      if (fused && e.tc_kind >= 1) {
         // the SpatialTransformer's fp16-split path on loose q / k / v: ranges measured here, keys padded to a multiple of 8 per image
         e.pools_reset(s);
         const int Nks = (Nk + 7) & ~7, M = B * Nq, Mk = B * Nks;
@@ -921,7 +922,7 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
         split_rows_h16(e, q, M, C, C, qh, ql, C, qa, s);
         split_rows_h16(e, kp, Mk, C, C, kh, kl, C, ka, s);
         split_transpose_h16(e, vp, Mk, C, C, vh, vl, va, s);
-        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, heads, d, scale, s);
+        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s);
       }
       if (!done && e.mma_mode == 1 && Nq == Nk && (Nq % 32) == 0 && Nq >= 128 && (d % 4) == 0) {
         // same operand preparation as the SpatialTransformer: q|k side by side, V transposed, TF32 planes
@@ -933,19 +934,19 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
           CDX_CUDA(cudaMemcpy2DAsync(qk + C, (size_t)2 * C * 4, k, (size_t)C * 4, (size_t)C * 4, M, cudaMemcpyDeviceToDevice, s));
         }
         nhwc_to_nchw(e, v, vt, 1, C, M, s);
-        if (e.flash_attn && (Nq % 128) == 0) {
+        if (fused) {
           float* qh = (float*)e.arena.alloc((size_t)M * 2 * C * sizeof(float));
           float* ql = (float*)e.arena.alloc((size_t)M * 2 * C * sizeof(float));
           float* vh = (float*)e.arena.alloc((size_t)C * M * sizeof(float));
           float* vl = (float*)e.arena.alloc((size_t)C * M * sizeof(float));
           split_planes(e, qk, qh, ql, (size_t)M * 2 * C, s);
           split_planes(e, vt, vh, vl, (size_t)C * M, s);
-          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, heads, d, scale, s);
+          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s);
         }
         if (!done) done = attention_tc(e, qk, 2 * C, qk + C, 2 * C, d, vt, out, C, B, Nq, Nk, heads, d, scale, s);
       }
-      if (!done && e.mma_mode == 1 && e.flash_attn && Nq != Nk && (Nq % 128) == 0) {
-        // cross-attention shape: keys padded to a multiple of 4 per image (TMA strides), masked inside the kernel
+      if (!done && fused) {
+        // cross-attention shape, or a key count off the TMA granule: keys padded to a multiple of 4 per image, masked inside the kernel
         const int Nks = (Nk + 3) & ~3, M = B * Nq, Mk = B * Nks;
         float* kp = (float*)e.arena.alloc((size_t)Mk * C * sizeof(float));
         float* vp = (float*)e.arena.alloc((size_t)Mk * C * sizeof(float));
@@ -966,7 +967,7 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
         split_planes(e, q, qh, ql, (size_t)M * C, s);
         split_planes(e, kp, kh, kl, (size_t)Mk * C, s);
         split_planes(e, vt, vh, vl, (size_t)C * Mk, s);
-        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, heads, d, scale, s);
+        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s);
       }
       if (!done) attention(e, q, C, k, C, v, C, out, C, B, Nq, Nk, heads, d, d, scale, s);
     });

@@ -175,18 +175,22 @@ struct GemmArgs {
 void gemm(Engine& e, const GemmArgs& a, cudaStream_t s);
 // wgmma back end (kernels_tc.cu); returns false when the shape is not eligible
 bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done = nullptr);   // side_done bit 0: c_amax fused, bit 1: c_stats fused
+// fused attention (kernels_attn.cu): true when the engine's mode runs N queries over Nk keys at head width d (C channels) fused
+bool flash_eligible(const Engine& e, int N, int Nk, int d, int C);
 bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
-                        const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int heads, int d,
+                        const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d,
                         float scale, cudaStream_t s);
 // fp16-split operands (the default scheme): planes made by split_rows_h16 / split_transpose_h16 from fp32 q | k and v with the
 // tensors' tracked ranges (device slots); halves the tensor-pipe time and the operand bytes of the TF32-plane version.
 // q_lo, k_lo and vt_lo all null: one-term products on the hi planes (mode 5); the split functions then write hi only.
 bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
                          const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
-                         int Nk, int Nks, int heads, int d, float scale, cudaStream_t s);
+                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s);
 void split_rows_h16(Engine& e, const float* src, long long rows, int cols, long long ld, void* hi, void* lo, long long ldh, const float* amax,
                     cudaStream_t s);
-void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long ld, void* hi, void* lo, const float* amax, cudaStream_t s);
+// R rows = `images` images of R / images rows each; Rp > 0: each image's columns padded with zeros to a stride of Rp (V^T key stride)
+void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long ld, void* hi, void* lo, const float* amax, cudaStream_t s,
+                         int images = 1, int Rp = 0);
 void split_planes(Engine& e, const float* w, float* hi, float* lo, size_t n, cudaStream_t s);   // hi = rn_tf32(w), lo = rn_tf32(w - hi)
 // fp16 split of w * 2^exp: hi = fp16(w'), lo = fp16(w' - hi)  (hi / lo: __half arrays)
 void split_planes_h16(Engine& e, const float* w, void* hi, void* lo, size_t n, int exp, cudaStream_t s);

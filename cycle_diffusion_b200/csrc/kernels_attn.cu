@@ -18,6 +18,10 @@
 //                   of the next wgmma; F16: fp16(p * 2^10)) -> O_j = P_j V_j (m64nNV, V^T tiles from smem) written fresh per block ->
 //                   O_total = O_total * corr + O_j with round-to-nearest fp32 adds (the tensor core's accumulation truncates, see
 //                   kernels_tc.cu; accumulating per block in registers also makes the online-softmax rescale free).  Final O / l -> global.
+// Any token count: ceil(N / 128) query tiles (TMA zero-fills Q rows >= N; RAG instantiations, chosen on the host by N % 128, store no
+// row >= N) and keys >= Nk in the last block masked.  d = 160 (fp16 variants): 64 queries per CTA, the two consumer warpgroups take
+// alternate key blocks and merge their softmax states at the end (KSPLIT), and O_j is formed in two n80 halves (PVH) so that O_total,
+// O_j, S and the P fragments fit the 232-register budget; see ACfg.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -30,6 +34,8 @@ using namespace tc;
 constexpr int AQ = 128;        // queries per CTA
 constexpr int AKV = 64;        // keys per block
 constexpr int ATHREADS = 384;
+// queries per CTA: d = 160 takes 64 (its two Q planes are 48 KB per 64 rows; at 128 the K / V ring would be one stage deep)
+constexpr int flash_qrows(int d) { return d > 80 ? 64 : AQ; }
 
 // F16: operands are fp16 hi / lo planes (x * 2^e split as in kernels_tc.cu's KIND_H16) and the three product terms run as
 // wgmma .f16 (K = 16 per instruction): half the tensor-pipe time and half the operand bytes of the TF32 planes.  P is split as
@@ -37,9 +43,15 @@ constexpr int ATHREADS = 384;
 // ONE (F16 only): hi planes alone, one product term; P rounded once as fp16(p * 2^10) (the scale keeps small probabilities out of
 // the subnormals).  The stages are half the size, so the ring is as deep as shared memory allows (up to 4; the three-term
 // variants keep depth 2).
+// d = 160 (fp16 only): QROWS = 64 queries shared by both consumer warpgroups, which walk alternate key blocks with their own online
+// softmax state (KSPLIT) and merge it through shared memory at the end; P.V as two m64n80 halves (PVH = 2), each added into O_total
+// before the next, so a thread holds O_total (80) + one half of O_j (40) + S (32) + the P fragments (32) instead of 80 + 80 + 64.
 template <int D, bool F16, bool ONE = false>
 struct ACfg {
   static_assert(!ONE || F16, "the one-term variant is fp16 only");
+  static constexpr int QROWS = flash_qrows(D);
+  static constexpr bool KSPLIT = QROWS < AQ;
+  static constexpr int PVH = D > 80 ? 2 : 1;
   static constexpr int NPL = ONE ? 1 : 2;                   // operand planes per tensor (hi, or hi + lo)
   static constexpr int KD = F16 ? (D + 15) / 16 * 16 : D;    // head dim as the QK products see it (F16: zero-padded to K = 16 steps by the TMA fill)
   static constexpr int KW = F16 ? 64 : 32;                  // elements per 128-byte k-block row
@@ -50,7 +62,7 @@ struct ACfg {
   static constexpr int K_STAGE = NPL * KB2 * KTILE;         // hi (+ lo)
   static constexpr int VTILE = NV * 128;                    // one 128-byte block of V^T (32 keys; F16: 64 keys): NV rows x 128 B
   static constexpr int V_STAGE = (F16 ? 1 : 2) * NPL * VTILE; // (key sub-blocks) x (hi (+ lo))
-  static constexpr int Q_PLANE = KB2 * AQ * 128;            // one plane of Q
+  static constexpr int Q_PLANE = KB2 * QROWS * 128;         // one plane of Q
   // ring depth: the deepest up to RING_MAX that fits (TF32 at d = 80 has room for one K and one V stage only)
   static constexpr int RING_MAX = ONE ? 4 : 2;
   static constexpr int RING_FIT = (232448 - 2048 - NPL * Q_PLANE) / (K_STAGE + V_STAGE);
@@ -61,10 +73,13 @@ struct ACfg {
   static constexpr int OFF_V = OFF_K + KS * K_STAGE;
   static constexpr int OFF_BAR = OFF_V + VS * V_STAGE;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;   // 1 KB slack: the tiles are placed at the next 1024-byte boundary
-  static_assert(D % 8 == 0 && D >= 16 && D <= 80, "head dim must be a multiple of 8 in [16, 80]");
+  static_assert(D % 8 == 0 && D >= 16 && (D <= 80 || (F16 && D == 160)), "head dim must be a multiple of 8 in [16, 80], or 160 (fp16)");
   static_assert(SMEM_BYTES <= 232448, "smem overflow");
   static_assert(8 + 32 * RING <= 256, "barrier area");
-  static_assert(NV % 16 == 0, "NV");
+  static_assert(NV % 16 == 0 && (NV / PVH) % 16 == 0, "NV");
+  // key split: each warpgroup owns the stages of its key-block parity (an even ring); the merge reuses the K / V rings
+  static_assert(!KSPLIT || (RING >= 2 && RING % 2 == 0), "key-split ring");
+  static_assert(!KSPLIT || (NV / 2 + 4) * 128 * 4 <= KS * K_STAGE + VS * V_STAGE, "merge buffer");
 };
 
 struct AttnParams {
@@ -88,13 +103,14 @@ __device__ __forceinline__ void split_h16_pair(float x0, float x1, uint32_t& hi,
   lo = *reinterpret_cast<const uint32_t*>(&ll);
 }
 
-template <int D, bool F16, bool ONE>
+template <int D, bool F16, bool ONE, bool RAG>
 __global__ void __launch_bounds__(ATHREADS, 1)
 flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_constant__ CUtensorMap mapQl,
                   const __grid_constant__ CUtensorMap mapKh, const __grid_constant__ CUtensorMap mapKl,
                   const __grid_constant__ CUtensorMap mapVh, const __grid_constant__ CUtensorMap mapVl, const AttnParams p) {
   using C = ACfg<D, F16, ONE>;
-  constexpr int KB2 = C::KB2, NV = C::NV, KW = C::KW, KS = C::KS, VS = C::VS;
+  constexpr int KB2 = C::KB2, NV = C::NV, KW = C::KW, KS = C::KS, VS = C::VS, QR = C::QROWS;
+  constexpr bool KSPLIT = C::KSPLIT;
   constexpr int NO = NV / 2;                       // O accumulators per thread (m64nNV)
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -107,13 +123,13 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   auto bar_v_empty = [&](int s) { return bars + 8u + 8u * (2 * KS + VS + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * AQ, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * QR, h = blockIdx.y, b = blockIdx.z;
   const int nb = (p.Nk + AKV - 1) / AKV;
 
   if (threadIdx.x == 0) {
     mbar_init(bar_q_full, 1);
-    for (int s = 0; s < KS; ++s) { mbar_init(bar_k_full(s), 1); mbar_init(bar_k_empty(s), 8); }
-    for (int s = 0; s < VS; ++s) { mbar_init(bar_v_full(s), 1); mbar_init(bar_v_empty(s), 8); }
+    for (int s = 0; s < KS; ++s) { mbar_init(bar_k_full(s), 1); mbar_init(bar_k_empty(s), KSPLIT ? 4 : 8); }
+    for (int s = 0; s < VS; ++s) { mbar_init(bar_v_full(s), 1); mbar_init(bar_v_empty(s), KSPLIT ? 4 : 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -126,8 +142,8 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
       const uint32_t sq = base + C::OFF_Q;
       mbar_expect_tx(bar_q_full, C::NPL * C::Q_PLANE);
       for (int kb = 0; kb < KB2; ++kb) {
-        tma_load_4d(sq + kb * AQ * 128, &mapQh, kb * KW, h, q0, b, bar_q_full);
-        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * AQ * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
+        tma_load_4d(sq + kb * QR * 128, &mapQh, kb * KW, h, q0, b, bar_q_full);
+        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * QR * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
       }
       for (int j = 0; j < nb; ++j) {
         // K block j: [64 keys x d] hi + lo
@@ -160,7 +176,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
 
   // ============================================================================= consumer warpgroups
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  const int wg = (warp >> 2) - 1;                  // rows [64 wg, 64 wg + 64) of the CTA's queries
+  const int wg = (warp >> 2) - 1;                  // rows [64 wg, 64 wg + 64) of the CTA's queries (KSPLIT: key blocks j = wg mod 2)
   const int wi = warp & 3, g = lane >> 2, qd = lane & 3;
   // F16: the planes carry 2^eq q, 2^ek k, 2^ev v -> scores rescaled by the exact 2^-(eq+ek), output by 2^-ev; P is handed to the
   // tensor core as p * 2^10 (folded into the exponent; the row sum carries the same factor, so O / l is unchanged)
@@ -174,11 +190,11 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   float o[NO], ob[NO], sc[32];
 #pragma unroll
   for (int c = 0; c < NO; ++c) o[c] = 0.f;
-  const uint32_t qh_base = base + C::OFF_Q + (uint32_t)wg * 64u * 128u, ql_base = qh_base + C::Q_PLANE;
+  const uint32_t qh_base = base + C::OFF_Q + (KSPLIT ? 0u : (uint32_t)wg * 64u * 128u), ql_base = qh_base + C::Q_PLANE;
   mbar_wait(bar_q_full, 0);
 
 #pragma unroll 1
-  for (int j = 0; j < nb; ++j) {
+  for (int j = KSPLIT ? wg : 0; j < nb; j += KSPLIT ? 2 : 1) {
     // ---- S = Q K_j^T
     const int ks = j % KS;
     mbar_wait(bar_k_full(ks), (j / KS) & 1);
@@ -191,7 +207,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     for (int c = 0; c < C::NG; ++c) {
       const int kb = c >> 2;
       const uint64_t adv = (uint64_t)((c & 3) * 2);
-      const uint64_t q_hi = make_desc(qh_base + kb * AQ * 128) + adv, q_lo = make_desc(ql_base + kb * AQ * 128) + adv;
+      const uint64_t q_hi = make_desc(qh_base + kb * QR * 128) + adv, q_lo = make_desc(ql_base + kb * QR * 128) + adv;
       const uint64_t k_hi = make_desc(sk + kb * C::KTILE) + adv, k_lo = make_desc(sk + (KB2 + kb) * C::KTILE) + adv;
       if (ONE) {
         Wgmma<64>::f16_ss(sc, q_hi, k_hi);
@@ -245,75 +261,149 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     const int vs = j % VS;
     mbar_wait(bar_v_full(vs), (j / VS) & 1);
     const uint32_t sv = base + C::OFF_V + vs * C::V_STAGE;
-#pragma unroll
-    for (int c = 0; c < NO; ++c) ob[c] = 0.f;
-    if (ONE) {
-      uint32_t ph[4][4];
+    if constexpr (C::PVH == 2) {
+      // channels [0, NV/2) then [NV/2, NV): rows NV/2.. of the V^T tile start on a 1024-byte swizzle atom
+      constexpr int NH = NV / 2, NOH = NO / 2;
+      uint32_t ph[4][4], pl[4][4];
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
           const int e = (2 * kk + (r >> 1)) * 4 + (r & 1) * 2;
-          const __half2 hh = __floats2half2_rn(sc[e], sc[e + 1]);
-          ph[kk][r] = *reinterpret_cast<const uint32_t*>(&hh);
+          if (ONE) {
+            const __half2 hh = __floats2half2_rn(sc[e], sc[e + 1]);
+            ph[kk][r] = *reinterpret_cast<const uint32_t*>(&hh);
+          } else {
+            split_h16_pair(sc[e], sc[e + 1], ph[kk][r], pl[kk][r]);
+          }
         }
-      wgmma_pin(ob);
-      wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) Wgmma<NV>::f16_rs(ob, ph[kk], make_desc(sv) + (uint64_t)(kk * 2));
-    } else if (F16) {
-      uint32_t ph[4][4], pl[4][4];
+      for (int hv = 0; hv < 2; ++hv) {
+        float oh[NOH];
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)               // keys 16 kk .. 16 kk + 15: accumulator groups 2 kk, 2 kk + 1
+        for (int c = 0; c < NOH; ++c) oh[c] = 0.f;
+        wgmma_pin(oh);
+        wgmma_fence();
+        const uint32_t svh = sv + hv * NH * 128;
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int e = (2 * kk + (r >> 1)) * 4 + (r & 1) * 2;
-          split_h16_pair(sc[e], sc[e + 1], ph[kk][r], pl[kk][r]);
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t adv = (uint64_t)(kk * 2);
+          const uint64_t v_hi = make_desc(svh) + adv;
+          if (ONE) {
+            Wgmma<NH>::f16_rs(oh, ph[kk], v_hi);
+          } else {
+            const uint64_t v_lo = make_desc(svh + C::VTILE) + adv;
+            Wgmma<NH>::f16_rs(oh, pl[kk], v_hi);
+            Wgmma<NH>::f16_rs(oh, ph[kk], v_lo);
+            Wgmma<NH>::f16_rs(oh, ph[kk], v_hi);
+          }
         }
-      wgmma_pin(ob);
-      wgmma_fence();
+        wgmma_commit();
+        wgmma_wait0();
+        wgmma_pin(oh);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const uint64_t adv = (uint64_t)(kk * 2);
-        const uint64_t v_hi = make_desc(sv) + adv, v_lo = make_desc(sv + C::VTILE) + adv;
-        Wgmma<NV>::f16_rs(ob, pl[kk], v_hi);
-        Wgmma<NV>::f16_rs(ob, ph[kk], v_lo);
-        Wgmma<NV>::f16_rs(ob, ph[kk], v_hi);
+        for (int c = 0; c < NOH; ++c) o[hv * NOH + c] = o[hv * NOH + c] * corr[(c >> 1) & 1] + oh[c];
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_v_empty(vs));
     } else {
-      // TF32 A fragment of keys 8 kk .. 8 kk + 7: (row, key qd) and (row, key qd + 4); this thread holds keys 2 qd, 2 qd + 1
-      uint32_t ph[8][4], pl[8][4];
-      const int src1 = (lane & ~3) | (qd >> 1), src2 = src1 + 2;
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk)
+      for (int c = 0; c < NO; ++c) ob[c] = 0.f;
+      if (ONE) {
+        uint32_t ph[4][4];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float a0 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2], src1), a1 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2 + 1], src1);
-          const float b0 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2], src2), b1 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2 + 1], src2);
-          const float xa = (qd & 1) ? a1 : a0, xb = (qd & 1) ? b1 : b0;
-          ph[kk][i] = rn_tf32(__float_as_uint(xa));
-          pl[kk][i] = __float_as_uint(xa - __uint_as_float(ph[kk][i]));   // lo left to the tensor core's own truncation
-          ph[kk][2 + i] = rn_tf32(__float_as_uint(xb));
-          pl[kk][2 + i] = __float_as_uint(xb - __uint_as_float(ph[kk][2 + i]));
+        for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int e = (2 * kk + (r >> 1)) * 4 + (r & 1) * 2;
+            const __half2 hh = __floats2half2_rn(sc[e], sc[e + 1]);
+            ph[kk][r] = *reinterpret_cast<const uint32_t*>(&hh);
+          }
+        wgmma_pin(ob);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) Wgmma<NV>::f16_rs(ob, ph[kk], make_desc(sv) + (uint64_t)(kk * 2));
+      } else if (F16) {
+        uint32_t ph[4][4], pl[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)               // keys 16 kk .. 16 kk + 15: accumulator groups 2 kk, 2 kk + 1
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int e = (2 * kk + (r >> 1)) * 4 + (r & 1) * 2;
+            split_h16_pair(sc[e], sc[e + 1], ph[kk][r], pl[kk][r]);
+          }
+        wgmma_pin(ob);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t adv = (uint64_t)(kk * 2);
+          const uint64_t v_hi = make_desc(sv) + adv, v_lo = make_desc(sv + C::VTILE) + adv;
+          Wgmma<NV>::f16_rs(ob, pl[kk], v_hi);
+          Wgmma<NV>::f16_rs(ob, ph[kk], v_lo);
+          Wgmma<NV>::f16_rs(ob, ph[kk], v_hi);
         }
-      wgmma_pin(ob);
-      wgmma_fence();
+      } else {
+        // TF32 A fragment of keys 8 kk .. 8 kk + 7: (row, key qd) and (row, key qd + 4); this thread holds keys 2 qd, 2 qd + 1
+        uint32_t ph[8][4], pl[8][4];
+        const int src1 = (lane & ~3) | (qd >> 1), src2 = src1 + 2;
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        const uint64_t adv = (uint64_t)((kk & 3) * 2);
-        const uint64_t v_hi = make_desc(sv + (kk >> 2) * C::VTILE) + adv, v_lo = make_desc(sv + (2 + (kk >> 2)) * C::VTILE) + adv;
-        Wgmma<NV>::tf32_rs(ob, pl[kk], v_hi);
-        Wgmma<NV>::tf32_rs(ob, ph[kk], v_lo);
-        Wgmma<NV>::tf32_rs(ob, ph[kk], v_hi);
+        for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const float a0 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2], src1), a1 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2 + 1], src1);
+            const float b0 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2], src2), b1 = __shfl_sync(0xffffffffu, sc[kk * 4 + i * 2 + 1], src2);
+            const float xa = (qd & 1) ? a1 : a0, xb = (qd & 1) ? b1 : b0;
+            ph[kk][i] = rn_tf32(__float_as_uint(xa));
+            pl[kk][i] = __float_as_uint(xa - __uint_as_float(ph[kk][i]));   // lo left to the tensor core's own truncation
+            ph[kk][2 + i] = rn_tf32(__float_as_uint(xb));
+            pl[kk][2 + i] = __float_as_uint(xb - __uint_as_float(ph[kk][2 + i]));
+          }
+        wgmma_pin(ob);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const uint64_t adv = (uint64_t)((kk & 3) * 2);
+          const uint64_t v_hi = make_desc(sv + (kk >> 2) * C::VTILE) + adv, v_lo = make_desc(sv + (2 + (kk >> 2)) * C::VTILE) + adv;
+          Wgmma<NV>::tf32_rs(ob, pl[kk], v_hi);
+          Wgmma<NV>::tf32_rs(ob, ph[kk], v_lo);
+          Wgmma<NV>::tf32_rs(ob, ph[kk], v_hi);
+        }
       }
-    }
-    wgmma_commit();
-    wgmma_wait0();
-    wgmma_pin(ob);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_v_empty(vs));
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_pin(ob);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_v_empty(vs));
 #pragma unroll
-    for (int c = 0; c < NO; ++c) o[c] = o[c] * corr[(c >> 1) & 1] + ob[c];
+      for (int c = 0; c < NO; ++c) o[c] = o[c] * corr[(c >> 1) & 1] + ob[c];
+    }
+  }
+
+  if constexpr (KSPLIT) {
+    // warpgroup 1 hands (m, l, O) of its key blocks to warpgroup 0.  Once both have left the loop every K / V stage has been
+    // consumed, so the rings hold the exchange.  O = O_0 2^(m_0 - m) + O_1 2^(m_1 - m): the online-softmax rescale, fp32 adds
+    float* xch = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + C::OFF_K);
+    const int tl = threadIdx.x & 127;
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (wg == 1) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) { xch[i * 128 + tl] = m_run[i]; xch[(2 + i) * 128 + tl] = l_run[i]; }
+#pragma unroll
+      for (int c = 0; c < NO; ++c) xch[(4 + c) * 128 + tl] = o[c];
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (wg == 1) return;
+    float c0[2], c1[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float m1 = xch[i * 128 + tl], l1 = xch[(2 + i) * 128 + tl];
+      const float m = fmaxf(m_run[i], m1);                 // finite: block 0 (warpgroup 0's) holds key 0
+      c0[i] = ex2_approx(m_run[i] - m);
+      c1[i] = ex2_approx(m1 - m);                          // 0 when warpgroup 1 had no key block (m1 = -inf)
+      l_run[i] = l_run[i] * c0[i] + l1 * c1[i];
+    }
+#pragma unroll
+    for (int c = 0; c < NO; ++c) o[c] = o[c] * c0[(c >> 1) & 1] + xch[(4 + c) * 128 + tl] * c1[(c >> 1) & 1];
   }
 
   // total row sums over the quad, fixed order: every thread of the row gets the same sum
@@ -322,7 +412,8 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     const float l0 = __shfl_sync(0xffffffffu, l_run[i], lane & ~3), l1 = __shfl_sync(0xffffffffu, l_run[i], (lane & ~3) | 1);
     const float l2 = __shfl_sync(0xffffffffu, l_run[i], (lane & ~3) | 2), l3 = __shfl_sync(0xffffffffu, l_run[i], (lane & ~3) | 3);
     const float inv_l = oscale / (((l0 + l1) + l2) + l3);
-    const int row = wg * 64 + wi * 16 + g + 8 * i;
+    const int row = (KSPLIT ? 0 : wg * 64) + wi * 16 + g + 8 * i;
+    if (RAG && q0 + row >= p.N) continue;          // ragged last query tile: rows >= N belong to the next image
     float* dst = p.out + ((long long)b * p.N + q0 + row) * p.ldo + h * p.d;
 #pragma unroll
     for (int j8 = 0; j8 < NV / 8; ++j8) {
@@ -332,18 +423,27 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   }
 }
 
-template <int D, bool F16, bool ONE = false>
-void launch_flash(const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMap& kh, const CUtensorMap& kl, const CUtensorMap& vh,
-                  const CUtensorMap& vl, const AttnParams& p, cudaStream_t s) {
+template <int D, bool F16, bool ONE, bool RAG>
+void launch_flash_k(const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMap& kh, const CUtensorMap& kl, const CUtensorMap& vh,
+                    const CUtensorMap& vl, const AttnParams& p, cudaStream_t s) {
+  using C = ACfg<D, F16, ONE>;
   static bool attr[64] = {};          // per device (cudaFuncSetAttribute is device state); engines are single-threaded per device
   int dev = 0;
   CDX_CUDA(cudaGetDevice(&dev));
   if (!attr[dev & 63]) {
-    CDX_CUDA(cudaFuncSetAttribute(flash_attn_kernel<D, F16, ONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, ACfg<D, F16, ONE>::SMEM_BYTES));
+    CDX_CUDA(cudaFuncSetAttribute(flash_attn_kernel<D, F16, ONE, RAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr[dev & 63] = true;
   }
-  launch_ex(flash_attn_kernel<D, F16, ONE>, dim3(p.N / AQ, p.heads, p.B), dim3(ATHREADS), ACfg<D, F16, ONE>::SMEM_BYTES, s, 1, qh, ql, kh, kl, vh,
-            vl, p);
+  launch_ex(flash_attn_kernel<D, F16, ONE, RAG>, dim3((p.N + C::QROWS - 1) / C::QROWS, p.heads, p.B), dim3(ATHREADS), C::SMEM_BYTES, s, 1, qh, ql,
+            kh, kl, vh, vl, p);
+}
+
+// N a multiple of the query tile: the instantiation without the row guard
+template <int D, bool F16, bool ONE = false>
+void launch_flash(const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMap& kh, const CUtensorMap& kl, const CUtensorMap& vh,
+                  const CUtensorMap& vl, const AttnParams& p, cudaStream_t s) {
+  if (p.N % ACfg<D, F16, ONE>::QROWS) launch_flash_k<D, F16, ONE, true>(qh, ql, kh, kl, vh, vl, p, s);
+  else launch_flash_k<D, F16, ONE, false>(qh, ql, kh, kl, vh, vl, p, s);
 }
 
 // x * 2^e -> fp16 hi / lo planes, e = h16_exp_of(*amax) (the exponent the attention kernel derives from the same slot).
@@ -376,9 +476,10 @@ __global__ void split_rows_h16_kernel(const float* src, long long rows, int cols
 }
 
 // the same split, transposed: src [R, ld] columns 0..C-1 -> hi / lo [C, R] (V^T: both P.V operands K-major for wgmma).
-// 64 (rows) x 32 (columns) tiles through shared memory; R % 2 == 0
+// Per image (blockIdx.z of gridDim.z): its Ri source rows -> output columns [z Rp, z Rp + Rp), columns Ri..Rp-1 zero (a key stride
+// padded to the TMA granule).  64 (rows) x 32 (columns) tiles through shared memory; Rp % 2 == 0
 template <bool LO>
-__global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* src, int R, int Cc, long long ld, __half* hi,
+__global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* src, int Ri, int Rp, int Cc, long long ld, __half* hi,
                                                                    __half* lo, const float* amax) {
   __shared__ float tile[64][33];
   pdl_trigger();
@@ -386,22 +487,25 @@ __global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* s
   const float sc = exp2i(h16_exp_of(*amax));
   const int r0 = blockIdx.x * 64, c0 = blockIdx.y * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;      // 32 x 8
+  const long long R = (long long)gridDim.z * Rp;               // output row length
+  src += (long long)blockIdx.z * Ri * ld;
+  const long long o0 = (long long)blockIdx.z * Rp;
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const int r = r0 + ty + 8 * k, c = c0 + tx;
-    tile[ty + 8 * k][tx] = (r < R && c < Cc) ? src[(long long)r * ld + c] * sc : 0.f;
+    tile[ty + 8 * k][tx] = (r < Ri && c < Cc) ? src[(long long)r * ld + c] * sc : 0.f;
   }
   __syncthreads();
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const int c = c0 + ty + 8 * k, r = r0 + 2 * tx;            // one warp: 64 consecutive rows of one output row = 128 B
-    if (c < Cc && r < R) {
+    if (c < Cc && r < Rp) {
       const float x0 = tile[2 * tx][ty + 8 * k], x1 = tile[2 * tx + 1][ty + 8 * k];
       const __half2 h = __floats2half2_rn(x0, x1);
-      *reinterpret_cast<__half2*>(hi + (long long)c * R + r) = h;
+      *reinterpret_cast<__half2*>(hi + (long long)c * R + o0 + r) = h;
       if (LO) {
         const float2 f = __half22float2(h);
-        *reinterpret_cast<__half2*>(lo + (long long)c * R + r) = __floats2half2_rn(x0 - f.x, x1 - f.y);
+        *reinterpret_cast<__half2*>(lo + (long long)c * R + o0 + r) = __floats2half2_rn(x0 - f.x, x1 - f.y);
       }
     }
   }
@@ -410,12 +514,23 @@ __global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* s
 }  // namespace
 
 // q_hi / q_lo: TF32 planes of the query projection [B*N, ldq] (head h at column h*d); k_hi / k_lo: planes of the key
-// projection [B*Nks, ldk] (Nks = stored keys per image >= Nk); vt_hi / vt_lo: planes of V^T [heads*d, B*Nks].
+// projection [B*Nks, ldk] (Nks = stored keys per image >= Nk); vt_hi / vt_lo: planes of V^T [heads*d, B*Nvs] (Nvs % 4 == 0).
 // out [B, N, ldo], head h at column h*d.  Self-attention: q and k are two column ranges of one fused projection.
+// The fused kernels' shape rule, in one place: every caller routes by it.  Any N >= 1 queries and Nk >= 1 keys (callers lay K and V^T
+// out at a per-image key stride padded to 8 (fp16) / 4 (TF32) keys); head widths with an instantiation: 16, 32, 40, 64, 80, and 160
+// for the fp16 planes (tc_kind >= 1; mma mode 3's TF32 planes at d = 160 keep the unfused route).  Mode 0 (FFMA) and mode 2 (unfused
+// attention) never take it.
+bool flash_eligible(const Engine& e, int N, int Nk, int d, int C) {
+  if (e.mma_mode != 1 || !e.flash_attn || N < 1 || Nk < 1) return false;
+  const bool h16 = e.tc_kind >= 1;
+  if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || (h16 && d == 160))) return false;
+  return C % (h16 ? 8 : 4) == 0;
+}
+
 bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
-                        const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int heads, int d,
+                        const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d,
                         float scale, cudaStream_t s) {
-  if ((N % AQ) || (d % 8) || d < 16 || d > 80 || (ldq & 3) || (ldk & 3) || (ldo & 3) || (Nks & 3) || Nk < 1 || Nk > Nks) return false;
+  if (N < 1 || (d % 8) || d < 16 || d > 80 || (ldq & 3) || (ldk & 3) || (ldo & 3) || (Nvs & 3) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
   if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) return false;
   if (!a16(q_hi) || !a16(q_lo) || !a16(k_hi) || !a16(k_lo) || !a16(vt_hi) || !a16(vt_lo) || !a16(out)) return false;
   if (e.dry()) return true;
@@ -424,9 +539,9 @@ bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq
   uint64_t sq[3] = {(uint64_t)d * 4, (uint64_t)ldq * 4, (uint64_t)N * ldq * 4};
   uint64_t dk[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)Nks, (uint64_t)B};
   uint64_t sk[3] = {(uint64_t)d * 4, (uint64_t)ldk * 4, (uint64_t)Nks * ldk * 4};
-  uint32_t bq[4] = {32, 1, AQ, 1}, bk[4] = {32, 1, AKV, 1};
-  uint64_t dv[4] = {(uint64_t)Nks, (uint64_t)B, (uint64_t)heads * d, 1};
-  uint64_t sv[3] = {(uint64_t)Nks * 4, (uint64_t)B * Nks * 4, (uint64_t)B * Nks * 4 * heads * d};
+  uint32_t bq[4] = {32, 1, (uint32_t)flash_qrows(d), 1}, bk[4] = {32, 1, AKV, 1};
+  uint64_t dv[4] = {(uint64_t)Nvs, (uint64_t)B, (uint64_t)heads * d, 1};
+  uint64_t sv[3] = {(uint64_t)Nvs * 4, (uint64_t)B * Nvs * 4, (uint64_t)B * Nvs * 4 * heads * d};
   uint32_t bv[4] = {32, 1, (uint32_t)NV, 1};
   const CUtensorMap& qh = get_map(q_hi, 4, dq, sq, bq);
   const CUtensorMap& ql = get_map(q_lo, 4, dq, sq, bq);
@@ -466,23 +581,28 @@ void split_rows_h16(Engine& e, const float* src, long long rows, int cols, long 
   e.launches++;
 }
 
-void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long ld, void* hi, void* lo, const float* amax, cudaStream_t s) {
-  CDX_CHECK((R & 1) == 0 && a16(hi) && (!lo || a16(lo)), "split_transpose_h16: even row count");
+void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long ld, void* hi, void* lo, const float* amax, cudaStream_t s, int images,
+                         int Rp) {
+  CDX_CHECK(images >= 1 && R % images == 0, "split_transpose_h16: rows not a whole number of images");
+  int Ri = R / images;
+  if (Rp <= 0 || Rp == Ri) { Rp = Ri = R; images = 1; }      // no padding: one image of all R rows
+  CDX_CHECK((Rp & 1) == 0 && Rp >= Ri && a16(hi) && (!lo || a16(lo)), "split_transpose_h16: even row count");
   if (e.dry()) return;
-  launch_ex(lo ? split_transpose_h16_kernel<true> : split_transpose_h16_kernel<false>, dim3((unsigned)((R + 63) / 64), (unsigned)((Cc + 31) / 32)),
-            dim3(256), 0, s, 1, src, R, Cc, ld, (__half*)hi, (__half*)lo, amax);
+  launch_ex(lo ? split_transpose_h16_kernel<true> : split_transpose_h16_kernel<false>,
+            dim3((unsigned)((Rp + 63) / 64), (unsigned)((Cc + 31) / 32), (unsigned)images), dim3(256), 0, s, 1, src, Ri, Rp, Cc, ld, (__half*)hi,
+            (__half*)lo, amax);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
 }
 
-// fp16-split variant: q / k planes [rows, ld] halves (head h at column h*d), V^T planes [heads*d, B*Nks] halves, each tensor's
-// planes scaled by 2^h16_exp_of(*amax) of its slot (split_rows_h16 / split_transpose_h16 above).  ld and Nks multiples of 8.
-// All three lo planes null: the one-term kernel (hi * hi products only, mma mode 5).
+// fp16-split variant: q / k planes [rows, ld] halves (head h at column h*d; Nks key rows per image), V^T planes [heads*d, B*Nvs] halves
+// (Nvs keys per image, the padding columns zero), each tensor's planes scaled by 2^h16_exp_of(*amax) of its slot (split_rows_h16 /
+// split_transpose_h16 above).  ld and Nvs multiples of 8.  All three lo planes null: the one-term kernel (hi * hi products only, mma mode 5).
 bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
                          const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
-                         int Nk, int Nks, int heads, int d, float scale, cudaStream_t s) {
-  if ((N % AQ) || (ldq & 7) || (ldk & 7) || (ldo & 3) || (Nks & 7) || Nk < 1 || Nk > Nks) return false;
-  if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) return false;
+                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s) {
+  if (N < 1 || (ldq & 7) || (ldk & 7) || (ldo & 3) || (Nvs & 7) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
+  if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || d == 160)) return false;
   const bool one = q_lo == nullptr;
   if (one ? (k_lo || vt_lo) : (!k_lo || !vt_lo)) return false;
   if (!a16(q_hi) || !a16(k_hi) || !a16(vt_hi) || !a16(out)) return false;
@@ -493,9 +613,9 @@ bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq,
   uint64_t sq[3] = {(uint64_t)d * 2, (uint64_t)ldq * 2, (uint64_t)N * ldq * 2};
   uint64_t dk[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)Nks, (uint64_t)B};
   uint64_t sk[3] = {(uint64_t)d * 2, (uint64_t)ldk * 2, (uint64_t)Nks * ldk * 2};
-  uint32_t bq[4] = {64, 1, AQ, 1}, bk[4] = {64, 1, AKV, 1};
-  uint64_t dv[4] = {(uint64_t)Nks, (uint64_t)B, (uint64_t)heads * d, 1};
-  uint64_t sv[3] = {(uint64_t)Nks * 2, (uint64_t)B * Nks * 2, (uint64_t)B * Nks * 2 * heads * d};
+  uint32_t bq[4] = {64, 1, (uint32_t)flash_qrows(d), 1}, bk[4] = {64, 1, AKV, 1};
+  uint64_t dv[4] = {(uint64_t)Nvs, (uint64_t)B, (uint64_t)heads * d, 1};
+  uint64_t sv[3] = {(uint64_t)Nvs * 2, (uint64_t)B * Nvs * 2, (uint64_t)B * Nvs * 2 * heads * d};
   uint32_t bv[4] = {64, 1, (uint32_t)NV, 1};
   const CUtensorMap& qh = get_map(q_hi, 4, dq, sq, bq, nullptr, 2);
   const CUtensorMap& kh = get_map(k_hi, 4, dk, sk, bk, nullptr, 2);
@@ -518,6 +638,7 @@ bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq,
       case 40: launch_flash<40, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
       case 64: launch_flash<64, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
       case 80: launch_flash<80, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+      case 160: launch_flash<160, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
       default: return false;
     }
     CDX_CUDA(cudaGetLastError());
@@ -530,6 +651,7 @@ bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq,
     case 40: launch_flash<40, true>(qh, ql, kh, kl, vh, vl, p, s); break;
     case 64: launch_flash<64, true>(qh, ql, kh, kl, vh, vl, p, s); break;
     case 80: launch_flash<80, true>(qh, ql, kh, kl, vh, vl, p, s); break;
+    case 160: launch_flash<160, true>(qh, ql, kh, kl, vh, vl, p, s); break;
     default: return false;
   }
   CDX_CUDA(cudaGetLastError());

@@ -820,25 +820,50 @@ struct UNetExec : Exec {
       Tensor a = alloc(B, x.H, x.W, C);
       a.amax = e.amax_slot();                   // <- max |V| (written by whichever projection produces V)
       bool done = false;
-      const bool flash_ok = e.mma_mode == 1 && e.flash_attn && (HW % 128) == 0 && (d == 16 || d == 32 || d == 40 || d == 64 || d == 80);
-      if (flash_ok && e.tc_kind >= 1 && (C % 8) == 0) {
+      const bool flash_ok = flash_eligible(e, HW, HW, d, C);
+      if (flash_ok && e.tc_kind >= 1) {
         // fp16-split fused attention: ONE plain fp32 q|k|v projection (its range tracked by the epilogue), then one pass that
-        // writes the fp16 hi / lo planes of q|k and of V^T (both P.V operands K-major for wgmma) with the tensor's exponent
+        // writes the fp16 hi / lo planes of q|k and of V^T (both P.V operands K-major for wgmma) with the tensor's exponent.
+        // V^T keeps Nvs = HW rounded up to 8 keys per image (zero columns): its TMA map needs 16-byte key strides
         Scope sa(e.arena);
         float* qkv = (float*)e.arena.alloc((size_t)M * 3 * C * sizeof(float));
         linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_q.weight"), 3 * C, nullptr, nullptr, 0, qkv, 3 * C, nullptr, n1.amax, nullptr,
                     a.amax);                    // range of q | k | v (v bounds the attention output: a convex combination of V rows)
         // (mode 5: hi planes only, one-term kernel)
         const bool lo = !e.attn_one;
+        const int Nvs = (HW + 7) & ~7;
         void* qk_hi = e.arena.alloc((size_t)M * 2 * C * 2);
         void* qk_lo = lo ? e.arena.alloc((size_t)M * 2 * C * 2) : nullptr;
-        void* vt_hi = e.arena.alloc((size_t)C * M * 2);
-        void* vt_lo = lo ? e.arena.alloc((size_t)C * M * 2) : nullptr;
+        void* vt_hi = e.arena.alloc((size_t)C * B * Nvs * 2);
+        void* vt_lo = lo ? e.arena.alloc((size_t)C * B * Nvs * 2) : nullptr;
         split_rows_h16(e, qkv, M, 2 * C, 3 * C, qk_hi, qk_lo, 2 * C, a.amax, s);
-        split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s);
+        split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s, B, Nvs);
         done = flash_attention_h16(e, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr, 2 * C,
-                                   vt_hi, vt_lo, a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, heads, d, scale, s);
+                                   vt_hi, vt_lo, a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s);
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
+      } else if (flash_ok && (HW % 4) != 0) {
+        // TF32 planes with a per-image key count off the 16-byte TMA granule: V row-major, copied into rows padded to Nvs keys
+        // per image (zero rows), transposed and split; q|k planes from the projection's epilogue as below
+        Scope sa(e.arena);
+        const int Nvs = (HW + 3) & ~3;
+        const size_t nqk = (size_t)M * 2 * C, nvt = (size_t)C * B * Nvs;
+        float* qk_hi = (float*)e.arena.alloc(nqk * sizeof(float));
+        float* qk_lo = (float*)e.arena.alloc(nqk * sizeof(float));
+        float* vr = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+        float* vp = (float*)e.arena.alloc(nvt * sizeof(float));
+        float* vt = (float*)e.arena.alloc(nvt * sizeof(float));
+        float* vt_hi = (float*)e.arena.alloc(nvt * sizeof(float));
+        float* vt_lo = (float*)e.arena.alloc(nvt * sizeof(float));
+        linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_q.weight"), 2 * C, nullptr, nullptr, 0, qk_hi, 2 * C, qk_lo, n1.amax);
+        linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_v.weight"), C, nullptr, nullptr, 0, vr, C, nullptr, n1.amax, nullptr, a.amax);
+        if (!e.dry()) {
+          CDX_CUDA(cudaMemsetAsync(vp, 0, nvt * sizeof(float), s));
+          CDX_CUDA(cudaMemcpy2DAsync(vp, (size_t)Nvs * C * 4, vr, (size_t)HW * C * 4, (size_t)HW * C * 4, B, cudaMemcpyDeviceToDevice, s));
+        }
+        nhwc_to_nchw(e, vp, vt, 1, C, B * Nvs, s);
+        split_planes(e, vt, vt_hi, vt_lo, nvt, s);
+        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s);
+        CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands
         // are K-major for wgmma) are written by their GEMM epilogues directly as TF32 hi / lo planes
@@ -867,7 +892,7 @@ struct UNetExec : Exec {
           linear_into(n.P(t + ".attn1.to_v.weight"), C, C, nullptr, 0, 0, C, n1.p, M, nullptr, nullptr, 0, vt_hi, M, vt_lo, nullptr, nullptr,
                       a.amax);   // V^T = Wv . X^T
         }
-        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, heads, d, scale, s);
+        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (e.mma_mode >= 1 && (HW % 32) == 0 && HW >= 128 && (d % 4) == 0) {
         // unfused tensor-core attention (mode 2, or shapes the fused kernel does not cover)
@@ -904,7 +929,8 @@ struct UNetExec : Exec {
       a.amax = kv_amax();                       // <- max |V| of the context projection (lives with the cached K / V in loop mode)
       bool done = false;
       Tensor q;
-      if (ctx_pad && e.tc_kind >= 1 && (C % 8) == 0 && (HW % 128) == 0 && (d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) {
+      const bool flash_ok = ctx_pad && flash_eligible(e, HW, ctx_len, d, C);
+      if (flash_ok && e.tc_kind >= 1) {
         // fp16-split fused attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the kernel):
         // q projected as plain fp32 (range tracked), K | V from one fused projection of the context; fp16 planes by the split pass.
         // K and V share the layer's slot (one exponent for both); in loop mode planes and slot are computed by the first call only.
@@ -929,10 +955,10 @@ struct UNetExec : Exec {
           split_rows_h16(e, kvf, Mk, C, 2 * C, k_hi, k_lo, C, a.amax, s);
           split_transpose_h16(e, kvf + C, Mk, C, 2 * C, vt_hi, vt_lo, a.amax, s);
         }
-        done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, vt_hi, vt_lo, qf.amax, a.amax, a.amax, a.p, C, B, HW, ctx_len, ctx_lp, heads, d,
-                                   scale, s);
+        done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, vt_hi, vt_lo, qf.amax, a.amax, a.amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads,
+                                   d, scale, s);
         CDX_CHECK(done, "flash cross-attention (fp16-split) rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
-      } else if (ctx_pad && (HW % 128) == 0 && (d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) {
+      } else if (flash_ok) {
         // fused tensor-core attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the
         // kernel): q = n2.Wq^T, K = ctx.Wk^T, V^T = Wv.ctx^T (swapped-role GEMM), all written as TF32 planes
         Scope sa(e.arena);
@@ -950,7 +976,7 @@ struct UNetExec : Exec {
           linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctx_pad, Mk, nullptr, nullptr, 0, vt_hi, Mk, vt_lo, nullptr, nullptr,
                       a.amax);
         }
-        done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, vt_hi, vt_lo, a.p, C, B, HW, ctx_len, ctx_lp, heads, d, scale, s);
+        done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, vt_hi, vt_lo, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s);
         CDX_CHECK(done, "flash cross-attention rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
       }
       if (!done) q = linear(n2, t + ".attn2.to_q", false);

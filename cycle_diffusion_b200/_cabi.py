@@ -96,6 +96,10 @@ SIGNATURES = {
                                _P]),
     'cdx_cycle_lockstep': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I, _I, _I,
                                 _P]),
+    'cdx_cycle_lockstep_masked': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I, _I,
+                                       _I, _P, _P]),
+    'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_latent_loop_ens': (_I, [_P, _I, _P, _P, _P, _P, _I, _P, _P, C.POINTER(DdimCoef), C.POINTER(_F), _I, _I, _P, _F, _F, _P, _I, _P, _P, _P,
                                  _I, _I, _I, _I, _P]),
     'cdx_clip_preprocess': (_I, [_P, _P, _I, _I, _I, _P, _P]),
@@ -109,6 +113,8 @@ SIGNATURES = {
     'cdx_latent_cycle_pair': (_I, [_P, _P, _P, C.POINTER(DdimCoef), C.POINTER(_F), _I, _I, _P, _F, _F, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_latent_cycle_fan': (_I, [_P, _I, _I, _P, _P, _P, _P, _I, C.POINTER(_F), C.POINTER(_F), C.POINTER(DdimCoef), C.POINTER(_F), _I, _P,
                                   _F, _F, _P, _P, _I, _I, _I, _P]),
+    'cdx_latent_cycle_fan_masked': (_I, [_P, _I, _I, _P, _P, _P, _P, _I, C.POINTER(_F), C.POINTER(_F), C.POINTER(DdimCoef), C.POINTER(_F), _I,
+                                         _P, _F, _F, _P, _P, _I, _I, _I, _P, _P]),
     'cdx_ensemble_select': (_I, [_P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_op_conv3x3': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     'cdx_op_linear': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),

@@ -162,6 +162,7 @@ struct ChainLoopArgs {
   const float* z_in = nullptr; int n_eps = 0;       // no src: [n_src, n_eps+1, chw], x_T then the recovered noises
   const float* extra = nullptr;                     // noise of the steps past n_eps (no src) / past n_rec (src)
   float* x_out = nullptr;                           // K > 0: [n_src*K, chw]
+  const float* mask = nullptr;                      // optional [n_src, 1, h, w]: masked editing (LatentChains::mask)
   int C = 0, h = 0, w = 0;
 };
 
@@ -203,6 +204,8 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   place(ch.data() + a.n_src, n_tgt_chains, a.t_scales);
   const int loop_steps = a.K ? a.n_steps : a.n_rec;
   CDX_CHECK(!tgt_net || (!unet.pred && !tgt_net->pred), "two-model latent loop: eps-prediction U-Nets only");
+  // a masked target chain takes its source chain's x_{t-1} outside the mask, so every step needs one
+  CDX_CHECK(!a.mask || (a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net), "masked latent loop: needs a source chain at every step");
   check_v_steps(unet, a.t_host, loop_steps);
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
@@ -243,7 +246,7 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   // the noise of a step no source chain recovers: the z_in slots while they last, then `extra`
   const int n_given = a.src ? a.n_rec : a.n_eps;
   LatentChains f;
-  f.n = n; f.chw = chw; f.n_src = a.n_src; f.K = a.K; f.chains = chd; f.x0 = a.x0; f.xin = xin;
+  f.n = n; f.chw = chw; f.n_src = a.n_src; f.K = a.K; f.chains = chd; f.x0 = a.x0; f.xin = xin; f.mask = a.mask; f.hw = a.h * a.w;
   f.z_stride = (long long)(a.n_rec + 1) * chw;
   {
     LatentChains in = f;
@@ -617,6 +620,14 @@ int cdx_latent_decode(cdx_net* un, const float* z, int n_eps, const float* c, co
 int cdx_cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
                        float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                        float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream) {
+  return cdx_cycle_lockstep_masked(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T,
+                                   x_out, z_out, B, C, h, w, stream, nullptr);
+}
+
+int cdx_cycle_lockstep_masked(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                              float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                              float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                              const float* mask) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -626,7 +637,7 @@ int cdx_cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, const f
     a.n_src = B; a.K = 1; a.src = true;
     a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scales = s_scales.data(); a.t_scales = t_scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
-    a.z_out = z_out; a.x_out = x_out; a.C = C; a.h = h; a.w = w;
+    a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.C = C; a.h = h; a.w = w;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -789,6 +800,14 @@ int cdx_latent_cycle_pair(cdx_net* src, cdx_net* tgt, const float* x0, const cdx
 int cdx_latent_cycle_fan(cdx_net* un, int n_src, int K, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
                          const float* src_scales, const float* tgt_scales, const cdx_ddim_coef* coef, const float* t_host, int n_steps,
                          const float* noise, float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int C, int h, int w, void* stream) {
+  return cdx_latent_cycle_fan_masked(un, n_src, K, x0, c_src, c_tgt, uc, L, src_scales, tgt_scales, coef, t_host, n_steps, noise, sqrt_a_T,
+                                     sqrt_1ma_T, x_out, z_out, C, h, w, stream, nullptr);
+}
+
+int cdx_latent_cycle_fan_masked(cdx_net* un, int n_src, int K, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                                int L, const float* src_scales, const float* tgt_scales, const cdx_ddim_coef* coef, const float* t_host,
+                                int n_steps, const float* noise, float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int C, int h,
+                                int w, void* stream, const float* mask) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && uc && src_scales && tgt_scales && coef && t_host && noise && x_out,
               "latent_cycle_fan: null argument");
@@ -799,9 +818,16 @@ int cdx_latent_cycle_fan(cdx_net* un, int n_src, int K, const float* x0, const f
     ChainLoopArgs a;
     a.n_src = n_src; a.K = K; a.src = true; a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L;
     a.s_scales = src_scales; a.t_scales = tgt_scales; a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps;
-    a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T; a.x_out = x_out; a.z_out = z_out; a.C = C; a.h = h; a.w = w;
+    a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T; a.x_out = x_out; a.z_out = z_out; a.mask = mask; a.C = C; a.h = h; a.w = w;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
+}
+
+int cdx_mask_pool(cdx_engine* e, const float* mask, float* out, int B, int H, int W, int f, void* s) {
+  ENG_CALL(e, CDX_CHECK(mask && out, "mask_pool: null argument"); mask_pool(e->e, mask, out, B, H, W, f, S(s)));
+}
+int cdx_mask_composite(cdx_engine* e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H, int W, void* s) {
+  ENG_CALL(e, CDX_CHECK(dec && image && mask && out, "mask_composite: null argument"); mask_composite(e->e, dec, image, mask, out, B, C, H, W, S(s)));
 }
 
 int cdx_ensemble_select(cdx_engine* eh, int n, const float* scores, const int64_t* cand_idx, const int* sample_idx, const float* images,

@@ -288,9 +288,19 @@ struct LatentChains {
   // v-prediction (SD 2.x "-v" models): the U-Net output is v; after the guidance combine, e_t = vsa*v + vs1*x_t and
   // pred_x0 = vsa*x_t - vs1*v with vsa = sqrt(abar_t), vs1 = sqrt(1 - abar_t) of the step's timestep (both chains share the step)
   int pred = 0; float vsa = 0.f, vs1 = 0.f;
+  // masked editing (step, source chain present): a target chain's x_{t-1} becomes m*y + (1 - m)*x of its group's source x_{t-1},
+  // m = mask[j*hw + p] for latent pixel p, broadcast over the C channels; m == 1 keeps y and m == 0 takes x exactly.  Kept last
+  // so that the offsets of the fields above, and the unmasked kernels' code, do not change.
+  const float* mask = nullptr; int hw = 0;
 };
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s);
 void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s);
+// image-resolution mask [B,1,H,W] -> [B,1,H/f,W/f]: mean of each f x f block, summed row by row then divided by f*f (avg_pool2d)
+void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, int f, cudaStream_t s);
+// paste-back at image resolution: out = m*clamp((dec + 1)*0.5, 0, 1) + (1 - m)*image, mask [B,1,H,W] broadcast over C channels;
+// m == 0 gives image, m == 1 the clamped decode, exactly
+void mask_composite(Engine& e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H, int W,
+                    cudaStream_t s);
 // Running per-sample best of the ensemble search over candidates that arrive in chunks, in any order: candidate c of the chunk
 // (image images[c], score scores[c], reference candidate index cand[c], sample sample[c]) replaces the best of its sample when it
 // wins under torch.argmax's rule over the [B, n_total] score matrix (larger score; NaN beats any number; ties and NaNs: lower

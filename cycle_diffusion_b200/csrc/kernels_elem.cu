@@ -284,16 +284,19 @@ __global__ void latent_chains_init_kernel(const LatentChains a) {
   }
 }
 // One step of the loop: the source half once per source chain, the target half once per target chain with the recovered noise held
-// in a register.  Under v-prediction each target chain forms e_t and pred_x0 from its own x_t and v.
-template <int PRED>
+// in a register.  Under v-prediction each target chain forms e_t and pred_x0 from its own x_t and v.  MASK (the driver guarantees a
+// source chain at every step): each target x_{t-1} is blended with the source's x_{t-1}, a posterior sample of q(x_{t-1} | x_t, x0)
+// of the real image at the same noise level (x0 itself on the last step), so the unmasked region stays on the image's trajectory.
+template <int PRED, int MASK>
 __global__ void latent_chains_step_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
-    float eps;
+    float eps, xn = 0.f;
     if (a.src) {
       const Chain src = a.chains[j];
       const float o = chain_eps_hat(a.eout, src, r, a.chw);
-      const float xt = __ldcg(a.xt + i), xn = __ldcg(a.xn + i);
+      const float xt = __ldcg(a.xt + i);
+      xn = __ldcg(a.xn + i);
       float e_t, pred_x0;
       eps_x0<PRED>(o, xt, a.c, a.vsa, a.vs1, e_t, pred_x0);                                     // ddim.py:576
       const float dir = MUL(a.c.dir_coef, e_t);                                                  // :578
@@ -305,6 +308,8 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
     } else {
       eps = __ldcg(a.eps_in + j * a.eps_stride + r);
     }
+    float m = 1.f;
+    if constexpr (MASK) m = __ldcg(a.mask + j * a.hw + (int)r % a.hw);
     for (int k = 0; k < a.K; ++k) {
       const size_t t = j * a.K + k, ti = t * a.chw + r;
       const Chain tc = a.chains[a.n_src + t];
@@ -314,10 +319,42 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
       eps_x0<PRED>(ot, y, a.c, a.vsa, a.vs1, et, px0);                                          // ddim.py:634
       const float tdir = MUL(a.c.dir_coef, et);                                                 // :638
       const float noise = MUL(MUL(a.c.sigma, eps), 1.0f);                                       // :642
-      const float yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                         // :645
+      float yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                               // :645
+      if constexpr (MASK) {
+        if (m == 0.0f) yn = xn;
+        else if (m != 1.0f) yn = ADD(xn, MUL(m, SUB(yn, xn)));
+      }
       a.y_out[ti] = yn;
       chain_put(a.xin, tc, r, a.chw, yn);
     }
+  }
+}
+
+// [B,1,H,W] -> [B,1,H/f,W/f]: the f x f block summed row by row, left to right, then divided by f*f (ATen's avg_pool2d order)
+__global__ void mask_pool_kernel(const float* __restrict__ m, float* __restrict__ out, int B, int H, int W, int f) {
+  const int Ho = H / f, Wo = W / f;
+  const size_t n = (size_t)B * Ho * Wo;
+  GRID_STRIDE(i, n) {
+    const int ox = (int)(i % Wo);
+    const size_t r = i / Wo;
+    const int oy = (int)(r % Ho);
+    const size_t b = r / Ho;
+    const float* p = m + (b * H + (size_t)oy * f) * W + (size_t)ox * f;
+    float sum = 0.f;
+    for (int dy = 0; dy < f; ++dy)
+      for (int dx = 0; dx < f; ++dx) sum = ADD(sum, p[(size_t)dy * W + dx]);
+    out[i] = DIV(sum, (float)(f * f));
+  }
+}
+// paste-back: out = m*clamp((dec + 1)*0.5, 0, 1) + (1 - m)*image over [B,C,H,W], m = mask[b, 0, y, x]; the decode is post-processed
+// as shift_scale + clamp do it, so m == 1 gives exactly the unmasked output and m == 0 exactly the input image
+__global__ void mask_composite_kernel(const float* __restrict__ dec, const float* __restrict__ img, const float* __restrict__ mask,
+                                      float* __restrict__ out, int C, size_t hw, size_t n) {
+  GRID_STRIDE(i, n) {
+    const size_t p = i % hw, b = i / hw / C;
+    const float m = mask[b * hw + p], x = img[i];
+    const float d = fminf(fmaxf(MUL(ADD(dec[i], 1.0f), 0.5f), 0.f), 1.f);
+    out[i] = m == 0.0f ? x : (m == 1.0f ? d : ADD(MUL(m, d), MUL(SUB(1.0f, m), x)));
   }
 }
 
@@ -612,8 +649,23 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
 
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s) { LAUNCH1(latent_chains_init_kernel, a.n, a); }
 void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
-  if (a.pred) LAUNCH1(latent_chains_step_kernel<1>, a.n, a);
-  else LAUNCH1(latent_chains_step_kernel<0>, a.n, a);
+  if (a.mask) {
+    if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1>), a.n, a);
+    else LAUNCH1((latent_chains_step_kernel<0, 1>), a.n, a);
+  } else {
+    if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0>), a.n, a);
+    else LAUNCH1((latent_chains_step_kernel<0, 0>), a.n, a);
+  }
+}
+void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, int f, cudaStream_t s) {
+  CDX_CHECK(B >= 1 && f >= 1 && H >= f && W >= f && H % f == 0 && W % f == 0, "mask_pool: %dx%d mask, factor %d", H, W, f);
+  LAUNCH1(mask_pool_kernel, (size_t)B * (H / f) * (W / f), mask, out, B, H, W, f);
+}
+void mask_composite(Engine& e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H, int W,
+                    cudaStream_t s) {
+  CDX_CHECK(B >= 1 && C >= 1 && H >= 1 && W >= 1, "mask_composite: B=%d C=%d %dx%d", B, C, H, W);
+  const size_t n = (size_t)B * C * H * W;
+  LAUNCH1(mask_composite_kernel, n, dec, image, mask, out, C, (size_t)H * W, n);
 }
 void ensemble_select(Engine& e, int n, const float* scores, const long long* cand, const int* sample, const float* images, float* best_score,
                      long long* best_idx, float* best_img, float* score_mat, int B, int n_total, size_t img_n, cudaStream_t s) {

@@ -25,6 +25,18 @@ def _f32c(t, device):
     return t.contiguous()
 
 
+def check_mask(mask, shape, device, what='mask'):
+    """A masked-editing mask from the caller: float32 of exactly ``shape`` ([B,1,h,w]), finite, every value in [0, 1] (1 = may
+    change).  Raises ValueError otherwise; returns it contiguous on ``device``."""
+    if not torch.is_tensor(mask) or mask.dtype != torch.float32:
+        raise ValueError(f'{what}: expected a float32 tensor, got {getattr(mask, "dtype", type(mask))}')
+    if tuple(mask.shape) != tuple(shape):
+        raise ValueError(f'{what}: shape {tuple(mask.shape)}, expected {tuple(shape)}')
+    if not bool(torch.isfinite(mask).all()) or bool((mask < 0).any()) or bool((mask > 1).any()):
+        raise ValueError(f'{what}: values must be finite and within [0, 1]')
+    return _f32c(mask, device)
+
+
 class Engine:
     """One per CUDA device / rank.  Not thread-safe; all work is enqueued on the current torch stream."""
 
@@ -116,6 +128,29 @@ class Engine:
         x = _f32c(x, self.device)
         out = torch.empty_like(x)
         check(lib.cdx_shift_scale(self.h, _ptr(x), b, a, _ptr(out), x.numel(), self.stream))
+        return out
+
+    def mask_pool(self, mask, f):
+        """Image-resolution mask [B,1,H,W] in [0,1] -> latent-resolution [B,1,H/f,W/f], the mean of each f x f block (f: the first
+        stage's factor); equals torch.nn.functional.avg_pool2d(mask, f) to within 1 ulp."""
+        if mask.dim() != 4 or mask.shape[1] != 1 or mask.shape[2] % f or mask.shape[3] % f:
+            raise ValueError(f'mask: expected [B,1,H,W] with H, W multiples of {f}, got {tuple(mask.shape)}')
+        mask = check_mask(mask, mask.shape, self.device)
+        B, _, H, W = mask.shape
+        out = self.empty(B, 1, H // f, W // f)
+        check(lib.cdx_mask_pool(self.h, _ptr(mask), _ptr(out), B, H, W, int(f), self.stream))
+        return out
+
+    def mask_composite(self, dec, image, mask):
+        """Paste-back: dec [B,C,H,W] (first-stage output in [-1,1]), image [B,C,H,W] in [0,1], mask [B,1,H,W] ->
+        m * clamp((dec + 1) * 0.5, 0, 1) + (1 - m) * image; exactly the image where m == 0, the clamped decode where m == 1."""
+        dec, image = _f32c(dec, self.device), _f32c(image, self.device)
+        B, Cc, H, W = dec.shape
+        if tuple(image.shape) != tuple(dec.shape):
+            raise ValueError(f'image shape {tuple(image.shape)} != decode shape {tuple(dec.shape)}')
+        mask = check_mask(mask, (B, 1, H, W), self.device)
+        out = torch.empty_like(dec)
+        check(lib.cdx_mask_composite(self.h, _ptr(dec), _ptr(image), _ptr(mask), _ptr(out), B, Cc, H, W, self.stream))
         return out
 
     def q_sample(self, x0, noise, sqrt_a, sqrt_1ma):
@@ -519,10 +554,11 @@ class UNet(Net):
                                       B, Cc, h, w, e.stream))
         return out
 
-    def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False):
+    def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False, mask=None):
         """Both chains in one loop (one U-Net call + one fused elementwise kernel per step, no z buffer unless asked for):
         x0 [B,C,h,w] -> translated latent [B,C,h,w] (and z [B, n+1, C,h,w] when return_z).  noise as for latent_encode with
-        n_rec == sched.refine_steps."""
+        n_rec == sched.refine_steps.  mask [B,1,h,w] in [0,1] (1 = may change): masked editing (cdx_cycle_lockstep_masked), the
+        target chain is blended with the source chain's x_{t-1} after every step; ones give the unmasked result, zeros give x0."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -530,19 +566,21 @@ class UNet(Net):
         n = sched.refine_steps
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
+        mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
         out = e.empty(B, Cc, h, w)
         z = e.empty(B, n + 1, Cc, h, w) if return_z else None
-        check(lib.cdx_cycle_lockstep(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale), float(tgt_scale),
-                                     sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out), _ptr(z),
-                                     B, Cc, h, w, e.stream))
+        check(lib.cdx_cycle_lockstep_masked(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale),
+                                            float(tgt_scale), sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T,
+                                            sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask)))
         return (out, z) if return_z else out
 
-    def cycle_fan(self, x0, c_src, c_tgt, uc, src_scales, tgt_scales, sched, noise, return_z=False):
+    def cycle_fan(self, x0, c_src, c_tgt, uc, src_scales, tgt_scales, sched, noise, return_z=False, mask=None):
         """The ensemble search's lock-step loop (cdx_latent_cycle_fan): source chain j (x0[j], c_src[j] at src_scales[j]) drives K
         target chains (c_tgt[j] at tgt_scales[j][k]) with the noise it recovers; one U-Net call per step over only the rows the
         scales need.  x0 [n_src,C,h,w]; c_src, c_tgt, uc [n_src,L,D]; src_scales [n_src] and tgt_scales [n_src][K] host numbers;
         noise [n+1, n_src,C,h,w] as for latent_encode with n_rec == sched.refine_steps -> latents [n_src*K,C,h,w] (row j*K + k)
-        and, when return_z, z [n_src, n+1, C,h,w]."""
+        and, when return_z, z [n_src, n+1, C,h,w].  mask [n_src,1,h,w]: source chain j's targets are masked by mask[j] as in
+        cycle_lockstep."""
         e = self.engine
         x0, c_src, c_tgt, uc, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, uc, noise))
         n_src, Cc, h, w = x0.shape
@@ -553,12 +591,13 @@ class UNet(Net):
         n = sched.refine_steps
         assert noise.shape == (n + 1, n_src, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape == uc.shape and c_src.shape[0] == n_src
+        mask = check_mask(mask, (n_src, 1, h, w), e.device) if mask is not None else None
         out = e.empty(n_src * K, Cc, h, w)
         z = e.empty(n_src, n + 1, Cc, h, w) if return_z else None
-        check(lib.cdx_latent_cycle_fan(self.h, n_src, K, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1],
-                                       (C.c_float * n_src)(*src), (C.c_float * (n_src * K))(*[s for r in tgt for s in r]),
-                                       sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out),
-                                       _ptr(z), Cc, h, w, e.stream))
+        check(lib.cdx_latent_cycle_fan_masked(self.h, n_src, K, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1],
+                                              (C.c_float * n_src)(*src), (C.c_float * (n_src * K))(*[s for r in tgt for s in r]),
+                                              sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T,
+                                              _ptr(out), _ptr(z), Cc, h, w, e.stream, _ptr(mask)))
         return (out, z) if return_z else out
 
     def pixel_encode(self, x0, sched, noise):

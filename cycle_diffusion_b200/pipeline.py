@@ -14,6 +14,7 @@ from dataclasses import dataclass
 
 import torch
 
+from .engine import check_mask
 from .schedule import DDIMSchedule
 
 
@@ -44,11 +45,21 @@ class CycleDiffusionPipeline:
     @torch.no_grad()
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
                  source_guidance_scale=1, num_images_per_prompt=1, eta=0.1, generator=None, prompt_embeds=None, output_type='pt',
-                 return_dict=True, callback=None, callback_steps=1, cross_attention_kwargs=None, clip_skip=None, two_phase=False):
+                 return_dict=True, callback=None, callback_steps=1, cross_attention_kwargs=None, clip_skip=None, two_phase=False,
+                 mask_image=None, paste_back=False):
+        """mask_image: optional float tensor [B,1,H,W] or [1,1,H,W] in [0,1] at the image's size, 1 = "may change" (diffusers'
+        convention).  Outside the mask the latent stays on the source image's own chain (cdx_cycle_lockstep_masked), so the
+        unmasked region decodes to the image's VAE reconstruction.  paste_back: additionally composite the output with the input
+        image at image resolution, so pixels where the mask is 0 are the input image exactly.  A mask needs the lock-step loop:
+        ``two_phase=True`` with a mask raises ValueError."""
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')
         if not isinstance(callback_steps, int) or callback_steps <= 0:
             raise ValueError('`callback_steps` has to be a positive integer')
+        if mask_image is not None and two_phase:
+            raise ValueError('mask_image needs the lock-step loop: the two-phase z holds noises, not the source chain (two_phase=False)')
+        if paste_back and mask_image is None:
+            raise ValueError('paste_back needs a mask_image')
         assert eta > 0, 'CycleDiffusion needs a stochastic sampler (eta > 0), ddim.py:268'
         g, e = self.g, self.engine
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
@@ -60,6 +71,15 @@ class CycleDiffusionPipeline:
             raise ValueError(f'image height and width must both be multiples of {side} (the first stage\'s factor {g.vae.down} x '
                              f'2^(len(channel_mult) - 1)), got {image.shape[2]}x{image.shape[3]}')
         B = image.shape[0] * num_images_per_prompt
+        if mask_image is not None:
+            if not (torch.is_tensor(mask_image) and mask_image.dim() == 4 and mask_image.shape[0] in (1, image.shape[0])
+                    and tuple(mask_image.shape[1:]) == (1,) + tuple(image.shape[2:])):
+                raise ValueError(f'mask_image: expected [{image.shape[0]} or 1, 1, {image.shape[2]}, {image.shape[3]}], got '
+                                 f'{tuple(mask_image.shape) if torch.is_tensor(mask_image) else type(mask_image)}')
+            mask_image = check_mask(mask_image, mask_image.shape, e.device, 'mask_image')
+            if mask_image.shape[0] == 1:
+                mask_image = mask_image.expand(image.shape[0], -1, -1, -1)
+            mask_image = mask_image.repeat_interleave(num_images_per_prompt, dim=0).contiguous()
         if num_images_per_prompt > 1:
             image = image.repeat_interleave(num_images_per_prompt, dim=0)
             prompts = [p for p in prompts for _ in range(num_images_per_prompt)]
@@ -88,10 +108,14 @@ class CycleDiffusionPipeline:
                 z = g.unet.latent_encode(x0, c_src, uc, source_guidance_scale, sched, n_rec, noise)
                 latents = g.unet.latent_decode(z, c_tgt, uc, guidance_scale, sched)
             else:
-                latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise)
+                mask = e.mask_pool(mask_image, g.vae.down) if mask_image is not None else None
+                latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise, mask=mask)
             if callback is not None:
                 callback(n_rec - 1, sched.t_loop[-1], latents)
-            img = e.shift_scale(g.decode_first_stage(latents), 1.0, 0.5).clamp(0, 1)
+            if paste_back:
+                img = e.mask_composite(g.decode_first_stage(latents), image, mask_image)
+            else:
+                img = e.shift_scale(g.decode_first_stage(latents), 1.0, 0.5).clamp(0, 1)
         if output_type == 'np':
             img = img.permute(0, 2, 3, 1).float().cpu().numpy()
         elif output_type == 'pil':

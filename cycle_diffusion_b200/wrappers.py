@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 from . import specs
-from .engine import Engine, UNet, VAE
+from .engine import Engine, UNet, VAE, check_mask
 from .ensemble import EnsemblePlan, MemberNoise
 from .schedule import DDIMSchedule, PixelSchedule, same_schedule
 
@@ -373,28 +373,40 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         sched = DDIMSchedule(self.custom_steps, self.eta, self.skip_steps[0], self.generator.alphas_cumprod)
         return self.white_box_steps != -1 and self.white_box_steps - self.skip_steps[0] - 1 >= sched.refine_steps
 
-    def cycle(self, image, encode_text, decode_text):
+    def cycle(self, image, encode_text, decode_text, mask=None):
         """encode(image, encode_text) followed by forward(z, image, encode_text, decode_text) for a single-member ensemble, on the
         engine's lock-step driver (cdx_cycle_lockstep): both chains advance together, one U-Net call per step on the batch
         [source | target uncond | target cond], and the noise recovered at a step is consumed by the target chain at once -- the
         ``z`` tensor of SDW:169-206 is never materialised.  Same random draws in the same order as encode(); same result per sample
         as the two calls (tests/test_cycle_gpu.py).  Called by TextUnsupervisedTranslation.forward when single_member().  The whole
-        cycle runs in the wrapper's precision scope, as encode() and generate() do."""
+        cycle runs in the wrapper's precision scope, as encode() and generate() do.
+
+        mask: optional [B,1,R,R] in [0,1] at image resolution, 1 = may change (masked editing): pooled to the latent grid, and
+        outside it the translated latent stays on the source image's chain (cdx_cycle_lockstep_masked)."""
         assert self.single_member(), 'cycle(): single-member ensembles only (use encode() + forward())'
         with self._precision_scope():
-            return self._cycle(image, encode_text, decode_text)
+            return self._cycle(image, encode_text, decode_text, mask)
 
-    def _cycle(self, image, encode_text, decode_text):
+    def _latent_mask(self, mask, bsz):
+        """Image-resolution mask [B,1,R,R] -> the latent grid (mean over the first stage's f x f blocks), or None."""
+        if mask is None:
+            return None
+        R = self.resolution
+        mask = check_mask(mask, (bsz, 1, R, R), self.engine.device)
+        return self.engine.mask_pool(mask, self.generator.vae.down)
+
+    def _cycle(self, image, encode_text, decode_text, mask=None):
         g, e = self.generator, self.engine
-        x0 = g.encode_image(image, self.resolution)
         bsz = image.shape[0]
+        m = self._latent_mask(mask, bsz)                  # checked before the first random draw
+        x0 = g.encode_image(image, self.resolution)
         c_src, uc = self._get_condition(encode_text, bsz)
         c_tgt, _ = self._get_condition(decode_text, bsz)
         assert self.eta > 0
         sched = DDIMSchedule(self.custom_steps, self.eta, self.skip_steps[0], g.alphas_cumprod)
         noise = self._encode_noise(sched, sched.refine_steps, x0.shape)
         sample = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, self.encoder_unconditional_guidance_scales[0],
-                                       self.decoder_unconditional_guidance_scales[0], sched, noise)
+                                       self.decoder_unconditional_guidance_scales[0], sched, noise, mask=m)
         return e.shift_scale(g.decode_first_stage(sample), 1.0, 0.5)
 
     def forward(self, z_ensemble, original_img, encode_text, decode_text):
@@ -440,7 +452,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         return EnsemblePlan(self.n_trials, self.encoder_unconditional_guidance_scales, self.skip_steps, self.decoder_unconditional_guidance_scales,
                             bsz, {k: s.refine_steps for k, s in scheds.items()}, self.ensemble_rows), scheds
 
-    def cycle_ensemble(self, image, encode_text, decode_text):
+    def cycle_ensemble(self, image, encode_text, decode_text, mask=None):
         """encode(image, encode_text) followed by forward(z, image, encode_text, decode_text) for an ensemble (lockstep_ensemble()),
         in lock-step and streamed: each (member, sample) pair's DPM-Encoder chain drives its decoder-scale chains with the noise it
         recovers (cdx_latent_cycle_fan), a chain runs a CFG row only when its scale needs one, and each chunk's candidates are
@@ -448,12 +460,16 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         candidate images is kept.  Same random draws in the same order as encode().
 
         -> (img [B,3,R,R] in [0,1], unclamped; best_idx [B] int64 in the reference's candidate order, member * n_dec + k;
-        scores [B, candidates]).  Loops and VAE run in the wrapper's precision scope, ranking outside it, as in encode + forward."""
+        scores [B, candidates]).  Loops and VAE run in the wrapper's precision scope, ranking outside it, as in encode + forward.
+
+        mask: optional [B,1,R,R] in [0,1] at image resolution (masked editing, as in cycle()): every candidate of sample b is
+        edited under mask[b] only; the masks are gathered on the device in each chunk's chain order."""
         assert self.lockstep_ensemble(), 'cycle_ensemble(): needs an ensemble with every step recovered, eta > 0 and a ranker'
         g, e, rank = self.generator, self.engine, self.directional_clip
+        bsz = image.shape[0]
+        m_lat = self._latent_mask(mask, bsz)
         with self._precision_scope():
             x0 = g.encode_image(image, self.resolution)
-            bsz = image.shape[0]
             c_src, uc = self._get_condition(encode_text, bsz)
             c_tgt, _ = self._get_condition(decode_text, bsz)
         plan, scheds = self.ensemble_plan(bsz)
@@ -468,7 +484,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
             pick = lambda t: t[samples.to(t.device)]
             with self._precision_scope():
                 lat = g.unet.cycle_fan(pick(x0), pick(c_src), pick(c_tgt), pick(uc), [plan.members[m][1] for m, _ in chunk.chains],
-                                       [plan.dec_scales] * len(chunk.chains), scheds[chunk.skip], noise.chunk(chunk))
+                                       [plan.dec_scales] * len(chunk.chains), scheds[chunk.skip], noise.chunk(chunk),
+                                       mask=pick(m_lat) if m_lat is not None else None)
                 imgs = torch.cat([g.decode_first_stage(lat[i:i + eb]) for i in range(0, lat.shape[0], eb)])
             imgs = e.shift_scale(imgs, 1.0, 0.5)                                            # Normalize(mean=-1, std=2)
             cand = [plan.candidate(m, k) for m, _ in chunk.chains for k in range(K)]

@@ -296,6 +296,28 @@ int cdx_cycle_lockstep(cdx_net* unet, const float* x0, const float* c_src, const
                        const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                        float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                        void* stream);
+/* Mask-guided local editing (Blended Latent Diffusion on the lock-step loop; diffusers' inpaint / DiffEdit `mask_image`):
+ * cdx_cycle_lockstep with mask [B,1,h,w] in [0,1] at latent resolution, 1 = "may change".  After each step the target chain's
+ * x_{t-1} becomes m * x_{t-1}(target) + (1 - m) * x_{t-1}(source), per latent pixel and broadcast over the C channels, where the
+ * source chain's x_{t-1} is its posterior sample of q(x_{t-1} | x_t, x0) of the real image (x0 itself on the last step).  The
+ * blended value is also the next U-Net input, so the edited region is denoised in the context of the real surroundings.
+ * m == 1 keeps the target value and m == 0 takes the source value EXACTLY: a mask of ones gives cdx_cycle_lockstep's output bit for
+ * bit, a mask of zeros gives x0.  The source chain reads no mask; its z_out moves only in the last bits, through the one U-Net
+ * call the rows share (fp16-split operands take one exponent per tensor).  mask == NULL is cdx_cycle_lockstep. */
+int cdx_cycle_lockstep_masked(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                              int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                              const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                              float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                              void* stream, const float* mask);
+/* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
+ * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
+ *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
+ * cdx_mask_composite: paste-back, out = m * clamp((dec + 1) * 0.5, 0, 1) + (1 - m) * image over [B,C,H,W] (dec the first stage's
+ *   output in [-1,1], image in [0,1]); where m == 0 out is image exactly, where m == 1 the clamped decode exactly (the value of
+ *   cdx_shift_scale(dec, 1, 0.5) followed by a clamp). */
+int cdx_mask_pool(cdx_engine* e, const float* mask, float* out, int B, int H, int W, int f, void* stream);
+int cdx_mask_composite(cdx_engine* e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H,
+                       int W, void* stream);
 /* The same three loops with PER-SAMPLE guidance scales (device arrays of B floats): the ensemble driver of the text wrappers
  * (SDW:146-165 generate, :189-204 encode -- the reference loops trial x encoder-scale x skip, then x decoder-scale, one chain at a
  * time, recomputing the conditioning and every context K/V projection per member).  Members that share a schedule are batched
@@ -383,6 +405,13 @@ int cdx_latent_cycle_fan(cdx_net* unet, int n_src, int K, const float* x0, const
                          const float* uc, int ctx_len, const float* src_scales_host, const float* tgt_scales_host,
                          const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                          float sqrt_1ma_T, float* x_out, float* z_out, int C, int h, int w, void* stream);
+/* cdx_latent_cycle_fan with mask [n_src,1,h,w]: source chain j's K target chains are blended with its x_{t-1} under mask[j] as in
+ * cdx_cycle_lockstep_masked (m == 1 / m == 0 exact).  mask == NULL is cdx_latent_cycle_fan. */
+int cdx_latent_cycle_fan_masked(cdx_net* unet, int n_src, int K, const float* x0, const float* c_src, const float* c_tgt,
+                                const float* uc, int ctx_len, const float* src_scales_host, const float* tgt_scales_host,
+                                const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                                float sqrt_1ma_T, float* x_out, float* z_out, int C, int h, int w, void* stream,
+                                const float* mask);
 int cdx_ensemble_select(cdx_engine* e, int n, const float* scores, const int64_t* cand_idx, const int* sample_idx,
                         const float* images, float* best_score, int64_t* best_idx, float* best_img, float* score_mat, int B,
                         int n_total, int H, int W, void* stream);

@@ -19,7 +19,9 @@
 //                 channel-concatenated sources), or for conv3x3 a 4D box of the NHWC activation -- per (tap, 32-channel block) {32 ch, bw,
 //                 bh, bn} shifted by (dy-1, dx-1): TMA's out-of-bounds zero fill *is* the conv's zero padding, im2col is never
 //                 materialised; or (batched mode) 4D maps over (k, head, row, batch) for the attention contractions.  B: pre-split
-//                 weight planes (fp16 or TF32), or raw fp32 (KIND_SS).  128B-swizzled smem, STAGES-deep ring.
+//                 weight planes (fp16 or TF32), or raw fp32 (KIND_SS).  One ring of 32-K stages in shared memory, as deep as
+//                 227 KB allows (Cfg: 7 stages at BN 128 and 9 at BN 64 for the fp16 split, whose B rows are 64 B with the 64B
+//                 swizzle; 4 / 7 for TF32, 128B swizzle), so the producer runs up to STAGES - 2 stages ahead of the consumers.
 //   warpgroups 1-2  64 rows each: raw fp32 A from smem -> hi / lo split in registers (the wgmma A fragment layout) -> three wgmmas
 //                 per K step against the B tiles in smem -> chunk accumulator -> total, software-pipelined (the next stage's A
 //                 is split into a second fragment set while the current stage's wgmmas run, one batch per stage); then the
@@ -45,24 +47,34 @@ namespace {
 using namespace tc;
 
 constexpr int TBM = 128, TBN = 128, TBK = 32;
-constexpr int TILE_BYTES = TBM * TBK * 4;          // 16 KB: one 32-float A sub-block of 128 rows
+constexpr int TILE_BYTES = TBM * TBK * 4;          // 16 KB: one 32-float A block of 128 rows
 constexpr int TC_THREADS = 384;                     // producer warpgroup + two consumer warpgroups (setmaxnreg is per warpgroup)
-constexpr int STAGES = 3;
+constexpr int SMEM_MAX = 232448;                    // sm_90 opt-in dynamic shared memory per block
+constexpr int BAR_BYTES = 256, ALIGN_SLACK = 1024;  // the ring's mbarriers; slack to align the ring base to 1024 B
 
 // KIND_H16_FAST: the separately reported reduced-precision path (hi*hi term only), a compile-time variant of KIND_H16 so that no
 // runtime branch sits inside a batch of wgmmas
 enum { KIND_SS = 0, KIND_TS = 1, KIND_H16 = 2, KIND_H16_FAST = 3 };
 
+// One ring stage = 32 K elements: the fp32 A block (128 rows x 128 B, 128B swizzle) + two B planes (hi / lo; KIND_SS: raw fp32
+// and its in-place lo), BN rows each: 32 fp16 = 64 B (64B swizzle) or 32 fp32 = 128 B (128B swizzle).  The ring is as deep as the
+// shared memory allows: the deeper it is, the more operand bytes the producer keeps in flight ahead of the consumers
+// (H16: 7 stages at BN 128, 9 at BN 64; TS / SS: 4 at BN 128, 7 at BN 64).
 template <int KIND, int BN>
 struct Cfg {
   static constexpr bool H16 = KIND == KIND_H16 || KIND == KIND_H16_FAST;
-  static constexpr int BK = H16 ? 64 : 32;           // K elements per pipeline stage
+  static constexpr int BK = TBK;                     // K elements per pipeline stage
+  static constexpr int KSTEPS = H16 ? 2 : 4;         // wgmma K steps per stage: k16 (fp16) or k8 (tf32)
   static constexpr int KCHUNK = 256 / BK;            // stages per accumulation chunk (256 K elements)
-  static constexpr int A_BYTES = (H16 ? 2 : 1) * TILE_BYTES;
-  static constexpr int B_PLANE = BN * 128;          // one B plane of a stage: BN rows x 128 B
+  static constexpr int A_BYTES = TILE_BYTES;
+  static constexpr int B_ROW = H16 ? 64 : 128;       // bytes of one B row of a stage
+  static constexpr int B_PLANE = BN * B_ROW;
   static constexpr int STAGE_BYTES = A_BYTES + 2 * B_PLANE;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/ + 1024 /*alignment slack*/;
-  static_assert(SMEM_BYTES <= 232448, "smem overflow");
+  static constexpr int STAGES = (SMEM_MAX - BAR_BYTES - ALIGN_SLACK) / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + ALIGN_SLACK;
+  static_assert(STAGES >= 3 && 2 * STAGES * 8 <= BAR_BYTES, "barrier area holds a full and an empty barrier per stage");
+  static_assert(STAGE_BYTES % 1024 == 0 && B_PLANE % 1024 == 0, "stage and plane bases stay 1024-byte aligned (swizzle atoms)");
+  static_assert(SMEM_BYTES <= SMEM_MAX, "smem overflow");
 };
 
 struct TcParams {
@@ -158,7 +170,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapBlo, const TcParams p) {
   using CF = Cfg<KIND, BN>;
   constexpr bool H16 = CF::H16, FAST = KIND == KIND_H16_FAST;
-  constexpr int BK = CF::BK, A_BYTES = CF::A_BYTES, B_PLANE = CF::B_PLANE, STAGE_BYTES = CF::STAGE_BYTES;
+  constexpr int BK = CF::BK, KSTEPS = CF::KSTEPS, A_BYTES = CF::A_BYTES, B_PLANE = CF::B_PLANE, STAGE_BYTES = CF::STAGE_BYTES;
+  constexpr int STAGES = CF::STAGES;
   constexpr int NACC = BN / 2;                     // fp32 accumulators per thread of an m64nBN tile
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
@@ -193,7 +206,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         const uint32_t st = base + s * STAGE_BYTES;
         const uint32_t sb = st + A_BYTES;
         const int k0 = kb * BK;
-        const int nsub = (H16 && k0 + TBK < p.K) ? 2 : 1;        // K % 32 == 0; an odd tail stage carries one sub-block
         if (p.mode == 2) {
           mbar_expect_tx(bar_full(s), TILE_BYTES + BN * 128);
           int ca[4], cb4[4];
@@ -207,21 +219,16 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           tma_load_4d(sb, &mapB, cb4[0], cb4[1], cb4[2], cb4[3], bar_full(s));
           continue;
         }
-        mbar_expect_tx(bar_full(s), nsub * TILE_BYTES + (KIND == KIND_SS ? 1 : 2) * BN * 128);
-        for (int sub = 0; sub < nsub; ++sub) {
-          const int ks = k0 + sub * TBK;
-          const uint32_t dst = st + sub * TILE_BYTES;
-          if (p.mode == 0) {
-            if (ks < p.C1) tma_load_2d(dst, &mapA, ks, tc_.m0, bar_full(s));
-            else tma_load_2d(dst, &mapA2, ks - p.C1, tc_.m0, bar_full(s));
-          } else {
-            const int kq = ks / TBK;
-            const int tap = kq / cblocks, cb = kq - tap * cblocks;
-            const int dy = tap / 3, dx = tap - dy * 3;
-            const int c = cb * TBK;                               // channel concat: blocks >= C1 come from the second source
-            tma_load_4d(dst, c < p.C1 ? &mapA : &mapA2, c < p.C1 ? c : c - p.C1, tc_.x0 * p.cstride + dx - p.cpad,
-                        tc_.y0 * p.cstride + dy - p.cpad, tc_.b0, bar_full(s));      // OOB -> zeros = padding
-          }
+        mbar_expect_tx(bar_full(s), TILE_BYTES + (KIND == KIND_SS ? 1 : 2) * B_PLANE);
+        if (p.mode == 0) {
+          if (k0 < p.C1) tma_load_2d(st, &mapA, k0, tc_.m0, bar_full(s));
+          else tma_load_2d(st, &mapA2, k0 - p.C1, tc_.m0, bar_full(s));
+        } else {
+          const int tap = kb / cblocks, cb = kb - tap * cblocks;
+          const int dy = tap / 3, dx = tap - dy * 3;
+          const int c = cb * TBK;                                 // channel concat: blocks >= C1 come from the second source
+          tma_load_4d(st, c < p.C1 ? &mapA : &mapA2, c < p.C1 ? c : c - p.C1, tc_.x0 * p.cstride + dx - p.cpad,
+                      tc_.y0 * p.cstride + dy - p.cpad, tc_.b0, bar_full(s));        // OOB -> zeros = padding
         }
         tma_load_2d(sb, &mapB, k0, tc_.n0, bar_full(s));
         if (KIND != KIND_SS) tma_load_2d(sb + B_PLANE, &mapBlo, k0, tc_.n0, bar_full(s));
@@ -255,10 +262,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 
   // Software pipeline over the stages of the work item: while the wgmmas of stage it run, stage it + 1's A is split into the
   // other fragment set; wgmma.wait_group 1 then retires stage it - 1, whose smem slot goes back to the producer.
-  struct Frag { uint32_t h[4][4], l[4][4]; };     // A fragments of one stage's K steps (rows r0 / r0 + 8), hi / lo
-  const int nst = tc_.kb1 - tc_.kb0;               // stages of this work item (>= 1)
-  // H16: a stage whose second 32-element sub-block lies beyond K (odd K tail, only the last stage of the K range) has 2 K steps
-  auto tail = [&](int it) { return H16 && (tc_.kb0 + it) * BK + TBK >= p.K; };
+  struct Frag { uint32_t h[KSTEPS][4], l[KSTEPS][4]; };     // A fragments of one stage's K steps (rows r0 / r0 + 8), hi / lo
+  const int nst = tc_.kb1 - tc_.kb0;               // stages of this work item (>= 1; K % 32 == 0: every stage is full)
 
   // wait for stage it to land, then split its A into f
   auto load_split = [&](int it, Frag& f) {
@@ -282,30 +287,25 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
       asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    const int k0 = (tc_.kb0 + it) * BK;
-    const int nsl = tail(it) ? 2 : 4;
+    // fused GroupNorm: tap / channel block of this stage
+    int tap = 0, cbase = 0;
+    if (H16 && p.gn_ab) {
+      const int kq = tc_.kb0 + it;
+      tap = kq / cblocks;
+      cbase = (kq - tap * cblocks) * TBK;
+    }
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      if (kk >= nsl) break;
+    for (int kk = 0; kk < KSTEPS; ++kk) {
       if (H16) {
-        const int sub = kk >> 1;
-        const uint32_t sa = st + sub * TILE_BYTES;
-        // fused GroupNorm: tap / channel block of this sub-block
-        int tap = 0, cbase = 0;
-        if (p.gn_ab) {
-          const int kq = (k0 + sub * TBK) / TBK;
-          tap = kq / cblocks;
-          cbase = (kq - tap * cblocks) * TBK;
-        }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {                 // i: row r0 + 8 i
           const int r = r0 + 8 * i;
 #pragma unroll
           for (int hk = 0; hk < 2; ++hk) {            // hk: k 2qd (+1) or 2qd + 8 (+1)
-            const int k = (kk & 1) * 16 + hk * 8 + 2 * qd;
+            const int k = kk * 16 + hk * 8 + 2 * qd;
             float2 x;
             asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x.x), "=f"(x.y)
-                         : "r"(sa + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
+                         : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
             if (p.gn_ab) {
               const int yy = py[i] + tap / 3 - 1, xx = px[i] + tap % 3 - 1;
               const bool inside = xx >= 0 && xx < p.W && yy >= 0 && yy < p.H && pb[i] < p.B;
@@ -347,16 +347,15 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
   };
 
-  // the wgmmas of stage it (NSL K steps) from f: one straight-line batch, small terms first
-  auto mma = [&](auto nsl_c, int it, const Frag& f) {
-    constexpr int NSL = decltype(nsl_c)::value;
+  // the wgmmas of stage it from f: one straight-line batch, small terms first
+  auto mma = [&](int it, const Frag& f) {
     const uint32_t sb = base + (it % STAGES) * STAGE_BYTES + A_BYTES;
-    const uint64_t bhi = make_desc(sb), blo = make_desc(sb + B_PLANE);
+    const uint64_t bhi = H16 ? make_desc_sw64(sb) : make_desc(sb), blo = H16 ? make_desc_sw64(sb + B_PLANE) : make_desc(sb + B_PLANE);
     wgmma_pin(acc);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < NSL; ++kk) {
-      const uint64_t adv = (uint64_t)kk * 2u;       // 32 bytes per K step along the 128-byte row
+    for (int kk = 0; kk < KSTEPS; ++kk) {
+      const uint64_t adv = (uint64_t)kk * 2u;       // 32 bytes per K step along the B row (64 B fp16 / 128 B fp32)
       if (H16) {
         if (!FAST) {
           Wgmma<BN>::f16_rs(acc, f.l[kk], bhi + adv);
@@ -375,8 +374,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   // stage it: its fragments are in cur; nxt held stage it - 1's
   int kin = 0;
   auto step = [&](int it, const Frag& cur, Frag& nxt) {
-    if (tail(it)) mma(std::integral_constant<int, 2>(), it, cur);
-    else mma(std::integral_constant<int, 4>(), it, cur);
+    mma(it, cur);
     wgmma_wait1();                                  // stage it - 1 has retired: its slot and its fragment set are free
     if (it > 0) {
       __syncwarp();
@@ -889,11 +887,13 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
     p.tiles_m = p.tiles_x * p.tiles_y * cdiv(B, bn);
   }
   // ---- operand path: fp16-split (KIND_H16) when the engine selects it, the weights have fp16 planes and the geometry allows it
-  // (K a multiple of 32: the stage's two 32-float A sub-blocks; fp16 B rows 16-byte aligned); else TF32 planes (KIND_TS); else SS
+  // (K a multiple of 32: whole 32-K ring stages; fp16 B rows 16-byte aligned); else TF32 planes (KIND_TS); else SS
   const bool ts = a.Bw_hi != nullptr && a.Bw_lo != nullptr && a16(a.Bw_hi) && a16(a.Bw_lo);
   const bool h16 = e.tc_kind >= 1 && a.Bw_h_hi && a.Bw_h_lo && a16(a.Bw_h_hi) && a16(a.Bw_h_lo) && (a.K % TBK) == 0 && (a.ldb % 8) == 0 &&
                    (a.mode == 1 || !a.A2 || (a.C2 % TBK) == 0);
   CDX_CHECK(!(a.mode == 1 && (a.A2 || a.gn_ab)) || h16, "conv3x3: concat / fused GroupNorm input without the fp16-split path");
+  // The planner counts fp16-split work in 64-K blocks (its cost constants are per 64 K), so its choice of (w, S) -- and with it the
+  // split-K boundaries -- does not depend on the ring's stage size; kb_per_split is converted to 32-K stages below.
   const int bk = h16 ? 64 : TBK;
   const int num_kb = cdiv(a.K, bk);
   // Work partition: tile width w (128 or 64 columns: the two wgmma widths compiled in) and split-K factor S, chosen together against
@@ -938,6 +938,7 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   const int tiles = p.tiles_m * p.tiles_n;
   p.kb_per_split = cdiv(num_kb, best_s);
   p.splits = cdiv(num_kb, p.kb_per_split);            // no empty splits
+  p.kb_per_split *= bk / TBK;                         // in the kernel's 32-K stages
   p.total_tiles = tiles * p.splits;
   Scope ws_scope(e.arena);
   if (p.splits > 1) p.ws = (float*)e.arena.alloc((size_t)p.splits * a.M * a.N * sizeof(float));
@@ -969,9 +970,9 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   if (e.dry()) return true;
   if (h16) {
     uint64_t d[2] = {(uint64_t)a.K, (uint64_t)a.N}, st[1] = {(uint64_t)a.ldb * 2};
-    uint32_t bx[2] = {64u, (uint32_t)p.tn_w};
-    mB = &get_map(a.Bw_h_hi, 2, d, st, bx, nullptr, 2);
-    mBlo = &get_map(a.Bw_h_lo, 2, d, st, bx, nullptr, 2);
+    uint32_t bx[2] = {(uint32_t)TBK, (uint32_t)p.tn_w};          // 32 fp16 = 64-byte rows, 64B swizzle
+    mB = &get_map(a.Bw_h_hi, 2, d, st, bx, nullptr, 2, 64);
+    mBlo = &get_map(a.Bw_h_lo, 2, d, st, bx, nullptr, 2, 64);
   } else {
     uint64_t d[2] = {(uint64_t)a.K, (uint64_t)a.N}, st[1] = {(uint64_t)a.ldb * 4};
     uint32_t bx[2] = {TBK, (uint32_t)p.tn_w};

@@ -1,5 +1,5 @@
 // tc_common.cuh -- shared pieces of the sm_90a tensor-core kernels: PTX wrappers (mbarrier, TMA, programmatic dependent launch),
-// the K-major 128B-swizzle wgmma smem descriptor, fp16 / TF32 split helpers, and the host-side CUtensorMap cache.
+// the K-major 128B / 64B-swizzle wgmma smem descriptors, fp16 / TF32 split helpers, and the host-side CUtensorMap cache.
 #pragma once
 #include <cuda.h>
 
@@ -86,6 +86,16 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset: 8 rows * 128 B
   d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
+  return d;
+}
+// K-major, 64-byte-swizzled variant (rows of 64 B = 32 fp16, 8-row atoms of 512 B; the tile base is 1024-byte aligned).  Advancing
+// one k16 step (32 B) along the row = adding 2 to the start-address field, as with make_desc.
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);       // start address
+  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(512 >> 4) << 32;               // stride byte offset: 8 rows * 64 B
+  d |= (uint64_t)2 << 62;                        // SWIZZLE_64B
   return d;
 }
 

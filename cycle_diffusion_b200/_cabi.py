@@ -123,6 +123,10 @@ SIGNATURES = {
     'cdx_op_attention': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
     'cdx_op_nchw_to_nhwc': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_nhwc_to_nchw': (_I, [_P, _P, _P, _I, _I, _I, _P]),
+    'cdx_op_groupnorm_ex': (_I, [_P, _P, _I, _P, _I, _P, _P, _F, _I, _P, _P, _I, _P, _P, _P, _I, _I, _P]),
+    'cdx_op_layernorm_ex': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
+    'cdx_op_softmax_rows': (_I, [_P, _P, C.c_int64, _I, _I, _I, _P]),
+    'cdx_op_produce_norm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, C.POINTER(_I), _P]),
 }
 
 

@@ -1002,4 +1002,94 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
 int cdx_op_nchw_to_nhwc(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nchw_to_nhwc(eh->e, x, y, B, C, HW, S(stream))); }
 int cdx_op_nhwc_to_nchw(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nhwc_to_nchw(eh->e, x, y, B, C, HW, S(stream))); }
 
+int cdx_op_groupnorm_ex(cdx_engine* eh, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta, float eps,
+                        int silu_, const float* scale, const float* shift, int ld_ss, float* y, float* amax_out, float* ab_out, int B, int HW,
+                        void* stream) {
+  return guard([&] {
+    CDX_CHECK(eh && x1 && gamma && beta && y && B > 0 && HW > 0 && C1 > 0 && C2 >= 0 && (C2 == 0) == (x2 == nullptr),
+              "op_groupnorm_ex: bad arguments");
+    CDX_CHECK(!scale == !shift && (!scale || ld_ss >= C1 + C2), "op_groupnorm_ex: scale and shift go together, with ld_ss >= C");
+    Engine& e = eh->e;
+    cudaStream_t s = S(stream);
+    with_arena(e, s, [&] {
+      Scope sc(e.arena);
+      e.pools_reset(s);
+      // the statistics of sources whose producer did not fuse them (one pass each), shared by the norm and the table
+      const double* st1 = gn_channel_stats(e, x1, C1, B, HW, s);
+      const double* st2 = x2 ? gn_channel_stats(e, x2, C2, B, HW, s) : nullptr;
+      float* slot = e.amax_slot();
+      groupnorm(e, x1, C1, x2, C2, gamma, beta, eps, silu_ != 0, scale, shift, ld_ss, y, B, HW, s, st1, st2, slot);
+      const float* ab = ab_out ? gn_affine(e, x1, C1, x2, C2, gamma, beta, eps, scale, shift, ld_ss, B, HW, s, st1, st2) : nullptr;
+      if (e.dry()) return;
+      if (amax_out) CDX_CUDA(cudaMemcpyAsync(amax_out, slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
+      if (ab_out) CDX_CUDA(cudaMemcpyAsync(ab_out, ab, (size_t)B * (C1 + C2) * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    });
+  });
+}
+int cdx_op_layernorm_ex(cdx_engine* eh, const float* x, const float* gamma, const float* beta, float* y, float* amax_out, int M, int C,
+                        void* stream) {
+  return guard([&] {
+    CDX_CHECK(eh && x && gamma && beta && y && M > 0, "op_layernorm_ex: bad arguments");
+    Engine& e = eh->e;
+    cudaStream_t s = S(stream);
+    with_arena(e, s, [&] {
+      e.pools_reset(s);
+      float* slot = e.amax_slot();
+      layernorm(e, x, gamma, beta, y, M, C, s, slot);
+      if (!e.dry() && amax_out) CDX_CUDA(cudaMemcpyAsync(amax_out, slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
+    });
+  });
+}
+int cdx_op_softmax_rows(cdx_engine* eh, float* x, int64_t rows, int L, int ld, int causal_nq, void* stream) {
+  ENG_CALL(eh, CDX_CHECK(x && rows > 0 && L > 0 && ld >= L && causal_nq >= 0, "op_softmax_rows: bad arguments");
+           softmax_rows(eh->e, x, (long long)rows, L, ld, S(stream), causal_nq));
+}
+int cdx_op_produce_norm(cdx_engine* eh, const float* x, const float* w, const float* bias, int conv, int B, int H, int W, int Cin, int Cout,
+                        const float* gamma, const float* beta, float eps, float* y, float* amax_out, double* stats_out, float* yn, int* path_out,
+                        void* stream) {
+  return guard([&] {
+    CDX_CHECK(eh && x && w && gamma && beta && y && amax_out && stats_out && yn && path_out, "op_produce_norm: null argument");
+    CDX_CHECK((conv == 0 || conv == 1) && B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && Cout % 4 == 0,
+              "op_produce_norm: conv=%d B=%d %dx%d Cin=%d Cout=%d", conv, B, H, W, Cin, Cout);
+    Engine& e = eh->e;
+    cudaStream_t s = S(stream);
+    with_arena(e, s, [&] {
+      Scope sc(e.arena);
+      e.pools_reset(s);
+      const int K = conv ? 9 * Cin : Cin;
+      const float* wk = w;
+      if (conv) {
+        float* wr = (float*)e.arena.alloc((size_t)Cout * K * sizeof(float));
+        repack_conv3x3(e, w, wr, Cout, Cin, s);
+        wk = wr;
+      }
+      GemmArgs g;
+      g.mode = conv;
+      g.M = B * H * W; g.N = Cout; g.K = K;
+      g.A = x; g.lda = Cin; g.C1 = Cin;
+      if (conv) { g.Hin = H; g.Win = W; g.Hout = H; g.Wout = W; g.stride = 1; g.pad = 1; g.up = 1; }
+      g.Bw = wk; g.ldb = K;
+      g.Cout = y; g.ldc = Cout;
+      g.bias = bias;
+      if (e.mma_mode == 1) {
+        float* hi = (float*)e.arena.alloc((size_t)Cout * K * sizeof(float));
+        float* lo = (float*)e.arena.alloc((size_t)Cout * K * sizeof(float));
+        split_planes(e, wk, hi, lo, (size_t)Cout * K, s);
+        g.Bw_hi = hi; g.Bw_lo = lo;
+        hook_h16_planes(e, wk, (size_t)Cout * K, g, s);
+      }
+      Tensor t;
+      t.p = y; t.B = B; t.H = H; t.W = W; t.C = Cout;
+      track_outputs(e, t, g, true);
+      int route = 0;
+      gemm(e, g, s, &route);          // statistics the epilogue could not fuse come from the standalone pass inside
+      *path_out = (route & 2) ? 1 : (route & 4) ? 3 : (route & 8) ? 2 : 0;
+      groupnorm(e, y, Cout, nullptr, 0, gamma, beta, eps, false, nullptr, nullptr, 0, yn, B, H * W, s, t.stats, nullptr, e.amax_slot());
+      if (e.dry()) return;
+      CDX_CUDA(cudaMemcpyAsync(amax_out, t.amax, sizeof(float), cudaMemcpyDeviceToDevice, s));
+      CDX_CUDA(cudaMemcpyAsync(stats_out, t.stats, (size_t)B * Cout * 2 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    });
+  });
+}
+
 }  // extern "C"

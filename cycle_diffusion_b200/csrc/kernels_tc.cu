@@ -966,7 +966,7 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   // (a tile that overhangs its map may start a warp on a masked row: its statistics are left to the standalone pass)
   const bool quad_ok = a.mode == 1 ? ((p.bw * p.bh) % 32 == 0 && p.tiles_x * p.bw == p.W && p.tiles_y * p.bh == p.H) : (a.rows_per_batch % 32 == 0);
   p.c_stats = (a.c_stats && quad_ok && p.splits == 1 && !a.out_nchw && !a.geglu && !a.Ct_hi && !a.Cout_lo && a.ldc == a.N) ? a.c_stats : nullptr;
-  if (side_done) *side_done = (p.c_amax ? 1 : 0) | (p.c_stats ? 2 : 0);
+  if (side_done) *side_done = (p.c_amax ? 1 : 0) | (p.c_stats ? 2 : 0) | (p.splits > 1 ? 4 : 0);
   if (e.dry()) return true;
   if (h16) {
     uint64_t d[2] = {(uint64_t)a.K, (uint64_t)a.N}, st[1] = {(uint64_t)a.ldb * 2};

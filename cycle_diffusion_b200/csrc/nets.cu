@@ -515,6 +515,16 @@ void net_finalize(Net& n) {
 }
 
 // ================================================================================================ executors
+void track_outputs(Engine& e, Tensor& t, GemmArgs& g, bool stats) {
+  t.amax = e.amax_slot();
+  g.c_amax = t.amax;
+  if (stats && (t.C % 4) == 0) {          // (few-channel outputs -- a 3-channel VQ latent -- are never GroupNorm inputs)
+    t.stats = e.stat_alloc((size_t)t.B * t.C * 2);
+    g.c_stats = t.stats;
+    g.rows_per_batch = t.H * t.W;
+  }
+}
+
 namespace {
 
 struct Exec {
@@ -538,17 +548,7 @@ struct Exec {
     gemm(e, g, s);
   }
 
-  // side outputs of a GEMM that writes tensor t: its range (for a consumer fp16-split GEMM) and, optionally, its per-(image,
-  // channel) sums (for a consumer GroupNorm) -- both produced by the epilogue that holds the tile in registers
-  void track(Tensor& t, GemmArgs& g, bool stats) {
-    t.amax = e.amax_slot();
-    g.c_amax = t.amax;
-    if (stats && (t.C % 4) == 0) {          // (few-channel outputs -- a 3-channel VQ latent -- are never GroupNorm inputs)
-      t.stats = e.stat_alloc((size_t)t.B * t.C * 2);
-      g.c_stats = t.stats;
-      g.rows_per_batch = t.H * t.W;
-    }
-  }
+  void track(Tensor& t, GemmArgs& g, bool stats) { track_outputs(e, t, g, stats); }
 
   // y = conv3x3(x [, x2 concat]) + bias (+ rowvec per sample) (+ residual); up: nearest-2x folded into the gather
   Tensor conv3(const Tensor& x0, const std::string& name, int stride = 1, int pad = 1, int up = 1, const float* rowvec = nullptr,

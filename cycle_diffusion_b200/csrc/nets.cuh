@@ -75,6 +75,10 @@ void net_load_param(Net& n, const char* name, const float* data, bool on_device,
 void net_finalize(Net& n);
 void net_ensure_blob(Net& n);
 
+// side outputs of a GEMM that writes tensor t: its range slot (for a consumer fp16-split GEMM) and, with `stats`, its per-(image,
+// channel) sums (for a consumer GroupNorm) -- both produced by the epilogue that holds the tile in registers where it can
+void track_outputs(Engine& e, Tensor& t, GemmArgs& g, bool stats);
+
 // forward executors (enqueue only; caller handles arena dry-run)
 // reuse_ctx: the caller guarantees `ctx` is unchanged since the previous call with reuse_ctx (and n.ctxkv was invalidated
 // at the start of the loop) -> context K / V projections are taken from n.ctxkv instead of being recomputed

@@ -281,6 +281,68 @@ class Engine:
         check(lib.cdx_op_layernorm(self.h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(y), M, Cc, self.stream))
         return y
 
+    def op_groupnorm_ex(self, x1, x2, gamma, beta, eps, silu, scale=None, shift=None):
+        """GroupNorm(32) of the channel concat [x1 | x2] (NHWC [B,H,W,C1], [B,H,W,C2] or None) as the network executors run it,
+        optional gn(x) * (1 + scale) + shift and SiLU.  scale / shift: [B, C] device views with unit column stride and one common
+        row stride (e.g. the two halves of a [B, 2C] embedding projection).  Returns (y, amax, ab): y [B,H,W,C], amax [1] the
+        tracked range slot of y, ab [B, C, 2] the fused conv's (a, o) table, y = silu?(x * a + o)."""
+        x1, gamma, beta = (_f32c(t, self.device) for t in (x1, gamma, beta))
+        B, H, W, C1 = x1.shape
+        x2 = _f32c(x2, self.device) if x2 is not None else None
+        C2 = x2.shape[3] if x2 is not None else 0
+        assert (scale is None) == (shift is None)
+        ld_ss = 0
+        if scale is not None:
+            for t in (scale, shift):
+                assert t.dtype == torch.float32 and t.device == self.device and tuple(t.shape) == (B, C1 + C2) and t.stride(1) == 1
+            assert scale.stride(0) == shift.stride(0), 'scale and shift share one row stride'
+            ld_ss = scale.stride(0)
+        y = self.empty(B, H, W, C1 + C2)
+        amax = torch.zeros(1, dtype=torch.float32, device=self.device)
+        ab = self.empty(B, C1 + C2, 2)
+        check(lib.cdx_op_groupnorm_ex(self.h, _ptr(x1), C1, _ptr(x2), C2, _ptr(gamma), _ptr(beta), eps, int(silu), _ptr(scale), _ptr(shift),
+                                      ld_ss, _ptr(y), _ptr(amax), _ptr(ab), B, H * W, self.stream))
+        return y, amax, ab
+
+    def op_layernorm_ex(self, x, gamma, beta):
+        """LayerNorm over the last dim of x [M, C] (eps 1e-5) -> (y, amax [1] the tracked range slot of y)."""
+        x, gamma, beta = (_f32c(t, self.device) for t in (x, gamma, beta))
+        M, Cc = x.shape
+        y = torch.empty_like(x)
+        amax = torch.zeros(1, dtype=torch.float32, device=self.device)
+        check(lib.cdx_op_layernorm_ex(self.h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(y), _ptr(amax), M, Cc, self.stream))
+        return y, amax
+
+    def op_softmax_rows(self, x, causal_nq=0):
+        """Row softmax of x [rows, L] in place (x is returned); causal_nq > 0: row r sees columns j <= r % causal_nq only."""
+        assert x.dtype == torch.float32 and x.device == self.device and x.is_contiguous()
+        rows, L = x.shape
+        check(lib.cdx_op_softmax_rows(self.h, _ptr(x), rows, L, L, int(causal_nq), self.stream))
+        return x
+
+    PRODUCE_PATHS = ('ffma', 'fused', 'tc_standalone', 'splitk')
+
+    def op_produce_norm(self, x, w, bias, gamma, beta, eps, conv=False):
+        """A producer GEMM with its GroupNorm side outputs wired as the executors wire them, then the GroupNorm that trusts them.
+        Linear: x [B, HW, Cin], w [Cout, Cin]; conv: NHWC x [B, H, W, Cin], w OIHW [Cout, Cin, 3, 3] (stride 1, pad 1).
+        Returns (y [B*HW, Cout], amax [1], stats [B, Cout, 2] float64, yn [B*HW, Cout], path), path one of PRODUCE_PATHS."""
+        x, w, gamma, beta = (_f32c(t, self.device) for t in (x, w, gamma, beta))
+        bias = _f32c(bias, self.device) if bias is not None else None
+        if conv:
+            B, H, W, Cin = x.shape
+        else:
+            B, HW, Cin = x.shape
+            H, W = HW, 1
+        Cout = w.shape[0]
+        y = self.empty(B * H * W, Cout)
+        yn = self.empty(B * H * W, Cout)
+        amax = torch.zeros(1, dtype=torch.float32, device=self.device)
+        stats = torch.empty(B, Cout, 2, dtype=torch.float64, device=self.device)
+        path = C.c_int(-1)
+        check(lib.cdx_op_produce_norm(self.h, _ptr(x), _ptr(w), _ptr(bias), int(bool(conv)), B, H, W, Cin, Cout, _ptr(gamma), _ptr(beta),
+                                      eps, _ptr(y), _ptr(amax), _ptr(stats), _ptr(yn), C.byref(path), self.stream))
+        return y, amax, stats, yn, self.PRODUCE_PATHS[path.value]
+
     def op_attention(self, q, k, v, heads, scale):
         q, k, v = (_f32c(t, self.device) for t in (q, k, v))
         B, Nq, Cc = q.shape

@@ -432,6 +432,30 @@ int cdx_op_attention(cdx_engine* e, const float* q, const float* k, const float*
                      int Nq, int Nk, int heads, int d, float scale, void* stream);
 int cdx_op_nchw_to_nhwc(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
+/* The normalisation kernels in the forms the network executors call them, with their side outputs (tests/test_norms_gpu.py).
+ * cdx_op_groupnorm_ex: GroupNorm(32) over the channel concat [x1 | x2] (NHWC [B,HW,C1] and [B,HW,C2]; x2 NULL when C2 == 0), then
+ *   optionally * (1 + scale) + shift (scale / shift [B, ld_ss] or NULL) and SiLU -> y [B,HW,C1+C2].  amax_out (optional, device
+ *   float): the tracked range slot of y as the norm left it.  ab_out (optional, device [B, C1+C2, 2] floats): the (a, o) table of
+ *   the fused GroupNorm conv for the same inputs and statistics, y = silu?(x * a + o).
+ * cdx_op_layernorm_ex: cdx_op_layernorm plus the tracked range slot of y in amax_out (optional, device float).
+ * cdx_op_softmax_rows: in-place softmax over `rows` rows of length L (row stride ld); causal_nq > 0: row r sees only columns
+ *   j <= r % causal_nq, the others become exactly 0.
+ * cdx_op_produce_norm: a producer GEMM with its GroupNorm side outputs, then the GroupNorm that trusts them.  conv == 0: linear,
+ *   x [B*H*W, Cin] @ w[Cout, Cin]^T + bias; conv == 1: stride-1 pad-1 conv3x3 of NHWC x [B,H,W,Cin] with w OIHW [Cout,Cin,3,3].
+ *   y [B*H*W, Cout] receives the product, amax_out (device float) its range slot, stats_out (device [B, Cout, 2] doubles) its
+ *   per-(image, channel) {sum, sum of squares} -- from the epilogue or, where it cannot, the standalone pass -- and yn (device
+ *   [B*H*W, Cout]) GroupNorm(32)(y) with those statistics (eps, no SiLU).  *path_out (host): how the statistics were made --
+ *   0 FFMA tiles + standalone pass, 1 fused into the tensor-core epilogue, 2 tensor cores + standalone pass, 3 split-K reduce +
+ *   standalone pass. */
+int cdx_op_groupnorm_ex(cdx_engine* e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta,
+                        float eps, int silu, const float* scale, const float* shift, int ld_ss, float* y, float* amax_out,
+                        float* ab_out, int B, int HW, void* stream);
+int cdx_op_layernorm_ex(cdx_engine* e, const float* x, const float* gamma, const float* beta, float* y, float* amax_out, int M,
+                        int C, void* stream);
+int cdx_op_softmax_rows(cdx_engine* e, float* x, int64_t rows, int L, int ld, int causal_nq, void* stream);
+int cdx_op_produce_norm(cdx_engine* e, const float* x, const float* w, const float* bias, int conv, int B, int H, int W, int Cin,
+                        int Cout, const float* gamma, const float* beta, float eps, float* y, float* amax_out, double* stats_out,
+                        float* yn, int* path_out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1009,20 +1009,20 @@ int cdx_op_groupnorm_ex(cdx_engine* eh, const float* x1, int C1, const float* x2
     CDX_CHECK(eh && x1 && gamma && beta && y && B > 0 && HW > 0 && C1 > 0 && C2 >= 0 && (C2 == 0) == (x2 == nullptr),
               "op_groupnorm_ex: bad arguments");
     CDX_CHECK(!scale == !shift && (!scale || ld_ss >= C1 + C2), "op_groupnorm_ex: scale and shift go together, with ld_ss >= C");
+    CDX_CHECK(((uintptr_t)ab_out & 7) == 0, "op_groupnorm_ex: ab_out must be 8-byte aligned");
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
     with_arena(e, s, [&] {
       Scope sc(e.arena);
       e.pools_reset(s);
-      // the statistics of sources whose producer did not fuse them (one pass each), shared by the norm and the table
+      // the statistics of sources whose producer did not fuse them (one pass each)
       const double* st1 = gn_channel_stats(e, x1, C1, B, HW, s);
       const double* st2 = x2 ? gn_channel_stats(e, x2, C2, B, HW, s) : nullptr;
       float* slot = e.amax_slot();
-      groupnorm(e, x1, C1, x2, C2, gamma, beta, eps, silu_ != 0, scale, shift, ld_ss, y, B, HW, s, st1, st2, slot);
-      const float* ab = ab_out ? gn_affine(e, x1, C1, x2, C2, gamma, beta, eps, scale, shift, ld_ss, B, HW, s, st1, st2) : nullptr;
+      groupnorm(e, x1, C1, x2, C2, gamma, beta, eps, silu_ != 0, scale, shift, ld_ss, y, B, HW, s, st1, st2, slot,
+                reinterpret_cast<float2*>(ab_out));
       if (e.dry()) return;
       if (amax_out) CDX_CUDA(cudaMemcpyAsync(amax_out, slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
-      if (ab_out) CDX_CUDA(cudaMemcpyAsync(ab_out, ab, (size_t)B * (C1 + C2) * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     });
   });
 }

@@ -141,7 +141,7 @@ struct GemmArgs {
   int M = 0, N = 0, K = 0;
   int mode = 0;                       // 0 dense rows, 1 conv3x3 gather
   const float* A = nullptr;  int lda = 0;  int C1 = 0;   // first source: C1 channels, row/pixel stride lda
-  const float* A2 = nullptr; int lda2 = 0; int C2 = 0;   // optional second source (channel concat)
+  const float* A2 = nullptr; int lda2 = 0; int C2 = 0;   // optional second source (channel concat; dense mode only)
   // conv geometry (mode 1): stored input [B,Hin,Win,*], logical input is up x larger (nearest)
   int Hin = 0, Win = 0, Hout = 0, Wout = 0, stride = 1, pad = 1, up = 1;
   const float* Bw = nullptr; int ldb = 0; int b_kn = 0;   // weights [N][K] (b_kn=0) or [K][N] (b_kn=1)
@@ -151,10 +151,6 @@ struct GemmArgs {
   const void* Bw_h_hi = nullptr; const void* Bw_h_lo = nullptr; int b_exp = 0;
   const float* a_amax = nullptr; const float* a2_amax = nullptr;
   float* c_amax = nullptr;
-  // conv3x3 halo schedule only: the A operand is silu?(x * a + o) with the per-(image, channel) table gn_ab [B, C1+C2] of float2 --
-  // GroupNorm (+SiLU) of the input applied while the halo is converted; padding pixels stay exactly 0 (the reference pads the
-  // normalised tensor).  A2 / C2: second source of a channel concat (C1 % 64 == 0)
-  const float* gn_ab = nullptr; int gn_silu = 0;
   double* c_stats = nullptr;         // optional: += per-(image, channel) {sum, sum sq} of C (rows_per_batch rows per image), zeroed by the caller
   float* Cout = nullptr; int ldc = 0;
   float* Cout_lo = nullptr;           // if set: Cout receives rn_tf32(C) and Cout_lo rn_tf32(C - hi) (operand planes for the tensor-core kernels)
@@ -209,14 +205,10 @@ bool attention_tc(Engine& e, const float* q, int ldq, const float* k, int ldk, i
 // GroupNorm(32) over NHWC, optionally over the channel-concat of two sources; y = [silu]( gn(x)*(1+scale)+shift )
 // st1 / st2: per-(image, channel) fp64 {sum, sum of squares} of the sources when their producer already accumulated them
 // (stats[(b*C + c)*2 + k]); null -> computed here by one extra read.  amax: optional device scalar <- atomic max |y|.
+// ab_out: optional [B, C1+C2] table of the (a, o) the norm applies, y = silu?(x*a + o).
 void groupnorm(Engine& e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta,
                float eps, bool silu, const float* scale, const float* shift, int ld_ss, float* y, int B, int HW,
-               cudaStream_t s, const double* st1 = nullptr, const double* st2 = nullptr, float* amax = nullptr);
-// the GroupNorm's per-(image, channel) affine table [B, C1+C2] of (a, o), y = x*a + o, for a conv that applies norm (+SiLU) itself
-const float* gn_affine(Engine& e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta, float eps,
-                       const float* scale, const float* shift, int ld_ss, int B, int HW, cudaStream_t s, const double* st1, const double* st2);
-// can a stride-1 conv3x3 over [B,H,W,C1(+C2)] take the halo schedule (and with it a fused GroupNorm + SiLU of its input)?
-bool conv_halo_eligible(const Engine& e, int B, int H, int W, int C1, int C2, int Cout, bool out_nchw);
+               cudaStream_t s, const double* st1 = nullptr, const double* st2 = nullptr, float* amax = nullptr, float2* ab_out = nullptr);
 double* gn_channel_stats(Engine& e, const float* x, int C, int B, int HW, cudaStream_t s);
 void gn_channel_stats_into(Engine& e, const float* x, int C, int B, int HW, double* stats, cudaStream_t s);   // stats += (zeroed by the caller)
 void layernorm(Engine& e, const float* x, const float* gamma, const float* beta, float* y, int M, int C, cudaStream_t s, float* amax = nullptr);

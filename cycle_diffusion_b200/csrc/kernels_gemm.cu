@@ -315,6 +315,7 @@ void gemm(Engine& e, const GemmArgs& a, cudaStream_t s, int* route) {
   CDX_CHECK(a.M > 0 && a.N > 0 && a.K > 0, "gemm: empty problem M=%d N=%d K=%d", a.M, a.N, a.K);
   CDX_CHECK(a.batch >= 1 && a.heads >= 1, "gemm: bad batch");
   if (a.mode == 1) CDX_CHECK(a.K == 9 * (a.C1 + a.C2), "conv3x3: K != 9*Cin");
+  if (a.mode == 1) CDX_CHECK(!a.A2, "conv3x3: one input source only (M=%d N=%d)", a.M, a.N);
   if (a.mode == 0) CDX_CHECK(a.K == a.C1 + a.C2, "dense: K != C1+C2");
   if (e.mma_mode == 1) {
     int done = 0;                                          // bit 0: c_amax written, bit 1: c_stats written
@@ -325,8 +326,6 @@ void gemm(Engine& e, const GemmArgs& a, cudaStream_t s, int* route) {
     }
   }
   if (route) *route = 0;
-  CDX_CHECK(!a.gn_ab && !(a.mode == 1 && a.A2), "gemm: a fused-GroupNorm / concat conv3x3 reached the FFMA back end (M=%d N=%d): the caller must ask conv_halo_eligible()",
-            a.M, a.N);
   if (a.c_amax || a.c_stats) {
     GemmArgs b = a;
     b.c_amax = nullptr; b.c_stats = nullptr;

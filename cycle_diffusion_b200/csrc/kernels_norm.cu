@@ -83,13 +83,15 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
 }
 
 // grid (row chunks, B); thread (tr, tc) owns channel vectors tc, tc+ncol, ... (so group / affine coefficients are hoisted out
-// of the row loop) and walks the chunk's rows 4 at a time.  Dynamic smem: float2 (sc, sh) per channel.
+// of the row loop) and walks the chunk's rows 4 at a time.  Dynamic smem: float2 (sc, sh) per channel.  ab_out (optional): the
+// first row chunk of each image stores that table, ab_out[b*C + c] = (a, o) with y = silu?(x * a + o).
 __global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, const float* x2, int C2,
                                                        const float* gamma, const float* beta,
                                                        const double* st1, const double* st2, double inv_count,
                                                        float eps, int silu,
                                                        const float* scale, const float* shift,
-                                                       int ld_ss, float* y, int HW, int rows_per_chunk, float* amax) {
+                                                       int ld_ss, float* y, int HW, int rows_per_chunk, float* amax,
+                                                       float2* ab_out) {
   tc::pdl_trigger();
   tc::pdl_wait();
   const int C = C1 + C2;
@@ -137,6 +139,8 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, 
     s_aff[c] = make_float2(a, o);
   }
   __syncthreads();
+  if (ab_out && blockIdx.x == 0)
+    for (int c = threadIdx.x; c < C; c += blockDim.x) ab_out[(long long)b * C + c] = s_aff[c];
   float vmax = 0.f;
   if (tr < nrow_par) {
     for (int c4 = tc; c4 < C4; c4 += ncol) {
@@ -167,51 +171,6 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, 
     }
   }
   if (amax) block_amax(vmax, amax);
-}
-
-// The per-(image, channel) affine table of a GroupNorm, ab[b*C + c] = (a, o) with y = x * a + o -- exactly the table gn_apply_kernel
-// builds in shared memory -- written to HBM for a consumer that applies the norm itself: the conv3x3 kernel's halo conversion
-// (kernels_tc.cu), which turns GroupNorm + SiLU on the ResBlock path into arithmetic on data that is already in shared memory.
-__global__ void __launch_bounds__(256) gn_affine_kernel(int C1, int C2, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                        const double* __restrict__ st1, const double* __restrict__ st2, double inv_count, float eps,
-                                                        const float* __restrict__ scale, const float* __restrict__ shift, int ld_ss,
-                                                        float2* __restrict__ ab) {
-  const int C = C1 + C2;
-  const int cpg = C / GN_GROUPS;
-  const int b = blockIdx.x;
-  __shared__ float mean_rstd[GN_GROUPS * 2];
-  {
-    const int g = threadIdx.x >> 3, l8 = threadIdx.x & 7;     // 8 threads per group
-    double s = 0.0, q = 0.0;
-    for (int j = l8; j < cpg; j += 8) {
-      const int c = g * cpg + j;
-      const double* o = (c < C1) ? st1 + ((long long)b * C1 + c) * 2 : st2 + ((long long)b * C2 + (c - C1)) * 2;
-      s += o[0];
-      q += o[1];
-    }
-#pragma unroll
-    for (int o = 4; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
-    if (l8 == 0) {
-      const double mean = s * inv_count;
-      double var = q * inv_count - mean * mean;
-      if (var < 0.0) var = 0.0;
-      mean_rstd[g * 2 + 0] = (float)mean;
-      mean_rstd[g * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
-    }
-  }
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const int g = c / cpg;
-    const float mean = mean_rstd[g * 2 + 0], rstd = mean_rstd[g * 2 + 1];
-    float a = rstd * gamma[c];
-    float o = beta[c] - mean * a;
-    if (scale) {
-      const float s1 = 1.f + scale[(long long)b * ld_ss + c];
-      a *= s1;
-      o = o * s1 + shift[(long long)b * ld_ss + c];
-    }
-    ab[(long long)b * C + c] = make_float2(a, o);
-  }
 }
 
 // one warp per row, the row held in registers (NV float4 per lane: C <= 128 NV): one read, one write.  Persistent warps walk the
@@ -335,7 +294,7 @@ void gn_channel_stats_into(Engine& e, const float* x, int C, int B, int HW, doub
 
 void groupnorm(Engine& e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta, float eps,
                bool silu, const float* scale, const float* shift, int ld_ss, float* y, int B, int HW, cudaStream_t s,
-               const double* st1, const double* st2, float* amax) {
+               const double* st1, const double* st2, float* amax, float2* ab_out) {
   const int C = C1 + C2;
   CDX_CHECK(C % GN_GROUPS == 0, "groupnorm: C=%d not divisible by 32", C);
   CDX_CHECK(C1 % 4 == 0 && C2 % 4 == 0, "groupnorm: channel counts must be multiples of 4 (C1=%d C2=%d)", C1, C2);
@@ -348,23 +307,9 @@ void groupnorm(Engine& e, const float* x1, int C1, const float* x2, int C2, cons
   const int arows = cdiv(HW, achunk);
   achunk = cdiv(HW, arows);
   tc::launch_ex(gn_apply_kernel, dim3((unsigned)achunk, (unsigned)B), dim3(256), (size_t)C * sizeof(float2), s, 1, x1, C1, x2, C2, gamma, beta, st1, st2,
-                1.0 / ((double)HW * (C / GN_GROUPS)), eps, silu ? 1 : 0, scale, shift, ld_ss, y, HW, arows, amax);
+                1.0 / ((double)HW * (C / GN_GROUPS)), eps, silu ? 1 : 0, scale, shift, ld_ss, y, HW, arows, amax, ab_out);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
-}
-
-const float* gn_affine(Engine& e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta, float eps,
-                       const float* scale, const float* shift, int ld_ss, int B, int HW, cudaStream_t s, const double* st1, const double* st2) {
-  const int C = C1 + C2;
-  CDX_CHECK(C % GN_GROUPS == 0 && C1 % 4 == 0 && C2 % 4 == 0, "gn_affine: C1=%d C2=%d", C1, C2);
-  if (!st1) st1 = gn_channel_stats(e, x1, C1, B, HW, s);
-  if (x2 && !st2) st2 = gn_channel_stats(e, x2, C2, B, HW, s);
-  float2* ab = (float2*)e.arena.alloc((size_t)B * C * sizeof(float2));
-  if (e.dry()) return reinterpret_cast<const float*>(ab);
-  gn_affine_kernel<<<B, 256, 0, s>>>(C1, C2, gamma, beta, st1, st2, 1.0 / ((double)HW * (C / GN_GROUPS)), eps, scale, shift, ld_ss, ab);
-  CDX_CUDA(cudaGetLastError());
-  e.launches++;
-  return reinterpret_cast<const float*>(ab);
 }
 
 void layernorm(Engine& e, const float* x, const float* gamma, const float* beta, float* y, int M, int C, cudaStream_t s, float* amax) {

@@ -80,15 +80,12 @@ struct Cfg {
 struct TcParams {
   int M, N, K;
   int mode;                 // 0 dense, 1 conv3x3, 2 batched dense
-  int C1, C2;               // channels of source 1 / 2 (k-blocks never straddle: C1 % 32 == 0 when C2 > 0)
-  int Cin;                  // conv: input channels (multiple of 32)
+  int C1, C2;               // channels of source 1 / 2 (dense: k-blocks never straddle, C1 % 32 == 0 when C2 > 0; conv: one
+                            // source, C1 = input channels, a multiple of 32)
   int H, W, B;              // conv: spatial size of the output and batch
   int bw, bh, bn;           // conv: pixel box of one M tile (bw*bh*bn == 128)
   int tiles_x, tiles_y;     // conv: tiles per row / column (cdiv: a tile may overhang the map; its outside rows are masked)
   int cstride, cpad;        // conv: stride (1 or 2: TMA element traversal stride) and low-side padding
-  // conv3x3, optional: the A operand is silu?(x * a + o), (a, o) = gn_ab[b * Cin + c] (GroupNorm of the input applied while A is
-  // split; out-of-image pixels stay 0, as the reference pads the normalised tensor).  C1 < Cin: channels >= C1 come from mapA2
-  const float2* gn_ab; int gn_silu;
   float* C; int ldc;
   float* C_lo;              // optional: C <- rn_tf32(result), C_lo <- rn_tf32(result - hi)
   float* Ct_hi; float* Ct_lo; int t_col0; long long ldt;   // optional transposed plane output for columns >= t_col0
@@ -119,7 +116,6 @@ struct TcParams {
 };
 
 __device__ __forceinline__ int h16_a_exp(const TcParams& p) {
-  if (p.gn_ab) return 0;         // normalised (+SiLU) activations are O(1..100): inside the no-rescale range by construction
   float m = p.a_amax ? *p.a_amax : 0.f;
   if (p.a2_amax) m = fmaxf(m, *p.a2_amax);
   return h16_exp_of(m);
@@ -198,7 +194,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     // =========================================================================== TMA producer
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
-      const int cblocks = p.mode == 1 ? p.Cin / TBK : 0;
+      const int cblocks = p.mode == 1 ? p.C1 / TBK : 0;
       int it = 0;
       for (int kb = tc_.kb0; kb < tc_.kb1; ++kb, ++it) {
         const int s = it % STAGES;
@@ -226,9 +222,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         } else {
           const int tap = kb / cblocks, cb = kb - tap * cblocks;
           const int dy = tap / 3, dx = tap - dy * 3;
-          const int c = cb * TBK;                                 // channel concat: blocks >= C1 come from the second source
-          tma_load_4d(st, c < p.C1 ? &mapA : &mapA2, c < p.C1 ? c : c - p.C1, tc_.x0 * p.cstride + dx - p.cpad,
-                      tc_.y0 * p.cstride + dy - p.cpad, tc_.b0, bar_full(s));        // OOB -> zeros = padding
+          tma_load_4d(st, &mapA, cb * TBK, tc_.x0 * p.cstride + dx - p.cpad, tc_.y0 * p.cstride + dy - p.cpad, tc_.b0,
+                      bar_full(s));                                                   // OOB -> zeros = padding
         }
         tma_load_2d(sb, &mapB, k0, tc_.n0, bar_full(s));
         if (KIND != KIND_SS) tma_load_2d(sb + B_PLANE, &mapBlo, k0, tc_.n0, bar_full(s));
@@ -245,8 +240,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const int ea = H16 ? h16_a_exp(p) : 0;
   const float asc = exp2i(ea);
   const int kchunk = (tc_.kb1 - tc_.kb0) <= 2 * CF::KCHUNK ? 2 * CF::KCHUNK : CF::KCHUNK;
-  const int cblocks = p.mode == 1 ? p.Cin / TBK : 1;
-  // conv + fused GroupNorm: pixel of each of this thread's two rows
+  // conv: pixel of each of this thread's two rows (the epilogue masks rows outside the map)
   int px[2] = {0, 0}, py[2] = {0, 0}, pb[2] = {0, 0};
   if (p.mode == 1) {
 #pragma unroll
@@ -287,13 +281,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
       asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    // fused GroupNorm: tap / channel block of this stage
-    int tap = 0, cbase = 0;
-    if (H16 && p.gn_ab) {
-      const int kq = tc_.kb0 + it;
-      tap = kq / cblocks;
-      cbase = (kq - tap * cblocks) * TBK;
-    }
 #pragma unroll
     for (int kk = 0; kk < KSTEPS; ++kk) {
       if (H16) {
@@ -306,18 +293,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
             float2 x;
             asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x.x), "=f"(x.y)
                          : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
-            if (p.gn_ab) {
-              const int yy = py[i] + tap / 3 - 1, xx = px[i] + tap % 3 - 1;
-              const bool inside = xx >= 0 && xx < p.W && yy >= 0 && yy < p.H && pb[i] < p.B;
-              if (inside) {
-                const float2 a0 = p.gn_ab[(long long)pb[i] * p.Cin + cbase + k], a1 = p.gn_ab[(long long)pb[i] * p.Cin + cbase + k + 1];
-                x.x = fmaf(x.x, a0.x, a0.y);
-                x.y = fmaf(x.y, a1.x, a1.y);
-                if (p.gn_silu) { x.x = __fdividef(x.x, 1.f + __expf(-x.x)); x.y = __fdividef(x.y, 1.f + __expf(-x.y)); }
-              } else {
-                x.x = 0.f; x.y = 0.f;
-              }
-            }
             if (ea != 0) { x.x *= asc; x.y *= asc; }
             const __half2 h = __floats2half2_rn(x.x, x.y);       // .x (low half) = even k
             f.h[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&h);
@@ -765,17 +740,6 @@ bool attention_tc(Engine& e, const float* q, int ldq, const float* k, int ldk, i
   return true;
 }
 
-bool conv_halo_eligible(const Engine& e, int B, int H, int W, int C1, int C2, int Cout, bool out_nchw) {
-  // Can a stride-1 conv3x3 over [B,H,W,C1(+C2)] take its input's GroupNorm (+SiLU) and a channel concat inside the A-operand split?
-  // Opt-in (CDX_GN_FUSION=1): every N tile of a conv re-applies the norm and the SiLU (two MUFU ops per element) while splitting A,
-  // which puts the conversion back on the critical path of the wide convs.
-  static const bool no_fuse = getenv("CDX_GN_FUSION") == nullptr;
-  const long long M = (long long)B * H * W;
-  if (no_fuse || e.mma_mode != 1 || e.tc_kind < 1 || !pow2(H) || !pow2(W) || (C1 % 64) || (C2 % 64) || M < 64) return false;
-  if ((Cout < 32 && M < 2048) || (!out_nchw && (Cout & 3))) return false;       // (the shapes gemm_tc leaves to the FFMA tiles)
-  return true;
-}
-
 // Pixel box of a conv3x3 M tile for an output map whose sides are not both powers of two: bw x bh pixels of bn images, bw*bh*bn == 128,
 // so every factor is a power of two and the box generally overhangs the map.  The box that covers [B, H, W] with the fewest tiles
 // wins (fewest masked rows); ties go to the smallest halo per tile, bn * (bw + 2) * (bh + 2) pixels fetched (then the wider box: longer
@@ -846,13 +810,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
     }
     p.tiles_m = cdiv(a.M, TBM);
   } else {
-    const int Cin = a.C1 + (a.A2 ? a.C2 : 0);
     if ((a.stride != 1 && a.stride != 2) || a.up != 1) return false;
-    if (Cin % TBK) return false;
-    // a channel-concat input or a fused GroupNorm: the caller asks conv_halo_eligible() first
-    const bool fused_in = a.A2 != nullptr || a.gn_ab != nullptr;
-    CDX_CHECK(!a.A2 || a.gn_ab, "conv3x3: a channel-concat input is only supported together with the fused GroupNorm");
-    CDX_CHECK(!fused_in || (a.stride == 1 && a.pad == 1 && (a.C1 % TBK) == 0), "conv3x3: concat / fused GroupNorm input needs stride 1, pad 1, C1 %% 32 == 0");
+    if (a.C1 % TBK) return false;
     if (a.Hin != a.Hout * a.stride || a.Win != a.Wout * a.stride) return false;
     const int B = a.M / (a.Hout * a.Wout);
     int bw, bh, bn;
@@ -861,11 +820,10 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
       bh = a.Hout < TBM / bw ? a.Hout : TBM / bw;
       bn = TBM / (bw * bh);
     } else {
-      CDX_CHECK(!fused_in, "conv3x3: fused GroupNorm / concat input on a %dx%d map (power-of-two maps only)", a.Hout, a.Wout);
       conv_ragged_tile(a.Wout, a.Hout, B, a.stride, &bw, &bh, &bn);
     }
     if (bn > 256 || bw * a.stride > 256 || bh * a.stride > 256) return false;
-    p.mode = 1; p.Cin = Cin; p.H = a.Hout; p.W = a.Wout; p.B = B;      // H, W: OUTPUT grid (tile -> row mapping)
+    p.mode = 1; p.C1 = a.C1; p.H = a.Hout; p.W = a.Wout; p.B = B;      // H, W: OUTPUT grid (tile -> row mapping)
     p.bw = bw; p.bh = bh; p.bn = bn;
     p.cstride = a.stride; p.cpad = a.pad;
     p.tiles_x = cdiv(a.Wout, bw); p.tiles_y = cdiv(a.Hout, bh);
@@ -874,24 +832,15 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
     // stride 2 (Downsample convs): TMA traverses every 2nd pixel; box = 2x the number of pixels wanted
     uint32_t bx[4] = {TBK, (uint32_t)(bw * a.stride), (uint32_t)(bh * a.stride), (uint32_t)bn};
     uint32_t es[4] = {1, (uint32_t)a.stride, (uint32_t)a.stride, 1};
-    p.C1 = a.C1;
-    p.gn_ab = reinterpret_cast<const float2*>(a.gn_ab); p.gn_silu = a.gn_silu;
     mA = &get_map(a.A, 4, d, st, bx, es);
     mA2 = mA;
-    if (a.A2) {
-      CDX_CHECK(a16(a.A2) && (a.lda2 & 3) == 0, "conv3x3: misaligned second source");
-      uint64_t d2[4] = {(uint64_t)a.C2, (uint64_t)a.Win, (uint64_t)a.Hin, (uint64_t)B};
-      uint64_t st2[3] = {(uint64_t)a.lda2 * 4, (uint64_t)a.lda2 * 4 * a.Win, (uint64_t)a.lda2 * 4 * a.Win * a.Hin};
-      mA2 = &get_map(a.A2, 4, d2, st2, bx, es);
-    }
     p.tiles_m = p.tiles_x * p.tiles_y * cdiv(B, bn);
   }
   // ---- operand path: fp16-split (KIND_H16) when the engine selects it, the weights have fp16 planes and the geometry allows it
   // (K a multiple of 32: whole 32-K ring stages; fp16 B rows 16-byte aligned); else TF32 planes (KIND_TS); else SS
   const bool ts = a.Bw_hi != nullptr && a.Bw_lo != nullptr && a16(a.Bw_hi) && a16(a.Bw_lo);
   const bool h16 = e.tc_kind >= 1 && a.Bw_h_hi && a.Bw_h_lo && a16(a.Bw_h_hi) && a16(a.Bw_h_lo) && (a.K % TBK) == 0 && (a.ldb % 8) == 0 &&
-                   (a.mode == 1 || !a.A2 || (a.C2 % TBK) == 0);
-  CDX_CHECK(!(a.mode == 1 && (a.A2 || a.gn_ab)) || h16, "conv3x3: concat / fused GroupNorm input without the fp16-split path");
+                   (!a.A2 || (a.C2 % TBK) == 0);
   // The planner counts fp16-split work in 64-K blocks (its cost constants are per 64 K), so its choice of (w, S) -- and with it the
   // split-K boundaries -- does not depend on the ring's stage size; kb_per_split is converted to 32-K stages below.
   const int bk = h16 ? 64 : TBK;
@@ -946,13 +895,13 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   if (h16) {
     p.a_amax = a.a_amax;
     p.a2_amax = a.A2 ? a.a2_amax : nullptr;
-    if (!p.a_amax && !p.gn_ab) {
+    if (!p.a_amax) {
       float* slot = e.amax_slot();
       if (a.mode == 1) amax_rows(e, a.A, (long long)(a.M / (a.Hout * a.Wout)) * a.Hin * a.Win, a.C1, a.lda, slot, s);
       else amax_rows(e, a.A, a.M, a.C1, a.lda, slot, s);
       p.a_amax = slot;
     }
-    if (a.A2 && !p.a2_amax && !p.gn_ab && a.mode == 0) {
+    if (a.A2 && !p.a2_amax) {
       float* slot = e.amax_slot();
       amax_rows(e, a.A2, a.M, a.C2, a.lda2, slot, s);
       p.a2_amax = slot;
@@ -982,8 +931,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   ensure_attr(e.device);
   ProfScope ps(e, s, a.mode == 1 ? PROF_CONV_TC : PROF_DENSE_TC, 2.0 * a.M * a.N * a.K,
                4.0 * ((double)a.M * a.K / (a.mode == 1 ? 9 : 1) + (double)a.N * a.K + (double)a.M * a.N), 1);
-  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s%s box%dx%dx%d", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
-          p.gn_ab ? " gn" : "", a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "", p.bw, p.bh, p.bn);
+  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s box%dx%dx%d", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
+          a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "", p.bw, p.bh, p.bn);
   if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (fast) launch_gemm<KIND_H16_FAST, 64>(p, *mA, *mA2, *mB, *mBlo, s);
   else if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, s);

@@ -550,9 +550,10 @@ struct Exec {
 
   void track(Tensor& t, GemmArgs& g, bool stats) { track_outputs(e, t, g, stats); }
 
-  // y = conv3x3(x [, x2 concat]) + bias (+ rowvec per sample) (+ residual); up: nearest-2x folded into the gather
+  // y = conv3x3(x) + bias (+ rowvec per sample) (+ residual); up: nearest-2x folded into the gather
+  // out_nchw (optional): store y there in NCHW layout; into (optional): preallocated NHWC output, its range and statistics tracked
   Tensor conv3(const Tensor& x0, const std::string& name, int stride = 1, int pad = 1, int up = 1, const float* rowvec = nullptr,
-               int ld_rowvec = 0, const float* residual = nullptr, float* out_nchw = nullptr) {
+               int ld_rowvec = 0, const float* residual = nullptr, float* out_nchw = nullptr, Tensor* into = nullptr) {
     const Param& w = n.param(name + ".weight");
     const int Cout = (int)w.dims[0];
     CDX_CHECK((int)w.dims[1] == x0.C, "conv %s: input has %d channels, weight expects %d", name.c_str(), x0.C, (int)w.dims[1]);
@@ -569,7 +570,7 @@ struct Exec {
       Tensor xu = alloc(x.B, x.H * 2, x.W * 2, x.C);
       upsample2(e, x.p, xu.p, x.B, x.H, x.W, x.C, s);
       xu.amax = x.amax;
-      return conv3(xu, name, stride, pad, 1, rowvec, ld_rowvec, residual, out_nchw);
+      return conv3(xu, name, stride, pad, 1, rowvec, ld_rowvec, residual, out_nchw, into);
     }
     const int Hl = x.H * up, Wl = x.W * up;
     int Ho, Wo;
@@ -577,6 +578,7 @@ struct Exec {
     else { Ho = Hl / 2; Wo = Wl / 2; }
     Tensor y;
     if (out_nchw) { y.p = out_nchw; y.B = x.B; y.H = Ho; y.W = Wo; y.C = Cout; }
+    else if (into) y = *into;
     else y = alloc(x.B, Ho, Wo, Cout);
     GemmArgs g;
     g.mode = 1;
@@ -592,6 +594,7 @@ struct Exec {
     else track(y, g, true);
     g.a_amax = x.amax;
     run(g);
+    if (into) *into = y;
     return y;
   }
 
@@ -644,58 +647,13 @@ struct Exec {
   }
 
   // GroupNorm(32)(+ scale-shift) + SiLU + conv3x3 (stride 1, pad 1) of x (optionally the channel concat [x | x2]): the ResBlock pattern
-  // of all four network families (OAI:255-275, IU:241-261, AEM:121-141, ddpm/diffusion.py:117-139).  When the conv can take the halo
-  // schedule the norm and the activation are applied INSIDE the conv kernel while it converts the halo box that TMA staged in shared
-  // memory: the normalised tensor never exists in HBM (one read of x instead of read + write + read), and the concat is never
-  // materialised either.  Otherwise: the standalone GroupNorm kernel, then the conv.  `into` (optional): preallocated output.
+  // of all four network families (OAI:255-275, IU:241-261, AEM:121-141, ddpm/diffusion.py:117-139).  The GroupNorm kernel reads
+  // both sources and writes the normalised concat, which the conv then reads as its one source.  `into` (optional): preallocated output.
   Tensor gn_silu_conv3(const Tensor& x, const Tensor* x2, const std::string& norm, float eps, const std::string& conv, const float* scale = nullptr,
                        const float* shift = nullptr, int ld_ss = 0, const float* rowvec = nullptr, int ld_rowvec = 0, const float* residual = nullptr,
                        Tensor* into = nullptr, float* out_nchw = nullptr) {
-    const Param& w = n.param(conv + ".weight");
-    const int Cout = (int)w.dims[0], Cin = x.C + (x2 ? x2->C : 0);
-    CDX_CHECK((int)w.dims[1] == Cin, "conv %s: input has %d channels, weight expects %d", conv.c_str(), Cin, (int)w.dims[1]);
-    const bool fused = !w.cin_pad && n.planes_valid && conv_halo_eligible(e, x.B, x.H, x.W, x.C, x2 ? x2->C : 0, Cout, out_nchw != nullptr);
-    if (!fused) {
-      Tensor h = gn(x, x2, norm, eps, true, scale, shift, ld_ss);
-      if (!into) return conv3(h, conv, 1, 1, 1, rowvec, ld_rowvec, residual, out_nchw);
-      GemmArgs g;
-      g.mode = 1;
-      g.M = h.rows(); g.N = Cout; g.K = 9 * h.C;
-      g.A = h.p; g.lda = h.C; g.C1 = h.C;
-      g.Hin = h.H; g.Win = h.W; g.Hout = h.H; g.Wout = h.W; g.stride = 1; g.pad = 1; g.up = 1;
-      g.Bw = n.blob + w.off; g.ldb = 9 * h.C;
-      g.Cout = into->p; g.ldc = Cout;
-      g.bias = n.P(conv + ".bias");
-      g.rowvec = rowvec; g.ld_rowvec = ld_rowvec; g.rows_per_batch = h.H * h.W;
-      g.residual = residual; g.ldr = Cout;
-      g.a_amax = h.amax;
-      track(*into, g, true);
-      run(g);
-      return *into;
-    }
-    const float* ab = gn_affine(e, x.p, x.C, x2 ? x2->p : nullptr, x2 ? x2->C : 0, n.P(norm + ".weight"), n.P(norm + ".bias"), eps, scale, shift, ld_ss,
-                                x.B, x.H * x.W, s, x.stats, x2 ? x2->stats : nullptr);
-    Tensor y;
-    if (out_nchw) { y.p = out_nchw; y.B = x.B; y.H = x.H; y.W = x.W; y.C = Cout; }
-    else if (into) y = *into;
-    else y = alloc(x.B, x.H, x.W, Cout);
-    GemmArgs g;
-    g.mode = 1;
-    g.M = x.rows(); g.N = Cout; g.K = 9 * Cin;
-    g.A = x.p; g.lda = x.C; g.C1 = x.C;
-    if (x2) { g.A2 = x2->p; g.lda2 = x2->C; g.C2 = x2->C; }
-    g.gn_ab = ab; g.gn_silu = 1;
-    g.Hin = x.H; g.Win = x.W; g.Hout = x.H; g.Wout = x.W; g.stride = 1; g.pad = 1; g.up = 1;
-    g.Bw = n.blob + w.off; g.ldb = 9 * Cin;
-    g.Cout = y.p; g.ldc = Cout;
-    g.bias = n.P(conv + ".bias");
-    g.rowvec = rowvec; g.ld_rowvec = ld_rowvec; g.rows_per_batch = x.H * x.W;
-    g.residual = residual; g.ldr = Cout;
-    if (out_nchw) { g.out_nchw = 1; g.rows_per_img = x.H * x.W; }
-    else track(y, g, true);
-    run(g);
-    if (into) *into = y;
-    return y;
+    const Tensor h = gn(x, x2, norm, eps, true, scale, shift, ld_ss);
+    return conv3(h, conv, 1, 1, 1, rowvec, ld_rowvec, residual, out_nchw, into);
   }
 
   // AttnBlock (AEM:178-202): single head, d = C, scale C^-1/2

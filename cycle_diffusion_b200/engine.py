@@ -285,7 +285,7 @@ class Engine:
         """GroupNorm(32) of the channel concat [x1 | x2] (NHWC [B,H,W,C1], [B,H,W,C2] or None) as the network executors run it,
         optional gn(x) * (1 + scale) + shift and SiLU.  scale / shift: [B, C] device views with unit column stride and one common
         row stride (e.g. the two halves of a [B, 2C] embedding projection).  Returns (y, amax, ab): y [B,H,W,C], amax [1] the
-        tracked range slot of y, ab [B, C, 2] the fused conv's (a, o) table, y = silu?(x * a + o)."""
+        tracked range slot of y, ab [B, C, 2] the (a, o) table the norm applies, y = silu?(x * a + o)."""
         x1, gamma, beta = (_f32c(t, self.device) for t in (x1, gamma, beta))
         B, H, W, C1 = x1.shape
         x2 = _f32c(x2, self.device) if x2 is not None else None

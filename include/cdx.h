@@ -435,8 +435,8 @@ int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, i
 /* The normalisation kernels in the forms the network executors call them, with their side outputs (tests/test_norms_gpu.py).
  * cdx_op_groupnorm_ex: GroupNorm(32) over the channel concat [x1 | x2] (NHWC [B,HW,C1] and [B,HW,C2]; x2 NULL when C2 == 0), then
  *   optionally * (1 + scale) + shift (scale / shift [B, ld_ss] or NULL) and SiLU -> y [B,HW,C1+C2].  amax_out (optional, device
- *   float): the tracked range slot of y as the norm left it.  ab_out (optional, device [B, C1+C2, 2] floats): the (a, o) table of
- *   the fused GroupNorm conv for the same inputs and statistics, y = silu?(x * a + o).
+ *   float): the tracked range slot of y as the norm left it.  ab_out (optional, device [B, C1+C2, 2] floats): the (a, o) table
+ *   the norm applies, y = silu?(x * a + o).
  * cdx_op_layernorm_ex: cdx_op_layernorm plus the tracked range slot of y in amax_out (optional, device float).
  * cdx_op_softmax_rows: in-place softmax over `rows` rows of length L (row stride ld); causal_nq > 0: row r sees only columns
  *   j <= r % causal_nq, the others become exactly 0.

@@ -5,8 +5,9 @@ torch.nn.functional where torch has the operation).
 Forms covered: two-source GroupNorm over the never-materialised U-Net skip concat, including groups that straddle the two
 sources; the improved-DDPM scale-shift norm gn(x)*(1+scale)+shift with scale / shift rows of stride 2C; SiLU; GroupNorm statistics
 made by the producing GEMM's epilogue (or, where it cannot, by the standalone pass) and trusted by the norm; the tracked range
-slot every norm and producer writes for the fp16-split GEMM that consumes its output; the (a, o) table of the fused
-GroupNorm conv; LayerNorm at the text-tower widths and across the kernel's register-blocking boundaries; causal softmax.
+slot every norm and producer writes for the fp16-split GEMM that consumes its output; the (a, o) table the GroupNorm kernel
+applies, as it stores it; LayerNorm at the text-tower widths and across the kernel's register-blocking boundaries; causal
+softmax.
 
 The fp32-affine bound.  With u = 2^-24, the kernels hold per channel a = fp32(rstd) * gamma (* (1 + scale)) and
 o = (beta - fp32(mean) * a') (* (1 + scale) + shift), a' = rstd * gamma, from float64 statistics, and store y = fma(x, a, o).
@@ -215,7 +216,7 @@ def test_groupnorm(eng, C1, C2, B, HW, eps, silu, ss, data):
     y64, t64, a64, o64, o_terms = groupnorm_ref(x1, x2, gamma, beta, eps, scale, shift, silu)
     x = torch.cat([x1, x2], dim=-1) if x2 is not None else x1
     a, o = ab[..., 0].double(), ab[..., 1].double()
-    # the fused conv's table: the norm's own coefficients
+    # the table the norm applies, as the kernel stored it
     ra = worst((a - a64).abs(), 8 * U * a64.abs() + 1e-300)
     ro = worst((o - o64).abs(), 8 * U * o_terms + 1e-300)
     ry = worst((y.double() - y64).abs(), affine_bound(x, a64, o_terms, t64, y64, silu))
@@ -223,7 +224,7 @@ def test_groupnorm(eng, C1, C2, B, HW, eps, silu, ss, data):
           f'err/bound y {ry:.3f} a {ra:.3f} o {ro:.3f}')
     assert ra <= 1 and ro <= 1 and ry <= 1
     if not silu:
-        # gn_apply and gn_affine use one table: y is fma(x, a, o) of the returned table, within 1 ulp
+        # the kernel stores y = fma(x, a, o) from that same table: within 1 ulp of it
         v = x.double() * a[:, None, :] + o[:, None, :]
         ulp = (torch.nextafter(y.abs(), torch.tensor(math.inf, device=y.device)) - y.abs()).double()
         assert bool(((y.double() - v).abs() <= ulp).all())

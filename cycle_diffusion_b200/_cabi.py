@@ -100,6 +100,9 @@ SIGNATURES = {
                                        _I, _P, _P]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),
+    'cdx_edit_map_from_eps': (_I, [_P, _P, _P, _F, _I, _I, _P, _I, _I, _I, _I, _P]),
+    'cdx_edit_mask': (_I, [_P, _P, _I, _F, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     'cdx_latent_loop_ens': (_I, [_P, _I, _P, _P, _P, _P, _I, _P, _P, C.POINTER(DdimCoef), C.POINTER(_F), _I, _I, _P, _F, _F, _P, _I, _P, _P, _P,
                                  _I, _I, _I, _I, _P]),
     'cdx_clip_preprocess': (_I, [_P, _P, _I, _I, _I, _P, _P]),

@@ -291,6 +291,44 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   }
 }
 
+// DiffEdit's mask statistics (Couairon et al., 2022): for each image b and map k, x_t = q_sample(x0[b], noise[b, k]) at timestep t
+// runs under c_src[b] and c_tgt[b], and acc[b] += sum_c |e_tgt - e_src| (v nets: sa_v[t]*(v_tgt - v_src), in eps units).  The
+// (map, image) pairs are walked map-major, as many whole pairs per U-Net call as rows_per_call allows (two rows each): per call one
+// launch builds the rows, one U-Net call, one launch accumulates.  The accumulate kernel adds the maps of an image in map order, so
+// acc does not depend on rows_per_call.
+void run_edit_map(Net& unet, const float* x0, const float* c_src, const float* c_tgt, int L, float t, float sa, float s1, const float* noise,
+                  int n_maps, int rows_per_call, float* acc, int B, int C, int h, int w, cudaStream_t s) {
+  Engine& e = *unet.eng;
+  const int chw = C * h * w, hw = h * w, n_pairs = n_maps * B, per_call = std::min(rows_per_call / 2, n_pairs), rows = 2 * per_call;
+  const size_t ctx_n = (size_t)L * unet.ucfg.context_dim;
+  check_v_steps(unet, &t, 1);
+  const float vscale = unet.pred ? unet.sa_v[(int)t] : 1.f;
+  Scope sc(e.arena);
+  float* xin = (float*)e.arena.alloc((size_t)rows * chw * sizeof(float));
+  float* eout = (float*)e.arena.alloc((size_t)rows * chw * sizeof(float));
+  float* ctx_in = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
+  float* tdev = (float*)e.arena.alloc((size_t)rows * sizeof(float));
+  upload_timesteps(e, &t, 1, rows, tdev, s);
+  if (!e.dry()) CDX_CUDA(cudaMemsetAsync(acc, 0, (size_t)B * hw * sizeof(float), s));
+  // the sizing pass runs the first call, the largest
+  const int calls = e.dry() ? 1 : cdiv(n_pairs, per_call);
+  for (int c = 0; c < calls; ++c) {
+    const int p0 = c * per_call, p1 = std::min(p0 + per_call, n_pairs), nr = 2 * (p1 - p0);
+    for (int q = p0; q < p1; ++q) {
+      const int b = q % B, r = 2 * (q - p0);
+      copy_dd(e, c_src + (size_t)b * ctx_n, ctx_in + (size_t)r * ctx_n, ctx_n, s);
+      copy_dd(e, c_tgt + (size_t)b * ctx_n, ctx_in + (size_t)(r + 1) * ctx_n, ctx_n, s);
+    }
+    edit_rows(e, x0, noise, sa, s1, xin, B, n_maps, chw, p0, p1, s);
+    const size_t stat0 = e.stat_dry;
+    unet_forward(unet, xin, tdev, ctx_in, L, eout, nr, h, w, s);
+    CDX_CHECK(!e.dry() || e.stat_dry - stat0 <= e.stat_cap,
+              "edit_map: a %d-row U-Net call needs %zu GroupNorm statistics doubles, the pool holds %zu: lower rows_per_call", nr,
+              e.stat_dry - stat0, e.stat_cap);
+    edit_map_accum(e, eout, eout + chw, 2LL * chw, 2LL * B * chw, 2LL * p0 * chw, vscale, acc, B, C, hw, p0, p1, s);
+  }
+}
+
 }  // namespace
 }  // namespace cdx
 
@@ -828,6 +866,36 @@ int cdx_mask_pool(cdx_engine* e, const float* mask, float* out, int B, int H, in
 }
 int cdx_mask_composite(cdx_engine* e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H, int W, void* s) {
   ENG_CALL(e, CDX_CHECK(dec && image && mask && out, "mask_composite: null argument"); mask_composite(e->e, dec, image, mask, out, B, C, H, W, S(s)));
+}
+
+int cdx_edit_map(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, int L, float t, float sqrt_a, float sqrt_1ma,
+                 const float* noise, int n_maps, int rows_per_call, float* acc_out, int B, int C, int h, int w, void* stream) {
+  return guard([&] {
+    CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && noise && acc_out, "edit_map: null argument");
+    CDX_CHECK(n_maps >= 1 && B >= 1 && C >= 1 && h >= 1 && w >= 1, "edit_map: n_maps=%d B=%d C=%d %dx%d", n_maps, B, C, h, w);
+    CDX_CHECK(rows_per_call >= 2, "edit_map: rows_per_call=%d, a (map, image) pair takes 2 rows", rows_per_call);
+    CDX_CHECK(un->n->ucfg.context_dim > 0 && L > 0, "edit_map: needs a text-conditioned U-Net and its context");
+    with_arena(un->owner->e, S(stream), [&] {
+      run_edit_map(*un->n, x0, c_src, c_tgt, L, t, sqrt_a, sqrt_1ma, noise, n_maps, rows_per_call, acc_out, B, C, h, w, S(stream));
+    });
+  });
+}
+int cdx_edit_map_from_eps(cdx_engine* e, const float* e_src, const float* e_tgt, float vscale, int n_maps, int maps_per_launch,
+                          float* acc_out, int B, int C, int h, int w, void* s) {
+  ENG_CALL(e, CDX_CHECK(e_src && e_tgt && acc_out, "edit_map_from_eps: null argument");
+           CDX_CHECK(n_maps >= 1 && maps_per_launch >= 1 && B >= 1 && C >= 1 && h >= 1 && w >= 1,
+                     "edit_map_from_eps: n_maps=%d maps_per_launch=%d B=%d C=%d %dx%d", n_maps, maps_per_launch, B, C, h, w);
+           const long long chw = (long long)C * h * w;
+           CDX_CUDA(cudaMemsetAsync(acc_out, 0, (size_t)B * h * w * sizeof(float), S(s)));
+           for (int k0 = 0; k0 < n_maps; k0 += maps_per_launch)
+             edit_map_accum(e->e, e_src, e_tgt, n_maps * chw, chw, 0, vscale, acc_out, B, C, h * w, k0 * B,
+                            std::min(k0 + maps_per_launch, n_maps) * B, S(s)));
+}
+int cdx_edit_mask(cdx_engine* e, const float* acc, int n_maps, float ratio, float* map_out, float* mask_out, float* mask_img_out, int f, int B,
+                  int C, int h, int w, void* s) {
+  ENG_CALL(e, CDX_CHECK(acc && map_out && mask_out, "edit_mask: null argument");
+           CDX_CHECK(ratio > 0.f && ratio < INFINITY, "edit_mask: ratio %g", ratio);
+           edit_mask(e->e, acc, n_maps, ratio, map_out, mask_out, mask_img_out, f, B, C, h, w, S(s)));
 }
 
 int cdx_ensemble_select(cdx_engine* eh, int n, const float* scores, const int64_t* cand_idx, const int* sample_idx, const float* images,

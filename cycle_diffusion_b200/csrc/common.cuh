@@ -84,6 +84,7 @@ struct Engine {
   // per-(image, channel) fp64 statistics buffers of activation tensors (GroupNorm inputs), same life cycle as the amax slots
   double* stat_pool = nullptr;
   size_t stat_cap = (size_t)8 << 20, stat_used = 0, stat_high = 0;      // doubles (64 MB)
+  size_t stat_dry = 0;      // doubles the sizing passes have asked for, ever: a driver checks one call's share against stat_cap
   double* stat_alloc(size_t n);
   void pools_reset(cudaStream_t s);   // start of a network call: zero what the previous call dirtied, rewind
   Arena arena;
@@ -296,6 +297,17 @@ void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, in
 // m == 0 gives image, m == 1 the clamped decode, exactly
 void mask_composite(Engine& e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H, int W,
                     cudaStream_t s);
+// DiffEdit mask (cdx_edit_map / cdx_edit_mask).  Pairs q = k*B + b (map k of image b) in map-major order.
+// edit_rows: pairs [p0, p1) -> xin rows 2*(q - p0) and 2*(q - p0) + 1 both = q_sample(x0[b], noise[b, k]), noise [B, n_maps, chw]
+void edit_rows(Engine& e, const float* x0, const float* noise, float sa, float s1, float* xin, int B, int n_maps, int chw, int p0, int p1,
+               cudaStream_t s);
+// edit_map_accum: acc [B, hw] += sum_c |vscale*(tgt - src)| per pair of [p0, p1) in map order; pair q's [C, hw] predictions at
+// src / tgt + b*sb + k*sk - off0
+void edit_map_accum(Engine& e, const float* src, const float* tgt, long long sb, long long sk, long long off0, float vscale, float* acc, int B,
+                    int C, int hw, int p0, int p1, cudaStream_t s);
+// edit_mask: one block per image -> map = acc / (n_maps*C), latent mask and (img_out non-null) the mask nearest-upsampled by f
+void edit_mask(Engine& e, const float* acc, int n_maps, float ratio, float* map_out, float* mask_out, float* img_out, int f, int B, int C, int h,
+               int w, cudaStream_t s);
 // Running per-sample best of the ensemble search over candidates that arrive in chunks, in any order: candidate c of the chunk
 // (image images[c], score scores[c], reference candidate index cand[c], sample sample[c]) replaces the best of its sample when it
 // wins under torch.argmax's rule over the [B, n_total] score matrix (larger score; NaN beats any number; ties and NaNs: lower

@@ -86,7 +86,7 @@ float* Engine::amax_slot() {
 }
 double* Engine::stat_alloc(size_t n) {
   n = (n + 31) & ~(size_t)31;
-  if (dry()) return reinterpret_cast<double*>((uintptr_t)0x1000);   // never dereferenced
+  if (dry()) { stat_dry += n; return reinterpret_cast<double*>((uintptr_t)0x1000); }   // never dereferenced
   if (!stat_pool) {
     if (cudaMalloc(&stat_pool, stat_cap * sizeof(double)) != cudaSuccess) throw Error(CDX_E_NOMEM, "statistics pool allocation failed");
     if (cudaMemset(stat_pool, 0, stat_cap * sizeof(double)) != cudaSuccess) throw Error(CDX_E_CUDA, "statistics pool memset failed");

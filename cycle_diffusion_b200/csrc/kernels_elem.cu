@@ -358,6 +358,79 @@ __global__ void mask_composite_kernel(const float* __restrict__ dec, const float
   }
 }
 
+// DiffEdit mask.  Pair q = k*B + b (map k of image b) of pairs [p0, p1): both of its U-Net rows get q_sample(x0[b], noise[b, k]) in
+// q_sample_kernel's op order; a pair's rows are 2*(q - p0) (source condition) and 2*(q - p0) + 1 (target condition).
+__global__ void edit_rows_kernel(const float* __restrict__ x0, const float* __restrict__ noise, float sa, float s1, float* __restrict__ xin,
+                                 int B, int n_maps, int chw, int p0, size_t n) {
+  GRID_STRIDE(i, n) {
+    const int r = (int)(i / chw), q = p0 + r, b = q % B, k = q / B;
+    const size_t c = i - (size_t)r * chw;
+    const float v = ADD(MUL(sa, x0[(size_t)b * chw + c]), MUL(s1, noise[((size_t)b * n_maps + k) * chw + c]));
+    xin[(size_t)2 * r * chw + c] = v;
+    xin[(size_t)(2 * r + 1) * chw + c] = v;
+  }
+}
+// acc[b, p] += sum_c |vscale * (tgt - src)| (c ascending, fp32) for every pair q = k*B + b of [p0, p1), k ascending: one thread per
+// (image, latent pixel), so the adds into acc happen in map order however the maps are split over launches.  Pair q's predictions
+// sit at src + off(q), tgt + off(q), off(q) = b*sb + k*sk - off0.  vscale = 1 (eps) leaves the difference unchanged exactly.
+// Coherent loads: the predictions come from the U-Net launches just before, acc from the previous accumulate launch.
+__global__ void edit_map_accum_kernel(const float* src, const float* tgt, long long sb, long long sk, long long off0, float vscale,
+                                      float* acc, int B, int C, int hw, int p0, int p1) {
+  const size_t n = (size_t)B * hw;
+  GRID_STRIDE(i, n) {
+    const int b = (int)(i / hw), p = (int)(i - (size_t)b * hw);
+    int k = p0 > b ? (p0 - b + B - 1) / B : 0;
+    if (k * B + b >= p1) continue;
+    float a = __ldcg(acc + i);
+    for (; k * B + b < p1; ++k) {
+      const long long off = (long long)b * sb + (long long)k * sk - off0 + p;
+      float s = 0.f;
+      for (int c = 0; c < C; ++c) {
+        const long long o = off + (long long)c * hw;
+        s = ADD(s, fabsf(MUL(vscale, SUB(__ldcg(tgt + o), __ldcg(src + o)))));
+      }
+      a = ADD(a, s);
+    }
+    acc[i] = a;
+  }
+}
+// One block of EDIT_MASK_THREADS per image: map = acc / (n*C); mean = fp32(sum_p map in fp64 / hw), summed in a fixed order (each
+// thread strides the pixels, then a fixed tree over the block); M = ratio * mean; mask = min(map, M) / M > 0.5 when M > 0, else 0.
+// Writes the map, the latent mask and, optionally, the mask nearest-upsampled by f.
+constexpr int EDIT_MASK_THREADS = 256;
+__global__ void __launch_bounds__(EDIT_MASK_THREADS) edit_mask_kernel(const float* acc, float div, float ratio, float* __restrict__ map_out,
+                                                                      float* __restrict__ mask_out, float* __restrict__ img_out, int f, int h,
+                                                                      int w) {
+  __shared__ double part[EDIT_MASK_THREADS];
+  __shared__ float thr;
+  const int b = blockIdx.x, hw = h * w;
+  const float* a = acc + (size_t)b * hw;
+  double sum = 0.0;
+  for (int p = threadIdx.x; p < hw; p += EDIT_MASK_THREADS) sum += (double)DIV(__ldcg(a + p), div);
+  part[threadIdx.x] = sum;
+  __syncthreads();
+  for (int o = EDIT_MASK_THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) part[threadIdx.x] += part[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) thr = MUL(ratio, (float)(part[0] / (double)hw));
+  __syncthreads();
+  const float M = thr;
+  for (int p = threadIdx.x; p < hw; p += EDIT_MASK_THREADS) {
+    const float m = DIV(__ldcg(a + p), div);
+    map_out[(size_t)b * hw + p] = m;
+    mask_out[(size_t)b * hw + p] = (M > 0.f && DIV(fminf(m, M), M) > 0.5f) ? 1.f : 0.f;
+  }
+  if (!img_out) return;
+  const int W = w * f;
+  const size_t HW = (size_t)hw * f * f;
+  for (size_t i = threadIdx.x; i < HW; i += EDIT_MASK_THREADS) {
+    const int y = (int)(i / W), x = (int)(i - (size_t)y * W);
+    const float m = DIV(__ldcg(a + (y / f) * w + x / f), div);
+    img_out[(size_t)b * HW + i] = (M > 0.f && DIV(fminf(m, M), M) > 0.5f) ? 1.f : 0.f;
+  }
+}
+
 // does candidate (sa, ia) beat (sb, ib) under torch.argmax?  larger wins, NaN beats any number, ties and NaN pairs go to the lower
 // index; an index < 0 is an empty slot
 __device__ __forceinline__ bool select_better(float sa, long long ia, float sb, long long ib) {
@@ -666,6 +739,23 @@ void mask_composite(Engine& e, const float* dec, const float* image, const float
   CDX_CHECK(B >= 1 && C >= 1 && H >= 1 && W >= 1, "mask_composite: B=%d C=%d %dx%d", B, C, H, W);
   const size_t n = (size_t)B * C * H * W;
   LAUNCH1(mask_composite_kernel, n, dec, image, mask, out, C, (size_t)H * W, n);
+}
+void edit_rows(Engine& e, const float* x0, const float* noise, float sa, float s1, float* xin, int B, int n_maps, int chw, int p0, int p1,
+               cudaStream_t s) {
+  const size_t n = (size_t)(p1 - p0) * chw;
+  LAUNCH1(edit_rows_kernel, n, x0, noise, sa, s1, xin, B, n_maps, chw, p0, n);
+}
+void edit_map_accum(Engine& e, const float* src, const float* tgt, long long sb, long long sk, long long off0, float vscale, float* acc, int B,
+                    int C, int hw, int p0, int p1, cudaStream_t s) {
+  LAUNCH1(edit_map_accum_kernel, (size_t)B * hw, src, tgt, sb, sk, off0, vscale, acc, B, C, hw, p0, p1);
+}
+void edit_mask(Engine& e, const float* acc, int n_maps, float ratio, float* map_out, float* mask_out, float* img_out, int f, int B, int C, int h,
+               int w, cudaStream_t s) {
+  CDX_CHECK(B >= 1 && C >= 1 && h >= 1 && w >= 1 && n_maps >= 1 && f >= 1, "edit_mask: B=%d C=%d %dx%d n_maps=%d f=%d", B, C, h, w, n_maps, f);
+  if (e.dry()) return;
+  edit_mask_kernel<<<B, EDIT_MASK_THREADS, 0, s>>>(acc, (float)(n_maps * C), ratio, map_out, mask_out, img_out, f, h, w);
+  CDX_CUDA(cudaGetLastError());
+  e.launches++;
 }
 void ensemble_select(Engine& e, int n, const float* scores, const long long* cand, const int* sample, const float* images, float* best_score,
                      long long* best_idx, float* best_img, float* score_mat, int B, int n_total, size_t img_n, cudaStream_t s) {

@@ -153,6 +153,33 @@ class Engine:
         check(lib.cdx_mask_composite(self.h, _ptr(dec), _ptr(image), _ptr(mask), _ptr(out), B, Cc, H, W, self.stream))
         return out
 
+    def edit_map_from_eps(self, e_src, e_tgt, vscale=1.0, maps_per_launch=None):
+        """DiffEdit accumulation on given predictions (cdx_edit_map_from_eps): e_src, e_tgt [B,n,C,h,w] -> acc [B,h,w], acc[b] the
+        sum over maps k ascending of sum_c |vscale * (e_tgt[b,k] - e_src[b,k])|, fp32.  Bit-identical for any maps_per_launch
+        (default: all n maps in one launch)."""
+        e_src, e_tgt = _f32c(e_src, self.device), _f32c(e_tgt, self.device)
+        assert e_src.dim() == 5 and e_src.shape == e_tgt.shape, f'{tuple(e_src.shape)} vs {tuple(e_tgt.shape)}'
+        B, n, Cc, h, w = e_src.shape
+        acc = self.empty(B, h, w)
+        check(lib.cdx_edit_map_from_eps(self.h, _ptr(e_src), _ptr(e_tgt), float(vscale), n, int(maps_per_launch or n), _ptr(acc), B, Cc,
+                                        h, w, self.stream))
+        return acc
+
+    def edit_mask(self, acc, n_maps, ratio=3.0, f=None, channels=4):
+        """DiffEdit mask from the accumulator of UNet.edit_map (cdx_edit_mask): acc [B,h,w] over n_maps maps of a `channels`-channel
+        latent -> (map [B,1,h,w] = acc / (n_maps * channels), mask [B,1,h,w] in {0, 1}, mask_img [B,1,f*h,f*w] or None when f is
+        None).  Per image, mask = min(map, M) / M > 0.5 with M = ratio * mean(map); an all-zero map gives an all-zero mask.
+        mask_img is the mask nearest-upsampled by f (the first stage's factor), ready for the pipeline's ``mask_image``."""
+        if not ratio > 0:
+            raise ValueError(f'mask_thresholding_ratio must be > 0, got {ratio}')
+        acc = _f32c(acc, self.device)
+        B, h, w = acc.shape
+        emap, mask = self.empty(B, 1, h, w), self.empty(B, 1, h, w)
+        img = self.empty(B, 1, f * h, f * w) if f else None
+        check(lib.cdx_edit_mask(self.h, _ptr(acc), int(n_maps), float(ratio), _ptr(emap), _ptr(mask), _ptr(img), int(f or 1), B,
+                                int(channels), h, w, self.stream))
+        return emap, mask, img
+
     def q_sample(self, x0, noise, sqrt_a, sqrt_1ma):
         x0, noise = _f32c(x0, self.device), _f32c(noise, self.device)
         out = torch.empty_like(x0)
@@ -661,6 +688,23 @@ class UNet(Net):
                                               sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T,
                                               _ptr(out), _ptr(z), Cc, h, w, e.stream, _ptr(mask)))
         return (out, z) if return_z else out
+
+    def edit_map(self, x0, c_src, c_tgt, sched, noise, rows_per_call=None):
+        """DiffEdit's mask statistics (cdx_edit_map): x0 [B,C,h,w], c_src / c_tgt [B,L,D], noise [B,n,C,h,w] -> acc [B,h,w], the sum
+        over the n maps of sum_c |e_tgt - e_src| of x_t = q_sample(x0[b], noise[b,k]) at sched's first timestep (v nets: in eps
+        units).  Engine.edit_mask turns it into the mask.  rows_per_call: U-Net rows per call, two per (map, image) pair; default
+        min(48, max(12, 3B)) -- the lock-step cycle's own 3B rows from batch 4 up, at least 12, at most the 48 rows whose GroupNorm
+        statistics fit the engine's pool at SD width.  The result does not depend on it."""
+        e = self.engine
+        x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
+        B, Cc, h, w = x0.shape
+        assert noise.dim() == 5 and noise.shape[0] == B and noise.shape[2:] == x0.shape[1:], f'noise shape {tuple(noise.shape)}'
+        assert c_src.shape == c_tgt.shape and c_src.shape[0] == B
+        rows = int(rows_per_call) if rows_per_call is not None else min(48, max(12, 3 * B))
+        acc = e.empty(B, h, w)
+        check(lib.cdx_edit_map(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), c_src.shape[1], sched.t_loop[0], sched.sqrt_a_T,
+                               sched.sqrt_1ma_T, _ptr(noise), noise.shape[1], rows, _ptr(acc), B, Cc, h, w, e.stream))
+        return acc
 
     def pixel_encode(self, x0, sched, noise):
         e = self.engine

@@ -42,6 +42,57 @@ class CycleDiffusionPipeline:
     def from_wrapper(cls, wrapper):
         return cls(wrapper.generator, precision=wrapper.precision)
 
+    def _check_image(self, image):
+        g = self.g
+        assert torch.is_tensor(image) and image.dim() == 4, 'image: float tensor [B,3,H,W] in [0,1] (PIL preprocessing is host glue)'
+        # any H x W the first stage and the U-Net can both halve all the way down: no silent resize
+        side = g.vae.down * 2 ** (len(g.unet.cfg['channel_mult']) - 1)
+        if image.shape[2] % side or image.shape[3] % side:
+            raise ValueError(f'image height and width must both be multiples of {side} (the first stage\'s factor {g.vae.down} x '
+                             f'2^(len(channel_mult) - 1)), got {image.shape[2]}x{image.shape[3]}')
+
+    @torch.no_grad()
+    def generate_mask(self, image, source_prompt, target_prompt, num_maps_per_mask=10, mask_encode_strength=0.5,
+                      mask_thresholding_ratio=3.0, num_inference_steps=50, generator=None, output_type='pt', rows_per_call=None):
+        """DiffEdit's mask (Couairon et al., 2022): where the U-Net's predictions under the source and the target prompt disagree
+        on the noised image is where the edit goes.  image [B,3,H,W] in [0,1] -> float32 [B,1,H,W] in {0, 1} on the device, one mask
+        per image, ready for ``mask_image=`` (output_type='latent': [B,1,H/f,W/f] at latent resolution).
+        The latent is made as ``__call__`` makes it (same generator draw), then noised num_maps_per_mask times (one further draw,
+        [B, n, C, h, w]) to the first timestep of the S-step schedule at mask_encode_strength; the map is the mean over maps and
+        channels of |e_tgt - e_src| (UNet.edit_map), the mask is map > mask_thresholding_ratio * mean(map) / 2 per image
+        (Engine.edit_mask).  Unlike diffusers' generate_mask: the mean is per image, not over the batch; two U-Net rows per map,
+        not four (the guidance scale cancels in the normalisation, so there is none); an all-zero map gives an empty mask.
+        rows_per_call: U-Net rows per call (UNet.edit_map's default); the result does not depend on it."""
+        g, e = self.g, self.engine
+        self._check_image(image)
+        S = num_inference_steps
+        if not (0 < mask_encode_strength <= 1) or int(S * mask_encode_strength) < 1:
+            raise ValueError(f'mask_encode_strength must be in (0, 1] with int(num_inference_steps * strength) >= 1, got '
+                             f'{mask_encode_strength} at {S} steps')
+        if not (isinstance(num_maps_per_mask, int) and num_maps_per_mask >= 1):
+            raise ValueError(f'num_maps_per_mask must be an integer >= 1, got {num_maps_per_mask!r}')
+        if not mask_thresholding_ratio > 0:
+            raise ValueError(f'mask_thresholding_ratio must be > 0, got {mask_thresholding_ratio}')
+        if output_type not in ('pt', 'latent'):
+            raise ValueError(f"output_type must be 'pt' or 'latent', got {output_type!r}")
+        B = image.shape[0]
+        per_image = lambda p: [p] * B if isinstance(p, str) else (list(p) * B if len(p) == 1 else list(p))
+        sources, targets = per_image(source_prompt), per_image(target_prompt)
+        with e.precision(self.precision):
+            rnd = lambda shape: torch.randn(shape, generator=generator)
+            c_src = g.get_learned_conditioning(sources)
+            c_tgt = g.get_learned_conditioning(targets)
+            # t and its noise level from the tables the cycle uses; eta does not enter them
+            sched = DDIMSchedule(S, 0.0, S - int(S * mask_encode_strength), g.alphas_cumprod)
+            moments = g.encode_first_stage(e.shift_scale(image, -0.5, 2.0))
+            lat_shape = (B, moments.shape[1] // 2, moments.shape[2], moments.shape[3])
+            x0 = e.vae_posterior(moments, rnd(lat_shape) if g.sample_posterior else None, g.scale_factor)
+            noise = rnd((B, num_maps_per_mask) + lat_shape[1:])
+            acc = g.unet.edit_map(x0, c_src, c_tgt, sched, noise, rows_per_call)
+            _, mask, mask_img = e.edit_mask(acc, num_maps_per_mask, mask_thresholding_ratio,
+                                            f=None if output_type == 'latent' else g.vae.down, channels=lat_shape[1])
+        return mask if output_type == 'latent' else mask_img
+
     @torch.no_grad()
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
                  source_guidance_scale=1, num_images_per_prompt=1, eta=0.1, generator=None, prompt_embeds=None, output_type='pt',
@@ -51,7 +102,9 @@ class CycleDiffusionPipeline:
         convention).  Outside the mask the latent stays on the source image's own chain (cdx_cycle_lockstep_masked), so the
         unmasked region decodes to the image's VAE reconstruction.  paste_back: additionally composite the output with the input
         image at image resolution, so pixels where the mask is 0 are the input image exactly.  A mask needs the lock-step loop:
-        ``two_phase=True`` with a mask raises ValueError."""
+        ``two_phase=True`` with a mask raises ValueError.  mask_image='auto': the mask is generated from the prompts first, exactly
+        ``self.generate_mask(image, source_prompt, prompt, generator=generator, num_inference_steps=num_inference_steps)`` with its
+        defaults, on the same generator."""
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')
         if not isinstance(callback_steps, int) or callback_steps <= 0:
@@ -60,16 +113,17 @@ class CycleDiffusionPipeline:
             raise ValueError('mask_image needs the lock-step loop: the two-phase z holds noises, not the source chain (two_phase=False)')
         if paste_back and mask_image is None:
             raise ValueError('paste_back needs a mask_image')
+        if isinstance(mask_image, str):
+            if mask_image != 'auto':
+                raise ValueError(f"mask_image: a tensor or 'auto', got {mask_image!r}")
+            if prompt is None:
+                raise ValueError("mask_image='auto' generates the mask from the prompt text: pass prompt")
+            mask_image = self.generate_mask(image, source_prompt, prompt, generator=generator, num_inference_steps=num_inference_steps)
         assert eta > 0, 'CycleDiffusion needs a stochastic sampler (eta > 0), ddim.py:268'
         g, e = self.g, self.engine
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
         sources = [source_prompt] if isinstance(source_prompt, str) else list(source_prompt)
-        assert torch.is_tensor(image) and image.dim() == 4, 'image: float tensor [B,3,H,W] in [0,1] (PIL preprocessing is host glue)'
-        # any H x W the first stage and the U-Net can both halve all the way down: no silent resize
-        side = g.vae.down * 2 ** (len(g.unet.cfg['channel_mult']) - 1)
-        if image.shape[2] % side or image.shape[3] % side:
-            raise ValueError(f'image height and width must both be multiples of {side} (the first stage\'s factor {g.vae.down} x '
-                             f'2^(len(channel_mult) - 1)), got {image.shape[2]}x{image.shape[3]}')
+        self._check_image(image)
         B = image.shape[0] * num_images_per_prompt
         if mask_image is not None:
             if not (torch.is_tensor(mask_image) and mask_image.dim() == 4 and mask_image.shape[0] in (1, image.shape[0])

@@ -318,6 +318,36 @@ int cdx_cycle_lockstep_masked(cdx_net* unet, const float* x0, const float* c_src
 int cdx_mask_pool(cdx_engine* e, const float* mask, float* out, int B, int H, int W, int f, void* stream);
 int cdx_mask_composite(cdx_engine* e, const float* dec, const float* image, const float* mask, float* out, int B, int C, int H,
                        int W, void* stream);
+/* Edit masks from two prompts (DiffEdit, Couairon et al., 2022): where the source and target predictions of the noised image
+ * disagree is where the edit goes.  x0 [B,C,h,w] the encoded latent, c_src / c_tgt [B,ctx_len,D], noise [B,n_maps,C,h,w].
+ * For image b and map k (k = 0 .. n_maps-1):
+ *   x_t  = sqrt_a * x0[b] + sqrt_1ma * noise[b,k]               (cdx_q_sample's op order)
+ *   d    = e(x_t, t, c_tgt[b]) - e(x_t, t, c_src[b])            per element, two U-Net rows, no uncond row
+ *          (v-prediction nets: d = sa_v[t] * (v_tgt - v_src), so the map is in eps units; t must index the net's tables)
+ *   s[p] = sum over c ascending of |d[c,p]|                       fp32
+ *   acc[b,p] += s[p]                                              fp32, k ascending: one add per map
+ * cdx_edit_map: the whole computation.  acc_out [B,h,w] is zeroed first.  The (map, image) pairs are walked map-major, as many
+ *   whole pairs per U-Net call as rows_per_call (>= 2) allows, two rows per pair; the result does not depend on rows_per_call.  A
+ *   call whose GroupNorm statistics would exceed the engine's pool (a 96-row SD call does; 48 rows fit) is rejected by the
+ *   sizing pass, before anything runs.
+ *   t, sqrt_a, sqrt_1ma: the first timestep of DDIMSchedule(S, eta, S - int(S*strength)) and that schedule's sqrt_a_T /
+ *   sqrt_1ma_T.  Text-conditioned latent U-Nets only.
+ * cdx_edit_map_from_eps: the accumulation alone, on given predictions e_src / e_tgt [B,n_maps,C,h,w], vscale multiplying each
+ *   difference (1: eps nets, exactly), maps_per_launch maps per launch; acc_out [B,h,w] is zeroed first and is bit-identical for
+ *   any maps_per_launch.
+ * cdx_edit_mask: per image, map = acc / (n_maps*C) -> map_out [B,1,h,w]; mean = fp32(sum_p map in fp64 / (h*w)) (fixed
+ *   summation order); M = ratio * mean (ratio > 0); mask_out [B,1,h,w] = (min(map, M) / M > 0.5) ? 1 : 0 when M > 0, all 0 when
+ *   M == 0 (the two prompts predict the same: nothing to edit).  mask_img_out (nullable) [B,1,f*h,f*w]: the mask nearest-upsampled
+ *   by f, which cdx_mask_pool(.., f) turns back into mask_out exactly.
+ * Unlike diffusers' StableDiffusionDiffEditPipeline.generate_mask: the mean is per image (a mask never depends on its batch-mates),
+ * two rows per map (the guidance scale cancels in the normalisation), and an all-zero map gives an empty mask. */
+int cdx_edit_map(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, int ctx_len, float t, float sqrt_a,
+                 float sqrt_1ma, const float* noise, int n_maps, int rows_per_call, float* acc_out, int B, int C, int h,
+                 int w, void* stream);
+int cdx_edit_map_from_eps(cdx_engine* e, const float* e_src, const float* e_tgt, float vscale, int n_maps,
+                          int maps_per_launch, float* acc_out, int B, int C, int h, int w, void* stream);
+int cdx_edit_mask(cdx_engine* e, const float* acc, int n_maps, float ratio, float* map_out, float* mask_out,
+                  float* mask_img_out, int f, int B, int C, int h, int w, void* stream);
 /* The same three loops with PER-SAMPLE guidance scales (device arrays of B floats): the ensemble driver of the text wrappers
  * (SDW:146-165 generate, :189-204 encode -- the reference loops trial x encoder-scale x skip, then x decoder-scale, one chain at a
  * time, recomputing the conditioning and every context K/V projection per member).  Members that share a schedule are batched

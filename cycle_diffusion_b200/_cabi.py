@@ -46,6 +46,21 @@ class PixelCoef(C.Structure):
 
 
 _P = C.c_void_p          # device / opaque pointers
+
+
+class GemmDesc(C.Structure):
+    _fields_ = [('mode', C.c_int), ('M', C.c_int), ('N', C.c_int), ('K', C.c_int),
+                ('A', _P), ('lda', C.c_int), ('C1', C.c_int), ('A2', _P), ('lda2', C.c_int), ('C2', C.c_int),
+                ('Hin', C.c_int), ('Win', C.c_int), ('Hout', C.c_int), ('Wout', C.c_int), ('stride', C.c_int), ('pad', C.c_int),
+                ('w', _P), ('ldb', C.c_int), ('b_kn', C.c_int), ('bias', _P),
+                ('rowvec', _P), ('ld_rowvec', C.c_int), ('rows_per_batch', C.c_int), ('residual', _P), ('ldr', C.c_int),
+                ('alpha', C.c_float), ('geglu', C.c_int), ('out_nchw', C.c_int), ('rows_per_img', C.c_int),
+                ('C', _P), ('ldc', C.c_int), ('C_lo', _P), ('Ct_hi', _P), ('Ct_lo', _P), ('t_col0', C.c_int), ('ldt', C.c_int64),
+                ('a_amax', _P), ('a2_amax', _P), ('c_amax', _P), ('c_stats', _P), ('w_range', C.c_float),
+                ('batch', C.c_int), ('heads', C.c_int),
+                ('sA_b', C.c_int64), ('sA_h', C.c_int64), ('sB_b', C.c_int64), ('sB_h', C.c_int64), ('sC_b', C.c_int64), ('sC_h', C.c_int64)]
+
+
 _F = C.c_float
 _I = C.c_int
 _S = C.c_size_t
@@ -130,6 +145,7 @@ SIGNATURES = {
     'cdx_op_layernorm_ex': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
     'cdx_op_softmax_rows': (_I, [_P, _P, C.c_int64, _I, _I, _I, _P]),
     'cdx_op_produce_norm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, C.POINTER(_I), _P]),
+    'cdx_op_gemm': (_I, [_P, C.POINTER(GemmDesc), C.POINTER(_I), _P]),
 }
 
 

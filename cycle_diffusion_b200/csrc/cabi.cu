@@ -120,8 +120,15 @@ void copy_dd(Engine& e, const float* src, float* dst, size_t n, cudaStream_t s) 
   CDX_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
 }
 
-// test hooks: build the fp16-split planes of an ad-hoc weight matrix on the fly (networks do this once at finalize)
-void hook_h16_planes(Engine& e, const float* w, size_t n, GemmArgs& g, cudaStream_t s) {
+// test hooks: the tensor-core weight planes of an ad-hoc weight matrix, built on the fly (networks do this once at finalize):
+// TF32 hi / lo, and in the fp16-split modes the fp16 planes of w * 2^b_exp with b_exp from max(w_range, max |w|) -- w_range stands
+// in for the net-wide weight range a network's planes take their exponent from
+void hook_weight_planes(Engine& e, const float* w, size_t n, GemmArgs& g, cudaStream_t s, float w_range = 0.f) {
+  if (e.mma_mode != 1) return;
+  float* thi = (float*)e.arena.alloc(n * sizeof(float));
+  float* tlo = (float*)e.arena.alloc(n * sizeof(float));
+  split_planes(e, w, thi, tlo, n, s);
+  g.Bw_hi = thi; g.Bw_lo = tlo;
   if (e.tc_kind < 1 || (n & 7)) return;
   void* hi = e.arena.alloc(n * 2);
   void* lo = e.arena.alloc(n * 2);
@@ -131,7 +138,7 @@ void hook_h16_planes(Engine& e, const float* w, size_t n, GemmArgs& g, cudaStrea
   float wmax = 0.f;
   CDX_CUDA(cudaMemcpyAsync(&wmax, slot, sizeof(float), cudaMemcpyDeviceToHost, s));
   CDX_CUDA(cudaStreamSynchronize(s));
-  g.b_exp = h16_exp_host(wmax);
+  g.b_exp = h16_exp_host(std::max(wmax, w_range));
   split_planes_h16(e, w, hi, lo, n, g.b_exp, s);
   g.Bw_h_hi = hi; g.Bw_h_lo = lo;
 }
@@ -930,13 +937,7 @@ int cdx_op_conv3x3(cdx_engine* eh, const float* x, const float* w_oihw, const fl
       g.Bw = wr; g.ldb = 9 * Cin;
       g.Cout = y; g.ldc = Cout;
       g.bias = bias;
-      if (e.mma_mode == 1) {   // exercise the TS kernel: build the TF32 planes of the (repacked) weight on the fly
-        float* hi = (float*)e.arena.alloc((size_t)Cout * Cin * 9 * sizeof(float));
-        float* lo = (float*)e.arena.alloc((size_t)Cout * Cin * 9 * sizeof(float));
-        split_planes(e, wr, hi, lo, (size_t)Cout * Cin * 9, s);
-        g.Bw_hi = hi; g.Bw_lo = lo;
-        hook_h16_planes(e, wr, (size_t)Cout * Cin * 9, g, s);
-      }
+      hook_weight_planes(e, wr, (size_t)Cout * Cin * 9, g, s);
       gemm(e, g, s);
     });
   });
@@ -954,13 +955,7 @@ int cdx_op_linear(cdx_engine* eh, const float* x, const float* w, const float* b
       g.Bw = w; g.ldb = K;
       g.Cout = y; g.ldc = N;
       g.bias = bias;
-      if (e.mma_mode == 1) {
-        float* hi = (float*)e.arena.alloc((size_t)N * K * sizeof(float));
-        float* lo = (float*)e.arena.alloc((size_t)N * K * sizeof(float));
-        split_planes(e, w, hi, lo, (size_t)N * K, S(stream));
-        g.Bw_hi = hi; g.Bw_lo = lo;
-        hook_h16_planes(e, w, (size_t)N * K, g, S(stream));
-      }
+      hook_weight_planes(e, w, (size_t)N * K, g, S(stream));
       gemm(e, g, S(stream));
     });
   });
@@ -1139,13 +1134,7 @@ int cdx_op_produce_norm(cdx_engine* eh, const float* x, const float* w, const fl
       g.Bw = wk; g.ldb = K;
       g.Cout = y; g.ldc = Cout;
       g.bias = bias;
-      if (e.mma_mode == 1) {
-        float* hi = (float*)e.arena.alloc((size_t)Cout * K * sizeof(float));
-        float* lo = (float*)e.arena.alloc((size_t)Cout * K * sizeof(float));
-        split_planes(e, wk, hi, lo, (size_t)Cout * K, s);
-        g.Bw_hi = hi; g.Bw_lo = lo;
-        hook_h16_planes(e, wk, (size_t)Cout * K, g, s);
-      }
+      hook_weight_planes(e, wk, (size_t)Cout * K, g, s);
       Tensor t;
       t.p = y; t.B = B; t.H = H; t.W = W; t.C = Cout;
       track_outputs(e, t, g, true);
@@ -1157,6 +1146,58 @@ int cdx_op_produce_norm(cdx_engine* eh, const float* x, const float* w, const fl
       CDX_CUDA(cudaMemcpyAsync(amax_out, t.amax, sizeof(float), cudaMemcpyDeviceToDevice, s));
       CDX_CUDA(cudaMemcpyAsync(stats_out, t.stats, (size_t)B * Cout * 2 * sizeof(double), cudaMemcpyDeviceToDevice, s));
     });
+  });
+}
+int cdx_op_gemm(cdx_engine* eh, const cdx_gemm_desc* d, int* plan_out, void* stream) {
+  return guard([&] {
+    CDX_CHECK(eh && d && d->A && d->w && d->C, "op_gemm: null argument");
+    CDX_CHECK((d->mode == 0 || d->mode == 1) && d->M > 0 && d->N > 0 && d->K > 0 && d->C1 > 0 && d->C2 >= 0 && (d->C2 == 0) == !d->A2,
+              "op_gemm: mode=%d M=%d N=%d K=%d C1=%d C2=%d", d->mode, d->M, d->N, d->K, d->C1, d->C2);
+    CDX_CHECK(d->batch >= 0 && d->heads >= 0 && d->rows_per_batch >= 0 && (d->out_nchw ? d->rows_per_img > 0 : d->rows_per_img >= 0),
+              "op_gemm: bad batch / image counts");
+    const int batch = d->batch > 0 ? d->batch : 1, heads = d->heads > 0 ? d->heads : 1;
+    CDX_CHECK(d->mode == 0 || (!d->b_kn && batch * heads == 1), "op_gemm: a conv3x3 is one unbatched [N][K] product");
+    Engine& e = eh->e;
+    cudaStream_t s = S(stream);
+    int route = 0;
+    with_arena(e, s, [&] {
+      Scope sc(e.arena);
+      e.pools_reset(s);
+      GemmArgs g;
+      g.mode = d->mode;
+      g.M = d->M; g.N = d->N; g.K = d->K;
+      g.A = d->A; g.lda = d->lda; g.C1 = d->C1;
+      g.A2 = d->A2; g.lda2 = d->lda2; g.C2 = d->C2;
+      g.Hin = d->Hin; g.Win = d->Win; g.Hout = d->Hout; g.Wout = d->Wout; g.stride = d->stride; g.pad = d->pad;
+      const float* wk = d->w;
+      size_t wn;                                   // weight elements the planes cover (element index = float index)
+      if (d->mode == 1) {
+        float* wr = (float*)e.arena.alloc((size_t)d->N * d->K * sizeof(float));
+        repack_conv3x3(e, d->w, wr, d->N, d->C1, s);
+        wk = wr;
+        g.ldb = d->K;
+        wn = (size_t)d->N * d->K;
+      } else {
+        g.ldb = d->ldb;
+        wn = d->b_kn ? (size_t)(d->K - 1) * d->ldb + d->N : (size_t)(d->N - 1) * d->ldb + d->K;
+      }
+      g.Bw = wk; g.b_kn = d->b_kn;
+      if (!d->b_kn && batch * heads == 1) hook_weight_planes(e, wk, wn, g, s, d->w_range);
+      g.a_amax = d->a_amax; g.a2_amax = d->a2_amax;
+      g.c_amax = d->c_amax; g.c_stats = d->c_stats;
+      g.Cout = d->C; g.ldc = d->ldc; g.Cout_lo = d->C_lo;
+      g.Ct_hi = d->Ct_hi; g.Ct_lo = d->Ct_lo; g.t_col0 = d->t_col0; g.ldt = d->ldt;
+      g.bias = d->bias;
+      g.rowvec = d->rowvec; g.ld_rowvec = d->ld_rowvec; g.rows_per_batch = d->rows_per_batch > 0 ? d->rows_per_batch : 1;
+      g.residual = d->residual; g.ldr = d->ldr;
+      g.alpha = d->alpha;
+      g.geglu = d->geglu;
+      g.out_nchw = d->out_nchw; g.rows_per_img = d->rows_per_img;
+      g.batch = batch; g.heads = heads;
+      g.sA_b = d->sA_b; g.sA_h = d->sA_h; g.sB_b = d->sB_b; g.sB_h = d->sB_h; g.sC_b = d->sC_b; g.sC_h = d->sC_h;
+      gemm(e, g, s, &route);
+    });
+    if (plan_out) *plan_out = route;
   });
 }
 

@@ -169,12 +169,16 @@ struct GemmArgs {
   int batch = 1, heads = 1;
   long long sA_b = 0, sA_h = 0, sB_b = 0, sB_h = 0, sC_b = 0, sC_h = 0;
 };
-// route (optional): how the call ran, known on the host at enqueue time -- bits 0-2 as gemm_tc's side_done, bit 3: tensor cores
-// (0: the FFMA tiles, side outputs by the standalone passes)
+// route (optional): how the call ran, known on the host at enqueue time -- bits 0-2, 4-5, 8-23 as gemm_tc's side_done, bit 3:
+// tensor cores (0: the FFMA tiles, side outputs by the standalone passes; bits 8-15 then hold the FFMA tile side, 128 or 64, and
+// bits 16-23 a split count of 1)
 void gemm(Engine& e, const GemmArgs& a, cudaStream_t s, int* route = nullptr);
 // wgmma back end (kernels_tc.cu); returns false when the shape is not eligible
-// side_done bit 0: c_amax fused, bit 1: c_stats fused, bit 2: split-K (partial sums + reduce kernel)
+// side_done bit 0: c_amax fused, bit 1: c_stats fused, bit 2: split-K (partial sums + reduce kernel); the plan it ran:
+// bits 4-5 operand kind (ROUTE_KIND_*), bits 8-15 tile width (128 or 64), bits 16-23 split-K factor
 bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done = nullptr);
+enum { ROUTE_KIND_SS = 0, ROUTE_KIND_TS = 1, ROUTE_KIND_H16 = 2, ROUTE_KIND_H16_FAST = 3 };
+inline int route_plan(int kind, int width, int splits) { return kind << 4 | width << 8 | splits << 16; }
 // fused attention (kernels_attn.cu): true when the engine's mode runs N queries over Nk keys at head width d (C channels) fused
 bool flash_eligible(const Engine& e, int N, int Nk, int d, int C);
 bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,

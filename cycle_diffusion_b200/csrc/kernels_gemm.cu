@@ -325,25 +325,27 @@ void gemm(Engine& e, const GemmArgs& a, cudaStream_t s, int* route) {
       return;
     }
   }
-  if (route) *route = 0;
+  const long long ctas128 = (long long)cdiv(a.M, 128) * cdiv(a.N, 128) * a.batch * a.heads;
+  const bool big = ctas128 >= 2LL * e.num_sms && a.N > 64;
+  if (route) *route = route_plan(0, big ? 128 : 64, 1);     // (the fall-backs below pass it on: their inner GEMM may take the tensor cores)
   if (a.c_amax || a.c_stats) {
     GemmArgs b = a;
     b.c_amax = nullptr; b.c_stats = nullptr;
-    gemm(e, b, s);
+    gemm(e, b, s, route);
     gemm_side_outputs(e, a, false, false, s);
     return;
   }
   CDX_CHECK(!a.Ct_hi, "gemm: transposed plane output is only available on the tensor-core path (caller must check eligibility)");
   if (a.geglu) {       // fused only in the tensor-core epilogue; here: plain GEMM into a temporary, then the GEGLU kernel
     CDX_CHECK(a.N % 128 == 0 && a.batch * a.heads == 1 && !a.out_nchw && !a.Cout_lo, "gemm: bad GEGLU problem");
+    CDX_CHECK(a.ldc == a.N / 2, "gemm: GEGLU output must be dense [M, N/2]");
     Scope sc(e.arena);
     float* tmp = (float*)e.arena.alloc((size_t)a.M * a.N * sizeof(float));
     if (e.dry()) return;
     GemmArgs b = a;
     b.geglu = 0;
     b.Cout = tmp; b.ldc = a.N;
-    gemm(e, b, s);
-    CDX_CHECK(a.ldc == a.N / 2, "gemm: GEGLU output must be dense [M, N/2]");
+    gemm(e, b, s, route);
     geglu(e, tmp, a.Cout, a.M, a.N / 2, s, true);
     return;
   }
@@ -352,7 +354,7 @@ void gemm(Engine& e, const GemmArgs& a, cudaStream_t s, int* route) {
     CDX_CHECK(a.ldc == a.N && a.batch * a.heads == 1 && !a.out_nchw, "gemm: plane output needs a dense [M,N] result");
     GemmArgs b = a;
     b.Cout_lo = nullptr;
-    gemm(e, b, s);
+    gemm(e, b, s, route);
     split_planes(e, a.Cout, a.Cout, a.Cout_lo, (size_t)a.M * a.N, s);
     return;
   }
@@ -369,9 +371,6 @@ void gemm(Engine& e, const GemmArgs& a, cudaStream_t s, int* route) {
   vec = vec && aligned16(a.Cout) && (a.bias == nullptr || aligned16(a.bias)) &&
         (a.residual == nullptr || aligned16(a.residual)) && (a.rowvec == nullptr || aligned16(a.rowvec));
   if (a.b_kn) CDX_CHECK(a.mode == 0, "b_kn only for dense mode");
-
-  const long long ctas128 = (long long)cdiv(a.M, 128) * cdiv(a.N, 128) * a.batch * a.heads;
-  const bool big = ctas128 >= 2LL * e.num_sms && a.N > 64;
 
 #define CDX_LAUNCH(MODE, BKN, VEC)                                   \
   do {                                                               \

@@ -530,7 +530,7 @@ __global__ void splitk_reduce_kernel(const float* ws, int splits, TcParams p, in
       a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
     }
     a.x *= alpha; a.y *= alpha; a.z *= alpha; a.w *= alpha;
-    if (p.bias) { const float4 t = *reinterpret_cast<const float4*>(p.bias + n); a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w; }
+    if (p.bias) { a.x += p.bias[n]; a.y += p.bias[n + 1]; a.z += p.bias[n + 2]; a.w += p.bias[n + 3]; }    // any alignment: gemm_tc does not check the bias
     if (p.rowvec) { const float4 t = *reinterpret_cast<const float4*>(p.rowvec + (m / p.rows_per_batch) * p.ld_rowvec + n); a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w; }
     if (p.residual) { const float4 t = *reinterpret_cast<const float4*>(p.residual + m * p.ldr + n); a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w; }
     if (p.C_lo) {
@@ -915,7 +915,9 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   // (a tile that overhangs its map may start a warp on a masked row: its statistics are left to the standalone pass)
   const bool quad_ok = a.mode == 1 ? ((p.bw * p.bh) % 32 == 0 && p.tiles_x * p.bw == p.W && p.tiles_y * p.bh == p.H) : (a.rows_per_batch % 32 == 0);
   p.c_stats = (a.c_stats && quad_ok && p.splits == 1 && !a.out_nchw && !a.geglu && !a.Ct_hi && !a.Cout_lo && a.ldc == a.N) ? a.c_stats : nullptr;
-  if (side_done) *side_done = (p.c_amax ? 1 : 0) | (p.c_stats ? 2 : 0) | (p.splits > 1 ? 4 : 0);
+  if (side_done)
+    *side_done = (p.c_amax ? 1 : 0) | (p.c_stats ? 2 : 0) | (p.splits > 1 ? 4 : 0) |
+                 route_plan(fast ? ROUTE_KIND_H16_FAST : h16 ? ROUTE_KIND_H16 : ts ? ROUTE_KIND_TS : ROUTE_KIND_SS, p.tn_w, p.splits);
   if (e.dry()) return true;
   if (h16) {
     uint64_t d[2] = {(uint64_t)a.K, (uint64_t)a.N}, st[1] = {(uint64_t)a.ldb * 2};

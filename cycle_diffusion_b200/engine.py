@@ -370,6 +370,36 @@ class Engine:
                                       eps, _ptr(y), _ptr(amax), _ptr(stats), _ptr(yn), C.byref(path), self.stream))
         return y, amax, stats, yn, self.PRODUCE_PATHS[path.value]
 
+    GEMM_POINTERS = ('A', 'A2', 'w', 'bias', 'rowvec', 'residual', 'C', 'C_lo', 'Ct_hi', 'Ct_lo', 'a_amax', 'a2_amax', 'c_amax', 'c_stats')
+    GEMM_KINDS = ('ss', 'ts', 'h16', 'h16_fast')
+
+    def op_gemm(self, **fields):
+        """One contraction through the production GEMM with any of its epilogue terms (cdx_op_gemm in include/cdx.h, whose
+        cdx_gemm_desc fields are the keyword arguments).  Every buffer is a float32 tensor (c_stats: float64) on this engine's
+        device, passed as it is -- a view at an offset or a column slice keeps its address, so the strides (lda, ldc, ...) are the
+        caller's.  Outputs land in the caller's C / C_lo / Ct_hi / Ct_lo / c_amax / c_stats.  Defaults: alpha 1, stride 1, pad 1,
+        one image per row block.  Returns the plan the call ran: dict(kind: 'ffma' or one of GEMM_KINDS, width: tile width
+        (FFMA: tile side), splits: split-K factor, amax_fused, stats_fused: side outputs made by the tensor-core epilogue)."""
+        d = _cabi.GemmDesc(alpha=1.0, stride=1, pad=1, batch=1, heads=1, rows_per_batch=1)
+        for name, v in fields.items():
+            if name in self.GEMM_POINTERS:
+                if v is not None:
+                    want = torch.float64 if name == 'c_stats' else torch.float32
+                    assert torch.is_tensor(v) and v.dtype == want and v.device == self.device, f'op_gemm: {name} must be a {want} tensor on {self.device}'
+                setattr(d, name, v.data_ptr() if v is not None else None)
+            else:
+                assert hasattr(d, name), f'op_gemm: no field {name}'
+                setattr(d, name, v)
+        plan = C.c_int(0)
+        check(lib.cdx_op_gemm(self.h, C.byref(d), C.byref(plan), self.stream))
+        return self.gemm_plan(plan.value)
+
+    @classmethod
+    def gemm_plan(cls, p):
+        """decode the plan word cdx_op_gemm reports"""
+        return dict(kind=cls.GEMM_KINDS[(p >> 4) & 3] if p & 8 else 'ffma', width=(p >> 8) & 255, splits=(p >> 16) & 255,
+                    amax_fused=bool(p & 1), stats_fused=bool(p & 2))
+
     def op_attention(self, q, k, v, heads, scale):
         q, k, v = (_f32c(t, self.device) for t in (q, k, v))
         B, Nq, Cc = q.shape

@@ -487,6 +487,44 @@ int cdx_op_produce_norm(cdx_engine* e, const float* x, const float* w, const flo
                         int Cout, const float* gamma, const float* beta, float eps, float* y, float* amax_out, double* stats_out,
                         float* yn, int* path_out, void* stream);
 
+/* One contraction through the engine's production GEMM with every epilogue term the network executors use
+ * (tests/test_gemm_epilogue_gpu.py):
+ *   C[m, n] = alpha * sum_k A(m, k) W(n, k) (+ bias[n]) (+ rowvec[m / rows_per_batch, n]) (+ residual[m, n])
+ * mode 0: dense; A(m, k) = A[m * lda + k] for k < C1, else A2[m * lda2 + k - C1] (K = C1 + C2); W [N][K] with row stride ldb
+ *   (b_kn == 1: [K][N], FFMA only); batch * heads > 1: blockIdx.z-batched products with the s*_b / s*_h element strides (FFMA only).
+ * mode 1: conv3x3 of NHWC A [B, Hin, Win, C1] (pixel stride lda) to an [B, Hout, Wout] grid, stride 1 or 2, low-side padding pad;
+ *   w OIHW [N, C1, 3, 3], repacked here (K = 9 C1, ldb ignored).
+ * Outputs, caller-allocated with caller strides: C [M, ldc] (geglu: [M, N/2] of value * gelu(gate) over [32 value | 32 gate] row
+ * blocks of w; out_nchw: [M / rows_per_img, N, rows_per_img]); C_lo optional: C <- rn_tf32(result), C_lo <- rn_tf32(result - C);
+ * Ct_hi / Ct_lo optional: columns n >= t_col0 go transposed as TF32 planes to Ct[(n - t_col0) * ldt + m]; c_amax (device float)
+ * <- max(c_amax, max |stored C|); c_stats (device [M / rows_per_batch, N, 2] doubles) += per-(image, channel) {sum, sum sq}.
+ * a_amax / a2_amax: tracked range slots of A / A2 (device floats), or NULL (measured here).  w_range > 0: the fp16 weight planes
+ * take the exponent of max(w_range, max |w|), as in a net whose weight exponent comes from a larger weight elsewhere.
+ * *plan_out (host): how the call ran -- bit 3 tensor cores; bits 0-2 range fused, statistics fused, split-K; bits 4-5 operand kind
+ * (0 SS, 1 TS, 2 fp16 split, 3 one-term fp16); bits 8-15 tile width (FFMA: tile side); bits 16-23 split-K factor. */
+typedef struct cdx_gemm_desc {
+  int mode, M, N, K;
+  const float* A; int lda; int C1;
+  const float* A2; int lda2; int C2;
+  int Hin, Win, Hout, Wout, stride, pad;
+  const float* w; int ldb; int b_kn;
+  const float* bias;
+  const float* rowvec; int ld_rowvec; int rows_per_batch;
+  const float* residual; int ldr;
+  float alpha;
+  int geglu;
+  int out_nchw, rows_per_img;
+  float* C; int ldc;
+  float* C_lo;
+  float* Ct_hi; float* Ct_lo; int t_col0; int64_t ldt;
+  const float* a_amax; const float* a2_amax;
+  float* c_amax; double* c_stats;
+  float w_range;
+  int batch, heads;
+  int64_t sA_b, sA_h, sB_b, sB_h, sC_b, sC_h;
+} cdx_gemm_desc;
+int cdx_op_gemm(cdx_engine* e, const cdx_gemm_desc* desc, int* plan_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -48,6 +48,10 @@ class PixelCoef(C.Structure):
 _P = C.c_void_p          # device / opaque pointers
 
 
+class AttnControl(C.Structure):
+    _fields_ = [('cross_steps', C.c_int), ('self_steps', C.c_int), ('self_max_tokens', C.c_int), ('token_map', C.c_void_p)]
+
+
 class GemmDesc(C.Structure):
     _fields_ = [('mode', C.c_int), ('M', C.c_int), ('N', C.c_int), ('K', C.c_int),
                 ('A', _P), ('lda', C.c_int), ('C1', C.c_int), ('A2', _P), ('lda2', C.c_int), ('C2', C.c_int),
@@ -113,6 +117,8 @@ SIGNATURES = {
                                 _P]),
     'cdx_cycle_lockstep_masked': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I, _I,
                                        _I, _P, _P]),
+    'cdx_cycle_lockstep_ctl': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I, _I,
+                                    _I, _P, _P, C.POINTER(AttnControl)]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),
@@ -139,6 +145,7 @@ SIGNATURES = {
     'cdx_op_groupnorm': (_I, [_P, _P, _P, _P, _F, _I, _P, _I, _I, _I, _P]),
     'cdx_op_layernorm': (_I, [_P, _P, _P, _P, _P, _I, _I, _P]),
     'cdx_op_attention': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    'cdx_op_attention_rows': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, C.POINTER(_I), _P]),
     'cdx_op_nchw_to_nhwc': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_nhwc_to_nchw': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_groupnorm_ex': (_I, [_P, _P, _I, _P, _I, _P, _P, _F, _I, _P, _P, _I, _P, _P, _P, _I, _I, _P]),

@@ -1,0 +1,93 @@
+"""Prompt-to-Prompt attention control (Hertz et al., 2022; "Cross Attention Control") for the lock-step cycle.
+
+The "replace" edit: in the first steps of the loop the target chain's conditional row attends with the source row's attention
+probabilities (cross-attention remapped through a token map, self-attention copied), so the edit keeps the source image's layout.
+The engine does it inside the fused attention kernel (include/cdx.h, cdx_cycle_lockstep_ctl); this module holds the value the
+Python surfaces take and the host helper that builds a token map.
+"""
+from dataclasses import dataclass
+
+import torch
+
+from . import _cabi
+
+
+def _fraction(name, f):
+    if isinstance(f, bool) or not isinstance(f, (int, float)) or not 0.0 <= float(f) <= 1.0:
+        raise ValueError(f'{name} must be a fraction in [0, 1], got {f!r}')
+    return float(f)
+
+
+@dataclass(frozen=True)
+class AttentionControl:
+    """cross_steps / self_steps: fractions of the loop's n steps; steps i < int(f * n) are controlled.  self_max_tokens: the
+    self-attention layers of at most this many tokens are controlled (256: the 16x16 and 8x8 levels at 512^2).  token_map:
+    optional float tensor [L, L] or [B, L, L], source token -> target token (P2P's mapper times its equalizer); None is the
+    identity."""
+    cross_steps: float
+    self_steps: float
+    self_max_tokens: int = 256
+    token_map: object = None
+
+    def __post_init__(self):
+        _fraction('cross_steps', self.cross_steps)
+        _fraction('self_steps', self.self_steps)
+        if isinstance(self.self_max_tokens, bool) or not isinstance(self.self_max_tokens, int) or self.self_max_tokens < 0:
+            raise ValueError(f'self_max_tokens must be an integer >= 0, got {self.self_max_tokens!r}')
+        if self.token_map is not None and not torch.is_tensor(self.token_map):
+            raise ValueError(f'token_map must be a tensor [L, L] or [B, L, L], got {type(self.token_map)}')
+
+    def steps(self, n):
+        """(cross_steps, self_steps) as step counts of an n-step loop."""
+        return int(self.cross_steps * n), int(self.self_steps * n)
+
+    def device_map(self, B, L, device):
+        """The token map as a contiguous float32 [B, L, L] tensor on `device`, or None."""
+        A = self.token_map
+        if A is None:
+            return None
+        if A.dim() == 2:
+            A = A.unsqueeze(0).expand(B, -1, -1)
+        if A.dim() != 3 or tuple(A.shape) != (B, L, L):
+            raise ValueError(f'token_map: expected [{L}, {L}] or [{B}, {L}, {L}], got {tuple(self.token_map.shape)}')
+        A = A.to(device=device, dtype=torch.float32).contiguous()
+        if not bool(torch.isfinite(A).all()):
+            raise ValueError('token_map must be finite')
+        return A
+
+    def c_struct(self, n, B, L, device):
+        """-> (cdx_attn_control for an n-step loop, the device token map it points to; keep it alive over the call)."""
+        A = self.device_map(B, L, device)
+        cross, self_ = self.steps(n)
+        return _cabi.AttnControl(cross, self_, self.self_max_tokens, A.data_ptr() if A is not None else None), A
+
+
+def replace_token_map(src_ids, tgt_ids, L):
+    """P2P's "replace" mapper for two prompts' token ids (BOS and EOS included, before padding) that differ in one contiguous
+    run: -> float32 [L, L], source position -> target position.  Identity on the common prefix; the differing run one-to-one when both runs have the same length, else every
+    source token of the run to every target token of it with weight 1 / len(target run); the rest shifted by the length
+    difference, positions pushed past L dropped.  Identical sequences give the identity."""
+    src, tgt = [int(t) for t in src_ids], [int(t) for t in tgt_ids]
+    A = torch.zeros(L, L, dtype=torch.float32)
+    p = 0
+    while p < min(len(src), len(tgt)) and src[p] == tgt[p]:
+        p += 1
+    s = 0                                              # common suffix, not reaching into the prefix
+    while s < min(len(src), len(tgt)) - p and src[len(src) - 1 - s] == tgt[len(tgt) - 1 - s]:
+        s += 1
+    ns, nt = len(src) - p - s, len(tgt) - p - s       # the differing runs [p, p + ns) and [p, p + nt)
+    for i in range(min(p, L)):
+        A[i, i] = 1.0
+    if ns == nt:
+        for k in range(ns):
+            if p + k < L:
+                A[p + k, p + k] = 1.0
+    elif nt > 0:
+        for i in range(p, min(p + ns, L)):
+            for j in range(p, min(p + nt, L)):
+                A[i, j] = 1.0 / nt
+    shift = nt - ns
+    for i in range(p + ns, L):                          # the suffix, and the padding past the prompts, shifted
+        if i + shift < L:
+            A[i, i + shift] = 1.0
+    return A

@@ -170,7 +170,16 @@ struct ChainLoopArgs {
   const float* extra = nullptr;                     // noise of the steps past n_eps (no src) / past n_rec (src)
   float* x_out = nullptr;                           // K > 0: [n_src*K, chw]
   const float* mask = nullptr;                      // optional [n_src, 1, h, w]: masked editing (LatentChains::mask)
+  const cdx_attn_control* ctl = nullptr;           // optional: attention control of each target chain's cond row (cdx.h)
   int C = 0, h = 0, w = 0;
+};
+
+// RAII: the engine's contractions on the exact-fp32 FFMA path for one scope
+struct ExactFp32 {
+  Engine& e;
+  int mode;
+  explicit ExactFp32(Engine& eng) : e(eng), mode(eng.mma_mode) { e.mma_mode = 0; }
+  ~ExactFp32() { e.mma_mode = mode; }
 };
 
 // v-prediction nets (cdx_unet_set_prediction): every U-Net timestep of the loop must index the net's sqrt(abar) tables
@@ -214,6 +223,16 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   // a masked target chain takes its source chain's x_{t-1} outside the mask, so every step needs one
   CDX_CHECK(!a.mask || (a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net), "masked latent loop: needs a source chain at every step");
   check_v_steps(unet, a.t_host, loop_steps);
+  if (a.ctl) {
+    const cdx_attn_control& c = *a.ctl;
+    CDX_CHECK(a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net && !a.scales_on_device,
+              "attention control: needs the lock-step loop with a source chain at every step");
+    CDX_CHECK(ctx_n > 0 && a.c_src && a.c_tgt, "attention control: needs a net with a context and both prompts");
+    CDX_CHECK(e.mma_mode == 1 && e.flash_attn, "attention control: needs the fused attention kernel (mma modes 1, 3, 4 or 5)");
+    CDX_CHECK(c.cross_steps >= 0 && c.cross_steps <= a.n_steps && c.self_steps >= 0 && c.self_steps <= a.n_steps && c.self_max_tokens >= 0,
+              "attention control: cross_steps=%d self_steps=%d (of %d) self_max_tokens=%d", c.cross_steps, c.self_steps, a.n_steps,
+              c.self_max_tokens);
+  }
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
   struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
@@ -246,6 +265,42 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       for (int k = 0; k < a.K; ++k) ctx_rows(ch[a.n_src + (size_t)j * a.K + k], a.c_tgt, j);
     }
   }
+  // attention control: the row table maps each target chain's cond row to its group's source row (every other row to itself); with
+  // a token map, the V context holds A_j . c_tgt[j] on those rows and every other row's own context.  Both fixed for the loop
+  AttnControl actl;
+  if (a.ctl) {
+    std::vector<int> qk(rows);
+    for (int r = 0; r < rows; ++r) qk[r] = r;
+    for (int j = 0; j < a.n_src; ++j) {
+      CDX_CHECK(!a.uc || ch[j].scale != 0.0f, "attention control: the source chain at scale 0 has no source-prompt row");
+      for (int k = 0; k < a.K; ++k) {
+        const Chain& t = ch[a.n_src + (size_t)j * a.K + k];
+        CDX_CHECK(!a.uc || t.scale != 0.0f, "attention control: the target chain at scale 0 has no target-prompt row");
+        qk[t.row] = ch[j].row;
+      }
+    }
+    int* qk_dev = (int*)e.arena.alloc((size_t)rows * sizeof(int));
+    if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(qk_dev, qk.data(), qk.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+    actl.qk_row = qk_dev;
+    actl.self_max_tokens = a.ctl->self_max_tokens;
+    if (a.ctl->token_map) {
+      const int D = unet.ucfg.context_dim;
+      float* cv = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
+      copy_dd(e, ctx_in, cv, (size_t)rows * ctx_n, s);
+      ExactFp32 exact(e);
+      for (int j = 0; j < a.n_src; ++j)
+        for (int k = 0; k < a.K; ++k) {
+          GemmArgs g;                                // cv[row] = A_j [L, L] . c_tgt[j] [L, D]
+          g.mode = 0;
+          g.M = a.L; g.N = D; g.K = a.L;
+          g.A = a.ctl->token_map + (size_t)j * a.L * a.L; g.lda = a.L; g.C1 = a.L;
+          g.Bw = a.c_tgt + (size_t)j * ctx_n; g.ldb = D; g.b_kn = 1;
+          g.Cout = cv + (size_t)ch[a.n_src + (size_t)j * a.K + k].row * ctx_n; g.ldc = D;
+          gemm(e, g, s);
+        }
+      actl.ctx_v = cv;
+    }
+  }
   auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
     if (i_next >= a.n_rec) return 0;
     return (a.n_steps - 1 - i_next) == 0 ? 2 : 1;                               // ddim.py:583-584
@@ -270,7 +325,9 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   for (int i = 0; i < iters; ++i) {
     const bool src_i = a.src && i < a.n_rec;
     if (!tgt_net) {
-      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true);
+      actl.cross = a.ctl && i < a.ctl->cross_steps;
+      actl.self = a.ctl && i < a.ctl->self_steps;
+      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true, a.ctl ? &actl : nullptr);
     } else {
       ps.fork();
       if (src_i) unet_forward(unet, xin, tdev + (size_t)i * rows, nullptr, 0, eout, rows_src, a.h, a.w, s);
@@ -673,6 +730,14 @@ int cdx_cycle_lockstep_masked(cdx_net* un, const float* x0, const float* c_src, 
                               float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
                               float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
                               const float* mask) {
+  return cdx_cycle_lockstep_ctl(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T,
+                                x_out, z_out, B, C, h, w, stream, mask, nullptr);
+}
+
+int cdx_cycle_lockstep_ctl(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                           float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                           float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                           const float* mask, const cdx_attn_control* ctl) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -682,7 +747,7 @@ int cdx_cycle_lockstep_masked(cdx_net* un, const float* x0, const float* c_src, 
     a.n_src = B; a.K = 1; a.src = true;
     a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scales = s_scales.data(); a.t_scales = t_scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
-    a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.C = C; a.h = h; a.w = w;
+    a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.C = C; a.h = h; a.w = w;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -972,8 +1037,13 @@ int cdx_op_layernorm(cdx_engine* eh, const float* x, const float* gamma, const f
 }
 int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d, float scale,
                      void* stream) {
+  return cdx_op_attention_rows(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, stream);
+}
+int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
+                          float scale, const int* qk_rows, void* stream) {
   return guard([&] {
     CDX_CHECK(eh && q && k && v && out, "op_attention: null argument");
+    if (qk_rows) for (int b = 0; b < B; ++b) CDX_CHECK(qk_rows[b] >= 0 && qk_rows[b] < B, "op_attention: qk_rows[%d] = %d outside [0, %d)", b, qk_rows[b], B);
     const int C = heads * d;
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
@@ -981,6 +1051,12 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
       Scope sc(e.arena);
       bool done = false;
       const bool fused = flash_eligible(e, Nq, Nk, d, C);
+      CDX_CHECK(!qk_rows || fused, "op_attention: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, d);
+      int* rows_dev = nullptr;
+      if (qk_rows) {
+        rows_dev = (int*)e.arena.alloc((size_t)B * sizeof(int));
+        if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(rows_dev, qk_rows, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+      }
       if (fused && e.tc_kind >= 1) {
         // the SpatialTransformer's fp16-split path on loose q / k / v: ranges measured here, keys padded to a multiple of 8 per image
         e.pools_reset(s);
@@ -1011,7 +1087,7 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
         split_rows_h16(e, q, M, C, C, qh, ql, C, qa, s);
         split_rows_h16(e, kp, Mk, C, C, kh, kl, C, ka, s);
         split_transpose_h16(e, vp, Mk, C, C, vh, vl, va, s);
-        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s);
+        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev);
       }
       if (!done && e.mma_mode == 1 && Nq == Nk && (Nq % 32) == 0 && Nq >= 128 && (d % 4) == 0) {
         // same operand preparation as the SpatialTransformer: q|k side by side, V transposed, TF32 planes
@@ -1030,8 +1106,9 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
           float* vl = (float*)e.arena.alloc((size_t)C * M * sizeof(float));
           split_planes(e, qk, qh, ql, (size_t)M * 2 * C, s);
           split_planes(e, vt, vh, vl, (size_t)C * M, s);
-          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s);
+          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev);
         }
+        CDX_CHECK(done || !rows_dev, "op_attention: the fused kernel rejected a row-table shape");
         if (!done) done = attention_tc(e, qk, 2 * C, qk + C, 2 * C, d, vt, out, C, B, Nq, Nk, heads, d, scale, s);
       }
       if (!done && fused) {
@@ -1056,8 +1133,9 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
         split_planes(e, q, qh, ql, (size_t)M * C, s);
         split_planes(e, kp, kh, kl, (size_t)Mk * C, s);
         split_planes(e, vt, vh, vl, (size_t)C * Mk, s);
-        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s);
+        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev);
       }
+      CDX_CHECK(done || !rows_dev, "op_attention: the fused kernel rejected a row-table shape");
       if (!done) attention(e, q, C, k, C, v, C, out, C, B, Nq, Nk, heads, d, d, scale, s);
     });
   });

@@ -87,6 +87,9 @@ struct AttnParams {
   float scale_log2e;      // scale * log2(e): scores are kept in the log2 domain
   float* out; int ldo;
   const float *q_amax, *k_amax, *v_amax;   // F16: tracked max |q|, |k|, |v| (the planes hold x * 2^h16_exp_of(amax))
+  // optional [B]: image qk_row[b] supplies the Q and K tiles of image b (attention control: a target row attends with its source
+  // row's probabilities); V^T and the output stay image b's.  Null: every image its own
+  const int* qk_row;
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -139,11 +142,12 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     // =========================================================================== TMA producer
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
+      const int bqk = p.qk_row ? __ldcg(p.qk_row + b) : b;    // (coherent: read after the dependent-launch wait)
       const uint32_t sq = base + C::OFF_Q;
       mbar_expect_tx(bar_q_full, C::NPL * C::Q_PLANE);
       for (int kb = 0; kb < KB2; ++kb) {
-        tma_load_4d(sq + kb * QR * 128, &mapQh, kb * KW, h, q0, b, bar_q_full);
-        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * QR * 128, &mapQl, kb * KW, h, q0, b, bar_q_full);
+        tma_load_4d(sq + kb * QR * 128, &mapQh, kb * KW, h, q0, bqk, bar_q_full);
+        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * QR * 128, &mapQl, kb * KW, h, q0, bqk, bar_q_full);
       }
       for (int j = 0; j < nb; ++j) {
         // K block j: [64 keys x d] hi + lo
@@ -152,8 +156,8 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
         const uint32_t sk = base + C::OFF_K + s * C::K_STAGE;
         mbar_expect_tx(bar_k_full(s), C::K_STAGE);
         for (int kb = 0; kb < KB2; ++kb) {
-          tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, b, bar_k_full(s));
-          if (!ONE) tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, b, bar_k_full(s));
+          tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, bqk, bar_k_full(s));
+          if (!ONE) tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, bqk, bar_k_full(s));
         }
         // V^T block j: [NV channel rows x 64 keys] (TF32: two 32-key tiles), hi + lo
         const int sv_ = j % VS;
@@ -529,7 +533,7 @@ bool flash_eligible(const Engine& e, int N, int Nk, int d, int C) {
 
 bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
                         const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d,
-                        float scale, cudaStream_t s) {
+                        float scale, cudaStream_t s, const int* qk_row) {
   if (N < 1 || (d % 8) || d < 16 || d > 80 || (ldq & 3) || (ldk & 3) || (ldo & 3) || (Nvs & 3) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
   if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) return false;
   if (!a16(q_hi) || !a16(q_lo) || !a16(k_hi) || !a16(k_lo) || !a16(vt_hi) || !a16(vt_lo) || !a16(out)) return false;
@@ -554,6 +558,7 @@ bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq
   p.scale_log2e = scale * 1.4426950408889634f;
   p.out = out; p.ldo = ldo;
   p.q_amax = p.k_amax = p.v_amax = nullptr;
+  p.qk_row = qk_row;
   ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * B * heads, 4.0 * B * heads * (2.0 * N * d + 2.0 * (double)Nk * d), 1);
   switch (d) {
     case 16: launch_flash<16, false>(qh, ql, kh, kl, vh, vl, p, s); break;
@@ -600,7 +605,7 @@ void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long l
 // split_transpose_h16 above).  ld and Nvs multiples of 8.  All three lo planes null: the one-term kernel (hi * hi products only, mma mode 5).
 bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
                          const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
-                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s) {
+                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s, const int* qk_row) {
   if (N < 1 || (ldq & 7) || (ldk & 7) || (ldo & 3) || (Nvs & 7) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
   if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || d == 160)) return false;
   const bool one = q_lo == nullptr;
@@ -629,6 +634,7 @@ bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq,
   p.scale_log2e = scale * 1.4426950408889634f;
   p.out = out; p.ldo = ldo;
   p.q_amax = q_amax; p.k_amax = k_amax; p.v_amax = v_amax;
+  p.qk_row = qk_row;
   ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * B * heads,
                (one ? 1.0 : 2.0) * B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + 4.0 * B * heads * (double)N * d, 1);
   if (one) {

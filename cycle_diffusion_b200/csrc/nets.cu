@@ -694,6 +694,9 @@ struct UNetExec : Exec {
   const float* ctx_pad = nullptr;   // context zero-padded to ctx_lp rows per image (tensor-core cross-attention)
   int ctx_lp = 0;
   bool kv_reuse = false, kv_hit = false;   // loop mode: context K / V live in n.ctxkv (kv_hit: already computed)
+  const AttnControl* ctl = nullptr;        // attention control of this call, or null
+  const float* ctxv_pad = nullptr;         // ctl->ctx_v zero-padded to ctx_lp rows per image, and its range
+  float* ctxv_amax = nullptr;
   size_t kv_off = 0;
   float* kv_take(size_t floats) {
     if (!kv_reuse) return (float*)e.arena.alloc(floats * sizeof(float));
@@ -710,6 +713,11 @@ struct UNetExec : Exec {
     if (!kv_reuse) return e.amax_slot();
     CDX_CHECK(kv_layer < Net::CtxKV::MAX_LAYERS, "too many cross-attention layers for the context cache");
     return e.dry() ? reinterpret_cast<float*>((uintptr_t)0x100) : n.ctxkv.amax + 1 + kv_layer++;
+  }
+  // V' range slot = max(the layer's K | V range, max |V'|): starts as a copy of the K | V slot, the V' projection maxes into it, so
+  // an identity token map leaves every exponent (and the output's range) as without control
+  void v2_range(const float* kv_slot, float* v2_slot) {
+    if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(v2_slot, kv_slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
   }
   bool oai;
   UNetExec(Net& net, cudaStream_t st) : Exec(net, st), oai(net.kind == NET_UNET_OPENAI) {}
@@ -779,6 +787,9 @@ struct UNetExec : Exec {
       a.amax = e.amax_slot();                   // <- max |V| (written by whichever projection produces V)
       bool done = false;
       const bool flash_ok = flash_eligible(e, HW, HW, d, C);
+      const int* srow = (ctl && ctl->self && HW <= ctl->self_max_tokens) ? ctl->qk_row : nullptr;
+      CDX_CHECK(!srow || flash_ok, "attention control: self-attention at HW=%d d=%d would take the unfused route (mma mode and head width "
+                "must run the fused kernel)", HW, d);
       if (flash_ok && e.tc_kind >= 1) {
         // fp16-split fused attention: ONE plain fp32 q|k|v projection (its range tracked by the epilogue), then one pass that
         // writes the fp16 hi / lo planes of q|k and of V^T (both P.V operands K-major for wgmma) with the tensor's exponent.
@@ -797,7 +808,7 @@ struct UNetExec : Exec {
         split_rows_h16(e, qkv, M, 2 * C, 3 * C, qk_hi, qk_lo, 2 * C, a.amax, s);
         split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s, B, Nvs);
         done = flash_attention_h16(e, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr, 2 * C,
-                                   vt_hi, vt_lo, a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s);
+                                   vt_hi, vt_lo, a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow);
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok && (HW % 4) != 0) {
         // TF32 planes with a per-image key count off the 16-byte TMA granule: V row-major, copied into rows padded to Nvs keys
@@ -820,7 +831,8 @@ struct UNetExec : Exec {
         }
         nhwc_to_nchw(e, vp, vt, 1, C, B * Nvs, s);
         split_planes(e, vt, vt_hi, vt_lo, nvt, s);
-        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s);
+        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s,
+                                  srow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands
@@ -850,7 +862,8 @@ struct UNetExec : Exec {
           linear_into(n.P(t + ".attn1.to_v.weight"), C, C, nullptr, 0, 0, C, n1.p, M, nullptr, nullptr, 0, vt_hi, M, vt_lo, nullptr, nullptr,
                       a.amax);   // V^T = Wv . X^T
         }
-        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s);
+        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s,
+                                  srow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (e.mma_mode >= 1 && (HW % 32) == 0 && HW >= 128 && (d % 4) == 0) {
         // unfused tensor-core attention (mode 2, or shapes the fused kernel does not cover)
@@ -885,9 +898,17 @@ struct UNetExec : Exec {
       const int D = n.ucfg.context_dim;
       Tensor a = alloc(B, x.H, x.W, C);
       a.amax = kv_amax();                       // <- max |V| of the context projection (lives with the cached K / V in loop mode)
+      // attention control: controlled rows attend with their source row's Q / K; with a V context every row reads V'^T (the
+      // token-mapped context's projection; its range slot also bounds this call's output) instead of V^T
+      const bool vmap = ctl && ctl->ctx_v;
+      float* v2_amax = vmap ? kv_amax() : nullptr;
+      const int* crow = (ctl && ctl->cross) ? ctl->qk_row : nullptr;
+      const bool use_v2 = crow && vmap;
       bool done = false;
       Tensor q;
       const bool flash_ok = ctx_pad && flash_eligible(e, HW, ctx_len, d, C);
+      CDX_CHECK(!crow || flash_ok, "attention control: cross-attention at HW=%d d=%d would take the unfused route (mma mode "
+                "and head width must run the fused kernel)", HW, d);
       if (flash_ok && e.tc_kind >= 1) {
         // fp16-split fused attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the kernel):
         // q projected as plain fp32 (range tracked), K | V from one fused projection of the context; fp16 planes by the split pass.
@@ -901,6 +922,8 @@ struct UNetExec : Exec {
         float* k_lo = lo ? kv_take(nk / 2) : nullptr;
         float* vt_hi = kv_take(nk / 2);
         float* vt_lo = lo ? kv_take(nk / 2) : nullptr;
+        float* v2_hi = vmap ? kv_take(nk / 2) : nullptr;
+        float* v2_lo = vmap && lo ? kv_take(nk / 2) : nullptr;
         Tensor qf = linear(n2, t + ".attn2.to_q", false, nullptr, true);
         void* q_hi = e.arena.alloc((size_t)M * C * 2);
         void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
@@ -912,9 +935,15 @@ struct UNetExec : Exec {
                       a.amax);
           split_rows_h16(e, kvf, Mk, C, 2 * C, k_hi, k_lo, C, a.amax, s);
           split_transpose_h16(e, kvf + C, Mk, C, 2 * C, vt_hi, vt_lo, a.amax, s);
+          if (vmap) {             // the same fused K | V projection of the V context (its K half unused): an identity map gives V' == V
+            v2_range(a.amax, v2_amax);
+            linear_into(ctxv_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, ctxv_amax,
+                        nullptr, v2_amax);
+            split_transpose_h16(e, kvf + C, Mk, C, 2 * C, v2_hi, v2_lo, v2_amax, s);
+          }
         }
-        done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, vt_hi, vt_lo, qf.amax, a.amax, a.amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads,
-                                   d, scale, s);
+        done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, use_v2 ? v2_hi : vt_hi, use_v2 ? v2_lo : vt_lo, qf.amax, a.amax,
+                                   use_v2 ? v2_amax : a.amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, crow);
         CDX_CHECK(done, "flash cross-attention (fp16-split) rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
       } else if (flash_ok) {
         // fused tensor-core attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the
@@ -926,6 +955,8 @@ struct UNetExec : Exec {
         float* k_lo = kv_take(nk);
         float* vt_hi = kv_take(nk);
         float* vt_lo = kv_take(nk);
+        float* v2_hi = vmap ? kv_take(nk) : nullptr;
+        float* v2_lo = vmap ? kv_take(nk) : nullptr;
         float* q_hi = (float*)e.arena.alloc(nq * sizeof(float));
         float* q_lo = (float*)e.arena.alloc(nq * sizeof(float));
         linear_into(n2.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn2.to_q.weight"), C, nullptr, nullptr, 0, q_hi, C, q_lo, n2.amax);
@@ -933,10 +964,17 @@ struct UNetExec : Exec {
           linear_into(ctx_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), C, nullptr, nullptr, 0, k_hi, C, k_lo, ctx_amax);
           linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctx_pad, Mk, nullptr, nullptr, 0, vt_hi, Mk, vt_lo, nullptr, nullptr,
                       a.amax);
+          if (vmap) {
+            v2_range(a.amax, v2_amax);
+            linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctxv_pad, Mk, nullptr, nullptr, 0, v2_hi, Mk, v2_lo, nullptr, nullptr,
+                        v2_amax);
+          }
         }
-        done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, vt_hi, vt_lo, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s);
+        done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, use_v2 ? v2_hi : vt_hi, use_v2 ? v2_lo : vt_lo, a.p, C, B, HW, ctx_len, ctx_lp,
+                                  ctx_lp, heads, d, scale, s, crow);
         CDX_CHECK(done, "flash cross-attention rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
       }
+      if (use_v2) a.amax = v2_amax;             // the output is a convex combination of V' rows
       if (!done) q = linear(n2, t + ".attn2.to_q", false);
       if (!done) {
         Scope sa(e.arena);
@@ -1087,7 +1125,7 @@ struct UNetExec : Exec {
       size_t sumC = 0;
       for (const Param& pp : n.params)
         if (pp.name.size() > 17 && pp.name.compare(pp.name.size() - 17, 17, "attn2.to_k.weight") == 0) sumC += (size_t)pp.dims[0] + 64;
-      const size_t need = 4 * (size_t)B * ctx_lp * sumC;
+      const size_t need = (ctl && ctl->ctx_v ? 6 : 4) * (size_t)B * ctx_lp * sumC;      // K, V (and V') hi + lo planes
       if (kc.cap < need) {
         CDX_CUDA(cudaDeviceSynchronize());
         if (kc.buf) CDX_CUDA(cudaFree(kc.buf));
@@ -1095,7 +1133,7 @@ struct UNetExec : Exec {
         CDX_CUDA(cudaMalloc(&kc.buf, need * sizeof(float)));
         kc.cap = need;
       }
-      kv_hit = kc.valid && kc.ctx == context && kc.L == L && kc.B == B && !e.dry();
+      kv_hit = kc.valid && kc.ctx == context && kc.ctx_v == (ctl ? ctl->ctx_v : nullptr) && kc.L == L && kc.B == B && !e.dry();
       if (!kc.amax) {
         CDX_CUDA(cudaMalloc(&kc.amax, (Net::CtxKV::MAX_LAYERS + 1) * sizeof(float)));
         CDX_CUDA(cudaMemset(kc.amax, 0, (Net::CtxKV::MAX_LAYERS + 1) * sizeof(float)));
@@ -1107,6 +1145,10 @@ struct UNetExec : Exec {
       // range of the context (A operand of the K / V projections; measured once per loop)
       ctx_amax = kv_reuse ? (e.dry() ? reinterpret_cast<float*>((uintptr_t)0x100) : n.ctxkv.amax) : e.amax_slot();
       if (!kv_hit) amax_rows(e, context, (long long)B * L, c.context_dim, c.context_dim, ctx_amax, s);
+      if (ctl && ctl->ctx_v) {
+        ctxv_amax = kv_amax();
+        if (!kv_hit) amax_rows(e, ctl->ctx_v, (long long)B * L, c.context_dim, c.context_dim, ctxv_amax, s);
+      }
     }
     if (context && L > 0 && e.mma_mode == 1 && e.flash_attn) {
       // context rows padded to a multiple of 8 per image: TMA needs 16-byte strides for K and V^T of the cross-attention
@@ -1117,6 +1159,14 @@ struct UNetExec : Exec {
         CDX_CUDA(cudaMemcpy2DAsync(cp, (size_t)ctx_lp * D * 4, context, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
       }
       ctx_pad = cp;
+      if (ctl && ctl->ctx_v) {
+        float* vp = (float*)e.arena.alloc((size_t)B * ctx_lp * D * sizeof(float));
+        if (!e.dry() && !kv_hit) {
+          if (ctx_lp != L) CDX_CUDA(cudaMemsetAsync(vp, 0, (size_t)B * ctx_lp * D * sizeof(float), s));
+          CDX_CUDA(cudaMemcpy2DAsync(vp, (size_t)ctx_lp * D * 4, ctl->ctx_v, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
+        }
+        ctxv_pad = vp;
+      }
     }
     // --- timestep embedding MLP + all ResBlock emb projections in one GEMM
     Tensor temb = alloc(B, 1, 1, mc);
@@ -1243,7 +1293,7 @@ struct VaeExec : Exec {
 }  // namespace
 
 void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* ctx, int ctx_len, float* out_nchw, int B, int H, int W,
-                  cudaStream_t s, bool reuse_ctx) {
+                  cudaStream_t s, bool reuse_ctx, const AttnControl* ctl) {
   CDX_CHECK(n.kind == NET_UNET_OPENAI || n.kind == NET_UNET_IDDPM || n.kind == NET_UNET_DDPM, "unet_forward on a non-U-Net");
   CDX_CHECK(n.finalized, "unet_forward before finalize");
   if (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0) CDX_CHECK(ctx != nullptr && ctx_len > 0, "unet_forward: the SD/LDM U-Net needs a context");
@@ -1251,11 +1301,14 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
   CDX_CHECK(H % down == 0 && W % down == 0, "unet_forward: %dx%d not divisible by %d", H, W, down);
   UNetExec ex(n, s);
   ex.kv_reuse = reuse_ctx && n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0;
+  CDX_CHECK(!ctl || !ctl->qk_row || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0),
+            "attention control: SD / LDM U-Nets with a context only");
+  ex.ctl = ctl;
   if (n.kind == NET_UNET_DDPM) { ex.forward_ddpm(x_nchw, t_dev, out_nchw, B, H, W); return; }
   ex.forward(x_nchw, t_dev, ctx, ctx_len, out_nchw, B, H, W);
   if (ex.kv_reuse && !n.eng->dry()) {
     n.ctxkv.valid = true;
-    n.ctxkv.ctx = ctx; n.ctxkv.L = ctx_len; n.ctxkv.B = B;
+    n.ctxkv.ctx = ctx; n.ctxkv.ctx_v = ctl ? ctl->ctx_v : nullptr; n.ctxkv.L = ctx_len; n.ctxkv.B = B;
   }
 }
 

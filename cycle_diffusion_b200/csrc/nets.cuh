@@ -53,8 +53,9 @@ struct Net {
   // computed by the first U-Net call of the loop, reused by the others (the reference recomputes them every step)
   struct CtxKV {
     static constexpr int MAX_LAYERS = 63;
-    bool valid = false; const float* ctx = nullptr; int L = 0, B = 0; float* buf = nullptr; size_t cap = 0;
-    float* amax = nullptr;     // [0]: max |context|, [1 + layer]: max |V| of that layer's context projection (device)
+    bool valid = false; const float* ctx = nullptr; const float* ctx_v = nullptr; int L = 0, B = 0; float* buf = nullptr; size_t cap = 0;
+    // [0]: max |context|, then per layer max |K, V| of its context projection and, with a V context (AttnControl::ctx_v), max |V'|
+    float* amax = nullptr;
   } ctxkv;
   // concatenated ResBlock emb projections: weights [emb_rows][ted] at emb_w_off, biases at emb_b_off
   size_t emb_w_off = 0, emb_b_off = 0;
@@ -79,11 +80,25 @@ void net_ensure_blob(Net& n);
 // channel) sums (for a consumer GroupNorm) -- both produced by the epilogue that holds the tile in registers where it can
 void track_outputs(Engine& e, Tensor& t, GemmArgs& g, bool stats);
 
+// Attention control of one SD / LDM U-Net call (Prompt-to-Prompt's "replace" edit, driven by the lock-step loop in cabi.cu).
+// Row r's fused attention takes its Q and K from row qk_row[r], so its probabilities are that row's; its V stays its own.  Only the
+// fused kernels can do this: a layer that would take another route while control is on is an error.
+struct AttnControl {
+  const int* qk_row = nullptr;          // device [B]; null: no control
+  bool cross = false;                   // remap the cross-attention layers in this call
+  bool self = false;                    // remap the self-attention layers of at most self_max_tokens tokens in this call
+  int self_max_tokens = 0;
+  // optional device [B, L, D]: the context the cross-attention V' is projected from (a controlled row holds A_b . c_tgt[b], every
+  // other row its own context).  Given, the context cache also holds V'^T (own range slot), and cross-controlled calls read it
+  // instead of V^T.  Fixed over the loop, like the context
+  const float* ctx_v = nullptr;
+};
+
 // forward executors (enqueue only; caller handles arena dry-run)
 // reuse_ctx: the caller guarantees `ctx` is unchanged since the previous call with reuse_ctx (and n.ctxkv was invalidated
 // at the start of the loop) -> context K / V projections are taken from n.ctxkv instead of being recomputed
 void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* ctx, int ctx_len, float* out_nchw, int B, int H,
-                  int W, cudaStream_t s, bool reuse_ctx = false);
+                  int W, cudaStream_t s, bool reuse_ctx = false, const AttnControl* ctl = nullptr);
 void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int H, int W, cudaStream_t s);
 void vae_decode(Net& n, const float* z_nchw, float* img_nchw, int B, int h, int w, cudaStream_t s);
 void text_encode(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);

@@ -400,12 +400,20 @@ class Engine:
         return dict(kind=cls.GEMM_KINDS[(p >> 4) & 3] if p & 8 else 'ffma', width=(p >> 8) & 255, splits=(p >> 16) & 255,
                     amax_fused=bool(p & 1), stats_fused=bool(p & 2))
 
-    def op_attention(self, q, k, v, heads, scale):
+    def op_attention(self, q, k, v, heads, scale, qk_rows=None):
+        """softmax(q k^T * scale) v per head.  qk_rows: optional [B] ints, image b attends with image qk_rows[b]'s q and k and its
+        own v (cdx_op_attention_rows; fused kernel only)."""
         q, k, v = (_f32c(t, self.device) for t in (q, k, v))
         B, Nq, Cc = q.shape
         Nk = k.shape[1]
         out = torch.empty_like(q)
-        check(lib.cdx_op_attention(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale, self.stream))
+        if qk_rows is None:
+            check(lib.cdx_op_attention(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale, self.stream))
+        else:
+            rows = [int(r) for r in qk_rows]
+            assert len(rows) == B, f'qk_rows: {len(rows)} entries for {B} images'
+            check(lib.cdx_op_attention_rows(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale,
+                                            (C.c_int * B)(*rows), self.stream))
         return out
 
     def op_nchw_to_nhwc(self, x):
@@ -673,11 +681,13 @@ class UNet(Net):
                                       B, Cc, h, w, e.stream))
         return out
 
-    def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False, mask=None):
+    def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False, mask=None, attn_control=None):
         """Both chains in one loop (one U-Net call + one fused elementwise kernel per step, no z buffer unless asked for):
         x0 [B,C,h,w] -> translated latent [B,C,h,w] (and z [B, n+1, C,h,w] when return_z).  noise as for latent_encode with
         n_rec == sched.refine_steps.  mask [B,1,h,w] in [0,1] (1 = may change): masked editing (cdx_cycle_lockstep_masked), the
-        target chain is blended with the source chain's x_{t-1} after every step; ones give the unmasked result, zeros give x0."""
+        target chain is blended with the source chain's x_{t-1} after every step; ones give the unmasked result, zeros give x0.
+        attn_control: an attn_control.AttentionControl, Prompt-to-Prompt's "replace" edit on the target chain's cond row
+        (cdx_cycle_lockstep_ctl); it composes with mask."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -686,11 +696,13 @@ class UNet(Net):
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
         mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
+        ctl, _token_map = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None else (None, None)
         out = e.empty(B, Cc, h, w)
         z = e.empty(B, n + 1, Cc, h, w) if return_z else None
-        check(lib.cdx_cycle_lockstep_masked(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale),
-                                            float(tgt_scale), sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T,
-                                            sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask)))
+        check(lib.cdx_cycle_lockstep_ctl(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale),
+                                         float(tgt_scale), sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T,
+                                         sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask),
+                                         C.byref(ctl) if ctl is not None else None))
         return (out, z) if return_z else out
 
     def cycle_fan(self, x0, c_src, c_tgt, uc, src_scales, tgt_scales, sched, noise, return_z=False, mask=None):

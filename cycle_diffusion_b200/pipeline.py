@@ -14,6 +14,7 @@ from dataclasses import dataclass
 
 import torch
 
+from .attn_control import AttentionControl
 from .engine import check_mask
 from .schedule import DDIMSchedule
 
@@ -93,6 +94,46 @@ class CycleDiffusionPipeline:
                                             f=None if output_type == 'latent' else g.vae.down, channels=lat_shape[1])
         return mask if output_type == 'latent' else mask_img
 
+    P2P_KEYS = {'edit_type', 'cross_replace_steps', 'self_replace_steps', 'self_replace_max_tokens', 'token_map', 'equalizer'}
+
+    @classmethod
+    def _attn_control(cls, kw, source_guidance_scale, two_phase):
+        """cross_attention_kwargs -> AttentionControl or None (no 'edit_type'); ValueError for what the engine cannot do."""
+        if not kw or 'edit_type' not in kw:
+            return None
+        kind = kw['edit_type']
+        if kind == 'refine':
+            raise ValueError("edit_type='refine' is not supported: it needs both rows' softmaxes per key (use 'replace' or 'reweight')")
+        if kind not in ('replace', 'reweight'):
+            raise ValueError(f"edit_type must be 'replace' or 'reweight', got {kind!r}")
+        extra = set(kw) - cls.P2P_KEYS
+        if extra:
+            raise ValueError(f'cross_attention_kwargs: unsupported keys {sorted(extra)} (LocalBlend: use mask_image)')
+        for key in ('cross_replace_steps', 'self_replace_steps'):
+            if key not in kw:
+                raise ValueError(f'cross_attention_kwargs: {key} is required with edit_type')
+        if two_phase:
+            raise ValueError('attention control needs the lock-step loop: the source chain does not run during the decode (two_phase=False)')
+        if source_guidance_scale == 0:
+            raise ValueError('attention control needs the source prompt: source_guidance_scale 0 runs no source-prompt row')
+        A, eq = kw.get('token_map'), kw.get('equalizer')
+        if A is not None:
+            if not torch.is_tensor(A) or A.dim() not in (2, 3) or A.shape[-1] != A.shape[-2]:
+                raise ValueError(f'token_map: expected a tensor [L,L] or [B,L,L], got {tuple(A.shape) if torch.is_tensor(A) else type(A)}')
+            A = A.to(torch.float32)
+        if eq is not None:
+            if not torch.is_tensor(eq) or eq.dim() not in (1, 2) or (A is not None and eq.shape[-1] != A.shape[-1]):
+                raise ValueError(f'equalizer: expected a tensor [L] or [B,L] matching token_map, got '
+                                 f'{tuple(eq.shape) if torch.is_tensor(eq) else type(eq)}')
+            eq = eq.to(torch.float32)
+            L = eq.shape[-1]
+            base = A if A is not None else torch.eye(L)
+            A = base * eq.unsqueeze(-2)                   # token_map . diag(equalizer)
+        try:
+            return AttentionControl(kw['cross_replace_steps'], kw['self_replace_steps'], kw.get('self_replace_max_tokens', 256), A)
+        except ValueError as err:
+            raise ValueError(f'cross_attention_kwargs: {err}') from None
+
     @torch.no_grad()
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
                  source_guidance_scale=1, num_images_per_prompt=1, eta=0.1, generator=None, prompt_embeds=None, output_type='pt',
@@ -104,7 +145,15 @@ class CycleDiffusionPipeline:
         image at image resolution, so pixels where the mask is 0 are the input image exactly.  A mask needs the lock-step loop:
         ``two_phase=True`` with a mask raises ValueError.  mask_image='auto': the mask is generated from the prompts first, exactly
         ``self.generate_mask(image, source_prompt, prompt, generator=generator, num_inference_steps=num_inference_steps)`` with its
-        defaults, on the same generator."""
+        defaults, on the same generator.
+
+        cross_attention_kwargs: Prompt-to-Prompt attention control (Hertz et al., 2022) when it has an ``edit_type``:
+        {'edit_type': 'replace' | 'reweight', 'cross_replace_steps': f, 'self_replace_steps': f, ['self_replace_max_tokens': n],
+        ['token_map': [L,L] | [B,L,L]], ['equalizer': [L] | [B,L]]}, fractions f in [0, 1] of the loop's steps.  The target's
+        cond row takes the source row's attention maps, cross-attention through A = token_map . diag(equalizer)
+        (attn_control.replace_token_map builds token_map from two prompts' token ids).  'refine' edits, two_phase=True and a
+        source_guidance_scale of 0 raise ValueError; LocalBlend is mask_image's job.  A dict without 'edit_type' is ignored."""
+        attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')
         if not isinstance(callback_steps, int) or callback_steps <= 0:
@@ -163,7 +212,8 @@ class CycleDiffusionPipeline:
                 latents = g.unet.latent_decode(z, c_tgt, uc, guidance_scale, sched)
             else:
                 mask = e.mask_pool(mask_image, g.vae.down) if mask_image is not None else None
-                latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise, mask=mask)
+                latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise, mask=mask,
+                                                attn_control=attn_control)
             if callback is not None:
                 callback(n_rec - 1, sched.t_loop[-1], latents)
             if paste_back:

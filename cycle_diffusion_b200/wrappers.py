@@ -373,7 +373,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         sched = DDIMSchedule(self.custom_steps, self.eta, self.skip_steps[0], self.generator.alphas_cumprod)
         return self.white_box_steps != -1 and self.white_box_steps - self.skip_steps[0] - 1 >= sched.refine_steps
 
-    def cycle(self, image, encode_text, decode_text, mask=None):
+    def cycle(self, image, encode_text, decode_text, mask=None, attn_control=None):
         """encode(image, encode_text) followed by forward(z, image, encode_text, decode_text) for a single-member ensemble, on the
         engine's lock-step driver (cdx_cycle_lockstep): both chains advance together, one U-Net call per step on the batch
         [source | target uncond | target cond], and the noise recovered at a step is consumed by the target chain at once -- the
@@ -382,10 +382,11 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         cycle runs in the wrapper's precision scope, as encode() and generate() do.
 
         mask: optional [B,1,R,R] in [0,1] at image resolution, 1 = may change (masked editing): pooled to the latent grid, and
-        outside it the translated latent stays on the source image's chain (cdx_cycle_lockstep_masked)."""
+        outside it the translated latent stays on the source image's chain (cdx_cycle_lockstep_masked).
+        attn_control: optional attn_control.AttentionControl, Prompt-to-Prompt's "replace" edit (UNet.cycle_lockstep)."""
         assert self.single_member(), 'cycle(): single-member ensembles only (use encode() + forward())'
         with self._precision_scope():
-            return self._cycle(image, encode_text, decode_text, mask)
+            return self._cycle(image, encode_text, decode_text, mask, attn_control)
 
     def _latent_mask(self, mask, bsz):
         """Image-resolution mask [B,1,R,R] -> the latent grid (mean over the first stage's f x f blocks), or None."""
@@ -395,7 +396,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         mask = check_mask(mask, (bsz, 1, R, R), self.engine.device)
         return self.engine.mask_pool(mask, self.generator.vae.down)
 
-    def _cycle(self, image, encode_text, decode_text, mask=None):
+    def _cycle(self, image, encode_text, decode_text, mask=None, attn_control=None):
         g, e = self.generator, self.engine
         bsz = image.shape[0]
         m = self._latent_mask(mask, bsz)                  # checked before the first random draw
@@ -406,7 +407,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         sched = DDIMSchedule(self.custom_steps, self.eta, self.skip_steps[0], g.alphas_cumprod)
         noise = self._encode_noise(sched, sched.refine_steps, x0.shape)
         sample = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, self.encoder_unconditional_guidance_scales[0],
-                                       self.decoder_unconditional_guidance_scales[0], sched, noise, mask=m)
+                                       self.decoder_unconditional_guidance_scales[0], sched, noise, mask=m, attn_control=attn_control)
         return e.shift_scale(g.decode_first_stage(sample), 1.0, 0.5)
 
     def forward(self, z_ensemble, original_img, encode_text, decode_text):

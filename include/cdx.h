@@ -309,6 +309,29 @@ int cdx_cycle_lockstep_masked(cdx_net* unet, const float* x0, const float* c_src
                               const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                               float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                               void* stream, const float* mask);
+/* Prompt-to-Prompt attention control (Hertz et al., 2022; "Cross Attention Control"), the "replace" edit, on the lock-step loop.
+ * Only the target chain's cond row (the row under c_tgt[b]) is controlled; its uncond row and every source row run unchanged.  At
+ * loop step i (0-based, of n_steps):
+ *   - i < cross_steps, every cross-attention layer: the controlled row's probabilities are P_src . A_b, where P_src is the source
+ *     row's softmax(Q K^T) under c_src[b] (same layer and head) and A_b = token_map[b] [L,L] (source token -> target token; NULL
+ *     token_map: the identity).  Computed as softmax(Q_src K_src^T) . V', V' projected once per loop from A_b . c_tgt[b] (to_v has
+ *     no bias), A_b . c_tgt[b] formed by the engine's exact-fp32 GEMM.
+ *   - i < self_steps, self-attention layers of at most self_max_tokens tokens: the controlled row's probabilities are the source
+ *     row's.
+ * Inside the fused attention kernel the controlled row reads the source row's Q and K tiles: no score matrix is formed and no
+ * launch is added.  Needs a source row: src_scale != 0 (and tgt_scale != 0 with uc).  Every controlled layer must run the fused
+ * kernel: mma modes 0 and 2, and mode 3 at head width 160, are rejected (CDX_E_INVALID) rather than run uncontrolled. */
+typedef struct cdx_attn_control {
+  int cross_steps, self_steps, self_max_tokens;
+  const float* token_map;            /* device [B,L,L] or NULL */
+} cdx_attn_control;
+/* cdx_cycle_lockstep_masked with attention control: ctl and mask may each be NULL (both NULL: cdx_cycle_lockstep).  With
+ * cross_steps == self_steps == 0 the result is cdx_cycle_lockstep_masked's bit for bit, and so is it with an identity token_map. */
+int cdx_cycle_lockstep_ctl(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                           int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                           const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                           void* stream, const float* mask, const cdx_attn_control* ctl);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -460,6 +483,10 @@ int cdx_op_layernorm(cdx_engine* e, const float* x, const float* gamma, const fl
 /* softmax(q k^T * scale) v with q [B,Nq,heads*d], k/v [B,Nk,heads*d] -> [B,Nq,heads*d] */
 int cdx_op_attention(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
                      int Nq, int Nk, int heads, int d, float scale, void* stream);
+/* cdx_op_attention with a row table: image b attends with image qk_rows[b]'s q and k and its own v (qk_rows: host [B], each in
+ * [0, B)).  Fused kernel only: a shape or mode that would take another route is CDX_E_INVALID. */
+int cdx_op_attention_rows(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
+                          int Nq, int Nk, int heads, int d, float scale, const int* qk_rows, void* stream);
 int cdx_op_nchw_to_nhwc(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 /* The normalisation kernels in the forms the network executors call them, with their side outputs (tests/test_norms_gpu.py).

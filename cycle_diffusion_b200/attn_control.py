@@ -2,8 +2,10 @@
 
 The "replace" edit: in the first steps of the loop the target chain's conditional row attends with the source row's attention
 probabilities (cross-attention remapped through a token map, self-attention copied), so the edit keeps the source image's layout.
-The engine does it inside the fused attention kernel (include/cdx.h, cdx_cycle_lockstep_ctl); this module holds the value the
-Python surfaces take and the host helper that builds a token map.
+The "refine" edit aligns the two prompts instead: a target token matched to a source token takes that token's cross-attention map,
+a target token with no match keeps the row's own map (``own_weight``).  The engine does both inside the fused attention kernel
+(include/cdx.h, cdx_cycle_lockstep_ctl and cdx_cycle_lockstep_refine); this module holds the value the Python surfaces take and
+the host helpers that build token maps from two prompts' token ids.
 """
 from dataclasses import dataclass
 
@@ -23,11 +25,14 @@ class AttentionControl:
     """cross_steps / self_steps: fractions of the loop's n steps; steps i < int(f * n) are controlled.  self_max_tokens: the
     self-attention layers of at most this many tokens are controlled (256: the 16x16 and 8x8 levels at 512^2).  token_map:
     optional float tensor [L, L] or [B, L, L], source token -> target token (P2P's mapper times its equalizer); None is the
-    identity."""
+    identity.  own_weight: optional float tensor [L] or [B, L], finite and >= 0 (P2P's refine): at a controlled cross-attention
+    step target token j's probabilities become P_src . token_map[:, j] + own_weight[j] . P_own[j], P_own being the row's own; None
+    is the replace edit.  The pipeline's refine passes token_map = A . diag(eq) and own_weight = (1 - colsum(A)) . eq."""
     cross_steps: float
     self_steps: float
     self_max_tokens: int = 256
     token_map: object = None
+    own_weight: object = None
 
     def __post_init__(self):
         _fraction('cross_steps', self.cross_steps)
@@ -36,6 +41,11 @@ class AttentionControl:
             raise ValueError(f'self_max_tokens must be an integer >= 0, got {self.self_max_tokens!r}')
         if self.token_map is not None and not torch.is_tensor(self.token_map):
             raise ValueError(f'token_map must be a tensor [L, L] or [B, L, L], got {type(self.token_map)}')
+        if self.own_weight is not None:
+            if not torch.is_tensor(self.own_weight):
+                raise ValueError(f'own_weight must be a tensor [L] or [B, L], got {type(self.own_weight)}')
+            if not bool(torch.isfinite(self.own_weight).all()) or bool((self.own_weight < 0).any()):
+                raise ValueError('own_weight must be finite and >= 0')
 
     def steps(self, n):
         """(cross_steps, self_steps) as step counts of an n-step loop."""
@@ -55,11 +65,24 @@ class AttentionControl:
             raise ValueError('token_map must be finite')
         return A
 
+    def device_weight(self, B, L, device):
+        """own_weight as a contiguous float32 [B, L] tensor on `device`, or None."""
+        w = self.own_weight
+        if w is None:
+            return None
+        if w.dim() == 1:
+            w = w.unsqueeze(0).expand(B, -1)
+        if w.dim() != 2 or tuple(w.shape) != (B, L):
+            raise ValueError(f'own_weight: expected [{L}] or [{B}, {L}], got {tuple(self.own_weight.shape)}')
+        return w.to(device=device, dtype=torch.float32).contiguous()
+
     def c_struct(self, n, B, L, device):
-        """-> (cdx_attn_control for an n-step loop, the device token map it points to; keep it alive over the call)."""
+        """-> (cdx_attn_control for an n-step loop, the device token map it points to, the device own weight or None; keep both
+        alive over the call)."""
         A = self.device_map(B, L, device)
+        w = self.device_weight(B, L, device)
         cross, self_ = self.steps(n)
-        return _cabi.AttnControl(cross, self_, self.self_max_tokens, A.data_ptr() if A is not None else None), A
+        return _cabi.AttnControl(cross, self_, self.self_max_tokens, A.data_ptr() if A is not None else None), A, w
 
 
 def replace_token_map(src_ids, tgt_ids, L):
@@ -90,4 +113,36 @@ def replace_token_map(src_ids, tgt_ids, L):
     for i in range(p + ns, L):                          # the suffix, and the padding past the prompts, shifted
         if i + shift < L:
             A[i, i + shift] = 1.0
+    return A
+
+
+def refine_token_map(src_ids, tgt_ids, L):
+    """P2P's "refine" mapper for two prompts' token ids (BOS and EOS included, before padding): -> float32 [L, L], A[m(j), j] = 1
+    for every target position j aligned to source position m(j), a zero column for a target token with no source.
+
+    The alignment is global (Needleman-Wunsch): match +1, mismatch -1, gap 0, boundary row and column 0.  The traceback prefers, on
+    ties, a target token with no source, then a dropped source token, then the diagonal; a mismatch is never taken, so a
+    substituted word is a drop plus an insertion and attends on its own.  Target positions j >= len(tgt_ids) (padding) map to
+    source position j; anything past L is dropped.  Identical sequences give the identity."""
+    src, tgt = [int(t) for t in src_ids], [int(t) for t in tgt_ids]
+    n, m = len(src), len(tgt)
+    score = [[0] * (m + 1) for _ in range(n + 1)]
+    for i in range(1, n + 1):
+        for j in range(1, m + 1):
+            score[i][j] = max(score[i - 1][j - 1] + (1 if src[i - 1] == tgt[j - 1] else -1), score[i][j - 1], score[i - 1][j])
+    src_of = [-1] * m                                   # m(j) per target position of the prompt
+    i, j = n, m
+    while i > 0 or j > 0:
+        if j > 0 and score[i][j] == score[i][j - 1]:
+            j -= 1                                       # left: target token j - 1 has no source
+        elif i > 0 and score[i][j] == score[i - 1][j]:
+            i -= 1                                       # up: source token i - 1 is dropped
+        else:
+            src_of[j - 1] = i - 1                        # diagonal: a match (a mismatch never ties the better gap)
+            i, j = i - 1, j - 1
+    A = torch.zeros(L, L, dtype=torch.float32)
+    for j in range(L):
+        s_ = src_of[j] if j < m else j
+        if 0 <= s_ < L:
+            A[s_, j] = 1.0
     return A

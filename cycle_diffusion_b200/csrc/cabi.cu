@@ -171,6 +171,7 @@ struct ChainLoopArgs {
   float* x_out = nullptr;                           // K > 0: [n_src*K, chw]
   const float* mask = nullptr;                      // optional [n_src, 1, h, w]: masked editing (LatentChains::mask)
   const cdx_attn_control* ctl = nullptr;           // optional: attention control of each target chain's cond row (cdx.h)
+  const float* own_weight = nullptr;                // optional with ctl: [n_src, L], refine's weights of the rows' own attention
   int C = 0, h = 0, w = 0;
 };
 
@@ -233,6 +234,7 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
               "attention control: cross_steps=%d self_steps=%d (of %d) self_max_tokens=%d", c.cross_steps, c.self_steps, a.n_steps,
               c.self_max_tokens);
   }
+  CDX_CHECK(!a.own_weight || a.ctl, "refine: own_weight needs an attention control");
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
   struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
@@ -299,6 +301,39 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
           gemm(e, g, s);
         }
       actl.ctx_v = cv;
+    }
+    if (a.own_weight) {
+      // refine: the second term's context holds diag(w_j) . c_tgt[j] on the controlled rows and zeros elsewhere (those rows run no
+      // second term, and zeros keep them out of its range slot), formed by the same exact-fp32 GEMM with a diagonal A
+      const int D = unet.ucfg.context_dim;
+      float* cw = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
+      float* dg = (float*)e.arena.alloc((size_t)a.n_src * a.L * a.L * sizeof(float));
+      std::vector<int> own;
+      for (int j = 0; j < a.n_src; ++j)
+        for (int k = 0; k < a.K; ++k) own.push_back(ch[a.n_src + (size_t)j * a.K + k].row);
+      int* own_dev = (int*)e.arena.alloc(own.size() * sizeof(int));
+      if (!e.dry()) {
+        CDX_CUDA(cudaMemcpyAsync(own_dev, own.data(), own.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+        CDX_CUDA(cudaMemsetAsync(cw, 0, (size_t)rows * ctx_n * sizeof(float), s));
+        CDX_CUDA(cudaMemsetAsync(dg, 0, (size_t)a.n_src * a.L * a.L * sizeof(float), s));
+        for (int j = 0; j < a.n_src; ++j)      // w_j onto the diagonal: a stride of L + 1 floats
+          CDX_CUDA(cudaMemcpy2DAsync(dg + (size_t)j * a.L * a.L, (size_t)(a.L + 1) * sizeof(float), a.own_weight + (size_t)j * a.L, sizeof(float),
+                                     sizeof(float), a.L, cudaMemcpyDeviceToDevice, s));
+      }
+      ExactFp32 exact(e);
+      for (int j = 0; j < a.n_src; ++j)
+        for (int k = 0; k < a.K; ++k) {
+          GemmArgs g;                                // cw[row] = diag(w_j) [L, L] . c_tgt[j] [L, D]
+          g.mode = 0;
+          g.M = a.L; g.N = D; g.K = a.L;
+          g.A = dg + (size_t)j * a.L * a.L; g.lda = a.L; g.C1 = a.L;
+          g.Bw = a.c_tgt + (size_t)j * ctx_n; g.ldb = D; g.b_kn = 1;
+          g.Cout = cw + (size_t)ch[a.n_src + (size_t)j * a.K + k].row * ctx_n; g.ldc = D;
+          gemm(e, g, s);
+        }
+      actl.ctx_w = cw;
+      actl.own_rows = own_dev;
+      actl.n_own = (int)own.size();
     }
   }
   auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
@@ -738,6 +773,14 @@ int cdx_cycle_lockstep_ctl(cdx_net* un, const float* x0, const float* c_src, con
                            float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
                            float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
                            const float* mask, const cdx_attn_control* ctl) {
+  return cdx_cycle_lockstep_refine(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T,
+                                   x_out, z_out, B, C, h, w, stream, mask, ctl, nullptr);
+}
+
+int cdx_cycle_lockstep_refine(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                              float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                              float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                              const float* mask, const cdx_attn_control* ctl, const float* own_weight) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -747,7 +790,7 @@ int cdx_cycle_lockstep_ctl(cdx_net* un, const float* x0, const float* c_src, con
     a.n_src = B; a.K = 1; a.src = true;
     a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scales = s_scales.data(); a.t_scales = t_scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
-    a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.C = C; a.h = h; a.w = w;
+    a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -1035,15 +1078,14 @@ int cdx_op_groupnorm(cdx_engine* eh, const float* x, const float* gamma, const f
 int cdx_op_layernorm(cdx_engine* eh, const float* x, const float* gamma, const float* beta, float* y, int M, int C, void* stream) {
   ENG_CALL(eh, layernorm(eh->e, x, gamma, beta, y, M, C, S(stream)));
 }
-int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d, float scale,
-                     void* stream) {
-  return cdx_op_attention_rows(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, stream);
-}
-int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
-                          float scale, const int* qk_rows, void* stream) {
+// cdx_op_attention with the fused kernel's options: a Q / K row table (qk_rows, host [B]) or the accumulating launch over a row
+// list (acc_rows, host [n_acc]); either one needs the fused kernel
+static int op_attention(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
+                        float scale, const int* qk_rows, const int* acc_rows, int n_acc, void* stream) {
   return guard([&] {
     CDX_CHECK(eh && q && k && v && out, "op_attention: null argument");
     if (qk_rows) for (int b = 0; b < B; ++b) CDX_CHECK(qk_rows[b] >= 0 && qk_rows[b] < B, "op_attention: qk_rows[%d] = %d outside [0, %d)", b, qk_rows[b], B);
+    if (acc_rows) for (int r = 0; r < n_acc; ++r) CDX_CHECK(acc_rows[r] >= 0 && acc_rows[r] < B, "op_attention: acc_rows[%d] = %d outside [0, %d)", r, acc_rows[r], B);
     const int C = heads * d;
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
@@ -1051,11 +1093,16 @@ int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const 
       Scope sc(e.arena);
       bool done = false;
       const bool fused = flash_eligible(e, Nq, Nk, d, C);
-      CDX_CHECK(!qk_rows || fused, "op_attention: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, d);
+      CDX_CHECK((!qk_rows && !acc_rows) || fused, "op_attention: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, d);
       int* rows_dev = nullptr;
       if (qk_rows) {
         rows_dev = (int*)e.arena.alloc((size_t)B * sizeof(int));
         if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(rows_dev, qk_rows, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+      }
+      int* acc_dev = nullptr;
+      if (acc_rows) {
+        acc_dev = (int*)e.arena.alloc((size_t)n_acc * sizeof(int));
+        if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(acc_dev, acc_rows, (size_t)n_acc * sizeof(int), cudaMemcpyHostToDevice, s));
       }
       if (fused && e.tc_kind >= 1) {
         // the SpatialTransformer's fp16-split path on loose q / k / v: ranges measured here, keys padded to a multiple of 8 per image
@@ -1087,7 +1134,8 @@ int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const 
         split_rows_h16(e, q, M, C, C, qh, ql, C, qa, s);
         split_rows_h16(e, kp, Mk, C, C, kh, kl, C, ka, s);
         split_transpose_h16(e, vp, Mk, C, C, vh, vl, va, s);
-        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev);
+        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev,
+                                   n_acc);
       }
       if (!done && e.mma_mode == 1 && Nq == Nk && (Nq % 32) == 0 && Nq >= 128 && (d % 4) == 0) {
         // same operand preparation as the SpatialTransformer: q|k side by side, V transposed, TF32 planes
@@ -1106,9 +1154,10 @@ int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const 
           float* vl = (float*)e.arena.alloc((size_t)C * M * sizeof(float));
           split_planes(e, qk, qh, ql, (size_t)M * 2 * C, s);
           split_planes(e, vt, vh, vl, (size_t)C * M, s);
-          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev);
+          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev, acc_dev,
+                                    n_acc);
         }
-        CDX_CHECK(done || !rows_dev, "op_attention: the fused kernel rejected a row-table shape");
+        CDX_CHECK(done || (!rows_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
         if (!done) done = attention_tc(e, qk, 2 * C, qk + C, 2 * C, d, vt, out, C, B, Nq, Nk, heads, d, scale, s);
       }
       if (!done && fused) {
@@ -1133,12 +1182,25 @@ int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const 
         split_planes(e, q, qh, ql, (size_t)M * C, s);
         split_planes(e, kp, kh, kl, (size_t)Mk * C, s);
         split_planes(e, vt, vh, vl, (size_t)C * Mk, s);
-        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev);
+        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc);
       }
-      CDX_CHECK(done || !rows_dev, "op_attention: the fused kernel rejected a row-table shape");
+      CDX_CHECK(done || (!rows_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
       if (!done) attention(e, q, C, k, C, v, C, out, C, B, Nq, Nk, heads, d, d, scale, s);
     });
   });
+}
+int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d, float scale,
+                     void* stream) {
+  return cdx_op_attention_rows(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, stream);
+}
+int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
+                          float scale, const int* qk_rows, void* stream) {
+  return op_attention(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, qk_rows, nullptr, 0, stream);
+}
+int cdx_op_attention_accum(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
+                           float scale, const int* acc_rows, int n_acc, void* stream) {
+  if (!acc_rows || n_acc < 1) return guard([&] { CDX_CHECK(false, "op_attention_accum: an empty row list"); });
+  return op_attention(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, acc_rows, n_acc, stream);
 }
 int cdx_op_nchw_to_nhwc(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nchw_to_nhwc(eh->e, x, y, B, C, HW, S(stream))); }
 int cdx_op_nhwc_to_nchw(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nhwc_to_nchw(eh->e, x, y, B, C, HW, S(stream))); }

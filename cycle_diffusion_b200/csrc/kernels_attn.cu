@@ -22,6 +22,8 @@
 // row >= N) and keys >= Nk in the last block masked.  d = 160 (fp16 variants): 64 queries per CTA, the two consumer warpgroups take
 // alternate key blocks and merge their softmax states at the end (KSPLIT), and O_j is formed in two n80 halves (PVH) so that O_total,
 // O_j, S and the P fragments fit the 232-register budget; see ACfg.
+// Accumulating launch (AttnParams::acc_rows): CTAs only for the listed images, and the epilogue adds O / l into out instead of
+// storing it -- a second attention term on a few rows (Prompt-to-Prompt's refine) with every variant above as it is.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -83,13 +85,16 @@ struct ACfg {
 };
 
 struct AttnParams {
-  int N, Nk, heads, d, B;   // N queries, Nk keys (cross-attention: Nk != N; keys >= Nk in the last block are masked)
+  int N, Nk, heads, d, B;   // N queries, Nk keys (cross-attention: Nk != N; keys >= Nk in the last block are masked); B: CTAs along z
   float scale_log2e;      // scale * log2(e): scores are kept in the log2 domain
   float* out; int ldo;
   const float *q_amax, *k_amax, *v_amax;   // F16: tracked max |q|, |k|, |v| (the planes hold x * 2^h16_exp_of(amax))
   // optional [B]: image qk_row[b] supplies the Q and K tiles of image b (attention control: a target row attends with its source
   // row's probabilities); V^T and the output stay image b's.  Null: every image its own
   const int* qk_row;
+  // optional [gridDim.z]: the accumulating launch.  CTA z serves image acc_rows[z] and adds its result into out (out += O / l)
+  // instead of storing it; images not listed get no CTA and are not touched (refine's second term over the controlled rows)
+  const int* acc_rows;
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -126,7 +131,7 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   auto bar_v_empty = [&](int s) { return bars + 8u + 8u * (2 * KS + VS + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * QR, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = blockIdx.x * QR, h = blockIdx.y;
   const int nb = (p.Nk + AKV - 1) / AKV;
 
   if (threadIdx.x == 0) {
@@ -137,6 +142,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   }
   __syncthreads();
   pdl_wait();                     // everything above touched shared memory only
+  // (row list and, below, out of an accumulating launch: coherent reads after the dependent-launch wait, so they see everything
+  // the previous launch on the stream wrote)
+  const int b = p.acc_rows ? __ldcg(p.acc_rows + blockIdx.z) : (int)blockIdx.z;
 
   if (warp < 4) {
     // =========================================================================== TMA producer
@@ -422,7 +430,14 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
 #pragma unroll
     for (int j8 = 0; j8 < NV / 8; ++j8) {
       const int col = 8 * j8 + 2 * qd;
-      if (col < D) *reinterpret_cast<float2*>(dst + col) = make_float2(o[j8 * 4 + i * 2] * inv_l, o[j8 * 4 + i * 2 + 1] * inv_l);
+      if (col < D) {
+        float2 r = make_float2(o[j8 * 4 + i * 2] * inv_l, o[j8 * 4 + i * 2 + 1] * inv_l);
+        if (p.acc_rows) {                            // out + O / l: the product rounded first, never fused into an FMA
+          const float2 prev = __ldcg(reinterpret_cast<const float2*>(dst + col));
+          r = make_float2(__fadd_rn(prev.x, r.x), __fadd_rn(prev.y, r.y));
+        }
+        *reinterpret_cast<float2*>(dst + col) = r;
+      }
     }
   }
 }
@@ -533,10 +548,11 @@ bool flash_eligible(const Engine& e, int N, int Nk, int d, int C) {
 
 bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
                         const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d,
-                        float scale, cudaStream_t s, const int* qk_row) {
+                        float scale, cudaStream_t s, const int* qk_row, const int* acc_rows, int n_acc) {
   if (N < 1 || (d % 8) || d < 16 || d > 80 || (ldq & 3) || (ldk & 3) || (ldo & 3) || (Nvs & 3) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
   if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) return false;
   if (!a16(q_hi) || !a16(q_lo) || !a16(k_hi) || !a16(k_lo) || !a16(vt_hi) || !a16(vt_lo) || !a16(out)) return false;
+  if (acc_rows && n_acc < 1) return false;
   if (e.dry()) return true;
   const int NV = (d + 15) / 16 * 16;
   uint64_t dq[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)N, (uint64_t)B};
@@ -554,12 +570,15 @@ bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq
   const CUtensorMap& vh = get_map(vt_hi, 4, dv, sv, bv);
   const CUtensorMap& vl = get_map(vt_lo, 4, dv, sv, bv);
   AttnParams p;
-  p.N = N; p.Nk = Nk; p.heads = heads; p.d = d; p.B = B;
+  p.N = N; p.Nk = Nk; p.heads = heads; p.d = d;
+  p.B = acc_rows ? n_acc : B;           // CTAs along z: the images served
   p.scale_log2e = scale * 1.4426950408889634f;
   p.out = out; p.ldo = ldo;
   p.q_amax = p.k_amax = p.v_amax = nullptr;
   p.qk_row = qk_row;
-  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * B * heads, 4.0 * B * heads * (2.0 * N * d + 2.0 * (double)Nk * d), 1);
+  p.acc_rows = acc_rows;
+  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * p.B * heads,
+               4.0 * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 4.0 * p.B * (double)N * d * heads : 0.0), 1);
   switch (d) {
     case 16: launch_flash<16, false>(qh, ql, kh, kl, vh, vl, p, s); break;
     case 32: launch_flash<32, false>(qh, ql, kh, kl, vh, vl, p, s); break;
@@ -605,13 +624,15 @@ void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long l
 // split_transpose_h16 above).  ld and Nvs multiples of 8.  All three lo planes null: the one-term kernel (hi * hi products only, mma mode 5).
 bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
                          const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
-                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s, const int* qk_row) {
+                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s, const int* qk_row, const int* acc_rows,
+                         int n_acc) {
   if (N < 1 || (ldq & 7) || (ldk & 7) || (ldo & 3) || (Nvs & 7) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
   if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || d == 160)) return false;
   const bool one = q_lo == nullptr;
   if (one ? (k_lo || vt_lo) : (!k_lo || !vt_lo)) return false;
   if (!a16(q_hi) || !a16(k_hi) || !a16(vt_hi) || !a16(out)) return false;
   if (!one && (!a16(q_lo) || !a16(k_lo) || !a16(vt_lo))) return false;
+  if (acc_rows && n_acc < 1) return false;
   if (e.dry()) return true;
   const int NV = (d + 15) / 16 * 16;
   uint64_t dq[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)N, (uint64_t)B};
@@ -630,13 +651,15 @@ bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq,
   const CUtensorMap& kl = one ? kh : get_map(k_lo, 4, dk, sk, bk, nullptr, 2);
   const CUtensorMap& vl = one ? vh : get_map(vt_lo, 4, dv, sv, bv, nullptr, 2);
   AttnParams p;
-  p.N = N; p.Nk = Nk; p.heads = heads; p.d = d; p.B = B;
+  p.N = N; p.Nk = Nk; p.heads = heads; p.d = d;
+  p.B = acc_rows ? n_acc : B;           // CTAs along z: the images served
   p.scale_log2e = scale * 1.4426950408889634f;
   p.out = out; p.ldo = ldo;
   p.q_amax = q_amax; p.k_amax = k_amax; p.v_amax = v_amax;
   p.qk_row = qk_row;
-  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * B * heads,
-               (one ? 1.0 : 2.0) * B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + 4.0 * B * heads * (double)N * d, 1);
+  p.acc_rows = acc_rows;
+  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * p.B * heads,
+               (one ? 1.0 : 2.0) * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 8.0 : 4.0) * p.B * heads * (double)N * d, 1);
   if (one) {
     switch (d) {
       case 16: launch_flash<16, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;

@@ -697,6 +697,8 @@ struct UNetExec : Exec {
   const AttnControl* ctl = nullptr;        // attention control of this call, or null
   const float* ctxv_pad = nullptr;         // ctl->ctx_v zero-padded to ctx_lp rows per image, and its range
   float* ctxv_amax = nullptr;
+  const float* ctxw_pad = nullptr;         // ctl->ctx_w (refine) the same way
+  float* ctxw_amax = nullptr;
   size_t kv_off = 0;
   float* kv_take(size_t floats) {
     if (!kv_reuse) return (float*)e.arena.alloc(floats * sizeof(float));
@@ -902,8 +904,16 @@ struct UNetExec : Exec {
       // token-mapped context's projection; its range slot also bounds this call's output) instead of V^T
       const bool vmap = ctl && ctl->ctx_v;
       float* v2_amax = vmap ? kv_amax() : nullptr;
+      // refine: the controlled rows also add their own attention over V''^T (the refine context's projection) into the output.
+      // V'' takes its own slot, from zero: the context is zero outside the controlled rows, so own weights of zero give a zero
+      // slot.  The output is no longer a convex combination of one tensor's rows, |out| <= max |V'| + max |V''|: its slot is the
+      // sum, formed on the device with the projections (once per loop), and equal to the first term's slot when V'' is zero
+      const bool wmap = ctl && ctl->ctx_w;
+      float* v3_amax = wmap ? kv_amax() : nullptr;
+      float* sum_amax = wmap ? kv_amax() : nullptr;
       const int* crow = (ctl && ctl->cross) ? ctl->qk_row : nullptr;
       const bool use_v2 = crow && vmap;
+      const bool use_v3 = crow && wmap;
       bool done = false;
       Tensor q;
       const bool flash_ok = ctx_pad && flash_eligible(e, HW, ctx_len, d, C);
@@ -924,6 +934,8 @@ struct UNetExec : Exec {
         float* vt_lo = lo ? kv_take(nk / 2) : nullptr;
         float* v2_hi = vmap ? kv_take(nk / 2) : nullptr;
         float* v2_lo = vmap && lo ? kv_take(nk / 2) : nullptr;
+        float* v3_hi = wmap ? kv_take(nk / 2) : nullptr;
+        float* v3_lo = wmap && lo ? kv_take(nk / 2) : nullptr;
         Tensor qf = linear(n2, t + ".attn2.to_q", false, nullptr, true);
         void* q_hi = e.arena.alloc((size_t)M * C * 2);
         void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
@@ -941,10 +953,21 @@ struct UNetExec : Exec {
                         nullptr, v2_amax);
             split_transpose_h16(e, kvf + C, Mk, C, 2 * C, v2_hi, v2_lo, v2_amax, s);
           }
+          if (wmap) {             // V'' by the same fused projection of the refine context, then the output's slot
+            linear_into(ctxw_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, ctxw_amax,
+                        nullptr, v3_amax);
+            split_transpose_h16(e, kvf + C, Mk, C, 2 * C, v3_hi, v3_lo, v3_amax, s);
+            add(e, vmap ? v2_amax : a.amax, v3_amax, sum_amax, 1, s);
+          }
         }
         done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, use_v2 ? v2_hi : vt_hi, use_v2 ? v2_lo : vt_lo, qf.amax, a.amax,
                                    use_v2 ? v2_amax : a.amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, crow);
         CDX_CHECK(done, "flash cross-attention (fp16-split) rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
+        if (use_v3) {             // + the controlled rows' own attention over V'' (accumulating launch, those rows' CTAs only)
+          done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, v3_hi, v3_lo, qf.amax, a.amax, v3_amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp,
+                                     heads, d, scale, s, nullptr, ctl->own_rows, ctl->n_own);
+          CDX_CHECK(done, "flash cross-attention (fp16-split) rejected the refine term (HW=%d d=%d L=%d)", HW, d, ctx_len);
+        }
       } else if (flash_ok) {
         // fused tensor-core attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the
         // kernel): q = n2.Wq^T, K = ctx.Wk^T, V^T = Wv.ctx^T (swapped-role GEMM), all written as TF32 planes
@@ -957,6 +980,8 @@ struct UNetExec : Exec {
         float* vt_lo = kv_take(nk);
         float* v2_hi = vmap ? kv_take(nk) : nullptr;
         float* v2_lo = vmap ? kv_take(nk) : nullptr;
+        float* v3_hi = wmap ? kv_take(nk) : nullptr;
+        float* v3_lo = wmap ? kv_take(nk) : nullptr;
         float* q_hi = (float*)e.arena.alloc(nq * sizeof(float));
         float* q_lo = (float*)e.arena.alloc(nq * sizeof(float));
         linear_into(n2.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn2.to_q.weight"), C, nullptr, nullptr, 0, q_hi, C, q_lo, n2.amax);
@@ -969,12 +994,23 @@ struct UNetExec : Exec {
             linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctxv_pad, Mk, nullptr, nullptr, 0, v2_hi, Mk, v2_lo, nullptr, nullptr,
                         v2_amax);
           }
+          if (wmap) {
+            linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctxw_pad, Mk, nullptr, nullptr, 0, v3_hi, Mk, v3_lo, nullptr, nullptr,
+                        v3_amax);
+            add(e, vmap ? v2_amax : a.amax, v3_amax, sum_amax, 1, s);
+          }
         }
         done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, use_v2 ? v2_hi : vt_hi, use_v2 ? v2_lo : vt_lo, a.p, C, B, HW, ctx_len, ctx_lp,
                                   ctx_lp, heads, d, scale, s, crow);
         CDX_CHECK(done, "flash cross-attention rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
+        if (use_v3) {
+          done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, v3_hi, v3_lo, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, nullptr,
+                                    ctl->own_rows, ctl->n_own);
+          CDX_CHECK(done, "flash cross-attention rejected the refine term (HW=%d d=%d L=%d)", HW, d, ctx_len);
+        }
       }
-      if (use_v2) a.amax = v2_amax;             // the output is a convex combination of V' rows
+      if (use_v3) a.amax = sum_amax;            // the sum of a convex combination of V' rows and one of V'' rows
+      else if (use_v2) a.amax = v2_amax;        // the output is a convex combination of V' rows
       if (!done) q = linear(n2, t + ".attn2.to_q", false);
       if (!done) {
         Scope sa(e.arena);
@@ -1125,7 +1161,7 @@ struct UNetExec : Exec {
       size_t sumC = 0;
       for (const Param& pp : n.params)
         if (pp.name.size() > 17 && pp.name.compare(pp.name.size() - 17, 17, "attn2.to_k.weight") == 0) sumC += (size_t)pp.dims[0] + 64;
-      const size_t need = (ctl && ctl->ctx_v ? 6 : 4) * (size_t)B * ctx_lp * sumC;      // K, V (and V') hi + lo planes
+      const size_t need = (4 + (ctl && ctl->ctx_v ? 2 : 0) + (ctl && ctl->ctx_w ? 2 : 0)) * (size_t)B * ctx_lp * sumC;   // K, V (V', V'') hi + lo
       if (kc.cap < need) {
         CDX_CUDA(cudaDeviceSynchronize());
         if (kc.buf) CDX_CUDA(cudaFree(kc.buf));
@@ -1133,7 +1169,8 @@ struct UNetExec : Exec {
         CDX_CUDA(cudaMalloc(&kc.buf, need * sizeof(float)));
         kc.cap = need;
       }
-      kv_hit = kc.valid && kc.ctx == context && kc.ctx_v == (ctl ? ctl->ctx_v : nullptr) && kc.L == L && kc.B == B && !e.dry();
+      kv_hit = kc.valid && kc.ctx == context && kc.ctx_v == (ctl ? ctl->ctx_v : nullptr) && kc.ctx_w == (ctl ? ctl->ctx_w : nullptr) && kc.L == L &&
+               kc.B == B && !e.dry();
       if (!kc.amax) {
         CDX_CUDA(cudaMalloc(&kc.amax, (Net::CtxKV::MAX_LAYERS + 1) * sizeof(float)));
         CDX_CUDA(cudaMemset(kc.amax, 0, (Net::CtxKV::MAX_LAYERS + 1) * sizeof(float)));
@@ -1148,6 +1185,10 @@ struct UNetExec : Exec {
       if (ctl && ctl->ctx_v) {
         ctxv_amax = kv_amax();
         if (!kv_hit) amax_rows(e, ctl->ctx_v, (long long)B * L, c.context_dim, c.context_dim, ctxv_amax, s);
+      }
+      if (ctl && ctl->ctx_w) {
+        ctxw_amax = kv_amax();
+        if (!kv_hit) amax_rows(e, ctl->ctx_w, (long long)B * L, c.context_dim, c.context_dim, ctxw_amax, s);
       }
     }
     if (context && L > 0 && e.mma_mode == 1 && e.flash_attn) {
@@ -1166,6 +1207,14 @@ struct UNetExec : Exec {
           CDX_CUDA(cudaMemcpy2DAsync(vp, (size_t)ctx_lp * D * 4, ctl->ctx_v, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
         }
         ctxv_pad = vp;
+      }
+      if (ctl && ctl->ctx_w) {
+        float* wp = (float*)e.arena.alloc((size_t)B * ctx_lp * D * sizeof(float));
+        if (!e.dry() && !kv_hit) {
+          if (ctx_lp != L) CDX_CUDA(cudaMemsetAsync(wp, 0, (size_t)B * ctx_lp * D * sizeof(float), s));
+          CDX_CUDA(cudaMemcpy2DAsync(wp, (size_t)ctx_lp * D * 4, ctl->ctx_w, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
+        }
+        ctxw_pad = wp;
       }
     }
     // --- timestep embedding MLP + all ResBlock emb projections in one GEMM
@@ -1308,7 +1357,7 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
   ex.forward(x_nchw, t_dev, ctx, ctx_len, out_nchw, B, H, W);
   if (ex.kv_reuse && !n.eng->dry()) {
     n.ctxkv.valid = true;
-    n.ctxkv.ctx = ctx; n.ctxkv.ctx_v = ctl ? ctl->ctx_v : nullptr; n.ctxkv.L = ctx_len; n.ctxkv.B = B;
+    n.ctxkv.ctx = ctx; n.ctxkv.ctx_v = ctl ? ctl->ctx_v : nullptr; n.ctxkv.ctx_w = ctl ? ctl->ctx_w : nullptr; n.ctxkv.L = ctx_len; n.ctxkv.B = B;
   }
 }
 

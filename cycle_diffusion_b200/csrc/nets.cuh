@@ -52,9 +52,11 @@ struct Net {
   // cross-attention K / V of a context that stays fixed over a sampling loop (set up by the loop drivers in cabi.cu):
   // computed by the first U-Net call of the loop, reused by the others (the reference recomputes them every step)
   struct CtxKV {
-    static constexpr int MAX_LAYERS = 63;
-    bool valid = false; const float* ctx = nullptr; const float* ctx_v = nullptr; int L = 0, B = 0; float* buf = nullptr; size_t cap = 0;
-    // [0]: max |context|, then per layer max |K, V| of its context projection and, with a V context (AttnControl::ctx_v), max |V'|
+    static constexpr int MAX_LAYERS = 127;   // range slots after [0] (up to four per layer under refine control)
+    bool valid = false; const float* ctx = nullptr; const float* ctx_v = nullptr; const float* ctx_w = nullptr; int L = 0, B = 0;
+    float* buf = nullptr; size_t cap = 0;
+    // [0]: max |context|, then per layer max |K, V| of its context projection and, with a V context (AttnControl::ctx_v), max |V'|;
+    // with a refine context (AttnControl::ctx_w) also max |V''| and the bound of the output (see UNetExec)
     float* amax = nullptr;
   } ctxkv;
   // concatenated ResBlock emb projections: weights [emb_rows][ted] at emb_w_off, biases at emb_b_off
@@ -80,7 +82,7 @@ void net_ensure_blob(Net& n);
 // channel) sums (for a consumer GroupNorm) -- both produced by the epilogue that holds the tile in registers where it can
 void track_outputs(Engine& e, Tensor& t, GemmArgs& g, bool stats);
 
-// Attention control of one SD / LDM U-Net call (Prompt-to-Prompt's "replace" edit, driven by the lock-step loop in cabi.cu).
+// Attention control of one SD / LDM U-Net call (Prompt-to-Prompt's "replace" and "refine" edits, driven by the lock-step loop in cabi.cu).
 // Row r's fused attention takes its Q and K from row qk_row[r], so its probabilities are that row's; its V stays its own.  Only the
 // fused kernels can do this: a layer that would take another route while control is on is an error.
 struct AttnControl {
@@ -92,6 +94,12 @@ struct AttnControl {
   // other row its own context).  Given, the context cache also holds V'^T (own range slot), and cross-controlled calls read it
   // instead of V^T.  Fixed over the loop, like the context
   const float* ctx_v = nullptr;
+  // refine (optional): the context of the second term, device [B, L, D] (a controlled row holds diag(w_b) . c_tgt[b], every other
+  // row zeros), and the controlled rows, device [n_own].  Given, the context cache also holds V''^T (own range slot) and the
+  // range slot of the sum, and every cross-controlled layer adds softmax(Q K^T) . V'' of those rows into its output
+  const float* ctx_w = nullptr;
+  const int* own_rows = nullptr;
+  int n_own = 0;
 };
 
 // forward executors (enqueue only; caller handles arena dry-run)

@@ -102,10 +102,8 @@ class CycleDiffusionPipeline:
         if not kw or 'edit_type' not in kw:
             return None
         kind = kw['edit_type']
-        if kind == 'refine':
-            raise ValueError("edit_type='refine' is not supported: it needs both rows' softmaxes per key (use 'replace' or 'reweight')")
-        if kind not in ('replace', 'reweight'):
-            raise ValueError(f"edit_type must be 'replace' or 'reweight', got {kind!r}")
+        if kind not in ('replace', 'reweight', 'refine'):
+            raise ValueError(f"edit_type must be 'replace', 'reweight' or 'refine', got {kind!r}")
         extra = set(kw) - cls.P2P_KEYS
         if extra:
             raise ValueError(f'cross_attention_kwargs: unsupported keys {sorted(extra)} (LocalBlend: use mask_image)')
@@ -117,10 +115,18 @@ class CycleDiffusionPipeline:
         if source_guidance_scale == 0:
             raise ValueError('attention control needs the source prompt: source_guidance_scale 0 runs no source-prompt row')
         A, eq = kw.get('token_map'), kw.get('equalizer')
+        if kind == 'refine' and A is None:
+            raise ValueError("edit_type='refine' needs a token_map (the prompts' alignment: attn_control.refine_token_map)")
         if A is not None:
             if not torch.is_tensor(A) or A.dim() not in (2, 3) or A.shape[-1] != A.shape[-2]:
                 raise ValueError(f'token_map: expected a tensor [L,L] or [B,L,L], got {tuple(A.shape) if torch.is_tensor(A) else type(A)}')
             A = A.to(torch.float32)
+        own = None
+        if kind == 'refine':
+            colsum = A.sum(dim=-2)                        # per target token: how much of it the source supplies
+            if not bool(torch.isfinite(colsum).all()) or bool((colsum < -1e-6).any()) or bool((colsum > 1 + 1e-6).any()):
+                raise ValueError('token_map: with refine every column sum must lie in [0, 1]')
+            own = (1.0 - colsum).clamp_min(0.0)           # the rest of each target token is its own attention
         if eq is not None:
             if not torch.is_tensor(eq) or eq.dim() not in (1, 2) or (A is not None and eq.shape[-1] != A.shape[-1]):
                 raise ValueError(f'equalizer: expected a tensor [L] or [B,L] matching token_map, got '
@@ -129,8 +135,10 @@ class CycleDiffusionPipeline:
             L = eq.shape[-1]
             base = A if A is not None else torch.eye(L)
             A = base * eq.unsqueeze(-2)                   # token_map . diag(equalizer)
+            if own is not None:
+                own = own * eq                            # (1 - colsum) . equalizer
         try:
-            return AttentionControl(kw['cross_replace_steps'], kw['self_replace_steps'], kw.get('self_replace_max_tokens', 256), A)
+            return AttentionControl(kw['cross_replace_steps'], kw['self_replace_steps'], kw.get('self_replace_max_tokens', 256), A, own)
         except ValueError as err:
             raise ValueError(f'cross_attention_kwargs: {err}') from None
 
@@ -148,11 +156,14 @@ class CycleDiffusionPipeline:
         defaults, on the same generator.
 
         cross_attention_kwargs: Prompt-to-Prompt attention control (Hertz et al., 2022) when it has an ``edit_type``:
-        {'edit_type': 'replace' | 'reweight', 'cross_replace_steps': f, 'self_replace_steps': f, ['self_replace_max_tokens': n],
-        ['token_map': [L,L] | [B,L,L]], ['equalizer': [L] | [B,L]]}, fractions f in [0, 1] of the loop's steps.  The target's
-        cond row takes the source row's attention maps, cross-attention through A = token_map . diag(equalizer)
-        (attn_control.replace_token_map builds token_map from two prompts' token ids).  'refine' edits, two_phase=True and a
-        source_guidance_scale of 0 raise ValueError; LocalBlend is mask_image's job.  A dict without 'edit_type' is ignored."""
+        {'edit_type': 'replace' | 'reweight' | 'refine', 'cross_replace_steps': f, 'self_replace_steps': f,
+        ['self_replace_max_tokens': n], ['token_map': [L,L] | [B,L,L]], ['equalizer': [L] | [B,L]]}, fractions f in [0, 1] of the
+        loop's steps.  The target's cond row takes the source row's attention maps, cross-attention through A = token_map .
+        diag(equalizer) (attn_control.replace_token_map builds token_map from two prompts' token ids).  'refine' needs a
+        token_map (attn_control.refine_token_map aligns two prompts' token ids) whose column sums lie in [0, 1]: target token j
+        takes P_src . A[:, j] and keeps (1 - colsum_j) . eq_j of its own map, so a word the source prompt lacks attends on its own.
+        two_phase=True and a source_guidance_scale of 0 raise ValueError; LocalBlend is mask_image's job.  A dict without
+        'edit_type' is ignored."""
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')

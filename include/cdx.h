@@ -332,6 +332,23 @@ int cdx_cycle_lockstep_ctl(cdx_net* unet, const float* x0, const float* c_src, c
                            const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                            float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                            void* stream, const float* mask, const cdx_attn_control* ctl);
+/* Prompt-to-Prompt's "refine" edit: cdx_cycle_lockstep_ctl with own_weight (device [B,L], finite, >= 0; NULL: exactly
+ * cdx_cycle_lockstep_ctl, which calls this).  At a controlled cross-attention step the controlled row's probabilities for target
+ * token j become
+ *     attn[j] = P_src . A_b[:, j]  +  own_weight[b, j] . P_tgt[j]
+ * P_tgt being the row's own softmax(Q K^T) under c_tgt[b].  With A_b[i, j] = alpha_j [m(j) = i] eq_j and own_weight[b, j] =
+ * (1 - alpha_j) eq_j this is P2P's refine: a target token aligned to source token m(j) takes that token's map, an unaligned one
+ * keeps its own (times the equalizer eq).  Computed as
+ *     out = softmax(Q_src K_src^T) . V'  +  softmax(Q_tgt K_tgt^T) . V'',   V'' projected once per loop from diag(w_b) . c_tgt[b]
+ * the second term by one more fused-attention launch over the controlled rows only, which adds into the output.  Range bound: the
+ * output's range slot (it sets the fp16 exponent of the to_out projection's operand) is the first term's slot plus max |V''| over
+ * the controlled rows -- |out| <= max |V'| + max |V''| -- formed on the device once per loop; own_weight == 0 leaves it, and the
+ * result, bit for bit as without own_weight.  Self-attention control is unchanged (the source row's probabilities). */
+int cdx_cycle_lockstep_refine(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                              int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                              const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                              float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                              void* stream, const float* mask, const cdx_attn_control* ctl, const float* own_weight);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -487,6 +504,10 @@ int cdx_op_attention(cdx_engine* e, const float* q, const float* k, const float*
  * [0, B)).  Fused kernel only: a shape or mode that would take another route is CDX_E_INVALID. */
 int cdx_op_attention_rows(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
                           int Nq, int Nk, int heads, int d, float scale, const int* qk_rows, void* stream);
+/* The fused kernel's accumulating launch: out[r] += softmax(q[r] k[r]^T * scale) v[r] for each image r of acc_rows (host [n_acc],
+ * each in [0, B)); the other images of out are not touched.  Fused kernel only, as cdx_op_attention_rows. */
+int cdx_op_attention_accum(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
+                           int Nq, int Nk, int heads, int d, float scale, const int* acc_rows, int n_acc, void* stream);
 int cdx_op_nchw_to_nhwc(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 /* The normalisation kernels in the forms the network executors call them, with their side outputs (tests/test_norms_gpu.py).

@@ -7,10 +7,13 @@ Workload (config 2): SD v1-4 topology with synthetic weights (specs.sd_unet_conf
 CycleDiffusionPipeline at strength 0.8 -- VAE encode, a DPM-Encoder under the source prompt at scale 1 and a CFG 7.5 decode under
 the target prompt in lock-step (40 of the 50 steps), VAE decode.  The conditioning is a fixed random [B, 77, 768] context.  Three
 arms: no control; 'replace' with cross_replace_steps 0.8 and self_replace_steps 0.4 (no token map); the same with a non-identity
-token map (a one-token swap times an equalizer), which adds one V' projection per cross-attention layer per loop.  The arms are
+token map (a one-token swap times an equalizer), which adds one V' projection per cross-attention layer per loop; 'refine' with
+the same steps and an insertion alignment (attn_control.refine_token_map, "a cat" -> "a fluffy cat") times an equalizer, which also
+adds one V'' projection per cross-attention layer per loop and a second, accumulating attention launch over the controlled rows
+in every cross-attention layer of a controlled step.  The arms are
 alternated run by run after one warm-up call each; median and min-max of --runs runs, as ms per step (the whole call's host time
 between device synchronisations over the loop's steps, VAE included) and images/s.  Then the engine's event profiler times one
-12-row U-Net call (a 1-step loop at B = 4: source, target uncond, target cond) with and without control and reports the fused
+12-row U-Net call (a 1-step loop at B = 4: source, target uncond, target cond; every layer controlled) in each arm and reports the fused
 attention kernels' time (tag batched_tc).  Prints one JSON line per arm, one for the profile, and a final one with the card's
 name, power limit and maximum SM clock.
 """
@@ -27,13 +30,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
-from cycle_diffusion_b200.attn_control import AttentionControl  # noqa: E402
+from cycle_diffusion_b200.attn_control import AttentionControl, refine_token_map  # noqa: E402
 from cycle_diffusion_b200.engine import Engine  # noqa: E402
 from cycle_diffusion_b200.pipeline import CycleDiffusionPipeline  # noqa: E402
 from cycle_diffusion_b200.schedule import DDIMSchedule  # noqa: E402
 from cycle_diffusion_b200.wrappers import SDStochasticTextWrapper  # noqa: E402
 
-ARMS = ['no-control', 'replace', 'replace-token-map']
+ARMS = ['no-control', 'replace', 'replace-token-map', 'refine']
 L = 77
 
 
@@ -48,6 +51,14 @@ def token_map():
     eq = torch.ones(L)
     eq[2] = 2.0
     return A * eq
+
+
+def refine_map():
+    """Token map and equalizer of the refine arm: "a cat" -> "a fluffy cat", the inserted word weighted 2."""
+    A = refine_token_map([49406, 320, 2368, 49407], [49406, 320, 21416, 2368, 49407], L)
+    eq = torch.ones(L)
+    eq[2] = 2.0
+    return A, eq
 
 
 def main():
@@ -66,7 +77,9 @@ def main():
     pipe = CycleDiffusionPipeline(w.generator)
     image = torch.rand(a.B, 3, R, R, generator=torch.Generator().manual_seed(1)).to(eng.device)
     replace = {'edit_type': 'replace', 'cross_replace_steps': 0.8, 'self_replace_steps': 0.4}
-    kwargs = {'no-control': None, 'replace': replace, 'replace-token-map': {**replace, 'token_map': token_map()}}
+    A, eq = refine_map()
+    kwargs = {'no-control': None, 'replace': replace, 'replace-token-map': {**replace, 'token_map': token_map()},
+              'refine': {**replace, 'edit_type': 'refine', 'token_map': A, 'equalizer': eq}}
     n_loop = int(a.steps * 0.8)
 
     def run(arm):
@@ -100,7 +113,9 @@ def main():
     uc = torch.zeros(a.B, L, 768, device=eng.device)
     c = ctx.to(eng.device)
     prof = {}
-    for arm, ctl in (('no-control', None), ('replace', AttentionControl(1.0, 1.0)), ('replace-token-map', AttentionControl(1.0, 1.0, token_map=token_map()))):
+    ctls = (('no-control', None), ('replace', AttentionControl(1.0, 1.0)), ('replace-token-map', AttentionControl(1.0, 1.0, token_map=token_map())),
+            ('refine', AttentionControl(1.0, 1.0, token_map=A * eq, own_weight=(1 - A.sum(0)) * eq)))
+    for arm, ctl in ctls:
         for enable in (False, True):                  # a warm-up call, then the profiled one
             eng.profile(enable)
             g.unet.cycle_lockstep(x0, c, c.flip(0), uc, 1.0, 7.5, sched, noise, attn_control=ctl)

@@ -285,27 +285,30 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(qk_dev, qk.data(), qk.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
     actl.qk_row = qk_dev;
     actl.self_max_tokens = a.ctl->self_max_tokens;
-    if (a.ctl->token_map) {
+    // out[row] = A_j [L, L] . c_tgt[j] [L, D] on each target chain's cond row, in exact fp32 (A_j at A + j L L)
+    auto ctx_products = [&](const float* A, float* out) {
       const int D = unet.ucfg.context_dim;
-      float* cv = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
-      copy_dd(e, ctx_in, cv, (size_t)rows * ctx_n, s);
       ExactFp32 exact(e);
       for (int j = 0; j < a.n_src; ++j)
         for (int k = 0; k < a.K; ++k) {
-          GemmArgs g;                                // cv[row] = A_j [L, L] . c_tgt[j] [L, D]
+          GemmArgs g;
           g.mode = 0;
           g.M = a.L; g.N = D; g.K = a.L;
-          g.A = a.ctl->token_map + (size_t)j * a.L * a.L; g.lda = a.L; g.C1 = a.L;
+          g.A = A + (size_t)j * a.L * a.L; g.lda = a.L; g.C1 = a.L;
           g.Bw = a.c_tgt + (size_t)j * ctx_n; g.ldb = D; g.b_kn = 1;
-          g.Cout = cv + (size_t)ch[a.n_src + (size_t)j * a.K + k].row * ctx_n; g.ldc = D;
+          g.Cout = out + (size_t)ch[a.n_src + (size_t)j * a.K + k].row * ctx_n; g.ldc = D;
           gemm(e, g, s);
         }
+    };
+    if (a.ctl->token_map) {
+      float* cv = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
+      copy_dd(e, ctx_in, cv, (size_t)rows * ctx_n, s);
+      ctx_products(a.ctl->token_map, cv);
       actl.ctx_v = cv;
     }
     if (a.own_weight) {
       // refine: the second term's context holds diag(w_j) . c_tgt[j] on the controlled rows and zeros elsewhere (those rows run no
       // second term, and zeros keep them out of its range slot), formed by the same exact-fp32 GEMM with a diagonal A
-      const int D = unet.ucfg.context_dim;
       float* cw = (float*)e.arena.alloc((size_t)rows * ctx_n * sizeof(float));
       float* dg = (float*)e.arena.alloc((size_t)a.n_src * a.L * a.L * sizeof(float));
       std::vector<int> own;
@@ -320,17 +323,7 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
           CDX_CUDA(cudaMemcpy2DAsync(dg + (size_t)j * a.L * a.L, (size_t)(a.L + 1) * sizeof(float), a.own_weight + (size_t)j * a.L, sizeof(float),
                                      sizeof(float), a.L, cudaMemcpyDeviceToDevice, s));
       }
-      ExactFp32 exact(e);
-      for (int j = 0; j < a.n_src; ++j)
-        for (int k = 0; k < a.K; ++k) {
-          GemmArgs g;                                // cw[row] = diag(w_j) [L, L] . c_tgt[j] [L, D]
-          g.mode = 0;
-          g.M = a.L; g.N = D; g.K = a.L;
-          g.A = dg + (size_t)j * a.L * a.L; g.lda = a.L; g.C1 = a.L;
-          g.Bw = a.c_tgt + (size_t)j * ctx_n; g.ldb = D; g.b_kn = 1;
-          g.Cout = cw + (size_t)ch[a.n_src + (size_t)j * a.K + k].row * ctx_n; g.ldc = D;
-          gemm(e, g, s);
-        }
+      ctx_products(dg, cw);
       actl.ctx_w = cw;
       actl.own_rows = own_dev;
       actl.n_own = (int)own.size();
@@ -1134,8 +1127,8 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
         split_rows_h16(e, q, M, C, C, qh, ql, C, qa, s);
         split_rows_h16(e, kp, Mk, C, C, kh, kl, C, ka, s);
         split_transpose_h16(e, vp, Mk, C, C, vh, vl, va, s);
-        done = flash_attention_h16(e, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev,
-                                   n_acc);
+        const AttnPlanes pl{AttnPlanes::H16, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va};
+        done = flash_attention(e, pl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc);
       }
       if (!done && e.mma_mode == 1 && Nq == Nk && (Nq % 32) == 0 && Nq >= 128 && (d % 4) == 0) {
         // same operand preparation as the SpatialTransformer: q|k side by side, V transposed, TF32 planes
@@ -1154,8 +1147,8 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
           float* vl = (float*)e.arena.alloc((size_t)C * M * sizeof(float));
           split_planes(e, qk, qh, ql, (size_t)M * 2 * C, s);
           split_planes(e, vt, vh, vl, (size_t)C * M, s);
-          done = flash_attention_tc(e, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev, acc_dev,
-                                    n_acc);
+          const AttnPlanes pl{AttnPlanes::TF32, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl};
+          done = flash_attention(e, pl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev, acc_dev, n_acc);
         }
         CDX_CHECK(done || (!rows_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
         if (!done) done = attention_tc(e, qk, 2 * C, qk + C, 2 * C, d, vt, out, C, B, Nq, Nk, heads, d, scale, s);
@@ -1182,7 +1175,8 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
         split_planes(e, q, qh, ql, (size_t)M * C, s);
         split_planes(e, kp, kh, kl, (size_t)Mk * C, s);
         split_planes(e, vt, vh, vl, (size_t)C * Mk, s);
-        done = flash_attention_tc(e, qh, ql, C, kh, kl, C, vh, vl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc);
+        const AttnPlanes pl{AttnPlanes::TF32, qh, ql, C, kh, kl, C, vh, vl};
+        done = flash_attention(e, pl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc);
       }
       CDX_CHECK(done || (!rows_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
       if (!done) attention(e, q, C, k, C, v, C, out, C, B, Nq, Nk, heads, d, d, scale, s);

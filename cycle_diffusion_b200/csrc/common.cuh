@@ -181,20 +181,28 @@ enum { ROUTE_KIND_SS = 0, ROUTE_KIND_TS = 1, ROUTE_KIND_H16 = 2, ROUTE_KIND_H16_
 inline int route_plan(int kind, int width, int splits) { return kind << 4 | width << 8 | splits << 16; }
 // fused attention (kernels_attn.cu): true when the engine's mode runs N queries over Nk keys at head width d (C channels) fused
 bool flash_eligible(const Engine& e, int N, int Nk, int d, int C);
-bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
-                        const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d,
-                        float scale, cudaStream_t s, const int* qk_row = nullptr, const int* acc_rows = nullptr, int n_acc = 0);
-// fp16-split operands (the default scheme): planes made by split_rows_h16 / split_transpose_h16 from fp32 q | k and v with the
-// tensors' tracked ranges (device slots); halves the tensor-pipe time and the operand bytes of the TF32-plane version.
-// q_lo, k_lo and vt_lo all null: one-term products on the hi planes (mode 5); the split functions then write hi only.
-// qk_row (both fused variants, optional device [B]): image b takes its Q and K from image qk_row[b] and keeps its own V and output --
-// its probabilities are image qk_row[b]'s (attention control).  Null: every image its own.
-// acc_rows (both fused variants, optional device [n_acc]): the accumulating launch, out[r] += attention of image r for the listed
-// images only (CTAs for those alone); ordered after the stream's previous launch, whose out it reads after the dependent-launch wait.
-bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
-                         const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
-                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s, const int* qk_row = nullptr,
-                         const int* acc_rows = nullptr, int n_acc = 0);
+// The fused kernel's operands: hi / lo planes of q [B*N, ldq] and k [B*Nks, ldk] (head h at column h*d; Nks stored keys per image
+// >= Nk) and of V^T [heads*d, B*Nvs] (Nvs keys per image, the padding columns zero).  Self-attention: q and k are two column ranges
+// of one fused projection.
+// TF32: planes rn_tf32(x), rn_tf32(x - hi), as the GEMM epilogues write them; ldq, ldk and Nvs multiples of 4.
+// H16 (the default scheme): fp16 planes made by split_rows_h16 / split_transpose_h16 from fp32 q | k and v, each scaled by
+// 2^h16_exp_of(*amax) of its tensor's range slot (device); halves the tensor-pipe time and the operand bytes of the TF32 planes.
+// ldq, ldk and Nvs multiples of 8.  q_lo, k_lo and vt_lo all null: one-term products on the hi planes (mode 5; the split functions
+// then write hi only).
+struct AttnPlanes {
+  enum Fmt { TF32, H16 } fmt;
+  const void* q_hi; const void* q_lo; int ldq;
+  const void* k_hi; const void* k_lo; int ldk;
+  const void* vt_hi; const void* vt_lo;
+  const float* q_amax = nullptr; const float* k_amax = nullptr; const float* v_amax = nullptr;   // H16 only
+};
+// out [B, N, ldo], head h at column h*d.  False when the planes or the shape do not fit an instantiation.
+// qk_row (optional device [B]): image b takes its Q and K from image qk_row[b] and keeps its own V and output -- its probabilities
+// are image qk_row[b]'s (attention control).  Null: every image its own.
+// acc_rows (optional device [n_acc]): the accumulating launch, out[r] += attention of image r for the listed images only (CTAs for
+// those alone); ordered after the stream's previous launch, whose out it reads after the dependent-launch wait.
+bool flash_attention(Engine& e, const AttnPlanes& a, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d, float scale,
+                     cudaStream_t s, const int* qk_row = nullptr, const int* acc_rows = nullptr, int n_acc = 0);
 void split_rows_h16(Engine& e, const float* src, long long rows, int cols, long long ld, void* hi, void* lo, long long ldh, const float* amax,
                     cudaStream_t s);
 // R rows = `images` images of R / images rows each; Rp > 0: each image's columns padded with zeros to a stride of Rp (V^T key stride)

@@ -465,6 +465,23 @@ void launch_flash(const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMa
   else launch_flash_k<D, F16, ONE, false>(qh, ql, kh, kl, vh, vl, p, s);
 }
 
+// the instantiation for head width d (160: fp16 planes only); false for a width without one
+template <bool F16, bool ONE>
+bool launch_flash_d(int d, const CUtensorMap& qh, const CUtensorMap& ql, const CUtensorMap& kh, const CUtensorMap& kl, const CUtensorMap& vh,
+                    const CUtensorMap& vl, const AttnParams& p, cudaStream_t s) {
+  switch (d) {
+    case 16: launch_flash<16, F16, ONE>(qh, ql, kh, kl, vh, vl, p, s); return true;
+    case 32: launch_flash<32, F16, ONE>(qh, ql, kh, kl, vh, vl, p, s); return true;
+    case 40: launch_flash<40, F16, ONE>(qh, ql, kh, kl, vh, vl, p, s); return true;
+    case 64: launch_flash<64, F16, ONE>(qh, ql, kh, kl, vh, vl, p, s); return true;
+    case 80: launch_flash<80, F16, ONE>(qh, ql, kh, kl, vh, vl, p, s); return true;
+    case 160:
+      if constexpr (F16) { launch_flash<160, F16, ONE>(qh, ql, kh, kl, vh, vl, p, s); return true; }
+      return false;
+    default: return false;
+  }
+}
+
 // x * 2^e -> fp16 hi / lo planes, e = h16_exp_of(*amax) (the exponent the attention kernel derives from the same slot).
 // src [rows, ld] (cols % 4 == 0) -> hi / lo [rows, ldh].  LO = false: the hi plane only (one-term attention)
 template <bool LO>
@@ -532,9 +549,6 @@ __global__ void __launch_bounds__(256) split_transpose_h16_kernel(const float* s
 
 }  // namespace
 
-// q_hi / q_lo: TF32 planes of the query projection [B*N, ldq] (head h at column h*d); k_hi / k_lo: planes of the key
-// projection [B*Nks, ldk] (Nks = stored keys per image >= Nk); vt_hi / vt_lo: planes of V^T [heads*d, B*Nvs] (Nvs % 4 == 0).
-// out [B, N, ldo], head h at column h*d.  Self-attention: q and k are two column ranges of one fused projection.
 // The fused kernels' shape rule, in one place: every caller routes by it.  Any N >= 1 queries and Nk >= 1 keys (callers lay K and V^T
 // out at a per-image key stride padded to 8 (fp16) / 4 (TF32) keys); head widths with an instantiation: 16, 32, 40, 64, 80, and 160
 // for the fp16 planes (tc_kind >= 1; mma mode 3's TF32 planes at d = 160 keep the unfused route).  Mode 0 (FFMA) and mode 2 (unfused
@@ -546,47 +560,51 @@ bool flash_eligible(const Engine& e, int N, int Nk, int d, int C) {
   return C % (h16 ? 8 : 4) == 0;
 }
 
-bool flash_attention_tc(Engine& e, const float* q_hi, const float* q_lo, int ldq, const float* k_hi, const float* k_lo, int ldk,
-                        const float* vt_hi, const float* vt_lo, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d,
-                        float scale, cudaStream_t s, const int* qk_row, const int* acc_rows, int n_acc) {
-  if (N < 1 || (d % 8) || d < 16 || d > 80 || (ldq & 3) || (ldk & 3) || (ldo & 3) || (Nvs & 3) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
-  if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80)) return false;
-  if (!a16(q_hi) || !a16(q_lo) || !a16(k_hi) || !a16(k_lo) || !a16(vt_hi) || !a16(vt_lo) || !a16(out)) return false;
+bool flash_attention(Engine& e, const AttnPlanes& a, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d, float scale,
+                     cudaStream_t s, const int* qk_row, const int* acc_rows, int n_acc) {
+  const bool h16 = a.fmt == AttnPlanes::H16;
+  const int gm = h16 ? 7 : 3;            // strides in whole 16-byte granules (TMA)
+  if (N < 1 || (a.ldq & gm) || (a.ldk & gm) || (ldo & 3) || (Nvs & gm) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
+  if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || (h16 && d == 160))) return false;
+  const bool one = h16 && !a.q_lo;
+  if (h16 && (one ? (a.k_lo || a.vt_lo) : (!a.k_lo || !a.vt_lo))) return false;
+  if (!a16(a.q_hi) || !a16(a.k_hi) || !a16(a.vt_hi) || !a16(out)) return false;
+  if (!one && (!a16(a.q_lo) || !a16(a.k_lo) || !a16(a.vt_lo))) return false;
   if (acc_rows && n_acc < 1) return false;
   if (e.dry()) return true;
+  const int es = h16 ? 2 : 4;            // element bytes; every box row is 128 bytes
+  const uint32_t bw = 128 / es;
   const int NV = (d + 15) / 16 * 16;
   uint64_t dq[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)N, (uint64_t)B};
-  uint64_t sq[3] = {(uint64_t)d * 4, (uint64_t)ldq * 4, (uint64_t)N * ldq * 4};
+  uint64_t sq[3] = {(uint64_t)d * es, (uint64_t)a.ldq * es, (uint64_t)N * a.ldq * es};
   uint64_t dk[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)Nks, (uint64_t)B};
-  uint64_t sk[3] = {(uint64_t)d * 4, (uint64_t)ldk * 4, (uint64_t)Nks * ldk * 4};
-  uint32_t bq[4] = {32, 1, (uint32_t)flash_qrows(d), 1}, bk[4] = {32, 1, AKV, 1};
+  uint64_t sk[3] = {(uint64_t)d * es, (uint64_t)a.ldk * es, (uint64_t)Nks * a.ldk * es};
+  uint32_t bq[4] = {bw, 1, (uint32_t)flash_qrows(d), 1}, bk[4] = {bw, 1, AKV, 1};
   uint64_t dv[4] = {(uint64_t)Nvs, (uint64_t)B, (uint64_t)heads * d, 1};
-  uint64_t sv[3] = {(uint64_t)Nvs * 4, (uint64_t)B * Nvs * 4, (uint64_t)B * Nvs * 4 * heads * d};
-  uint32_t bv[4] = {32, 1, (uint32_t)NV, 1};
-  const CUtensorMap& qh = get_map(q_hi, 4, dq, sq, bq);
-  const CUtensorMap& ql = get_map(q_lo, 4, dq, sq, bq);
-  const CUtensorMap& kh = get_map(k_hi, 4, dk, sk, bk);
-  const CUtensorMap& kl = get_map(k_lo, 4, dk, sk, bk);
-  const CUtensorMap& vh = get_map(vt_hi, 4, dv, sv, bv);
-  const CUtensorMap& vl = get_map(vt_lo, 4, dv, sv, bv);
+  uint64_t sv[3] = {(uint64_t)Nvs * es, (uint64_t)B * Nvs * es, (uint64_t)B * Nvs * es * heads * d};
+  uint32_t bv[4] = {bw, 1, (uint32_t)NV, 1};
+  const CUtensorMap& qh = get_map(a.q_hi, 4, dq, sq, bq, nullptr, es);
+  const CUtensorMap& kh = get_map(a.k_hi, 4, dk, sk, bk, nullptr, es);
+  const CUtensorMap& vh = get_map(a.vt_hi, 4, dv, sv, bv, nullptr, es);
+  // (one-term: the lo maps are never read; the hi maps stand in for them)
+  const CUtensorMap& ql = one ? qh : get_map(a.q_lo, 4, dq, sq, bq, nullptr, es);
+  const CUtensorMap& kl = one ? kh : get_map(a.k_lo, 4, dk, sk, bk, nullptr, es);
+  const CUtensorMap& vl = one ? vh : get_map(a.vt_lo, 4, dv, sv, bv, nullptr, es);
   AttnParams p;
   p.N = N; p.Nk = Nk; p.heads = heads; p.d = d;
   p.B = acc_rows ? n_acc : B;           // CTAs along z: the images served
   p.scale_log2e = scale * 1.4426950408889634f;
   p.out = out; p.ldo = ldo;
-  p.q_amax = p.k_amax = p.v_amax = nullptr;
+  p.q_amax = a.q_amax; p.k_amax = a.k_amax; p.v_amax = a.v_amax;
   p.qk_row = qk_row;
   p.acc_rows = acc_rows;
-  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * p.B * heads,
-               4.0 * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 4.0 * p.B * (double)N * d * heads : 0.0), 1);
-  switch (d) {
-    case 16: launch_flash<16, false>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 32: launch_flash<32, false>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 40: launch_flash<40, false>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 64: launch_flash<64, false>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 80: launch_flash<80, false>(qh, ql, kh, kl, vh, vl, p, s); break;
-    default: return false;
-  }
+  const double bytes = h16 ? (one ? 1.0 : 2.0) * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 8.0 : 4.0) * p.B * heads * (double)N * d
+                           : 4.0 * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 4.0 * p.B * (double)N * d * heads : 0.0);
+  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * p.B * heads, bytes, 1);
+  const bool ok = one ? launch_flash_d<true, true>(d, qh, ql, kh, kl, vh, vl, p, s)
+                      : h16 ? launch_flash_d<true, false>(d, qh, ql, kh, kl, vh, vl, p, s)
+                            : launch_flash_d<false, false>(d, qh, ql, kh, kl, vh, vl, p, s);
+  if (!ok) return false;
   CDX_CUDA(cudaGetLastError());
   e.launches++;
   return true;
@@ -617,75 +635,6 @@ void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long l
             (__half*)lo, amax);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
-}
-
-// fp16-split variant: q / k planes [rows, ld] halves (head h at column h*d; Nks key rows per image), V^T planes [heads*d, B*Nvs] halves
-// (Nvs keys per image, the padding columns zero), each tensor's planes scaled by 2^h16_exp_of(*amax) of its slot (split_rows_h16 /
-// split_transpose_h16 above).  ld and Nvs multiples of 8.  All three lo planes null: the one-term kernel (hi * hi products only, mma mode 5).
-bool flash_attention_h16(Engine& e, const void* q_hi, const void* q_lo, int ldq, const void* k_hi, const void* k_lo, int ldk, const void* vt_hi,
-                         const void* vt_lo, const float* q_amax, const float* k_amax, const float* v_amax, float* out, int ldo, int B, int N,
-                         int Nk, int Nks, int Nvs, int heads, int d, float scale, cudaStream_t s, const int* qk_row, const int* acc_rows,
-                         int n_acc) {
-  if (N < 1 || (ldq & 7) || (ldk & 7) || (ldo & 3) || (Nvs & 7) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
-  if (!(d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || d == 160)) return false;
-  const bool one = q_lo == nullptr;
-  if (one ? (k_lo || vt_lo) : (!k_lo || !vt_lo)) return false;
-  if (!a16(q_hi) || !a16(k_hi) || !a16(vt_hi) || !a16(out)) return false;
-  if (!one && (!a16(q_lo) || !a16(k_lo) || !a16(vt_lo))) return false;
-  if (acc_rows && n_acc < 1) return false;
-  if (e.dry()) return true;
-  const int NV = (d + 15) / 16 * 16;
-  uint64_t dq[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)N, (uint64_t)B};
-  uint64_t sq[3] = {(uint64_t)d * 2, (uint64_t)ldq * 2, (uint64_t)N * ldq * 2};
-  uint64_t dk[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)Nks, (uint64_t)B};
-  uint64_t sk[3] = {(uint64_t)d * 2, (uint64_t)ldk * 2, (uint64_t)Nks * ldk * 2};
-  uint32_t bq[4] = {64, 1, (uint32_t)flash_qrows(d), 1}, bk[4] = {64, 1, AKV, 1};
-  uint64_t dv[4] = {(uint64_t)Nvs, (uint64_t)B, (uint64_t)heads * d, 1};
-  uint64_t sv[3] = {(uint64_t)Nvs * 2, (uint64_t)B * Nvs * 2, (uint64_t)B * Nvs * 2 * heads * d};
-  uint32_t bv[4] = {64, 1, (uint32_t)NV, 1};
-  const CUtensorMap& qh = get_map(q_hi, 4, dq, sq, bq, nullptr, 2);
-  const CUtensorMap& kh = get_map(k_hi, 4, dk, sk, bk, nullptr, 2);
-  const CUtensorMap& vh = get_map(vt_hi, 4, dv, sv, bv, nullptr, 2);
-  // (one-term: the lo maps are never read; the hi maps stand in for them)
-  const CUtensorMap& ql = one ? qh : get_map(q_lo, 4, dq, sq, bq, nullptr, 2);
-  const CUtensorMap& kl = one ? kh : get_map(k_lo, 4, dk, sk, bk, nullptr, 2);
-  const CUtensorMap& vl = one ? vh : get_map(vt_lo, 4, dv, sv, bv, nullptr, 2);
-  AttnParams p;
-  p.N = N; p.Nk = Nk; p.heads = heads; p.d = d;
-  p.B = acc_rows ? n_acc : B;           // CTAs along z: the images served
-  p.scale_log2e = scale * 1.4426950408889634f;
-  p.out = out; p.ldo = ldo;
-  p.q_amax = q_amax; p.k_amax = k_amax; p.v_amax = v_amax;
-  p.qk_row = qk_row;
-  p.acc_rows = acc_rows;
-  ProfScope ps(e, s, PROF_BATCHED_TC, 4.0 * N * (double)Nk * d * p.B * heads,
-               (one ? 1.0 : 2.0) * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 8.0 : 4.0) * p.B * heads * (double)N * d, 1);
-  if (one) {
-    switch (d) {
-      case 16: launch_flash<16, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-      case 32: launch_flash<32, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-      case 40: launch_flash<40, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-      case 64: launch_flash<64, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-      case 80: launch_flash<80, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-      case 160: launch_flash<160, true, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-      default: return false;
-    }
-    CDX_CUDA(cudaGetLastError());
-    e.launches++;
-    return true;
-  }
-  switch (d) {
-    case 16: launch_flash<16, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 32: launch_flash<32, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 40: launch_flash<40, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 64: launch_flash<64, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 80: launch_flash<80, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-    case 160: launch_flash<160, true>(qh, ql, kh, kl, vh, vl, p, s); break;
-    default: return false;
-  }
-  CDX_CUDA(cudaGetLastError());
-  e.launches++;
-  return true;
 }
 
 }  // namespace cdx

@@ -689,16 +689,18 @@ struct Exec {
 // ------------------------------------------------------------------------------------------------ U-Nets
 struct UNetExec : Exec {
   const float* E = nullptr;   // [B, emb_rows] all ResBlock emb projections
-  const float* ctx = nullptr;
   int ctx_len = 0;
-  const float* ctx_pad = nullptr;   // context zero-padded to ctx_lp rows per image (tensor-core cross-attention)
-  int ctx_lp = 0;
+  int ctx_lp = 0;                          // context rows per image, padded for the fused cross-attention
   bool kv_reuse = false, kv_hit = false;   // loop mode: context K / V live in n.ctxkv (kv_hit: already computed)
   const AttnControl* ctl = nullptr;        // attention control of this call, or null
-  const float* ctxv_pad = nullptr;         // ctl->ctx_v zero-padded to ctx_lp rows per image, and its range
-  float* ctxv_amax = nullptr;
-  const float* ctxw_pad = nullptr;         // ctl->ctx_w (refine) the same way
-  float* ctxw_amax = nullptr;
+  // the contexts the cross-attention projects: [0] the call's context, [1] the V' context (AttnControl::ctx_v), [2] the refine
+  // context (ctx_w); src null when absent.  pad: src zero-padded to ctx_lp rows per image (fused route only); amax: range slot of
+  // src (A operand of the K / V projections)
+  struct CtxIn {
+    const float* src = nullptr;
+    const float* pad = nullptr;
+    float* amax = nullptr;
+  } cx[3];
   size_t kv_off = 0;
   float* kv_take(size_t floats) {
     if (!kv_reuse) return (float*)e.arena.alloc(floats * sizeof(float));
@@ -707,9 +709,8 @@ struct UNetExec : Exec {
     CDX_CHECK(kv_off <= n.ctxkv.cap, "context K/V cache overflow (%zu > %zu floats)", kv_off, n.ctxkv.cap);
     return p;
   }
-  // range slots: of the context itself (A operand of the K / V projections) and of each layer's V (bounds the attention output).
-  // In loop mode the projections run only in the first call, so their slots live with the cached K / V, outside the per-call pool.
-  float* ctx_amax = nullptr;
+  // range slots: of the contexts (CtxIn::amax) and of each layer's V (bounds the attention output).  In loop mode the projections
+  // run only in the first call, so their slots live with the cached K / V, outside the per-call pool.
   int kv_layer = 0;
   float* kv_amax() {
     if (!kv_reuse) return e.amax_slot();
@@ -720,6 +721,23 @@ struct UNetExec : Exec {
   // an identity token map leaves every exponent (and the output's range) as without control
   void v2_range(const float* kv_slot, float* v2_slot) {
     if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(v2_slot, kv_slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
+  }
+  // V^T planes of one padded context (Mk rows) in the engine's format for the fused cross-attention of block t, maxing its range
+  // into `slot`; with k_hi also the K planes.  fp16: one fused K | V projection, K and V^T split from it with the slot of the whole
+  // output -- a V' or V'' context takes the same projection with its K half unused, so an identity token map gives V' == V.
+  // TF32: K and V^T = Wv . ctx^T (a swapped-role GEMM, so that both P.V operands are K-major) written as planes by the epilogues
+  void context_planes(const CtxIn& x, const std::string& t, int C, int Mk, float* slot, float* k_hi, float* k_lo, float* vt_hi, float* vt_lo) {
+    const int D = n.ucfg.context_dim;
+    if (e.tc_kind >= 1) {
+      Scope sk(e.arena);
+      float* kvf = (float*)e.arena.alloc((size_t)Mk * 2 * C * sizeof(float));
+      linear_into(x.pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, x.amax, nullptr, slot);
+      if (k_hi) split_rows_h16(e, kvf, Mk, C, 2 * C, k_hi, k_lo, C, slot, s);
+      split_transpose_h16(e, kvf + C, Mk, C, 2 * C, vt_hi, vt_lo, slot, s);
+    } else {
+      if (k_hi) linear_into(x.pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), C, nullptr, nullptr, 0, k_hi, C, k_lo, x.amax);
+      linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, x.pad, Mk, nullptr, nullptr, 0, vt_hi, Mk, vt_lo, nullptr, nullptr, slot);
+    }
   }
   bool oai;
   UNetExec(Net& net, cudaStream_t st) : Exec(net, st), oai(net.kind == NET_UNET_OPENAI) {}
@@ -809,8 +827,9 @@ struct UNetExec : Exec {
         void* vt_lo = lo ? e.arena.alloc((size_t)C * B * Nvs * 2) : nullptr;
         split_rows_h16(e, qkv, M, 2 * C, 3 * C, qk_hi, qk_lo, 2 * C, a.amax, s);
         split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s, B, Nvs);
-        done = flash_attention_h16(e, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr, 2 * C,
-                                   vt_hi, vt_lo, a.amax, a.amax, a.amax, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow);
+        const AttnPlanes pl{AttnPlanes::H16, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr,
+                            2 * C, vt_hi, vt_lo, a.amax, a.amax, a.amax};
+        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow);
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok && (HW % 4) != 0) {
         // TF32 planes with a per-image key count off the 16-byte TMA granule: V row-major, copied into rows padded to Nvs keys
@@ -833,8 +852,8 @@ struct UNetExec : Exec {
         }
         nhwc_to_nchw(e, vp, vt, 1, C, B * Nvs, s);
         split_planes(e, vt, vt_hi, vt_lo, nvt, s);
-        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s,
-                                  srow);
+        const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
+        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands
@@ -845,8 +864,7 @@ struct UNetExec : Exec {
         float* qk_lo = (float*)e.arena.alloc(nqk * sizeof(float));
         float* vt_hi = (float*)e.arena.alloc(nvt * sizeof(float));
         float* vt_lo = (float*)e.arena.alloc(nvt * sizeof(float));
-        static const bool no_fused_qkv = getenv("CDX_NO_FUSED_QKV") != nullptr;     // tuning aid
-        if (!no_fused_qkv && (2 * C) % 128 == 0 && M >= 64 && (C % 4) == 0) {
+        if ((2 * C) % 128 == 0 && M >= 64 && (C % 4) == 0) {
           // one fused q|k|v projection (weights adjacent in the blob): q|k stored row-major as planes, the v columns stored
           // transposed by the epilogue (thread = row, so a column is 32 consecutive floats per warp) -> V^T planes
           GemmArgs g;
@@ -864,8 +882,8 @@ struct UNetExec : Exec {
           linear_into(n.P(t + ".attn1.to_v.weight"), C, C, nullptr, 0, 0, C, n1.p, M, nullptr, nullptr, 0, vt_hi, M, vt_lo, nullptr, nullptr,
                       a.amax);   // V^T = Wv . X^T
         }
-        done = flash_attention_tc(e, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s,
-                                  srow);
+        const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
+        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s, srow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (e.mma_mode >= 1 && (HW % 32) == 0 && HW >= 128 && (d % 4) == 0) {
         // unfused tensor-core attention (mode 2, or shapes the fused kernel does not cover)
@@ -916,96 +934,57 @@ struct UNetExec : Exec {
       const bool use_v3 = crow && wmap;
       bool done = false;
       Tensor q;
-      const bool flash_ok = ctx_pad && flash_eligible(e, HW, ctx_len, d, C);
+      const bool flash_ok = cx[0].pad && flash_eligible(e, HW, ctx_len, d, C);
       CDX_CHECK(!crow || flash_ok, "attention control: cross-attention at HW=%d d=%d would take the unfused route (mma mode "
                 "and head width must run the fused kernel)", HW, d);
-      if (flash_ok && e.tc_kind >= 1) {
-        // fp16-split fused attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the kernel):
-        // q projected as plain fp32 (range tracked), K | V from one fused projection of the context; fp16 planes by the split pass.
-        // K and V share the layer's slot (one exponent for both); in loop mode planes and slot are computed by the first call only.
-        // Mode 5: hi planes only (the cache then holds no lo planes; it lives for one loop, which runs in one mode)
+      if (flash_ok) {
+        // fused attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the kernel).  fp16 planes:
+        // q projected as plain fp32 (range tracked) and split; K and V share the layer's slot (one exponent for both).  TF32 planes:
+        // q written as planes by its projection's epilogue.  In loop mode the context planes and slots are computed by the first call
+        // only.  Mode 5: hi planes only (the cache then holds no lo planes; it lives for one loop, which runs in one mode)
         Scope sa(e.arena);
-        const bool lo = !e.attn_one;
+        const bool h16 = e.tc_kind >= 1, lo = !e.attn_one;
         const int Mk = B * ctx_lp;
-        const size_t nk = (size_t)Mk * C;
-        float* k_hi = kv_take(nk / 2);
-        float* k_lo = lo ? kv_take(nk / 2) : nullptr;
-        float* vt_hi = kv_take(nk / 2);
-        float* vt_lo = lo ? kv_take(nk / 2) : nullptr;
-        float* v2_hi = vmap ? kv_take(nk / 2) : nullptr;
-        float* v2_lo = vmap && lo ? kv_take(nk / 2) : nullptr;
-        float* v3_hi = wmap ? kv_take(nk / 2) : nullptr;
-        float* v3_lo = wmap && lo ? kv_take(nk / 2) : nullptr;
-        Tensor qf = linear(n2, t + ".attn2.to_q", false, nullptr, true);
-        void* q_hi = e.arena.alloc((size_t)M * C * 2);
-        void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
-        split_rows_h16(e, qf.p, M, C, C, q_hi, q_lo, C, qf.amax, s);
-        if (!kv_hit) {
-          Scope sk(e.arena);
-          float* kvf = (float*)e.arena.alloc((size_t)Mk * 2 * C * sizeof(float));
-          linear_into(ctx_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, ctx_amax, nullptr,
-                      a.amax);
-          split_rows_h16(e, kvf, Mk, C, 2 * C, k_hi, k_lo, C, a.amax, s);
-          split_transpose_h16(e, kvf + C, Mk, C, 2 * C, vt_hi, vt_lo, a.amax, s);
-          if (vmap) {             // the same fused K | V projection of the V context (its K half unused): an identity map gives V' == V
-            v2_range(a.amax, v2_amax);
-            linear_into(ctxv_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, ctxv_amax,
-                        nullptr, v2_amax);
-            split_transpose_h16(e, kvf + C, Mk, C, 2 * C, v2_hi, v2_lo, v2_amax, s);
-          }
-          if (wmap) {             // V'' by the same fused projection of the refine context, then the output's slot
-            linear_into(ctxw_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, ctxw_amax,
-                        nullptr, v3_amax);
-            split_transpose_h16(e, kvf + C, Mk, C, 2 * C, v3_hi, v3_lo, v3_amax, s);
-            add(e, vmap ? v2_amax : a.amax, v3_amax, sum_amax, 1, s);
-          }
+        const size_t np = h16 ? (size_t)Mk * C / 2 : (size_t)Mk * C;     // floats per plane
+        float* k_hi = kv_take(np);
+        float* k_lo = lo ? kv_take(np) : nullptr;
+        float* vt_hi = kv_take(np);
+        float* vt_lo = lo ? kv_take(np) : nullptr;
+        float* v2_hi = vmap ? kv_take(np) : nullptr;
+        float* v2_lo = vmap && lo ? kv_take(np) : nullptr;
+        float* v3_hi = wmap ? kv_take(np) : nullptr;
+        float* v3_lo = wmap && lo ? kv_take(np) : nullptr;
+        AttnPlanes pl{h16 ? AttnPlanes::H16 : AttnPlanes::TF32, nullptr, nullptr, C, k_hi, k_lo, C, nullptr, nullptr};
+        if (h16) {
+          Tensor qf = linear(n2, t + ".attn2.to_q", false, nullptr, true);
+          void* q_hi = e.arena.alloc((size_t)M * C * 2);
+          void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
+          split_rows_h16(e, qf.p, M, C, C, q_hi, q_lo, C, qf.amax, s);
+          pl.q_hi = q_hi; pl.q_lo = q_lo; pl.q_amax = qf.amax;
+        } else {
+          float* q_hi = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+          float* q_lo = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+          linear_into(n2.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn2.to_q.weight"), C, nullptr, nullptr, 0, q_hi, C, q_lo, n2.amax);
+          pl.q_hi = q_hi; pl.q_lo = q_lo;
         }
-        done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, use_v2 ? v2_hi : vt_hi, use_v2 ? v2_lo : vt_lo, qf.amax, a.amax,
-                                   use_v2 ? v2_amax : a.amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, crow);
-        CDX_CHECK(done, "flash cross-attention (fp16-split) rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
-        if (use_v3) {             // + the controlled rows' own attention over V'' (accumulating launch, those rows' CTAs only)
-          done = flash_attention_h16(e, q_hi, q_lo, C, k_hi, k_lo, C, v3_hi, v3_lo, qf.amax, a.amax, v3_amax, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp,
-                                     heads, d, scale, s, nullptr, ctl->own_rows, ctl->n_own);
-          CDX_CHECK(done, "flash cross-attention (fp16-split) rejected the refine term (HW=%d d=%d L=%d)", HW, d, ctx_len);
-        }
-      } else if (flash_ok) {
-        // fused tensor-core attention over the zero-padded context (ctx_lp rows per image, keys >= ctx_len masked in the
-        // kernel): q = n2.Wq^T, K = ctx.Wk^T, V^T = Wv.ctx^T (swapped-role GEMM), all written as TF32 planes
-        Scope sa(e.arena);
-        const int Mk = B * ctx_lp;
-        const size_t nq = (size_t)M * C, nk = (size_t)Mk * C;
-        float* k_hi = kv_take(nk);
-        float* k_lo = kv_take(nk);
-        float* vt_hi = kv_take(nk);
-        float* vt_lo = kv_take(nk);
-        float* v2_hi = vmap ? kv_take(nk) : nullptr;
-        float* v2_lo = vmap ? kv_take(nk) : nullptr;
-        float* v3_hi = wmap ? kv_take(nk) : nullptr;
-        float* v3_lo = wmap ? kv_take(nk) : nullptr;
-        float* q_hi = (float*)e.arena.alloc(nq * sizeof(float));
-        float* q_lo = (float*)e.arena.alloc(nq * sizeof(float));
-        linear_into(n2.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn2.to_q.weight"), C, nullptr, nullptr, 0, q_hi, C, q_lo, n2.amax);
         if (!kv_hit) {
-          linear_into(ctx_pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), C, nullptr, nullptr, 0, k_hi, C, k_lo, ctx_amax);
-          linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctx_pad, Mk, nullptr, nullptr, 0, vt_hi, Mk, vt_lo, nullptr, nullptr,
-                      a.amax);
+          context_planes(cx[0], t, C, Mk, a.amax, k_hi, k_lo, vt_hi, vt_lo);
           if (vmap) {
             v2_range(a.amax, v2_amax);
-            linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctxv_pad, Mk, nullptr, nullptr, 0, v2_hi, Mk, v2_lo, nullptr, nullptr,
-                        v2_amax);
+            context_planes(cx[1], t, C, Mk, v2_amax, nullptr, nullptr, v2_hi, v2_lo);
           }
-          if (wmap) {
-            linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, ctxw_pad, Mk, nullptr, nullptr, 0, v3_hi, Mk, v3_lo, nullptr, nullptr,
-                        v3_amax);
+          if (wmap) {             // V'', then the output's slot
+            context_planes(cx[2], t, C, Mk, v3_amax, nullptr, nullptr, v3_hi, v3_lo);
             add(e, vmap ? v2_amax : a.amax, v3_amax, sum_amax, 1, s);
           }
         }
-        done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, use_v2 ? v2_hi : vt_hi, use_v2 ? v2_lo : vt_lo, a.p, C, B, HW, ctx_len, ctx_lp,
-                                  ctx_lp, heads, d, scale, s, crow);
+        pl.k_amax = a.amax;
+        pl.vt_hi = use_v2 ? v2_hi : vt_hi; pl.vt_lo = use_v2 ? v2_lo : vt_lo; pl.v_amax = use_v2 ? v2_amax : a.amax;
+        done = flash_attention(e, pl, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, crow);
         CDX_CHECK(done, "flash cross-attention rejected an eligible shape (HW=%d d=%d L=%d)", HW, d, ctx_len);
-        if (use_v3) {
-          done = flash_attention_tc(e, q_hi, q_lo, C, k_hi, k_lo, C, v3_hi, v3_lo, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, nullptr,
-                                    ctl->own_rows, ctl->n_own);
+        if (use_v3) {             // + the controlled rows' own attention over V'' (accumulating launch, those rows' CTAs only)
+          pl.vt_hi = v3_hi; pl.vt_lo = v3_lo; pl.v_amax = v3_amax;
+          done = flash_attention(e, pl, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, nullptr, ctl->own_rows, ctl->n_own);
           CDX_CHECK(done, "flash cross-attention rejected the refine term (HW=%d d=%d L=%d)", HW, d, ctx_len);
         }
       }
@@ -1015,8 +994,8 @@ struct UNetExec : Exec {
       if (!done) {
         Scope sa(e.arena);
         float* kv = kv_take((size_t)B * ctx_len * 2 * C);
-        if (!kv_hit) linear_into(ctx, D, D, nullptr, 0, 0, B * ctx_len, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kv, 2 * C, nullptr,
-                                 ctx_amax, nullptr, a.amax);
+        if (!kv_hit) linear_into(cx[0].src, D, D, nullptr, 0, 0, B * ctx_len, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kv, 2 * C,
+                                 nullptr, cx[0].amax, nullptr, a.amax);
         attention(e, q.p, C, kv, 2 * C, kv + C, 2 * C, a.p, C, B, HW, ctx_len, heads, d, d, scale, s);
       }
       h3 = linear(a, t + ".attn2.to_out.0", true, h2.p);
@@ -1147,9 +1126,7 @@ struct UNetExec : Exec {
 
   void forward(const float* x_nchw, const float* t_dev, const float* context, int L, float* out_nchw, int B, int H, int W) {
     const cdx_unet_config& c = n.ucfg;
-    ctx = context;
     ctx_len = L;
-    ctx_pad = nullptr;
     ctx_lp = (L + 7) & ~7;                // (fp16 planes: 16-byte TMA strides need 8 keys)
     const int mc = c.model_channels, half = mc / 2, ted = n.ted;
     Scope top(e.arena);
@@ -1179,42 +1156,24 @@ struct UNetExec : Exec {
     }
     kv_layer = 0;
     if (context && L > 0) {
-      // range of the context (A operand of the K / V projections; measured once per loop)
-      ctx_amax = kv_reuse ? (e.dry() ? reinterpret_cast<float*>((uintptr_t)0x100) : n.ctxkv.amax) : e.amax_slot();
-      if (!kv_hit) amax_rows(e, context, (long long)B * L, c.context_dim, c.context_dim, ctx_amax, s);
-      if (ctl && ctl->ctx_v) {
-        ctxv_amax = kv_amax();
-        if (!kv_hit) amax_rows(e, ctl->ctx_v, (long long)B * L, c.context_dim, c.context_dim, ctxv_amax, s);
-      }
-      if (ctl && ctl->ctx_w) {
-        ctxw_amax = kv_amax();
-        if (!kv_hit) amax_rows(e, ctl->ctx_w, (long long)B * L, c.context_dim, c.context_dim, ctxw_amax, s);
-      }
-    }
-    if (context && L > 0 && e.mma_mode == 1 && e.flash_attn) {
-      // context rows padded to a multiple of 8 per image: TMA needs 16-byte strides for K and V^T of the cross-attention
+      // each context's range (A operand of the K / V projections) and, for the fused route, its rows padded with zeros to ctx_lp per
+      // image (TMA needs 16-byte strides for K and V^T); in loop mode both once per loop
       const size_t D = (size_t)c.context_dim;
-      float* cp = (float*)e.arena.alloc((size_t)B * ctx_lp * D * sizeof(float));
-      if (!e.dry() && !kv_hit) {
-        if (ctx_lp != L) CDX_CUDA(cudaMemsetAsync(cp, 0, (size_t)B * ctx_lp * D * sizeof(float), s));
-        CDX_CUDA(cudaMemcpy2DAsync(cp, (size_t)ctx_lp * D * 4, context, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
-      }
-      ctx_pad = cp;
-      if (ctl && ctl->ctx_v) {
-        float* vp = (float*)e.arena.alloc((size_t)B * ctx_lp * D * sizeof(float));
+      const float* src[3] = {context, ctl ? ctl->ctx_v : nullptr, ctl ? ctl->ctx_w : nullptr};
+      for (int i = 0; i < 3; ++i) {
+        if (!src[i]) continue;
+        CtxIn& x = cx[i];
+        x.src = src[i];
+        // the context's slot is the cache's first; the V' and V'' contexts take the next ones
+        x.amax = i ? kv_amax() : kv_reuse ? (e.dry() ? reinterpret_cast<float*>((uintptr_t)0x100) : n.ctxkv.amax) : e.amax_slot();
+        if (!kv_hit) amax_rows(e, x.src, (long long)B * L, c.context_dim, c.context_dim, x.amax, s);
+        if (e.mma_mode != 1 || !e.flash_attn) continue;
+        float* pad = (float*)e.arena.alloc((size_t)B * ctx_lp * D * sizeof(float));
         if (!e.dry() && !kv_hit) {
-          if (ctx_lp != L) CDX_CUDA(cudaMemsetAsync(vp, 0, (size_t)B * ctx_lp * D * sizeof(float), s));
-          CDX_CUDA(cudaMemcpy2DAsync(vp, (size_t)ctx_lp * D * 4, ctl->ctx_v, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
+          if (ctx_lp != L) CDX_CUDA(cudaMemsetAsync(pad, 0, (size_t)B * ctx_lp * D * sizeof(float), s));
+          CDX_CUDA(cudaMemcpy2DAsync(pad, (size_t)ctx_lp * D * 4, x.src, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
         }
-        ctxv_pad = vp;
-      }
-      if (ctl && ctl->ctx_w) {
-        float* wp = (float*)e.arena.alloc((size_t)B * ctx_lp * D * sizeof(float));
-        if (!e.dry() && !kv_hit) {
-          if (ctx_lp != L) CDX_CUDA(cudaMemsetAsync(wp, 0, (size_t)B * ctx_lp * D * sizeof(float), s));
-          CDX_CUDA(cudaMemcpy2DAsync(wp, (size_t)ctx_lp * D * 4, ctl->ctx_w, (size_t)L * D * 4, (size_t)L * D * 4, B, cudaMemcpyDeviceToDevice, s));
-        }
-        ctxw_pad = wp;
+        x.pad = pad;
       }
     }
     // --- timestep embedding MLP + all ResBlock emb projections in one GEMM

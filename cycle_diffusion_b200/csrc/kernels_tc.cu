@@ -25,7 +25,12 @@
 //   warpgroups 1-2  64 rows each: raw fp32 A from smem -> hi / lo split in registers (the wgmma A fragment layout) -> three wgmmas
 //                 per K step against the B tiles in smem -> chunk accumulator -> total, software-pipelined (the next stage's A
 //                 is split into a second fragment set while the current stage's wgmmas run, one batch per stage); then the
-//                 epilogue straight from registers: alpha / rescale, +bias, +per-sample row vector (timestep embedding), GEGLU, +residual, range / GroupNorm side outputs.
+//                 epilogue from registers: alpha / rescale, +bias, +per-sample row vector (timestep embedding), GEGLU, +residual, range / GroupNorm side outputs.
+// Staged epilogue (every fp32 row output of a dense or conv3x3 work item that is not split along K): once the producer has issued
+// the last K stage it claims the ring slots that follow it and, with a residual, TMA-loads the residual tile there as 32-column
+// boxes (the A box's shape) while the last stages' wgmmas run; the consumers add it from shared memory, write the result back in
+// place (or into the claimed slots), and one thread stores the tile by TMA, which clips rows and columns outside C.  Split-K partials,
+// the NCHW store, TF32 / transposed planes and batched products store per element from registers.
 #include <algorithm>
 
 #include <mutex>
@@ -72,7 +77,16 @@ struct Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + 2 * B_PLANE;
   static constexpr int STAGES = (SMEM_MAX - BAR_BYTES - ALIGN_SLACK) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + ALIGN_SLACK;
-  static_assert(STAGES >= 3 && 2 * STAGES * 8 <= BAR_BYTES, "barrier area holds a full and an empty barrier per stage");
+  // Staged epilogue: the output tile (and the residual tile, loaded by TMA) as 32-column fp32 boxes of 128 rows (the A box's shape,
+  // 128B swizzle), EPI_PER_SLOT to a ring slot, in the slots of ring stages nst, nst + 1, ... after the work item's nst stages.  The
+  // producer claims each through its empty barrier, which frees the slot of stage nst + k - STAGES; the last stage's slot is never
+  // handed back, so every claimed slot must have held a stage before nst - 1, and for the residual to land while the last wgmmas
+  // run, before nst - 2: STAGES >= 2 + EPI_SLOTS.
+  static constexpr int EPI_BOX = TBM * TBK * 4;
+  static constexpr int EPI_PER_SLOT = STAGE_BYTES / EPI_BOX;
+  static constexpr int EPI_SLOTS = (BN / TBK + EPI_PER_SLOT - 1) / EPI_PER_SLOT;
+  static_assert(STAGES >= 2 + EPI_SLOTS, "the epilogue's slots never include the last stages' slots");
+  static_assert(STAGES >= 3 && (2 * STAGES + 1) * 8 <= BAR_BYTES, "barrier area holds a full and an empty barrier per stage and bar_res");
   static_assert(STAGE_BYTES % 1024 == 0 && B_PLANE % 1024 == 0, "stage and plane bases stay 1024-byte aligned (swizzle atoms)");
   static_assert(SMEM_BYTES <= SMEM_MAX, "smem overflow");
 };
@@ -114,6 +128,13 @@ struct TcParams {
   double* c_stats;          // optional: per-(image, channel) fp64 {sum, sum sq} of C, for the GroupNorm that consumes it; requires
                             // every 32-row quadrant of a tile to lie inside one image (checked on the host)
 };
+
+// Result tiles staged in shared memory and stored by TMA (mapC; the residual tile arrives by TMA through mapR): every fp32 row
+// output of a dense or conv3x3 work item.  Split-K partials, the NCHW store, TF32 / transposed planes and batched products keep the
+// per-element stores.
+__host__ __device__ __forceinline__ bool staged_store(const TcParams& p) {
+  return p.mode != 2 && p.splits == 1 && !p.out_nchw && !p.Ct_hi && !p.C_lo;
+}
 
 __device__ __forceinline__ int h16_a_exp(const TcParams& p) {
   float m = p.a_amax ? *p.a_amax : 0.f;
@@ -163,11 +184,12 @@ __device__ __forceinline__ uint32_t tf32_lo(float x, uint32_t hi) { return rn_tf
 template <int KIND, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2,
-               const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapBlo, const TcParams p) {
+               const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapBlo,
+               const __grid_constant__ CUtensorMap mapR, const __grid_constant__ CUtensorMap mapC, const TcParams p) {
   using CF = Cfg<KIND, BN>;
   constexpr bool H16 = CF::H16, FAST = KIND == KIND_H16_FAST;
   constexpr int BK = CF::BK, KSTEPS = CF::KSTEPS, A_BYTES = CF::A_BYTES, B_PLANE = CF::B_PLANE, STAGE_BYTES = CF::STAGE_BYTES;
-  constexpr int STAGES = CF::STAGES;
+  constexpr int STAGES = CF::STAGES, EPI_BOX = CF::EPI_BOX, EPI_PER_SLOT = CF::EPI_PER_SLOT, EPI_SLOTS = CF::EPI_SLOTS;
   constexpr int NACC = BN / 2;                     // fp32 accumulators per thread of an m64nBN tile
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
@@ -175,16 +197,22 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const uint32_t bars = base + STAGES * STAGE_BYTES;
   auto bar_full = [&](int s) { return bars + 8u * s; };
   auto bar_empty = [&](int s) { return bars + 8u * (STAGES + s); };
+  const uint32_t bar_res = bars + 16u * STAGES;    // the epilogue's slots are claimed (and the residual tile has landed)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = (p.K + BK - 1) / BK;
   const TileCoord tc_ = tile_coord(p, blockIdx.x, num_kb);
+  const int nst = tc_.kb1 - tc_.kb0;               // stages of this work item (>= 1; K % 32 == 0: every stage is full)
+  const bool staged = staged_store(p);
+  // shared address of 32-column box k of the staged output / residual tile
+  auto epi_box = [&](int k) { return base + ((nst + k / EPI_PER_SLOT) % STAGES) * STAGE_BYTES + (k % EPI_PER_SLOT) * EPI_BOX; };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(bar_full(s), 1);
       mbar_init(bar_empty(s), 8);                 // one arrival per consumer warp
     }
+    mbar_init(bar_res, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -228,6 +256,22 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         tma_load_2d(sb, &mapB, k0, tc_.n0, bar_full(s));
         if (KIND != KIND_SS) tma_load_2d(sb + B_PLANE, &mapBlo, k0, tc_.n0, bar_full(s));
       }
+      if (staged) {
+        // the epilogue's slots, as ring stages nst, nst + 1, ...: each frees as the consumers retire the stage it held, and the
+        // residual boxes land there while the last stages' wgmmas run
+        if (p.residual) mbar_expect_tx(bar_res, BN * TBM * 4);
+        for (int k = 0; k < EPI_SLOTS; ++k, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(bar_empty(s), ((it / STAGES) & 1) ^ 1);
+          if (!p.residual) continue;
+          for (int b = k * EPI_PER_SLOT; b < min(BN / TBK, (k + 1) * EPI_PER_SLOT); ++b) {
+            const uint32_t dst = epi_box(b);
+            if (p.mode == 0) tma_load_2d(dst, &mapR, tc_.n0 + b * TBK, tc_.m0, bar_res);
+            else tma_load_4d(dst, &mapR, tc_.n0 + b * TBK, tc_.x0, tc_.y0, tc_.b0, bar_res);
+          }
+        }
+        if (!p.residual) mbar_arrive(bar_res);
+      }
     }
     return;
   }
@@ -257,7 +301,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   // Software pipeline over the stages of the work item: while the wgmmas of stage it run, stage it + 1's A is split into the
   // other fragment set; wgmma.wait_group 1 then retires stage it - 1, whose smem slot goes back to the producer.
   struct Frag { uint32_t h[KSTEPS][4], l[KSTEPS][4]; };     // A fragments of one stage's K steps (rows r0 / r0 + 8), hi / lo
-  const int nst = tc_.kb1 - tc_.kb0;               // stages of this work item (>= 1; K % 32 == 0: every stage is full)
 
   // wait for stage it to land, then split its A into f
   auto load_split = [&](int it, Frag& f) {
@@ -457,52 +500,90 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   } else {
     float* const dst = p.C + tc_.zb * p.sC_b + tc_.zh * p.sC_h;
     float* const dst_lo = p.C_lo ? p.C_lo + tc_.zb * p.sC_b + tc_.zh * p.sC_h : nullptr;
-    // GEGLU tiles are [32 value | 32 gate] blocks: accumulator group j (value) pairs with j + 4 (gate)
+    // one loop body, compiled for each store path: STAGED writes every row and column of the tile into the epilogue's boxes (rows
+    // and columns outside C are clipped by the TMA store), the other path stores the valid elements to global memory
+    auto store_tile = [&](auto staged_c) {
+      constexpr bool STAGED = decltype(staged_c)::value;
+      // GEGLU tiles are [32 value | 32 gate] blocks: accumulator group j (value) pairs with j + 4 (gate)
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      if (p.geglu && (j & 4)) continue;
-      const int n = n0 + 8 * j + 2 * qd;             // even; N % 4 == 0 (eligibility), so n + 1 < nend whenever n < nend
-      const int nout = p.geglu ? (n >> 6) * 32 + (n & 63) : n;
-      float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
+      for (int j = 0; j < BN / 8; ++j) {
+        if (p.geglu && (j & 4)) continue;
+        const int n = n0 + 8 * j + 2 * qd;             // even; N % 4 == 0 (eligibility), so n + 1 < nend whenever n < nend
+        const int nout = p.geglu ? (n >> 6) * 32 + (n & 63) : n;
+        // STAGED: the column pair's box and its column in the box (GEGLU: boxes of the BN / 2 output columns)
+        const int box = p.geglu ? j >> 3 : j >> 2, cc = 8 * (j & 3) + 2 * qd;
+        float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        float2 o = make_float2(tot[j * 4 + i * 2], tot[j * 4 + i * 2 + 1]);
-        if (p.geglu) {
-          const float g0 = tot[(j + 4) * 4 + i * 2], g1 = tot[(j + 4) * 4 + i * 2 + 1];
-          o.x *= 0.5f * g0 * (1.f + erff(g0 * 0.70710678118654752440f));     // exact-erf GELU as F.gelu
-          o.y *= 0.5f * g1 * (1.f + erff(g1 * 0.70710678118654752440f));
+        for (int i = 0; i < 2; ++i) {
+          float2 o = make_float2(tot[j * 4 + i * 2], tot[j * 4 + i * 2 + 1]);
+          if (p.geglu) {
+            const float g0 = tot[(j + 4) * 4 + i * 2], g1 = tot[(j + 4) * 4 + i * 2 + 1];
+            o.x *= 0.5f * g0 * (1.f + erff(g0 * 0.70710678118654752440f));     // exact-erf GELU as F.gelu
+            o.y *= 0.5f * g1 * (1.f + erff(g1 * 0.70710678118654752440f));
+          }
+          if (STAGED) {
+            // the 128B-swizzled box layout; the residual box holds its value at the same address
+            const int r = r0 + 8 * i;
+            const uint32_t a = epi_box(box) + (uint32_t)r * 128u + ((((uint32_t)cc >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(cc & 3) * 4u;
+            if (p.residual) {
+              float2 rv;
+              asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rv.x), "=f"(rv.y) : "r"(a));
+              o.x += rv.x;
+              o.y += rv.y;
+            }
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(o.x), "f"(o.y) : "memory");
+          }
+          if (!rok[i] || n >= nend) continue;
+          if (!STAGED && p.residual) {
+            o.x += p.residual[mrow[i] * p.ldr + n];
+            o.y += p.residual[mrow[i] * p.ldr + n + 1];
+          }
+          if (p.c_stats) { cs[0] += o.x; cq[0] += o.x * o.x; cs[1] += o.y; cq[1] += o.y * o.y; }
+          if (!STAGED) {
+            float* const d = dst + mrow[i] * p.ldc + nout;
+            if (dst_lo) {                          // operand planes for a following tensor-core consumer
+              const uint32_t hx = rn_tf32(__float_as_uint(o.x)), hy = rn_tf32(__float_as_uint(o.y));
+              *reinterpret_cast<float2*>(dst_lo + mrow[i] * p.ldc + nout) = make_float2(__uint_as_float(tf32_lo(o.x, hx)), __uint_as_float(tf32_lo(o.y, hy)));
+              o = make_float2(__uint_as_float(hx), __uint_as_float(hy));
+            }
+            *reinterpret_cast<float2*>(d) = o;
+          }
+          omax = fmaxf(omax, fmaxf(fabsf(o.x), fabsf(o.y)));
         }
-        if (!rok[i] || n >= nend) continue;
-        if (p.residual) {
-          o.x += p.residual[mrow[i] * p.ldr + n];
-          o.y += p.residual[mrow[i] * p.ldr + n + 1];
-        }
-        if (p.c_stats) { cs[0] += o.x; cq[0] += o.x * o.x; cs[1] += o.y; cq[1] += o.y * o.y; }
-        float* const d = dst + mrow[i] * p.ldc + nout;
-        if (dst_lo) {                          // operand planes for a following tensor-core consumer
-          const uint32_t hx = rn_tf32(__float_as_uint(o.x)), hy = rn_tf32(__float_as_uint(o.y));
-          *reinterpret_cast<float2*>(dst_lo + mrow[i] * p.ldc + nout) = make_float2(__uint_as_float(tf32_lo(o.x, hx)), __uint_as_float(tf32_lo(o.y, hy)));
-          o = make_float2(__uint_as_float(hx), __uint_as_float(hy));
-        }
-        *reinterpret_cast<float2*>(d) = o;
-        omax = fmaxf(omax, fmaxf(fabsf(o.x), fabsf(o.y)));
-      }
-      if (p.c_stats) {
-        // GroupNorm statistics: fold the warp's 16 rows (one image: host-checked), one fp64 atomic per (column, statistic)
+        if (p.c_stats) {
+          // GroupNorm statistics: fold the warp's 16 rows (one image: host-checked), one fp64 atomic per (column, statistic)
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
+          for (int c = 0; c < 2; ++c) {
 #pragma unroll
-          for (int o2 = 4; o2 < 32; o2 <<= 1) {
-            cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], o2);
-            cq[c] += __shfl_xor_sync(0xffffffffu, cq[c], o2);
+            for (int o2 = 4; o2 < 32; o2 <<= 1) {
+              cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], o2);
+              cq[c] += __shfl_xor_sync(0xffffffffu, cq[c], o2);
+            }
+          }
+          const long long mq = __shfl_sync(0xffffffffu, rok[0] ? mrow[0] : -1LL, 0);     // first row of the warp
+          if (g == 0 && mq >= 0 && n < nend) {
+            double* sp = p.c_stats + ((mq / p.rows_per_batch) * p.N + n) * 2;
+            atomicAdd(sp, (double)cs[0]); atomicAdd(sp + 1, (double)cq[0]);
+            atomicAdd(sp + 2, (double)cs[1]); atomicAdd(sp + 3, (double)cq[1]);
           }
         }
-        const long long mq = __shfl_sync(0xffffffffu, rok[0] ? mrow[0] : -1LL, 0);     // first row of the warp
-        if (g == 0 && mq >= 0 && n < nend) {
-          double* sp = p.c_stats + ((mq / p.rows_per_batch) * p.N + n) * 2;
-          atomicAdd(sp, (double)cs[0]); atomicAdd(sp + 1, (double)cq[0]);
-          atomicAdd(sp + 2, (double)cs[1]); atomicAdd(sp + 3, (double)cq[1]);
+      }
+    };
+    if (!staged) {
+      store_tile(std::false_type());
+    } else {
+      mbar_wait(bar_res, 0);                       // the boxes' slots are free and the residual boxes have landed
+      store_tile(std::true_type());
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA store
+      asm volatile("bar.sync 2, 256;" ::: "memory");                 // the consumer warpgroups' rows are all written
+      if (threadIdx.x == 128) {
+        const int c0 = p.geglu ? n0 / 2 : n0, ncols = p.geglu ? p.N / 2 : p.N;
+        for (int b = 0; b < (p.geglu ? BN / 64 : BN / TBK) && c0 + b * TBK < ncols; ++b) {
+          if (p.mode == 0) tma_store_2d(epi_box(b), &mapC, c0 + b * TBK, tc_.m0);
+          else tma_store_4d(epi_box(b), &mapC, c0 + b * TBK, tc_.x0, tc_.y0, tc_.b0);
         }
+        bulk_commit();
+        bulk_wait0();                              // written, not only read: a dependent launch reads C after its griddepcontrol.wait
       }
     }
   }
@@ -624,8 +705,9 @@ void ensure_attr(int device) {
 }
 
 template <int KIND, int BN>
-void launch_gemm(const TcParams& p, const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mBlo, cudaStream_t s) {
-  launch_ex(tc_gemm_kernel<KIND, BN>, dim3((unsigned)p.total_tiles), dim3(TC_THREADS), Cfg<KIND, BN>::SMEM_BYTES, s, 1, mA, mA2, mB, mBlo, p);
+void launch_gemm(const TcParams& p, const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mBlo,
+                 const CUtensorMap& mR, const CUtensorMap& mC, cudaStream_t s) {
+  launch_ex(tc_gemm_kernel<KIND, BN>, dim3((unsigned)p.total_tiles), dim3(TC_THREADS), Cfg<KIND, BN>::SMEM_BYTES, s, 1, mA, mA2, mB, mBlo, mR, mC, p);
 }
 
 }  // namespace
@@ -706,7 +788,7 @@ bool attention_tc(Engine& e, const float* q, int ldq, const float* k, int ldk, i
     p.splits = 1; p.kb_per_split = cdiv(d, TBK);
     p.tn_w = TBN;
     p.tiles_m = cdiv(Nq, TBM); p.tiles_n = cdiv(Nk, TBN); p.total_tiles = p.tiles_m * p.tiles_n * B * heads;
-    launch_gemm<KIND_SS, 128>(p, mA, mA, mB, mB, s);
+    launch_gemm<KIND_SS, 128>(p, mA, mA, mB, mB, mA, mA, s);
     CDX_CUDA(cudaGetLastError());
     e.launches++;
   }
@@ -733,7 +815,7 @@ bool attention_tc(Engine& e, const float* q, int ldq, const float* k, int ldk, i
     p.splits = 1; p.kb_per_split = cdiv(Nk, TBK);
     p.tn_w = TBN;
     p.tiles_m = cdiv(Nq, TBM); p.tiles_n = cdiv(d, TBN); p.total_tiles = p.tiles_m * p.tiles_n * B * heads;
-    launch_gemm<KIND_SS, 128>(p, mA, mA, mB, mB, s);
+    launch_gemm<KIND_SS, 128>(p, mA, mA, mB, mB, mA, mA, s);
     CDX_CUDA(cudaGetLastError());
     e.launches++;
   }
@@ -930,18 +1012,36 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
     mB = &get_map(ts ? a.Bw_hi : a.Bw, 2, d, st, bx);
     mBlo = ts ? &get_map(a.Bw_lo, 2, d, st, bx) : mB;
   }
+  // staged epilogue: C (GEGLU: its N / 2 output columns) and the residual as 32-column boxes of the tile's 128 rows -- [M] rows, or
+  // for a conv the NHWC output grid in the A box's pixel order {bw, bh, bn}
+  const CUtensorMap *mR = mA, *mC = mA;
+  if (staged_store(p)) {
+    auto out_map = [&](const float* ptr, int cols, int ld) -> const CUtensorMap& {
+      if (a.mode == 0) {
+        uint64_t d[2] = {(uint64_t)cols, (uint64_t)a.M}, st[1] = {(uint64_t)ld * 4};
+        uint32_t bx[2] = {TBK, TBM};
+        return get_map(ptr, 2, d, st, bx);
+      }
+      uint64_t d[4] = {(uint64_t)cols, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.B};
+      uint64_t st[3] = {(uint64_t)ld * 4, (uint64_t)ld * 4 * p.W, (uint64_t)ld * 4 * p.W * p.H};
+      uint32_t bx[4] = {TBK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
+      return get_map(ptr, 4, d, st, bx);
+    };
+    mC = &out_map(a.Cout, a.geglu ? a.N / 2 : a.N, a.ldc);
+    if (a.residual) mR = &out_map(a.residual, a.N, a.ldr);
+  }
   ensure_attr(e.device);
   ProfScope ps(e, s, a.mode == 1 ? PROF_CONV_TC : PROF_DENSE_TC, 2.0 * a.M * a.N * a.K,
                4.0 * ((double)a.M * a.K / (a.mode == 1 ? 9 : 1) + (double)a.N * a.K + (double)a.M * a.N), 1);
   ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s box%dx%dx%d", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
           a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "", p.bw, p.bh, p.bn);
-  if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, s);
-  else if (fast) launch_gemm<KIND_H16_FAST, 64>(p, *mA, *mA2, *mB, *mBlo, s);
-  else if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, s);
-  else if (h16) launch_gemm<KIND_H16, 64>(p, *mA, *mA2, *mB, *mBlo, s);
-  else if (ts && p.tn_w == 128) launch_gemm<KIND_TS, 128>(p, *mA, *mA2, *mB, *mBlo, s);
-  else if (ts) launch_gemm<KIND_TS, 64>(p, *mA, *mA2, *mB, *mBlo, s);
-  else launch_gemm<KIND_SS, 128>(p, *mA, *mA2, *mB, *mBlo, s);
+  if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (fast) launch_gemm<KIND_H16_FAST, 64>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (h16) launch_gemm<KIND_H16, 64>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (ts && p.tn_w == 128) launch_gemm<KIND_TS, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (ts) launch_gemm<KIND_TS, 64>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else launch_gemm<KIND_SS, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
   if (p.splits > 1) {

@@ -64,7 +64,14 @@ __device__ __forceinline__ void tma_store_2d(uint32_t src, const CUtensorMap* ma
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src), "r"(c0), "r"(c1)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_4d(uint32_t src, const CUtensorMap* map, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map), "r"(src), "r"(c0), "r"(c1),
+               "r"(c2), "r"(c3)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all bulk stores of this thread have completed: their writes are performed in global memory
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // all bulk stores of this thread have finished READING their shared-memory source (it may be overwritten)
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }   // all but the newest

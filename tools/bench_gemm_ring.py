@@ -7,6 +7,9 @@ For each checkout (--root, imported in a fresh process per run; the runs alterna
   * every Linear / 1x1 shape and every conv3x3 shape of the SD v1-4 U-Net (the tools/bench_ops.py lists) at batch 12 -- the
     encode chain plus the two CFG rows of each of the four decode chains in lock-step: kernel time from the in-engine CUDA-event
     profiler (dense_tc / conv3x3_tc family), ms per call and TFLOP/s (2 M N K);
+  * the same shapes through Engine.op_gemm with the epilogue terms the U-Net fuses ('gemm' rows): bias and range slot, plus GroupNorm
+    statistics on the convs ('-stats': without them), '+res' a residual on the 320 / 640 / 1280-wide outputs, 'geglu' on the FF1
+    shapes -- the with / without difference is the epilogue's share of the kernel time;
   * one 12-row SD v1-4 U-Net call at 512x512 (synthetic weights): ms per call unprofiled, and the per-family profile in modes 1 and 5.
 Printed: the card, its power limit and max SM clock; median and min-max over the runs; max |delta| between the two checkouts'
 outputs on identical inputs (first run of each arm).
@@ -59,6 +62,48 @@ def weights(specs, cfg, cache):
     return sd
 
 
+def epilogue_arms(eng, x, w, b, M, N, conv, rows_per_img, g):
+    """Engine.op_gemm calls carrying the epilogue terms the U-Net fuses: label suffix -> (call, output).  Every arm has the bias and
+    the range slot; convs add the GroupNorm statistics (every U-Net conv3x3 tracks them), '+res' a residual at ldr = N, and the FF1
+    shapes (N = 8 * K) the GEGLU epilogue."""
+    import torch
+    K = w[0].numel() if conv else w.shape[1]
+    f = dict(M=M, N=N, K=K, A=x, C1=x.shape[-1], lda=x.shape[-1], w=w, bias=b, ldc=N, rows_per_batch=rows_per_img)
+    if conv:
+        h = x.shape[1]
+        f.update(mode=1, Hin=h, Win=h, Hout=h, Wout=h)
+    else:
+        f.update(mode=0, ldb=K)
+    res = torch.randn(M, N, device='cuda', generator=g)
+    amax = torch.zeros(1, device='cuda')
+    stats = torch.zeros(M // rows_per_img, N, 2, dtype=torch.float64, device='cuda')
+    arms = {}
+
+    def arm(name, out, **extra):
+        def call():
+            amax.zero_()
+            if 'c_stats' in extra:
+                stats.zero_()
+            eng.op_gemm(**f, C=out, c_amax=amax, **extra)
+        arms[name] = (call, out)
+
+    side = dict(c_stats=stats) if conv else {}
+    arm('', torch.empty(M, N, device='cuda'), **side)
+    if N in (320, 640, 1280):
+        arm(' +res', torch.empty(M, N, device='cuda'), residual=res, ldr=N, **side)
+    if conv:
+        arm(' -stats', torch.empty(M, N, device='cuda'))
+    if not conv and N == 8 * K:
+        f2 = dict(f, ldc=N // 2)
+        out = torch.empty(M, N // 2, device='cuda')
+
+        def geglu():
+            amax.zero_()
+            eng.op_gemm(**f2, C=out, c_amax=amax, geglu=1)
+        arms[' geglu'] = (geglu, out)
+    return arms
+
+
 def op_time(eng, fn, family, reps):
     """Kernel time of one call (ms) from the engine's CUDA-event profiler; the first call warms up the shape."""
     fn()
@@ -87,6 +132,11 @@ def worker(root, out, reps, cache, save):
         if save:
             tensors[label] = eng.op_conv3x3(x, w, b).cpu()
         res[label] = op_time(eng, lambda: eng.op_conv3x3(x, w, b), 'conv3x3_tc', reps)
+        for suffix, (fn, y) in epilogue_arms(eng, x, w, b, ROWS * h * h, cout, True, h * h, g).items():
+            res[label + ' gemm' + suffix] = op_time(eng, fn, 'conv3x3_tc', reps)
+            if save:
+                fn()
+                tensors[label + ' gemm' + suffix] = y.cpu()
         del x, w, b
     for m, k, n in LINEARS:
         g = torch.Generator(device='cuda').manual_seed(m * 7 + k + n)
@@ -97,6 +147,11 @@ def worker(root, out, reps, cache, save):
         if save:
             tensors[label] = eng.op_linear(x, w, b).cpu()
         res[label] = op_time(eng, lambda: eng.op_linear(x, w, b), 'dense_tc', reps)
+        for suffix, (fn, y) in epilogue_arms(eng, x, w, b, m * ROWS, n, False, m, g).items():
+            res[label + ' gemm' + suffix] = op_time(eng, fn, 'dense_tc', reps)
+            if save:
+                fn()
+                tensors[label + ' gemm' + suffix] = y.cpu()
         del x, w, b
     torch.cuda.empty_cache()
     cfg = specs.sd_unet_config(768)
@@ -163,24 +218,23 @@ def main():
     print(f'{args.runs} runs per arm, alternating; median (min-max) ms per call, kernel time (profiler) for the single ops\n')
     flops = {conv_label(ci, co, h): 2.0 * ROWS * h * h * co * 9 * ci for ci, co, h in CONVS}
     flops.update({lin_label(m, k, n): 2.0 * ROWS * m * k * n for m, k, n in LINEARS})
-    labels = [conv_label(*c) for c in CONVS] + [lin_label(*l) for l in LINEARS]
-    labels += [k for k in runs[roots[0]][0] if k.startswith('U-Net') or (k.startswith('  mode') and not k.endswith('flops'))]
+    labels = [k for k in runs[roots[0]][0] if k != 'card' and not k.endswith('flops')]
     hdr = ''.join(f'{"arm " + str(j):>36s}' for j in range(len(roots)))
-    print(f'{"shape":36s}{hdr}   {"arm1/arm0":>9s}  max|delta|')
+    print(f'{"shape":48s}{hdr}   {"arm1/arm0":>9s}  max|delta|')
     for label in labels:
         cells, meds = '', []
         for r in roots:
             v = [x.get(label, float('nan')) for x in runs[r]]
             med = statistics.median(v)
             meds.append(med)
-            fl = flops.get(label) or runs[r][0].get(label + ' flops', 0.0)
+            fl = flops.get(label.split(' gemm')[0]) or runs[r][0].get(label + ' flops', 0.0)
             tf = f' {fl / (med * 1e-3) / 1e12:5.1f} TF/s' if fl else ' ' * 11
             cells += f'{med:9.3f} ({min(v):.3f}-{max(v):.3f}){tf}'
         ratio = f'{meds[1] / meds[0]:9.3f}' if len(meds) > 1 else ''
         dl = ''
         if len(outs) > 1 and label in outs[0]:
             dl = f'{float((outs[0][label].double() - outs[1][label].double()).abs().max()):.2e}'
-        print(f'{label:36s}{cells}   {ratio}  {dl}')
+        print(f'{label:48s}{cells}   {ratio}  {dl}')
     shutil.rmtree(tmp, ignore_errors=True)
 
 

@@ -133,6 +133,8 @@ SIGNATURES = {
                                     _I, _P, _P, C.POINTER(AttnControl)]),
     'cdx_cycle_lockstep_refine': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
                                        _I, _I, _P, _P, C.POINTER(AttnControl), _P]),
+    'cdx_cycle_lockstep_mutual': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
+                                       _I, _I, _P, _P, _I, _I]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),
@@ -160,6 +162,7 @@ SIGNATURES = {
     'cdx_op_layernorm': (_I, [_P, _P, _P, _P, _P, _I, _I, _P]),
     'cdx_op_attention': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
     'cdx_op_attention_rows': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, C.POINTER(_I), _P]),
+    'cdx_op_attention_kv_rows': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, C.POINTER(_I), _P]),
     'cdx_op_attention_accum': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, C.POINTER(_I), _I, _P]),
     'cdx_op_nchw_to_nhwc': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_nhwc_to_nchw': (_I, [_P, _P, _P, _I, _I, _I, _P]),

@@ -6,6 +6,10 @@ The "refine" edit aligns the two prompts instead: a target token matched to a so
 a target token with no match keeps the row's own map (``own_weight``).  The engine does both inside the fused attention kernel
 (include/cdx.h, cdx_cycle_lockstep_ctl and cdx_cycle_lockstep_refine); this module holds the value the Python surfaces take and
 the host helpers that build token maps from two prompts' token ids.
+
+MasaCtrl's mutual self-attention (Cao et al., 2023; ``MutualSelfControl``) is the complementary control for non-rigid edits: in
+the decoder's self-attention layers the target rows keep their own queries and attend over the source row's keys and values
+(cdx_cycle_lockstep_mutual), so the layout follows the target prompt and the content comes from the real image.
 """
 from dataclasses import dataclass
 
@@ -83,6 +87,23 @@ class AttentionControl:
         w = self.device_weight(B, L, device)
         cross, self_ = self.steps(n)
         return _cabi.AttnControl(cross, self_, self.self_max_tokens, A.data_ptr() if A is not None else None), A, w
+
+
+@dataclass(frozen=True)
+class MutualSelfControl:
+    """MasaCtrl's mutual self-attention control: at loop steps i >= start_step (0-based, of the steps that run after strength's
+    skip), in every SpatialTransformer whose index in forward order (input blocks, middle block, output blocks; 16 in SD v1 / 2.x)
+    is >= start_layer, the target chain's rows attend with their own queries over the source chain's keys and values -- the cond
+    row over the source's cond row, the uncond row over the source's uncond row (its cond row when the source has none).  The
+    defaults are MasaCtrl's: the last six layers (the decoder's two finest levels) from step 4 on."""
+    start_step: int = 4
+    start_layer: int = 10
+
+    def __post_init__(self):
+        for name in ('start_step', 'start_layer'):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+                raise ValueError(f'{name} must be an integer >= 0, got {v!r}')
 
 
 def replace_token_map(src_ids, tgt_ids, L):

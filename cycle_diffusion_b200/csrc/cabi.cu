@@ -172,6 +172,8 @@ struct ChainLoopArgs {
   const float* mask = nullptr;                      // optional [n_src, 1, h, w]: masked editing (LatentChains::mask)
   const cdx_attn_control* ctl = nullptr;           // optional: attention control of each target chain's cond row (cdx.h)
   const float* own_weight = nullptr;                // optional with ctl: [n_src, L], refine's weights of the rows' own attention
+  // optional, exclusive with ctl: mutual self-attention (cdx.h, cdx_cycle_lockstep_mutual) at steps >= start_step, layers >= start_layer
+  bool mutual = false; int start_step = 0, start_layer = 0;
   int C = 0, h = 0, w = 0;
 };
 
@@ -235,6 +237,14 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
               c.self_max_tokens);
   }
   CDX_CHECK(!a.own_weight || a.ctl, "refine: own_weight needs an attention control");
+  if (a.mutual) {
+    CDX_CHECK(!a.ctl, "mutual self-attention and Prompt-to-Prompt control are exclusive in one loop");
+    CDX_CHECK(a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net && !a.scales_on_device,
+              "mutual self-attention: needs the lock-step loop with a source chain at every step");
+    CDX_CHECK(unet.kind == NET_UNET_OPENAI && ctx_n > 0 && a.c_src && a.c_tgt, "mutual self-attention: needs a U-Net with SpatialTransformers");
+    CDX_CHECK(e.mma_mode == 1 && e.flash_attn, "mutual self-attention: needs the fused attention kernel (mma modes 1, 3, 4 or 5)");
+    CDX_CHECK(a.start_step >= 0 && a.start_layer >= 0, "mutual self-attention: start_step=%d start_layer=%d", a.start_step, a.start_layer);
+  }
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
   struct Invalidate { Net& u; ~Invalidate() { u.ctxkv.valid = false; } } inval{unet};
@@ -329,6 +339,22 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.n_own = (int)own.size();
     }
   }
+  // mutual self-attention: each target chain's cond row reads its group's source cond row's K and V, its uncond row the source's
+  // uncond row (the cond row when the source runs without one); every other row its own.  Fixed for the loop
+  if (a.mutual) {
+    std::vector<int> kv(rows);
+    for (int r = 0; r < rows; ++r) kv[r] = r;
+    for (int j = 0; j < a.n_src; ++j)
+      for (int k = 0; k < a.K; ++k) {
+        const Chain& t = ch[a.n_src + (size_t)j * a.K + k];
+        kv[t.row] = ch[j].row;
+        if (t.row2 >= 0) kv[t.row2] = ch[j].row2 >= 0 ? ch[j].row2 : ch[j].row;
+      }
+    int* kv_dev = (int*)e.arena.alloc((size_t)rows * sizeof(int));
+    if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(kv_dev, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+    actl.kv_row = kv_dev;
+    actl.start_layer = a.start_layer;
+  }
   auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
     if (i_next >= a.n_rec) return 0;
     return (a.n_steps - 1 - i_next) == 0 ? 2 : 1;                               // ddim.py:583-584
@@ -355,7 +381,8 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     if (!tgt_net) {
       actl.cross = a.ctl && i < a.ctl->cross_steps;
       actl.self = a.ctl && i < a.ctl->self_steps;
-      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true, a.ctl ? &actl : nullptr);
+      actl.mutual = a.mutual && i >= a.start_step;
+      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true, a.ctl || a.mutual ? &actl : nullptr);
     } else {
       ps.fork();
       if (src_i) unet_forward(unet, xin, tdev + (size_t)i * rows, nullptr, 0, eout, rows_src, a.h, a.w, s);
@@ -770,10 +797,11 @@ int cdx_cycle_lockstep_ctl(cdx_net* un, const float* x0, const float* c_src, con
                                    x_out, z_out, B, C, h, w, stream, mask, ctl, nullptr);
 }
 
-int cdx_cycle_lockstep_refine(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
-                              float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
-                              float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
-                              const float* mask, const cdx_attn_control* ctl, const float* own_weight) {
+// the single-image lock-step cycle under the controls of ChainLoopArgs (ctl, own_weight; mutual with start_step >= 0)
+static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                          float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                          float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream, const float* mask,
+                          const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -784,8 +812,25 @@ int cdx_cycle_lockstep_refine(cdx_net* un, const float* x0, const float* c_src, 
     a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scales = s_scales.data(); a.t_scales = t_scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
     a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
+    a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
+}
+
+int cdx_cycle_lockstep_refine(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                              float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                              float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                              const float* mask, const cdx_attn_control* ctl, const float* own_weight) {
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, ctl, own_weight, false, 0, 0);
+}
+
+int cdx_cycle_lockstep_mutual(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                              float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                              float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                              const float* mask, int start_step, int start_layer) {
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, nullptr, nullptr, true, start_step, start_layer);
 }
 
 int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
@@ -1071,13 +1116,15 @@ int cdx_op_groupnorm(cdx_engine* eh, const float* x, const float* gamma, const f
 int cdx_op_layernorm(cdx_engine* eh, const float* x, const float* gamma, const float* beta, float* y, int M, int C, void* stream) {
   ENG_CALL(eh, layernorm(eh->e, x, gamma, beta, y, M, C, S(stream)));
 }
-// cdx_op_attention with the fused kernel's options: a Q / K row table (qk_rows, host [B]) or the accumulating launch over a row
-// list (acc_rows, host [n_acc]); either one needs the fused kernel
+// cdx_op_attention with the fused kernel's options: a Q / K row table (qk_rows, host [B]), a K / V row table (kv_rows, host [B]) or
+// the accumulating launch over a row list (acc_rows, host [n_acc]); each needs the fused kernel
 static int op_attention(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
-                        float scale, const int* qk_rows, const int* acc_rows, int n_acc, void* stream) {
+                        float scale, const int* qk_rows, const int* acc_rows, int n_acc, void* stream, const int* kv_rows = nullptr) {
   return guard([&] {
     CDX_CHECK(eh && q && k && v && out, "op_attention: null argument");
+    CDX_CHECK(!qk_rows || !kv_rows, "op_attention: qk_rows and kv_rows in one launch");
     if (qk_rows) for (int b = 0; b < B; ++b) CDX_CHECK(qk_rows[b] >= 0 && qk_rows[b] < B, "op_attention: qk_rows[%d] = %d outside [0, %d)", b, qk_rows[b], B);
+    if (kv_rows) for (int b = 0; b < B; ++b) CDX_CHECK(kv_rows[b] >= 0 && kv_rows[b] < B, "op_attention: kv_rows[%d] = %d outside [0, %d)", b, kv_rows[b], B);
     if (acc_rows) for (int r = 0; r < n_acc; ++r) CDX_CHECK(acc_rows[r] >= 0 && acc_rows[r] < B, "op_attention: acc_rows[%d] = %d outside [0, %d)", r, acc_rows[r], B);
     const int C = heads * d;
     Engine& e = eh->e;
@@ -1086,11 +1133,12 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
       Scope sc(e.arena);
       bool done = false;
       const bool fused = flash_eligible(e, Nq, Nk, d, C);
-      CDX_CHECK((!qk_rows && !acc_rows) || fused, "op_attention: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, d);
-      int* rows_dev = nullptr;
-      if (qk_rows) {
-        rows_dev = (int*)e.arena.alloc((size_t)B * sizeof(int));
-        if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(rows_dev, qk_rows, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+      CDX_CHECK((!qk_rows && !kv_rows && !acc_rows) || fused, "op_attention: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, d);
+      int *rows_dev = nullptr, *kv_dev = nullptr;
+      if (qk_rows || kv_rows) {
+        int*& dev = qk_rows ? rows_dev : kv_dev;
+        dev = (int*)e.arena.alloc((size_t)B * sizeof(int));
+        if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(dev, qk_rows ? qk_rows : kv_rows, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
       }
       int* acc_dev = nullptr;
       if (acc_rows) {
@@ -1128,7 +1176,7 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
         split_rows_h16(e, kp, Mk, C, C, kh, kl, C, ka, s);
         split_transpose_h16(e, vp, Mk, C, C, vh, vl, va, s);
         const AttnPlanes pl{AttnPlanes::H16, qh, ql, C, kh, kl, C, vh, vl, qa, ka, va};
-        done = flash_attention(e, pl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc);
+        done = flash_attention(e, pl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc, kv_dev);
       }
       if (!done && e.mma_mode == 1 && Nq == Nk && (Nq % 32) == 0 && Nq >= 128 && (d % 4) == 0) {
         // same operand preparation as the SpatialTransformer: q|k side by side, V transposed, TF32 planes
@@ -1148,9 +1196,9 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
           split_planes(e, qk, qh, ql, (size_t)M * 2 * C, s);
           split_planes(e, vt, vh, vl, (size_t)C * M, s);
           const AttnPlanes pl{AttnPlanes::TF32, qh, ql, 2 * C, qh + C, ql + C, 2 * C, vh, vl};
-          done = flash_attention(e, pl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev, acc_dev, n_acc);
+          done = flash_attention(e, pl, out, C, B, Nq, Nq, Nq, Nq, heads, d, scale, s, rows_dev, acc_dev, n_acc, kv_dev);
         }
-        CDX_CHECK(done || (!rows_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
+        CDX_CHECK(done || (!rows_dev && !kv_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
         if (!done) done = attention_tc(e, qk, 2 * C, qk + C, 2 * C, d, vt, out, C, B, Nq, Nk, heads, d, scale, s);
       }
       if (!done && fused) {
@@ -1176,9 +1224,9 @@ static int op_attention(cdx_engine* eh, const float* q, const float* k, const fl
         split_planes(e, kp, kh, kl, (size_t)Mk * C, s);
         split_planes(e, vt, vh, vl, (size_t)C * Mk, s);
         const AttnPlanes pl{AttnPlanes::TF32, qh, ql, C, kh, kl, C, vh, vl};
-        done = flash_attention(e, pl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc);
+        done = flash_attention(e, pl, out, C, B, Nq, Nk, Nks, Nks, heads, d, scale, s, rows_dev, acc_dev, n_acc, kv_dev);
       }
-      CDX_CHECK(done || (!rows_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
+      CDX_CHECK(done || (!rows_dev && !kv_dev && !acc_dev), "op_attention: the fused kernel rejected a row-table shape");
       if (!done) attention(e, q, C, k, C, v, C, out, C, B, Nq, Nk, heads, d, d, scale, s);
     });
   });
@@ -1190,6 +1238,10 @@ int cdx_op_attention(cdx_engine* eh, const float* q, const float* k, const float
 int cdx_op_attention_rows(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
                           float scale, const int* qk_rows, void* stream) {
   return op_attention(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, qk_rows, nullptr, 0, stream);
+}
+int cdx_op_attention_kv_rows(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
+                             float scale, const int* kv_rows, void* stream) {
+  return op_attention(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, nullptr, 0, stream, kv_rows);
 }
 int cdx_op_attention_accum(cdx_engine* eh, const float* q, const float* k, const float* v, float* out, int B, int Nq, int Nk, int heads, int d,
                            float scale, const int* acc_rows, int n_acc, void* stream) {

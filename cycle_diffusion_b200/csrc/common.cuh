@@ -201,8 +201,10 @@ struct AttnPlanes {
 // are image qk_row[b]'s (attention control).  Null: every image its own.
 // acc_rows (optional device [n_acc]): the accumulating launch, out[r] += attention of image r for the listed images only (CTAs for
 // those alone); ordered after the stream's previous launch, whose out it reads after the dependent-launch wait.
+// kv_row (optional device [B]): image b takes its K and V from image kv_row[b] and keeps its own Q and output -- its queries attend
+// over image kv_row[b]'s keys and values (mutual self-attention).  Giving both qk_row and kv_row is an error.
 bool flash_attention(Engine& e, const AttnPlanes& a, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d, float scale,
-                     cudaStream_t s, const int* qk_row = nullptr, const int* acc_rows = nullptr, int n_acc = 0);
+                     cudaStream_t s, const int* qk_row = nullptr, const int* acc_rows = nullptr, int n_acc = 0, const int* kv_row = nullptr);
 void split_rows_h16(Engine& e, const float* src, long long rows, int cols, long long ld, void* hi, void* lo, long long ldh, const float* amax,
                     cudaStream_t s);
 // R rows = `images` images of R / images rows each; Rp > 0: each image's columns padded with zeros to a stride of Rp (V^T key stride)

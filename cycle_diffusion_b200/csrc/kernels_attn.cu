@@ -24,6 +24,9 @@
 // O_j, S and the P fragments fit the 232-register budget; see ACfg.
 // Accumulating launch (AttnParams::acc_rows): CTAs only for the listed images, and the epilogue adds O / l into out instead of
 // storing it -- a second attention term on a few rows (Prompt-to-Prompt's refine) with every variant above as it is.
+// Row tables (AttnParams::qk_row, kv_row): the producer loads image b's Q and K tiles from image qk_row[b] (Prompt-to-Prompt: the
+// source row's probabilities), or its K and V^T tiles from image kv_row[b] (MasaCtrl: the row's own queries over the source row's
+// keys and values) -- a change of TMA coordinates only.
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -92,6 +95,9 @@ struct AttnParams {
   // optional [B]: image qk_row[b] supplies the Q and K tiles of image b (attention control: a target row attends with its source
   // row's probabilities); V^T and the output stay image b's.  Null: every image its own
   const int* qk_row;
+  // optional [B]: image kv_row[b] supplies the K and V^T tiles of image b (mutual self-attention: a target row's own queries
+  // attend over its source row's keys and values); Q and the output stay image b's.  Exclusive with qk_row.  Null: every image its own
+  const int* kv_row;
   // optional [gridDim.z]: the accumulating launch.  CTA z serves image acc_rows[z] and adds its result into out (out += O / l)
   // instead of storing it; images not listed get no CTA and are not touched (refine's second term over the controlled rows)
   const int* acc_rows;
@@ -150,12 +156,15 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
     // =========================================================================== TMA producer
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
-      const int bqk = p.qk_row ? __ldcg(p.qk_row + b) : b;    // (coherent: read after the dependent-launch wait)
+      // the images Q, K and V^T come from (coherent reads after the dependent-launch wait; qk_row and kv_row are exclusive)
+      const int bq = p.qk_row ? __ldcg(p.qk_row + b) : b;
+      const int bv = p.kv_row ? __ldcg(p.kv_row + b) : b;
+      const int bk = p.qk_row ? bq : bv;
       const uint32_t sq = base + C::OFF_Q;
       mbar_expect_tx(bar_q_full, C::NPL * C::Q_PLANE);
       for (int kb = 0; kb < KB2; ++kb) {
-        tma_load_4d(sq + kb * QR * 128, &mapQh, kb * KW, h, q0, bqk, bar_q_full);
-        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * QR * 128, &mapQl, kb * KW, h, q0, bqk, bar_q_full);
+        tma_load_4d(sq + kb * QR * 128, &mapQh, kb * KW, h, q0, bq, bar_q_full);
+        if (!ONE) tma_load_4d(sq + C::Q_PLANE + kb * QR * 128, &mapQl, kb * KW, h, q0, bq, bar_q_full);
       }
       for (int j = 0; j < nb; ++j) {
         // K block j: [64 keys x d] hi + lo
@@ -164,8 +173,8 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
         const uint32_t sk = base + C::OFF_K + s * C::K_STAGE;
         mbar_expect_tx(bar_k_full(s), C::K_STAGE);
         for (int kb = 0; kb < KB2; ++kb) {
-          tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, bqk, bar_k_full(s));
-          if (!ONE) tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, bqk, bar_k_full(s));
+          tma_load_4d(sk + kb * C::KTILE, &mapKh, kb * KW, h, j * AKV, bk, bar_k_full(s));
+          if (!ONE) tma_load_4d(sk + (KB2 + kb) * C::KTILE, &mapKl, kb * KW, h, j * AKV, bk, bar_k_full(s));
         }
         // V^T block j: [NV channel rows x 64 keys] (TF32: two 32-key tiles), hi + lo
         const int sv_ = j % VS;
@@ -173,12 +182,12 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
         const uint32_t sv = base + C::OFF_V + sv_ * C::V_STAGE;
         mbar_expect_tx(bar_v_full(sv_), C::V_STAGE);
         if (F16) {
-          tma_load_4d(sv, &mapVh, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
-          if (!ONE) tma_load_4d(sv + C::VTILE, &mapVl, j * AKV, b, h * p.d, 0, bar_v_full(sv_));
+          tma_load_4d(sv, &mapVh, j * AKV, bv, h * p.d, 0, bar_v_full(sv_));
+          if (!ONE) tma_load_4d(sv + C::VTILE, &mapVl, j * AKV, bv, h * p.d, 0, bar_v_full(sv_));
         } else {
           for (int kk = 0; kk < 2; ++kk) {
-            tma_load_4d(sv + kk * C::VTILE, &mapVh, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
-            tma_load_4d(sv + (2 + kk) * C::VTILE, &mapVl, j * AKV + kk * 32, b, h * p.d, 0, bar_v_full(sv_));
+            tma_load_4d(sv + kk * C::VTILE, &mapVh, j * AKV + kk * 32, bv, h * p.d, 0, bar_v_full(sv_));
+            tma_load_4d(sv + (2 + kk) * C::VTILE, &mapVl, j * AKV + kk * 32, bv, h * p.d, 0, bar_v_full(sv_));
           }
         }
       }
@@ -561,7 +570,8 @@ bool flash_eligible(const Engine& e, int N, int Nk, int d, int C) {
 }
 
 bool flash_attention(Engine& e, const AttnPlanes& a, float* out, int ldo, int B, int N, int Nk, int Nks, int Nvs, int heads, int d, float scale,
-                     cudaStream_t s, const int* qk_row, const int* acc_rows, int n_acc) {
+                     cudaStream_t s, const int* qk_row, const int* acc_rows, int n_acc, const int* kv_row) {
+  CDX_CHECK(!qk_row || !kv_row, "flash_attention: a Q / K row table and a K / V row table in one launch");
   const bool h16 = a.fmt == AttnPlanes::H16;
   const int gm = h16 ? 7 : 3;            // strides in whole 16-byte granules (TMA)
   if (N < 1 || (a.ldq & gm) || (a.ldk & gm) || (ldo & 3) || (Nvs & gm) || Nk < 1 || Nk > Nks || Nk > Nvs) return false;
@@ -597,6 +607,7 @@ bool flash_attention(Engine& e, const AttnPlanes& a, float* out, int ldo, int B,
   p.out = out; p.ldo = ldo;
   p.q_amax = a.q_amax; p.k_amax = a.k_amax; p.v_amax = a.v_amax;
   p.qk_row = qk_row;
+  p.kv_row = kv_row;
   p.acc_rows = acc_rows;
   const double bytes = h16 ? (one ? 1.0 : 2.0) * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 8.0 : 4.0) * p.B * heads * (double)N * d
                            : 4.0 * p.B * heads * (2.0 * N * d + 2.0 * (double)Nk * d) + (acc_rows ? 4.0 * p.B * (double)N * d * heads : 0.0);

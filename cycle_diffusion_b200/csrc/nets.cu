@@ -693,6 +693,7 @@ struct UNetExec : Exec {
   int ctx_lp = 0;                          // context rows per image, padded for the fused cross-attention
   bool kv_reuse = false, kv_hit = false;   // loop mode: context K / V live in n.ctxkv (kv_hit: already computed)
   const AttnControl* ctl = nullptr;        // attention control of this call, or null
+  int st_layer = 0;                        // SpatialTransformers run so far in this call (AttnControl::start_layer counts them)
   // the contexts the cross-attention projects: [0] the call's context, [1] the V' context (AttnControl::ctx_v), [2] the refine
   // context (ctx_w); src null when absent.  pad: src zero-padded to ctx_lp rows per image (fused route only); amax: range slot of
   // src (A operand of the K / V projections)
@@ -808,8 +809,11 @@ struct UNetExec : Exec {
       bool done = false;
       const bool flash_ok = flash_eligible(e, HW, HW, d, C);
       const int* srow = (ctl && ctl->self && HW <= ctl->self_max_tokens) ? ctl->qk_row : nullptr;
-      CDX_CHECK(!srow || flash_ok, "attention control: self-attention at HW=%d d=%d would take the unfused route (mma mode and head width "
-                "must run the fused kernel)", HW, d);
+      // mutual self-attention: the controlled rows' queries over their source rows' keys and values
+      const int* mrow = (ctl && ctl->mutual && st_layer >= ctl->start_layer) ? ctl->kv_row : nullptr;
+      ++st_layer;
+      CDX_CHECK((!srow && !mrow) || flash_ok, "attention control: self-attention at HW=%d d=%d would take the unfused route (mma mode and "
+                "head width must run the fused kernel)", HW, d);
       if (flash_ok && e.tc_kind >= 1) {
         // fp16-split fused attention: ONE plain fp32 q|k|v projection (its range tracked by the epilogue), then one pass that
         // writes the fp16 hi / lo planes of q|k and of V^T (both P.V operands K-major for wgmma) with the tensor's exponent.
@@ -829,7 +833,7 @@ struct UNetExec : Exec {
         split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s, B, Nvs);
         const AttnPlanes pl{AttnPlanes::H16, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr,
                             2 * C, vt_hi, vt_lo, a.amax, a.amax, a.amax};
-        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow);
+        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow, nullptr, 0, mrow);
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok && (HW % 4) != 0) {
         // TF32 planes with a per-image key count off the 16-byte TMA granule: V row-major, copied into rows padded to Nvs keys
@@ -853,7 +857,7 @@ struct UNetExec : Exec {
         nhwc_to_nchw(e, vp, vt, 1, C, B * Nvs, s);
         split_planes(e, vt, vt_hi, vt_lo, nvt, s);
         const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
-        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow);
+        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow, nullptr, 0, mrow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands
@@ -883,7 +887,7 @@ struct UNetExec : Exec {
                       a.amax);   // V^T = Wv . X^T
         }
         const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
-        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s, srow);
+        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, HW, heads, d, scale, s, srow, nullptr, 0, mrow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (e.mma_mode >= 1 && (HW % 32) == 0 && HW >= 128 && (d % 4) == 0) {
         // unfused tensor-core attention (mode 2, or shapes the fused kernel does not cover)
@@ -1309,8 +1313,9 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
   CDX_CHECK(H % down == 0 && W % down == 0, "unet_forward: %dx%d not divisible by %d", H, W, down);
   UNetExec ex(n, s);
   ex.kv_reuse = reuse_ctx && n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0;
-  CDX_CHECK(!ctl || !ctl->qk_row || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0),
+  CDX_CHECK(!ctl || (!ctl->qk_row && !ctl->kv_row) || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0),
             "attention control: SD / LDM U-Nets with a context only");
+  CDX_CHECK(!ctl || !ctl->qk_row || !ctl->kv_row, "attention control: Prompt-to-Prompt and mutual self-attention in one call");
   ex.ctl = ctl;
   if (n.kind == NET_UNET_DDPM) { ex.forward_ddpm(x_nchw, t_dev, out_nchw, B, H, W); return; }
   ex.forward(x_nchw, t_dev, ctx, ctx_len, out_nchw, B, H, W);

@@ -100,14 +100,18 @@ struct AttnControl {
   const float* ctx_w = nullptr;
   const int* own_rows = nullptr;
   int n_own = 0;
+  // mutual self-attention (MasaCtrl; exclusive with qk_row): with `mutual`, the self-attention of every SpatialTransformer whose
+  // index in forward order (input blocks, middle block, output blocks) is >= start_layer takes row r's K and V from row kv_row[r]
+  const int* kv_row = nullptr;          // device [B]
+  bool mutual = false;                  // control the self-attention layers >= start_layer in this call
+  int start_layer = 0;
 };
 
 // forward executors (enqueue only; caller handles arena dry-run)
 // reuse_ctx: the caller guarantees `ctx` is unchanged since the previous call with reuse_ctx (and n.ctxkv was invalidated
 // at the start of the loop) -> context K / V projections are taken from n.ctxkv instead of being recomputed
 void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* ctx, int ctx_len, float* out_nchw, int B, int H,
-                  int W, cudaStream_t s, bool reuse_ctx = false, const AttnControl* ctl = nullptr);
-void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int H, int W, cudaStream_t s);
+                  int W, cudaStream_t s, bool reuse_ctx = false, const AttnControl* ctl = nullptr);void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int H, int W, cudaStream_t s);
 void vae_decode(Net& n, const float* z_nchw, float* img_nchw, int B, int h, int w, cudaStream_t s);
 void text_encode(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);
 void text_features(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);                // CLIP.encode_text   -> [B, proj_dim]

@@ -12,6 +12,7 @@ import torch
 
 from . import _cabi
 from ._cabi import lib, check, UnetConfig, VaeConfig, TextConfig, DdimCoef, PixelCoef
+from .attn_control import MutualSelfControl
 
 
 def _ptr(t):
@@ -442,16 +443,18 @@ class Engine:
         check(lib.cdx_op_pixel_lockstep(self.h, _ptr(x0), _ptr(xs), _ptr(ys), _ptr(et_src), _ptr(et_tgt), _ptr(noise), C.byref(coef), B, chw,
                                         ns, nt, self.stream))
 
-    def op_attention(self, q, k, v, heads, scale, qk_rows=None, accumulate_rows=None, out=None):
+    def op_attention(self, q, k, v, heads, scale, qk_rows=None, accumulate_rows=None, out=None, kv_rows=None):
         """softmax(q k^T * scale) v per head.  qk_rows: optional [B] ints, image b attends with image qk_rows[b]'s q and k and its
-        own v (cdx_op_attention_rows; fused kernel only).  accumulate_rows: optional list of images r, out[r] += the attention of
-        image r, the other images of `out` (a [B, Nq, C] float32 tensor on the device, updated in place and returned) untouched
-        (cdx_op_attention_accum; fused kernel only)."""
+        own v (cdx_op_attention_rows; fused kernel only).  kv_rows: optional [B] ints, image b attends with its own q over image
+        kv_rows[b]'s k and v (cdx_op_attention_kv_rows; fused kernel only; not with qk_rows).  accumulate_rows: optional list of
+        images r, out[r] += the attention of image r, the other images of `out` (a [B, Nq, C] float32 tensor on the device, updated
+        in place and returned) untouched (cdx_op_attention_accum; fused kernel only)."""
         q, k, v = (_f32c(t, self.device) for t in (q, k, v))
         B, Nq, Cc = q.shape
         Nk = k.shape[1]
+        assert qk_rows is None or kv_rows is None, 'qk_rows and kv_rows are exclusive: one row table per launch'
         if accumulate_rows is not None:
-            assert qk_rows is None, 'qk_rows and accumulate_rows are separate launches'
+            assert qk_rows is None and kv_rows is None, 'row tables and accumulate_rows are separate launches'
             assert out is not None and out.shape == q.shape and out.dtype == torch.float32 and out.is_contiguous() and out.device == q.device, \
                 'accumulate_rows: out must be a contiguous float32 tensor shaped like q on the engine device'
             rows = [int(r) for r in accumulate_rows]
@@ -460,13 +463,14 @@ class Engine:
             return out
         assert out is None, 'out is the accumulation target of accumulate_rows'
         out = torch.empty_like(q)
-        if qk_rows is None:
+        table = qk_rows if qk_rows is not None else kv_rows
+        if table is None:
             check(lib.cdx_op_attention(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale, self.stream))
         else:
-            rows = [int(r) for r in qk_rows]
-            assert len(rows) == B, f'qk_rows: {len(rows)} entries for {B} images'
-            check(lib.cdx_op_attention_rows(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale,
-                                            (C.c_int * B)(*rows), self.stream))
+            rows = [int(r) for r in table]
+            assert len(rows) == B, f'{"qk" if qk_rows is not None else "kv"}_rows: {len(rows)} entries for {B} images'
+            fn = lib.cdx_op_attention_rows if qk_rows is not None else lib.cdx_op_attention_kv_rows
+            check(fn(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale, (C.c_int * B)(*rows), self.stream))
         return out
 
     def op_nchw_to_nhwc(self, x):
@@ -740,8 +744,9 @@ class UNet(Net):
         n_rec == sched.refine_steps.  mask [B,1,h,w] in [0,1] (1 = may change): masked editing (cdx_cycle_lockstep_masked), the
         target chain is blended with the source chain's x_{t-1} after every step; ones give the unmasked result, zeros give x0.
         attn_control: an attn_control.AttentionControl, Prompt-to-Prompt's "replace" edit on the target chain's cond row
-        (cdx_cycle_lockstep_ctl), or its "refine" edit when the control has an own_weight (cdx_cycle_lockstep_refine); it
-        composes with mask."""
+        (cdx_cycle_lockstep_ctl), or its "refine" edit when the control has an own_weight (cdx_cycle_lockstep_refine); or an
+        attn_control.MutualSelfControl, MasaCtrl's mutual self-attention on the target chain's rows (cdx_cycle_lockstep_mutual).
+        Each composes with mask."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -750,12 +755,17 @@ class UNet(Net):
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
         mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
-        ctl, _token_map, own = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None else (None, None, None)
+        mutual = isinstance(attn_control, MutualSelfControl)
+        ctl, _token_map, own = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None and not mutual \
+            else (None, None, None)
         out = e.empty(B, Cc, h, w)
         z = e.empty(B, n + 1, Cc, h, w) if return_z else None
         args = (self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale), float(tgt_scale), sched.coef_array(),
-                sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask),
-                C.byref(ctl) if ctl is not None else None)
+                sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask))
+        if mutual:
+            check(lib.cdx_cycle_lockstep_mutual(*args, attn_control.start_step, attn_control.start_layer))
+            return (out, z) if return_z else out
+        args += (C.byref(ctl) if ctl is not None else None,)
         if own is None:
             check(lib.cdx_cycle_lockstep_ctl(*args))
         else:

@@ -14,7 +14,7 @@ from dataclasses import dataclass
 
 import torch
 
-from .attn_control import AttentionControl
+from .attn_control import AttentionControl, MutualSelfControl
 from .engine import check_mask
 from .schedule import DDIMSchedule
 
@@ -95,15 +95,29 @@ class CycleDiffusionPipeline:
         return mask if output_type == 'latent' else mask_img
 
     P2P_KEYS = {'edit_type', 'cross_replace_steps', 'self_replace_steps', 'self_replace_max_tokens', 'token_map', 'equalizer'}
+    MUTUAL_KEYS = {'edit_type', 'start_step', 'start_layer'}
 
     @classmethod
     def _attn_control(cls, kw, source_guidance_scale, two_phase):
-        """cross_attention_kwargs -> AttentionControl or None (no 'edit_type'); ValueError for what the engine cannot do."""
+        """cross_attention_kwargs -> AttentionControl, MutualSelfControl or None (no 'edit_type'); ValueError for what the engine
+        cannot do."""
         if not kw or 'edit_type' not in kw:
             return None
         kind = kw['edit_type']
+        if kind == 'mutual_self':
+            extra = set(kw) - cls.MUTUAL_KEYS
+            if extra:
+                raise ValueError(f"cross_attention_kwargs: keys {sorted(extra)} do not apply to edit_type='mutual_self' (it takes "
+                                 f"start_step and start_layer; Prompt-to-Prompt edits are a separate edit_type)")
+            if two_phase:
+                raise ValueError('mutual self-attention needs the lock-step loop: the source chain does not run during the decode '
+                                 '(two_phase=False)')
+            try:
+                return MutualSelfControl(kw.get('start_step', 4), kw.get('start_layer', 10))
+            except ValueError as err:
+                raise ValueError(f'cross_attention_kwargs: {err}') from None
         if kind not in ('replace', 'reweight', 'refine'):
-            raise ValueError(f"edit_type must be 'replace', 'reweight' or 'refine', got {kind!r}")
+            raise ValueError(f"edit_type must be 'replace', 'reweight', 'refine' or 'mutual_self', got {kind!r}")
         extra = set(kw) - cls.P2P_KEYS
         if extra:
             raise ValueError(f'cross_attention_kwargs: unsupported keys {sorted(extra)} (LocalBlend: use mask_image)')
@@ -163,7 +177,12 @@ class CycleDiffusionPipeline:
         token_map (attn_control.refine_token_map aligns two prompts' token ids) whose column sums lie in [0, 1]: target token j
         takes P_src . A[:, j] and keeps (1 - colsum_j) . eq_j of its own map, so a word the source prompt lacks attends on its own.
         two_phase=True and a source_guidance_scale of 0 raise ValueError; LocalBlend is mask_image's job.  A dict without
-        'edit_type' is ignored."""
+        'edit_type' is ignored.
+        {'edit_type': 'mutual_self', ['start_step': 4], ['start_layer': 10]}: MasaCtrl's mutual self-attention (Cao et al., 2023)
+        instead, for non-rigid edits (a pose or a layout change): from loop step start_step on, in the SpatialTransformers from
+        index start_layer on (16 in SD v1 / 2.x; the defaults control the decoder's two finest levels), the target rows keep their
+        own queries and attend over the source rows' keys and values (attn_control.MutualSelfControl).  Prompt-to-Prompt keys,
+        other keys and two_phase=True raise ValueError; it composes with mask_image."""
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')

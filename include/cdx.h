@@ -349,6 +349,26 @@ int cdx_cycle_lockstep_refine(cdx_net* unet, const float* x0, const float* c_src
                               const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                               float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                               void* stream, const float* mask, const cdx_attn_control* ctl, const float* own_weight);
+/* Mutual self-attention control (MasaCtrl, Cao et al., 2023) on the lock-step loop: cdx_cycle_lockstep_masked (mask may be NULL)
+ * where the target chain's rows keep their own queries but attend over the source chain's keys and values in the decoder's
+ * self-attention layers, so the layout can follow the target prompt while identity, texture and background are fetched from the
+ * real image.  At loop step i (0-based, of n_steps) with i >= start_step, in every SpatialTransformer whose index (counted in
+ * forward order over the input blocks, the middle block and the output blocks; SD v1 / 2.x and LDM text2img have 16) is
+ * >= start_layer, each target row computes softmax(Q_own K_src^T * scale) . V_src, where for sample b
+ *   - the target's cond row (under c_tgt[b]) reads the source chain's cond row (under c_src[b]), and
+ *   - the target's uncond row (present when tgt_scale is neither 0 nor 1) reads the source chain's uncond row, or its cond row when
+ *     the source runs without one (src_scale 0 or 1).
+ * Source rows and every cross-attention layer run unchanged.  MasaCtrl's defaults are start_step = 4, start_layer = 10 (the last
+ * six layers: the decoder's two finest levels).  Inside the fused attention kernel a controlled row reads the source row's K and
+ * V^T tiles: no launch is added.  The output stays a convex combination of rows of the layer's V, so its range slot is unchanged.
+ * start_step >= n_steps or start_layer >= the net's layer count gives cdx_cycle_lockstep_masked's result bit for bit; negative
+ * values, nets without SpatialTransformers, and mma modes 0 and 2 (and mode 3 at head width 160) on a controlled layer are
+ * CDX_E_INVALID. */
+int cdx_cycle_lockstep_mutual(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                              int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                              const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                              float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                              void* stream, const float* mask, int start_step, int start_layer);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -504,6 +524,10 @@ int cdx_op_attention(cdx_engine* e, const float* q, const float* k, const float*
  * [0, B)).  Fused kernel only: a shape or mode that would take another route is CDX_E_INVALID. */
 int cdx_op_attention_rows(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
                           int Nq, int Nk, int heads, int d, float scale, const int* qk_rows, void* stream);
+/* cdx_op_attention with a key / value row table: image b attends with its own q over image kv_rows[b]'s k and v (kv_rows: host
+ * [B], each in [0, B)).  Fused kernel only, as cdx_op_attention_rows. */
+int cdx_op_attention_kv_rows(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
+                             int Nq, int Nk, int heads, int d, float scale, const int* kv_rows, void* stream);
 /* The fused kernel's accumulating launch: out[r] += softmax(q[r] k[r]^T * scale) v[r] for each image r of acc_rows (host [n_acc],
  * each in [0, B)); the other images of out are not touched.  Fused kernel only, as cdx_op_attention_rows. */
 int cdx_op_attention_accum(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,

@@ -65,6 +65,13 @@ class GemmDesc(C.Structure):
                 ('sA_b', C.c_int64), ('sA_h', C.c_int64), ('sB_b', C.c_int64), ('sB_h', C.c_int64), ('sC_b', C.c_int64), ('sC_h', C.c_int64)]
 
 
+class AttentionNetDesc(C.Structure):
+    _fields_ = [('kind', C.c_int), ('causal', C.c_int), ('qkv', C.c_void_p), ('q', C.c_void_p), ('kv', C.c_void_p), ('k', C.c_void_p),
+                ('v', C.c_void_p), ('B', C.c_int), ('N', C.c_int), ('L', C.c_int), ('ctx_lp', C.c_int), ('heads', C.c_int), ('d', C.c_int),
+                ('scale', C.c_float), ('qk_rows', C.POINTER(C.c_int)), ('kv_rows', C.POINTER(C.c_int)), ('acc_rows', C.POINTER(C.c_int)),
+                ('n_acc', C.c_int), ('slot', C.c_float), ('q_slot', C.c_float), ('out', C.c_void_p)]
+
+
 class LatentChain(C.Structure):
     _fields_ = [('row', C.c_int), ('row2', C.c_int), ('scale', C.c_float)]
 
@@ -171,6 +178,7 @@ SIGNATURES = {
     'cdx_op_softmax_rows': (_I, [_P, _P, C.c_int64, _I, _I, _I, _P]),
     'cdx_op_produce_norm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, C.POINTER(_I), _P]),
     'cdx_op_gemm': (_I, [_P, C.POINTER(GemmDesc), C.POINTER(_I), _P]),
+    'cdx_op_attention_net': (_I, [_P, C.POINTER(AttentionNetDesc), C.POINTER(_I), _P]),
     'cdx_op_latent_chains': (_I, [_P, C.POINTER(LatentChainsDesc), _I, _P]),
     'cdx_op_pixel_lockstep': (_I, [_P, _P, _P, _P, _P, _P, _P, C.POINTER(PixelCoef), _I, _I, _I, _I, _P]),
 }

@@ -1248,6 +1248,155 @@ int cdx_op_attention_accum(cdx_engine* eh, const float* q, const float* k, const
   if (!acc_rows || n_acc < 1) return guard([&] { CDX_CHECK(false, "op_attention_accum: an empty row list"); });
   return op_attention(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, acc_rows, n_acc, stream);
 }
+int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* plan_out, void* stream) {
+  return guard([&] {
+    CDX_CHECK(eh && d && d->out && d->kind >= 0 && d->kind <= 2, "op_attention_net: null argument or bad kind");
+    const int kind = d->kind, B = d->B, N = d->N, heads = d->heads, dh = d->d, C = heads * dh;
+    const int L = kind == 0 ? N : d->L;
+    CDX_CHECK(B > 0 && N > 0 && L > 0 && heads > 0 && dh > 0, "op_attention_net: B=%d N=%d L=%d heads=%d d=%d", B, N, L, heads, dh);
+    CDX_CHECK(kind != 0 || d->qkv, "op_attention_net: self-attention needs qkv");
+    CDX_CHECK(kind != 1 || (d->q && d->kv && d->ctx_lp >= L), "op_attention_net: cross-attention needs q and kv of ctx_lp >= L rows per image");
+    CDX_CHECK(kind != 2 || (d->q && d->k && d->v), "op_attention_net: generic attention needs q, k and v");
+    CDX_CHECK(!d->causal || kind == 2, "op_attention_net: the causal mask is the generic route's");
+    CDX_CHECK(!d->qk_rows || !d->kv_rows, "op_attention_net: qk_rows and kv_rows in one launch");
+    CDX_CHECK(!d->acc_rows || d->n_acc >= 1, "op_attention_net: an empty acc_rows list");
+    for (const int* t : {d->qk_rows, d->kv_rows})
+      if (t) for (int b = 0; b < B; ++b) CDX_CHECK(t[b] >= 0 && t[b] < B, "op_attention_net: row table entry %d = %d outside [0, %d)", b, t[b], B);
+    if (d->acc_rows) for (int r = 0; r < d->n_acc; ++r) CDX_CHECK(d->acc_rows[r] >= 0 && d->acc_rows[r] < B, "op_attention_net: acc_rows[%d] outside [0, %d)", r, B);
+    const bool tables = d->qk_rows || d->kv_rows || d->acc_rows;
+    Engine& e = eh->e;
+    cudaStream_t s = S(stream);
+    int plan[7] = {};
+    with_arena(e, s, [&] {
+      Scope sc(e.arena);
+      e.pools_reset(s);
+      auto stage = [&](const int* host, int n) -> const int* {
+        if (!host) return nullptr;
+        int* dev = (int*)e.arena.alloc((size_t)n * sizeof(int));
+        if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(dev, host, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, s));
+        return dev;
+      };
+      const int *qk_dev = stage(d->qk_rows, B), *kv_dev = stage(d->kv_rows, B), *acc_dev = stage(d->acc_rows, d->n_acc);
+      // a range slot as the network's producer leaves it: max |x| over the tensor, or the caller's (conservative) value
+      auto slot_of = [&](float value, const float* x, long long rows, int cols) {
+        float* slot = e.amax_slot();
+        if (value > 0.f) {
+          if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(slot, &value, sizeof(float), cudaMemcpyHostToDevice, s));
+        } else {
+          amax_rows(e, x, rows, cols, cols, slot, s);
+        }
+        return slot;
+      };
+      // TF32 planes of `cols` columns of x (row stride ld) as a projection epilogue writes them: hi = rn_tf32(x), lo = rn_tf32(x - hi)
+      auto tf32_planes = [&](const float* x, long long rows, int cols, long long ld, float*& hi, float*& lo) {
+        const size_t n = (size_t)rows * cols;
+        float* c = (float*)e.arena.alloc(n * sizeof(float));
+        hi = (float*)e.arena.alloc(n * sizeof(float));
+        lo = (float*)e.arena.alloc(n * sizeof(float));
+        if (!e.dry()) CDX_CUDA(cudaMemcpy2DAsync(c, (size_t)cols * 4, x, (size_t)ld * 4, (size_t)cols * 4, rows, cudaMemcpyDeviceToDevice, s));
+        split_planes(e, c, hi, lo, n, s);
+        return c;
+      };
+      auto fused_plan = [&](int route, bool h16, int Nq, int Nks, int Nvs) {
+        const FlashPlan f = flash_plan(dh, h16, e.attn_one, Nq);
+        plan[0] = route; plan[1] = f.qrows; plan[2] = f.rag; plan[3] = f.ksplit; plan[4] = f.ring; plan[5] = Nks; plan[6] = Nvs;
+      };
+      const long long M = (long long)B * N;
+      bool done = false;
+      if (kind == 0) {
+        const float* slot = slot_of(d->slot, d->qkv, M, 3 * C);
+        const bool flash_ok = flash_eligible(e, N, N, dh, C);
+        CDX_CHECK(!tables || flash_ok, "op_attention_net: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, dh);
+        if (flash_ok && e.tc_kind >= 1) {
+          int Nvs = 0;
+          done = self_attention_h16(e, d->qkv, slot, d->out, B, N, C, heads, dh, d->scale, !e.attn_one, s, qk_dev, kv_dev, acc_dev, d->n_acc, &Nvs);
+          fused_plan(e.attn_one ? 4 : 2, true, N, N, Nvs);
+        } else if (flash_ok) {
+          float *qk_hi, *qk_lo, *vt_hi, *vt_lo;
+          tf32_planes(d->qkv, M, 2 * C, 3 * C, qk_hi, qk_lo);
+          int Nvs = N;
+          if (N % 4) {
+            float* vr = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+            if (!e.dry()) CDX_CUDA(cudaMemcpy2DAsync(vr, (size_t)C * 4, d->qkv + 2 * C, (size_t)3 * C * 4, (size_t)C * 4, M, cudaMemcpyDeviceToDevice, s));
+            done = self_attention_tf32_padded(e, qk_hi, qk_lo, vr, d->out, B, N, C, heads, dh, d->scale, s, qk_dev, kv_dev, acc_dev, d->n_acc, &Nvs);
+          } else {
+            float* vr = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+            float* vt = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+            if (!e.dry()) CDX_CUDA(cudaMemcpy2DAsync(vr, (size_t)C * 4, d->qkv + 2 * C, (size_t)3 * C * 4, (size_t)C * 4, M, cudaMemcpyDeviceToDevice, s));
+            nhwc_to_nchw(e, vr, vt, 1, C, (int)M, s);
+            tf32_planes(vt, 1, (int)(M * C), M * C, vt_hi, vt_lo);
+            const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
+            done = flash_attention(e, pl, d->out, C, B, N, N, N, N, heads, dh, d->scale, s, qk_dev, acc_dev, d->n_acc, kv_dev);
+          }
+          fused_plan(3, false, N, N, Nvs);
+        } else if (e.mma_mode >= 1 && (N % 32) == 0 && N >= 128 && (dh % 4) == 0) {
+          float* qk = (float*)e.arena.alloc((size_t)M * 2 * C * sizeof(float));
+          float* vr = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+          float* vt = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
+          if (!e.dry()) {
+            CDX_CUDA(cudaMemcpy2DAsync(qk, (size_t)2 * C * 4, d->qkv, (size_t)3 * C * 4, (size_t)2 * C * 4, M, cudaMemcpyDeviceToDevice, s));
+            CDX_CUDA(cudaMemcpy2DAsync(vr, (size_t)C * 4, d->qkv + 2 * C, (size_t)3 * C * 4, (size_t)C * 4, M, cudaMemcpyDeviceToDevice, s));
+          }
+          nhwc_to_nchw(e, vr, vt, 1, C, (int)M, s);
+          done = attention_tc(e, qk, 2 * C, qk + C, 2 * C, dh, vt, d->out, C, B, N, N, heads, dh, d->scale, s);
+          plan[0] = 1;
+        }
+        if (!done) {
+          attention(e, d->qkv, 3 * C, d->qkv + C, 3 * C, d->qkv + 2 * C, 3 * C, d->out, C, B, N, N, heads, dh, dh, d->scale, s);
+          plan[0] = 0;
+        }
+      } else if (kind == 1) {
+        const int Lp = d->ctx_lp;
+        const long long Mk = (long long)B * Lp;
+        const bool flash_ok = flash_eligible(e, N, L, dh, C);
+        CDX_CHECK(!tables || flash_ok, "op_attention_net: a row table needs the fused kernel (mode %d, d=%d)", e.mma_mode, dh);
+        if (flash_ok) {
+          const bool h16 = e.tc_kind >= 1, lo = !e.attn_one;
+          AttnPlanes pl{h16 ? AttnPlanes::H16 : AttnPlanes::TF32, nullptr, nullptr, C, nullptr, nullptr, C, nullptr, nullptr};
+          if (h16) {
+            const float* kv_slot = slot_of(d->slot, d->kv, Mk, 2 * C);
+            const float* q_slot = slot_of(d->q_slot, d->q, M, C);
+            void* q_hi = e.arena.alloc((size_t)M * C * 2);
+            void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
+            void* k_hi = e.arena.alloc((size_t)Mk * C * 2);
+            void* k_lo = lo ? e.arena.alloc((size_t)Mk * C * 2) : nullptr;
+            void* vt_hi = e.arena.alloc((size_t)Mk * C * 2);
+            void* vt_lo = lo ? e.arena.alloc((size_t)Mk * C * 2) : nullptr;
+            split_rows_h16(e, d->q, M, C, C, q_hi, q_lo, C, q_slot, s);
+            context_split_h16(e, d->kv, (int)Mk, C, kv_slot, k_hi, k_lo, vt_hi, vt_lo, s);
+            pl.q_hi = q_hi; pl.q_lo = q_lo; pl.k_hi = k_hi; pl.k_lo = k_lo; pl.vt_hi = vt_hi; pl.vt_lo = vt_lo;
+            pl.q_amax = q_slot; pl.k_amax = kv_slot; pl.v_amax = kv_slot;
+          } else {
+            float *q_hi, *q_lo, *k_hi, *k_lo, *vt_hi, *vt_lo;
+            tf32_planes(d->q, M, C, C, q_hi, q_lo);
+            tf32_planes(d->kv, Mk, C, 2 * C, k_hi, k_lo);
+            float* vr = (float*)e.arena.alloc((size_t)Mk * C * sizeof(float));
+            float* vt = (float*)e.arena.alloc((size_t)Mk * C * sizeof(float));
+            if (!e.dry()) CDX_CUDA(cudaMemcpy2DAsync(vr, (size_t)C * 4, d->kv + C, (size_t)2 * C * 4, (size_t)C * 4, Mk, cudaMemcpyDeviceToDevice, s));
+            nhwc_to_nchw(e, vr, vt, 1, C, (int)Mk, s);
+            tf32_planes(vt, 1, (int)(Mk * C), Mk * C, vt_hi, vt_lo);
+            pl.q_hi = q_hi; pl.q_lo = q_lo; pl.k_hi = k_hi; pl.k_lo = k_lo; pl.vt_hi = vt_hi; pl.vt_lo = vt_lo;
+          }
+          done = flash_attention(e, pl, d->out, C, B, N, L, Lp, Lp, heads, dh, d->scale, s, qk_dev, acc_dev, d->n_acc, kv_dev);
+          fused_plan(h16 ? (e.attn_one ? 4 : 2) : 3, h16, N, Lp, Lp);
+        }
+        if (!done) {
+          // the unfused route reads the context unpadded, L rows per image
+          float* kv = (float*)e.arena.alloc((size_t)B * L * 2 * C * sizeof(float));
+          if (!e.dry())
+            CDX_CUDA(cudaMemcpy2DAsync(kv, (size_t)L * 2 * C * 4, d->kv, (size_t)Lp * 2 * C * 4, (size_t)L * 2 * C * 4, B, cudaMemcpyDeviceToDevice, s));
+          attention(e, d->q, C, kv, 2 * C, kv + C, 2 * C, d->out, C, B, N, L, heads, dh, dh, d->scale, s);
+          plan[0] = 0;
+        }
+      } else {
+        CDX_CHECK(!tables, "op_attention_net: row tables need a fused route");
+        attention(e, d->q, C, d->k, C, d->v, C, d->out, C, B, N, L, heads, dh, dh, d->scale, s, d->causal != 0);
+      }
+      CDX_CHECK(done || !tables, "op_attention_net: the fused kernel rejected a row-table shape");
+    });
+    if (plan_out) for (int i = 0; i < 7; ++i) plan_out[i] = plan[i];
+  });
+}
 int cdx_op_nchw_to_nhwc(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nchw_to_nhwc(eh->e, x, y, B, C, HW, S(stream))); }
 int cdx_op_nhwc_to_nchw(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nhwc_to_nchw(eh->e, x, y, B, C, HW, S(stream))); }
 

@@ -210,6 +210,26 @@ void split_rows_h16(Engine& e, const float* src, long long rows, int cols, long 
 // R rows = `images` images of R / images rows each; Rp > 0: each image's columns padded with zeros to a stride of Rp (V^T key stride)
 void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long ld, void* hi, void* lo, const float* amax, cudaStream_t s,
                          int images = 1, int Rp = 0);
+// The fused kernel variant flash_attention runs for head width d, plane format and N queries: queries per CTA, ragged last query
+// tile, key split across the two consumer warpgroups, K / V ring depth (all zero: no instantiation)
+struct FlashPlan { int qrows, rag, ksplit, ring; };
+FlashPlan flash_plan(int d, bool h16, bool one, int N);
+// The network executors' operand preparation after the projection, shared by UNetExec::spatial_transformer and
+// cdx_op_attention_net so that the op test feeds the kernel exactly as the network does.
+// Self-attention, fp16 planes: one plain fp32 q|k|v projection qkv [B*HW, 3C] whose single range slot sets the exponent of all
+// three operands.  q|k split in place at ld 3C; K keeps the per-image key stride HW (Nks = HW: an image's last 64-key box reads
+// into the next image, masked by Nk); V^T split per image at Nvs = HW rounded up to 8 keys.  lo = false: hi planes only (one-term)
+bool self_attention_h16(Engine& e, const float* qkv, const float* slot, float* out, int B, int HW, int C, int heads, int d, float scale, bool lo,
+                        cudaStream_t s, const int* qk_row, const int* kv_row, const int* acc_rows = nullptr, int n_acc = 0, int* Nvs_out = nullptr);
+// Self-attention, TF32 planes, HW % 4 != 0: q|k planes [B*HW, 2C] from the projection's epilogue and V row-major [B*HW, C], copied
+// into rows padded to Nvs = HW rounded up to 4 keys per image (zero rows), transposed and split
+bool self_attention_tf32_padded(Engine& e, const float* qk_hi, const float* qk_lo, const float* vr, float* out, int B, int HW, int C, int heads,
+                                int d, float scale, cudaStream_t s, const int* qk_row, const int* kv_row, const int* acc_rows = nullptr,
+                                int n_acc = 0, int* Nvs_out = nullptr);
+// Cross-attention, fp16 planes: K (when k_hi) and V^T of one fused K | V context projection kv [Mk, 2C] (Mk padded context rows),
+// both with the exponent of the one slot of the whole projection
+void context_split_h16(Engine& e, const float* kv, int Mk, int C, const float* slot, void* k_hi, void* k_lo, void* vt_hi, void* vt_lo,
+                       cudaStream_t s);
 void split_planes(Engine& e, const float* w, float* hi, float* lo, size_t n, cudaStream_t s);   // hi = rn_tf32(w), lo = rn_tf32(w - hi)
 // fp16 split of w * 2^exp: hi = fp16(w'), lo = fp16(w' - hi)  (hi / lo: __half arrays)
 void split_planes_h16(Engine& e, const float* w, void* hi, void* lo, size_t n, int exp, cudaStream_t s);

@@ -204,6 +204,9 @@ flash_attn_kernel(const __grid_constant__ CUtensorMap mapQh, const __grid_consta
   float scale_l2 = p.scale_log2e, oscale = 1.f;
   if (F16) {
     scale_l2 = scale_l2 * exp2i(-h16_exp_of(*p.q_amax)) * exp2i(-h16_exp_of(*p.k_amax));
+    // q and k both far below fp32's range (exponents near the +100 clamp) take the product under 2^-126, and a zero scale would turn
+    // the masked scores' -inf into NaN.  Every score is then below 2^-88 in the log2 domain (|raw| < 2^38), 0 to fp32 either way
+    scale_l2 = fmaxf(scale_l2, exp2i(-126));
     oscale = exp2i(-h16_exp_of(*p.v_amax));
   }
   constexpr float PEXP = F16 ? 10.f : 0.f;
@@ -646,6 +649,71 @@ void split_transpose_h16(Engine& e, const float* src, int R, int Cc, long long l
             (__half*)lo, amax);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
+}
+
+namespace {
+template <int D, bool F16, bool ONE>
+FlashPlan plan_of(int N) {
+  using C = ACfg<D, F16, ONE>;
+  return {C::QROWS, N % C::QROWS != 0, C::KSPLIT, C::RING};
+}
+template <bool F16, bool ONE>
+FlashPlan plan_d(int d, int N) {
+  switch (d) {
+    case 16: return plan_of<16, F16, ONE>(N);
+    case 32: return plan_of<32, F16, ONE>(N);
+    case 40: return plan_of<40, F16, ONE>(N);
+    case 64: return plan_of<64, F16, ONE>(N);
+    case 80: return plan_of<80, F16, ONE>(N);
+    case 160: if constexpr (F16) return plan_of<160, F16, ONE>(N); else return {};
+    default: return {};
+  }
+}
+}  // namespace
+
+FlashPlan flash_plan(int d, bool h16, bool one, int N) {
+  return one ? plan_d<true, true>(d, N) : h16 ? plan_d<true, false>(d, N) : plan_d<false, false>(d, N);
+}
+
+bool self_attention_h16(Engine& e, const float* qkv, const float* slot, float* out, int B, int HW, int C, int heads, int d, float scale, bool lo,
+                        cudaStream_t s, const int* qk_row, const int* kv_row, const int* acc_rows, int n_acc, int* Nvs_out) {
+  const int M = B * HW, Nvs = (HW + 7) & ~7;
+  void* qk_hi = e.arena.alloc((size_t)M * 2 * C * 2);
+  void* qk_lo = lo ? e.arena.alloc((size_t)M * 2 * C * 2) : nullptr;
+  void* vt_hi = e.arena.alloc((size_t)C * B * Nvs * 2);
+  void* vt_lo = lo ? e.arena.alloc((size_t)C * B * Nvs * 2) : nullptr;
+  split_rows_h16(e, qkv, M, 2 * C, 3 * C, qk_hi, qk_lo, 2 * C, slot, s);
+  split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, slot, s, B, Nvs);
+  const AttnPlanes pl{AttnPlanes::H16, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr,
+                      2 * C, vt_hi, vt_lo, slot, slot, slot};
+  if (Nvs_out) *Nvs_out = Nvs;
+  return flash_attention(e, pl, out, C, B, HW, HW, HW, Nvs, heads, d, scale, s, qk_row, acc_rows, n_acc, kv_row);
+}
+
+bool self_attention_tf32_padded(Engine& e, const float* qk_hi, const float* qk_lo, const float* vr, float* out, int B, int HW, int C, int heads,
+                                int d, float scale, cudaStream_t s, const int* qk_row, const int* kv_row, const int* acc_rows, int n_acc,
+                                int* Nvs_out) {
+  const int Nvs = (HW + 3) & ~3;
+  const size_t nvt = (size_t)C * B * Nvs;
+  float* vp = (float*)e.arena.alloc(nvt * sizeof(float));
+  float* vt = (float*)e.arena.alloc(nvt * sizeof(float));
+  float* vt_hi = (float*)e.arena.alloc(nvt * sizeof(float));
+  float* vt_lo = (float*)e.arena.alloc(nvt * sizeof(float));
+  if (!e.dry()) {
+    CDX_CUDA(cudaMemsetAsync(vp, 0, nvt * sizeof(float), s));
+    CDX_CUDA(cudaMemcpy2DAsync(vp, (size_t)Nvs * C * 4, vr, (size_t)HW * C * 4, (size_t)HW * C * 4, B, cudaMemcpyDeviceToDevice, s));
+  }
+  nhwc_to_nchw(e, vp, vt, 1, C, B * Nvs, s);
+  split_planes(e, vt, vt_hi, vt_lo, nvt, s);
+  const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
+  if (Nvs_out) *Nvs_out = Nvs;
+  return flash_attention(e, pl, out, C, B, HW, HW, HW, Nvs, heads, d, scale, s, qk_row, acc_rows, n_acc, kv_row);
+}
+
+void context_split_h16(Engine& e, const float* kv, int Mk, int C, const float* slot, void* k_hi, void* k_lo, void* vt_hi, void* vt_lo,
+                       cudaStream_t s) {
+  if (k_hi) split_rows_h16(e, kv, Mk, C, 2 * C, k_hi, k_lo, C, slot, s);
+  split_transpose_h16(e, kv + C, Mk, C, 2 * C, vt_hi, vt_lo, slot, s);
 }
 
 }  // namespace cdx

@@ -733,8 +733,7 @@ struct UNetExec : Exec {
       Scope sk(e.arena);
       float* kvf = (float*)e.arena.alloc((size_t)Mk * 2 * C * sizeof(float));
       linear_into(x.pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kvf, 2 * C, nullptr, x.amax, nullptr, slot);
-      if (k_hi) split_rows_h16(e, kvf, Mk, C, 2 * C, k_hi, k_lo, C, slot, s);
-      split_transpose_h16(e, kvf + C, Mk, C, 2 * C, vt_hi, vt_lo, slot, s);
+      context_split_h16(e, kvf, Mk, C, slot, k_hi, k_lo, vt_hi, vt_lo, s);
     } else {
       if (k_hi) linear_into(x.pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), C, nullptr, nullptr, 0, k_hi, C, k_lo, x.amax);
       linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, x.pad, Mk, nullptr, nullptr, 0, vt_hi, Mk, vt_lo, nullptr, nullptr, slot);
@@ -823,41 +822,19 @@ struct UNetExec : Exec {
         linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_q.weight"), 3 * C, nullptr, nullptr, 0, qkv, 3 * C, nullptr, n1.amax, nullptr,
                     a.amax);                    // range of q | k | v (v bounds the attention output: a convex combination of V rows)
         // (mode 5: hi planes only, one-term kernel)
-        const bool lo = !e.attn_one;
-        const int Nvs = (HW + 7) & ~7;
-        void* qk_hi = e.arena.alloc((size_t)M * 2 * C * 2);
-        void* qk_lo = lo ? e.arena.alloc((size_t)M * 2 * C * 2) : nullptr;
-        void* vt_hi = e.arena.alloc((size_t)C * B * Nvs * 2);
-        void* vt_lo = lo ? e.arena.alloc((size_t)C * B * Nvs * 2) : nullptr;
-        split_rows_h16(e, qkv, M, 2 * C, 3 * C, qk_hi, qk_lo, 2 * C, a.amax, s);
-        split_transpose_h16(e, qkv + 2 * C, M, C, 3 * C, vt_hi, vt_lo, a.amax, s, B, Nvs);
-        const AttnPlanes pl{AttnPlanes::H16, qk_hi, qk_lo, 2 * C, (const char*)qk_hi + (size_t)C * 2, lo ? (const char*)qk_lo + (size_t)C * 2 : nullptr,
-                            2 * C, vt_hi, vt_lo, a.amax, a.amax, a.amax};
-        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow, nullptr, 0, mrow);
+        done = self_attention_h16(e, qkv, a.amax, a.p, B, HW, C, heads, d, scale, !e.attn_one, s, srow, mrow);
         CDX_CHECK(done, "flash attention (fp16-split) rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok && (HW % 4) != 0) {
         // TF32 planes with a per-image key count off the 16-byte TMA granule: V row-major, copied into rows padded to Nvs keys
         // per image (zero rows), transposed and split; q|k planes from the projection's epilogue as below
         Scope sa(e.arena);
-        const int Nvs = (HW + 3) & ~3;
-        const size_t nqk = (size_t)M * 2 * C, nvt = (size_t)C * B * Nvs;
+        const size_t nqk = (size_t)M * 2 * C;
         float* qk_hi = (float*)e.arena.alloc(nqk * sizeof(float));
         float* qk_lo = (float*)e.arena.alloc(nqk * sizeof(float));
         float* vr = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
-        float* vp = (float*)e.arena.alloc(nvt * sizeof(float));
-        float* vt = (float*)e.arena.alloc(nvt * sizeof(float));
-        float* vt_hi = (float*)e.arena.alloc(nvt * sizeof(float));
-        float* vt_lo = (float*)e.arena.alloc(nvt * sizeof(float));
         linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_q.weight"), 2 * C, nullptr, nullptr, 0, qk_hi, 2 * C, qk_lo, n1.amax);
         linear_into(n1.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn1.to_v.weight"), C, nullptr, nullptr, 0, vr, C, nullptr, n1.amax, nullptr, a.amax);
-        if (!e.dry()) {
-          CDX_CUDA(cudaMemsetAsync(vp, 0, nvt * sizeof(float), s));
-          CDX_CUDA(cudaMemcpy2DAsync(vp, (size_t)Nvs * C * 4, vr, (size_t)HW * C * 4, (size_t)HW * C * 4, B, cudaMemcpyDeviceToDevice, s));
-        }
-        nhwc_to_nchw(e, vp, vt, 1, C, B * Nvs, s);
-        split_planes(e, vt, vt_hi, vt_lo, nvt, s);
-        const AttnPlanes pl{AttnPlanes::TF32, qk_hi, qk_lo, 2 * C, qk_hi + C, qk_lo + C, 2 * C, vt_hi, vt_lo};
-        done = flash_attention(e, pl, a.p, C, B, HW, HW, HW, Nvs, heads, d, scale, s, srow, nullptr, 0, mrow);
+        done = self_attention_tf32_padded(e, qk_hi, qk_lo, vr, a.p, B, HW, C, heads, d, scale, s, srow, mrow);
         CDX_CHECK(done, "flash attention rejected an eligible shape (HW=%d d=%d)", HW, d);
       } else if (flash_ok) {
         // fused tensor-core attention: q|k projection and V^T (= Wv . X^T, a swapped-role GEMM, so that both P.V operands

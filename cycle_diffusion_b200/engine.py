@@ -473,6 +473,31 @@ class Engine:
             check(fn(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, Nq, Nk, heads, Cc // heads, scale, (C.c_int * B)(*rows), self.stream))
         return out
 
+    ATTN_ROUTES = ('generic', 'unfused_tc', 'fused_h16', 'fused_tf32', 'fused_one')
+
+    def op_attention_net(self, kind, out, B, N, heads, d, scale, qkv=None, q=None, kv=None, k=None, v=None, L=0, ctx_lp=0, causal=False,
+                         qk_rows=None, kv_rows=None, acc_rows=None, slot=0.0, q_slot=0.0):
+        """One attention with its operands prepared as the network executors prepare them (cdx_op_attention_net in include/cdx.h,
+        whose descriptor fields are the arguments).  kind: 'self' (qkv [B*N, 3C], one range slot), 'cross' (q [B*N, C], kv
+        [B*ctx_lp, 2C] the padded context's K | V) or 'generic' (q, k, v; optional causal mask).  Every buffer is a float32 tensor on
+        this engine's device passed as it is; out [B*N, C] (a view inside a larger buffer is fine) is written, or added to for the
+        images of acc_rows.  slot / q_slot > 0 replace the measured range slots.  Returns the plan: dict(route, qrows, rag, ksplit,
+        ring, Nks, Nvs)."""
+        kinds = ('self', 'cross', 'generic')
+        assert kind in kinds, kind
+        for name, t in (('out', out), ('qkv', qkv), ('q', q), ('kv', kv), ('k', k), ('v', v)):
+            assert t is None or (torch.is_tensor(t) and t.dtype == torch.float32 and t.device == self.device), \
+                f'op_attention_net: {name} must be a float32 tensor on {self.device}'
+        rows = lambda r: None if r is None else (C.c_int * max(len(r), 1))(*[int(x) for x in r])
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        desc = _cabi.AttentionNetDesc(kind=kinds.index(kind), causal=int(bool(causal)), qkv=ptr(qkv), q=ptr(q), kv=ptr(kv), k=ptr(k), v=ptr(v),
+                                      B=B, N=N, L=L, ctx_lp=ctx_lp, heads=heads, d=d, scale=scale, qk_rows=rows(qk_rows), kv_rows=rows(kv_rows),
+                                      acc_rows=rows(acc_rows), n_acc=len(acc_rows) if acc_rows is not None else 0, slot=slot, q_slot=q_slot,
+                                      out=ptr(out))
+        plan = (C.c_int * 7)()
+        check(lib.cdx_op_attention_net(self.h, C.byref(desc), plan, self.stream))
+        return dict(zip(('route', 'qrows', 'rag', 'ksplit', 'ring', 'Nks', 'Nvs'), [self.ATTN_ROUTES[plan[0]]] + list(plan[1:])))
+
     def op_nchw_to_nhwc(self, x):
         x = _f32c(x, self.device)
         B, Cc, H, W = x.shape

@@ -532,6 +532,30 @@ int cdx_op_attention_kv_rows(cdx_engine* e, const float* q, const float* k, cons
  * each in [0, B)); the other images of out are not touched.  Fused kernel only, as cdx_op_attention_rows. */
 int cdx_op_attention_accum(cdx_engine* e, const float* q, const float* k, const float* v, float* out, int B,
                            int Nq, int Nk, int heads, int d, float scale, const int* acc_rows, int n_acc, void* stream);
+/* One attention with its operands prepared as the network executors prepare them after the projection
+ * (tests/test_attention_bound_gpu.py).  C = heads * d, out [B*N, C].
+ *   kind 0, self (the U-Net SpatialTransformer): qkv [B*N, 3C], one q|k|v projection with ONE range slot for all three operands
+ *     (`slot` > 0: that value, else max |qkv|); K at the per-image key stride N, V^T padded per image.  TF32 planes (mma mode 3):
+ *     q|k and V^T as the projection epilogues write them, on both of the network's V^T routes (N % 4 == 0 or not).
+ *   kind 1, cross: q [B*N, C] (its own slot, `q_slot` > 0 or max |q|) over a context padded to ctx_lp >= L rows per image,
+ *     kv [B*ctx_lp, 2C] one K | V projection with one slot (`slot` > 0 or max |kv|); keys >= L masked.
+ *   kind 2, generic (text towers, VAE): q [B*N, C], k / v [B*L, C], two contractions around the row softmax; causal: query i sees
+ *     keys j <= i.
+ * qk_rows / kv_rows (host [B]) and acc_rows (host [n_acc], out += for those images only) as cdx_op_attention_rows / _kv_rows /
+ * _accum; fused routes only.  plan_out (host int[7], optional): route (0 generic, 1 unfused tensor-core, 2 fused fp16 three-term,
+ * 3 fused TF32, 4 fused one-term), the fused kernel's queries per CTA, ragged query tile, key split, ring depth, and the K and V^T
+ * per-image key strides Nks, Nvs (zero where not fused). */
+typedef struct cdx_attention_net_desc {
+  int kind, causal;
+  const float* qkv;
+  const float* q; const float* kv; const float* k; const float* v;
+  int B, N, L, ctx_lp, heads, d;
+  float scale;
+  const int* qk_rows; const int* kv_rows; const int* acc_rows; int n_acc;
+  float slot, q_slot;
+  float* out;
+} cdx_attention_net_desc;
+int cdx_op_attention_net(cdx_engine* e, const cdx_attention_net_desc* desc, int* plan_out, void* stream);
 int cdx_op_nchw_to_nhwc(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 /* The normalisation kernels in the forms the network executors call them, with their side outputs (tests/test_norms_gpu.py).

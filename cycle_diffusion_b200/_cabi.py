@@ -142,6 +142,8 @@ SIGNATURES = {
                                        _I, _I, _P, _P, C.POINTER(AttnControl), _P]),
     'cdx_cycle_lockstep_mutual': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
                                        _I, _I, _P, _P, _I, _I]),
+    'cdx_cycle_lockstep_pnp': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
+                                    _I, _I, _P, _P, _I, _I, _I, C.POINTER(_I), _I]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),
@@ -174,6 +176,7 @@ SIGNATURES = {
     'cdx_op_nchw_to_nhwc': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_nhwc_to_nchw': (_I, [_P, _P, _P, _I, _I, _I, _P]),
     'cdx_op_groupnorm_ex': (_I, [_P, _P, _I, _P, _I, _P, _P, _F, _I, _P, _P, _I, _P, _P, _P, _I, _I, _P]),
+    'cdx_op_groupnorm_rows': (_I, [_P, _P, _I, _P, _I, _P, _P, _F, _I, _P, _P, _I, C.POINTER(_I), _P, _P, _P, _P, _I, _I, _P]),
     'cdx_op_layernorm_ex': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P]),
     'cdx_op_softmax_rows': (_I, [_P, _P, C.c_int64, _I, _I, _I, _P]),
     'cdx_op_produce_norm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, C.POINTER(_I), _P]),

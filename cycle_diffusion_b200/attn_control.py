@@ -10,6 +10,10 @@ the host helpers that build token maps from two prompts' token ids.
 MasaCtrl's mutual self-attention (Cao et al., 2023; ``MutualSelfControl``) is the complementary control for non-rigid edits: in
 the decoder's self-attention layers the target rows keep their own queries and attend over the source row's keys and values
 (cdx_cycle_lockstep_mutual), so the layout follows the target prompt and the content comes from the real image.
+
+Plug-and-Play diffusion features (Tumanyan et al., 2023; ``PnPControl``) keep the real image's spatial layout for text-guided
+translation: the target rows take the source row's decoder ResBlock features and its self-attention queries and keys
+(cdx_cycle_lockstep_pnp), and the target prompt sets the appearance.
 """
 from dataclasses import dataclass
 
@@ -104,6 +108,41 @@ class MutualSelfControl:
             v = getattr(self, name)
             if isinstance(v, bool) or not isinstance(v, int) or v < 0:
                 raise ValueError(f'{name} must be an integer >= 0, got {v!r}')
+
+
+@dataclass(frozen=True)
+class PnPControl:
+    """Plug-and-Play's feature and attention injection: at loop steps i < int(feature_steps * n) (0-based, of the n steps that run
+    after strength's skip), the ResBlock output_blocks.k.0 of every k in feature_blocks gives each target row its own skip plus
+    out_layers of the source row's in_layers output; at steps i < int(attention_steps * n), in every SpatialTransformer whose index
+    in forward order (input blocks, middle block, output blocks; 16 in SD v1 / 2.x) is >= attention_start_layer, the target rows
+    attend with the source row's queries and keys over their own values.  The target's cond row reads the source's cond row, its
+    uncond row the source's uncond row (the source's only row when it has none).  The defaults are PnP's: pnp_f_t = 0.8 and
+    pnp_attn_t = 0.5, block 4 (up_blocks[1].resnets[1]), layers from 8 (up_blocks[1].attentions[1]) on."""
+    feature_steps: float = 0.8
+    attention_steps: float = 0.5
+    feature_blocks: tuple = (4,)
+    attention_start_layer: int = 8
+
+    def __post_init__(self):
+        _fraction('feature_steps', self.feature_steps)
+        _fraction('attention_steps', self.attention_steps)
+        blocks = self.feature_blocks
+        if not isinstance(blocks, (tuple, list)):
+            raise ValueError(f'feature_blocks must be a tuple of output-block indices, got {blocks!r}')
+        for k in blocks:
+            if isinstance(k, bool) or not isinstance(k, int) or k < 0:
+                raise ValueError(f'feature_blocks: indices must be integers >= 0, got {k!r}')
+        if len(set(blocks)) != len(blocks):
+            raise ValueError(f'feature_blocks: duplicate index in {tuple(blocks)}')
+        object.__setattr__(self, 'feature_blocks', tuple(blocks))
+        v = self.attention_start_layer
+        if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+            raise ValueError(f'attention_start_layer must be an integer >= 0, got {v!r}')
+
+    def steps(self, n):
+        """(feature_steps, attention_steps) as step counts of an n-step loop."""
+        return int(self.feature_steps * n), int(self.attention_steps * n)
 
 
 def replace_token_map(src_ids, tgt_ids, L):

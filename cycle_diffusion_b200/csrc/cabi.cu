@@ -153,6 +153,14 @@ void hook_weight_planes(Engine& e, const float* w, size_t n, GemmArgs& g, cudaSt
 // Per step: one U-Net call over exactly the rows the chains need (a chain contributes [uncond, cond] when it runs with
 // classifier-free guidance, ddim.py:550-559, else one row) and ONE fused elementwise launch (latent_chains_step).
 // ---------------------------------------------------------------------------------------------------------------------
+// Plug-and-Play injection of one loop (cdx.h, cdx_cycle_lockstep_pnp): the ResBlocks of output blocks blocks[0 .. n_blocks) at
+// steps < feature_steps, the self-attention of layers >= start_layer at steps < attention_steps
+struct PnpLoop {
+  int feature_steps = 0, attention_steps = 0, start_layer = 0;
+  const int* blocks = nullptr;                      // host [n_blocks]
+  int n_blocks = 0;
+};
+
 struct ChainLoopArgs {
   int n_src = 0, K = 0;                            // element groups; target chains per group
   bool src = false;                                // a source chain per group
@@ -174,6 +182,7 @@ struct ChainLoopArgs {
   const float* own_weight = nullptr;                // optional with ctl: [n_src, L], refine's weights of the rows' own attention
   // optional, exclusive with ctl: mutual self-attention (cdx.h, cdx_cycle_lockstep_mutual) at steps >= start_step, layers >= start_layer
   bool mutual = false; int start_step = 0, start_layer = 0;
+  const PnpLoop* pnp = nullptr;                     // optional, exclusive with ctl and mutual: Plug-and-Play
   int C = 0, h = 0, w = 0;
 };
 
@@ -244,6 +253,23 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     CDX_CHECK(unet.kind == NET_UNET_OPENAI && ctx_n > 0 && a.c_src && a.c_tgt, "mutual self-attention: needs a U-Net with SpatialTransformers");
     CDX_CHECK(e.mma_mode == 1 && e.flash_attn, "mutual self-attention: needs the fused attention kernel (mma modes 1, 3, 4 or 5)");
     CDX_CHECK(a.start_step >= 0 && a.start_layer >= 0, "mutual self-attention: start_step=%d start_layer=%d", a.start_step, a.start_layer);
+  }
+  if (a.pnp) {
+    const PnpLoop& p = *a.pnp;
+    CDX_CHECK(!a.ctl && !a.mutual, "Plug-and-Play, Prompt-to-Prompt and mutual self-attention are exclusive in one loop");
+    CDX_CHECK(a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net && !a.scales_on_device,
+              "Plug-and-Play: needs the lock-step loop with a source chain at every step");
+    CDX_CHECK(unet.kind == NET_UNET_OPENAI && ctx_n > 0 && a.c_src && a.c_tgt, "Plug-and-Play: needs a U-Net with SpatialTransformers");
+    CDX_CHECK(e.mma_mode == 1 && e.flash_attn, "Plug-and-Play: needs the fused attention kernel (mma modes 1, 3, 4 or 5)");
+    CDX_CHECK(p.feature_steps >= 0 && p.feature_steps <= a.n_steps && p.attention_steps >= 0 && p.attention_steps <= a.n_steps &&
+              p.start_layer >= 0 && p.n_blocks >= 0 && (p.blocks || p.n_blocks == 0),
+              "Plug-and-Play: feature_steps=%d attention_steps=%d (of %d) attention_start_layer=%d n_blocks=%d", p.feature_steps,
+              p.attention_steps, a.n_steps, p.start_layer, p.n_blocks);
+    const int n_out = unet.ucfg.n_mult * (unet.ucfg.num_res_blocks + 1);
+    for (int i = 0; i < p.n_blocks; ++i) {
+      CDX_CHECK(p.blocks[i] >= 0 && p.blocks[i] < n_out, "Plug-and-Play: feature block %d outside the net's %d output blocks", p.blocks[i], n_out);
+      for (int j = 0; j < i; ++j) CDX_CHECK(p.blocks[j] != p.blocks[i], "Plug-and-Play: feature block %d given twice", p.blocks[i]);
+    }
   }
   Scope sc(e.arena);
   unet.ctxkv.valid = false;                    // the conditioning is fixed for this loop: its K / V are computed by the first step only
@@ -339,21 +365,28 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.n_own = (int)own.size();
     }
   }
-  // mutual self-attention: each target chain's cond row reads its group's source cond row's K and V, its uncond row the source's
-  // uncond row (the cond row when the source runs without one); every other row its own.  Fixed for the loop
-  if (a.mutual) {
-    std::vector<int> kv(rows);
-    for (int r = 0; r < rows; ++r) kv[r] = r;
+  // mutual self-attention and Plug-and-Play: each target chain's cond row reads its group's source cond row, its uncond row the
+  // source's uncond row (the source's only row when it runs without one); every other row its own.  Fixed for the loop
+  if (a.mutual || a.pnp) {
+    std::vector<int> src_row(rows);
+    for (int r = 0; r < rows; ++r) src_row[r] = r;
     for (int j = 0; j < a.n_src; ++j)
       for (int k = 0; k < a.K; ++k) {
         const Chain& t = ch[a.n_src + (size_t)j * a.K + k];
-        kv[t.row] = ch[j].row;
-        if (t.row2 >= 0) kv[t.row2] = ch[j].row2 >= 0 ? ch[j].row2 : ch[j].row;
+        src_row[t.row] = ch[j].row;
+        if (t.row2 >= 0) src_row[t.row2] = ch[j].row2 >= 0 ? ch[j].row2 : ch[j].row;
       }
-    int* kv_dev = (int*)e.arena.alloc((size_t)rows * sizeof(int));
-    if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(kv_dev, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
-    actl.kv_row = kv_dev;
-    actl.start_layer = a.start_layer;
+    int* dev = (int*)e.arena.alloc((size_t)rows * sizeof(int));
+    if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(dev, src_row.data(), src_row.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+    if (a.mutual) {
+      actl.kv_row = dev;
+      actl.start_layer = a.start_layer;
+    } else {
+      actl.pnp_row = dev;
+      actl.pnp_layer = a.pnp->start_layer;
+      actl.feat_blocks = a.pnp->blocks;
+      actl.n_feat = a.pnp->n_blocks;
+    }
   }
   auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
     if (i_next >= a.n_rec) return 0;
@@ -382,7 +415,10 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.cross = a.ctl && i < a.ctl->cross_steps;
       actl.self = a.ctl && i < a.ctl->self_steps;
       actl.mutual = a.mutual && i >= a.start_step;
-      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true, a.ctl || a.mutual ? &actl : nullptr);
+      actl.pnp_feat = a.pnp && i < a.pnp->feature_steps;
+      actl.pnp_attn = a.pnp && i < a.pnp->attention_steps;
+      unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true,
+                   a.ctl || a.mutual || a.pnp ? &actl : nullptr);
     } else {
       ps.fork();
       if (src_i) unet_forward(unet, xin, tdev + (size_t)i * rows, nullptr, 0, eout, rows_src, a.h, a.w, s);
@@ -797,11 +833,12 @@ int cdx_cycle_lockstep_ctl(cdx_net* un, const float* x0, const float* c_src, con
                                    x_out, z_out, B, C, h, w, stream, mask, ctl, nullptr);
 }
 
-// the single-image lock-step cycle under the controls of ChainLoopArgs (ctl, own_weight; mutual with start_step >= 0)
+// the single-image lock-step cycle under the controls of ChainLoopArgs (ctl, own_weight; mutual with start_step >= 0; pnp)
 static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
                           float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream, const float* mask,
-                          const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer) {
+                          const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer,
+                          const PnpLoop* pnp = nullptr) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -812,7 +849,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
     a.x0 = x0; a.c_src = c_src; a.c_tgt = c_tgt; a.uc = uc; a.L = L; a.s_scales = s_scales.data(); a.t_scales = t_scales.data();
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
     a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
-    a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer;
+    a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer; a.pnp = pnp;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -831,6 +868,18 @@ int cdx_cycle_lockstep_mutual(cdx_net* un, const float* x0, const float* c_src, 
                               const float* mask, int start_step, int start_layer) {
   return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
                         B, C, h, w, stream, mask, nullptr, nullptr, true, start_step, start_layer);
+}
+
+int cdx_cycle_lockstep_pnp(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                           float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                           float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                           const float* mask, int feature_steps, int attention_steps, int attention_start_layer, const int* feature_blocks,
+                           int n_feature_blocks) {
+  PnpLoop p;
+  p.feature_steps = feature_steps; p.attention_steps = attention_steps; p.start_layer = attention_start_layer;
+  p.blocks = feature_blocks; p.n_blocks = n_feature_blocks;
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, nullptr, nullptr, false, 0, 0, &p);
 }
 
 int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
@@ -1421,6 +1470,34 @@ int cdx_op_groupnorm_ex(cdx_engine* eh, const float* x1, int C1, const float* x2
                 reinterpret_cast<float2*>(ab_out));
       if (e.dry()) return;
       if (amax_out) CDX_CUDA(cudaMemcpyAsync(amax_out, slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
+    });
+  });
+}
+int cdx_op_groupnorm_rows(cdx_engine* eh, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta, float eps,
+                          int silu_, const float* scale, const float* shift, int ld_ss, const int* src_rows, float* y, float* amax_out,
+                          float* y_rows, float* amax_rows_out, int B, int HW, void* stream) {
+  return guard([&] {
+    CDX_CHECK(eh && x1 && gamma && beta && y && y_rows && src_rows && B > 0 && HW > 0 && C1 > 0 && C2 >= 0 && (C2 == 0) == (x2 == nullptr),
+              "op_groupnorm_rows: bad arguments");
+    CDX_CHECK(!scale == !shift && (!scale || ld_ss >= C1 + C2), "op_groupnorm_rows: scale and shift go together, with ld_ss >= C");
+    for (int b = 0; b < B; ++b) CDX_CHECK(src_rows[b] >= 0 && src_rows[b] < B, "op_groupnorm_rows: src_rows[%d] = %d outside [0, %d)", b, src_rows[b], B);
+    Engine& e = eh->e;
+    cudaStream_t s = S(stream);
+    with_arena(e, s, [&] {
+      Scope sc(e.arena);
+      e.pools_reset(s);
+      // one set of statistics for both norms (the statistics pass accumulates with atomics: two passes need not agree in the last bit)
+      const double* st1 = gn_channel_stats(e, x1, C1, B, HW, s);
+      const double* st2 = x2 ? gn_channel_stats(e, x2, C2, B, HW, s) : nullptr;
+      int* rows_dev = (int*)e.arena.alloc((size_t)B * sizeof(int));
+      if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(rows_dev, src_rows, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+      float* slot = e.amax_slot();
+      float* slot_rows = e.amax_slot();
+      groupnorm(e, x1, C1, x2, C2, gamma, beta, eps, silu_ != 0, scale, shift, ld_ss, y, B, HW, s, st1, st2, slot);
+      groupnorm(e, x1, C1, x2, C2, gamma, beta, eps, silu_ != 0, scale, shift, ld_ss, y_rows, B, HW, s, st1, st2, slot_rows, nullptr, rows_dev);
+      if (e.dry()) return;
+      if (amax_out) CDX_CUDA(cudaMemcpyAsync(amax_out, slot, sizeof(float), cudaMemcpyDeviceToDevice, s));
+      if (amax_rows_out) CDX_CUDA(cudaMemcpyAsync(amax_rows_out, slot_rows, sizeof(float), cudaMemcpyDeviceToDevice, s));
     });
   });
 }

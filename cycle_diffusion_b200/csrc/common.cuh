@@ -246,9 +246,12 @@ bool attention_tc(Engine& e, const float* q, int ldq, const float* k, int ldk, i
 // st1 / st2: per-(image, channel) fp64 {sum, sum of squares} of the sources when their producer already accumulated them
 // (stats[(b*C + c)*2 + k]); null -> computed here by one extra read.  amax: optional device scalar <- atomic max |y|.
 // ab_out: optional [B, C1+C2] table of the (a, o) the norm applies, y = silu?(x*a + o).
+// src_img: optional device [B]; image b of y is image src_img[b]'s norm (its input, statistics and scale / shift), bit for bit.
+// amax then covers the images written.  Null: every image its own.
 void groupnorm(Engine& e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta,
                float eps, bool silu, const float* scale, const float* shift, int ld_ss, float* y, int B, int HW,
-               cudaStream_t s, const double* st1 = nullptr, const double* st2 = nullptr, float* amax = nullptr, float2* ab_out = nullptr);
+               cudaStream_t s, const double* st1 = nullptr, const double* st2 = nullptr, float* amax = nullptr, float2* ab_out = nullptr,
+               const int* src_img = nullptr);
 double* gn_channel_stats(Engine& e, const float* x, int C, int B, int HW, cudaStream_t s);
 void gn_channel_stats_into(Engine& e, const float* x, int C, int B, int HW, double* stats, cudaStream_t s);   // stats += (zeroed by the caller)
 void layernorm(Engine& e, const float* x, const float* gamma, const float* beta, float* y, int M, int C, cudaStream_t s, float* amax = nullptr);

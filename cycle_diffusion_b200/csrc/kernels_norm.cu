@@ -11,6 +11,9 @@
 // every block folds the channel sums of its image into the 32 group means / rstds (fp64), y = x * sc + sh per channel (the form
 // ATen's CPU kernel uses), optional (1 + scale) / shift of the improved-DDPM scale-shift norm, optional SiLU, and it tracks
 // max |y| for the fp16-split GEMM that consumes y.
+// Row-mapped apply (src_img): the block writing image b reads image src_img[b]'s input, statistics and scale / shift, so image b
+// receives exactly image src_img[b]'s normalised activation (Plug-and-Play feature injection: the conv after the norm sees the
+// source row's operand and adds the target's own residual).  The bytes moved and the launch are the plain apply's.
 #include <algorithm>
 
 #include "tc_common.cuh"      // pdl_trigger / pdl_wait / launch_ex
@@ -84,20 +87,22 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
 
 // grid (row chunks, B); thread (tr, tc) owns channel vectors tc, tc+ncol, ... (so group / affine coefficients are hoisted out
 // of the row loop) and walks the chunk's rows 4 at a time.  Dynamic smem: float2 (sc, sh) per channel.  ab_out (optional): the
-// first row chunk of each image stores that table, ab_out[b*C + c] = (a, o) with y = silu?(x * a + o).
+// first row chunk of each image stores that table, ab_out[b*C + c] = (a, o) with y = silu?(x * a + o).  src_img (optional,
+// device [B]): image b is written from image src_img[b]'s input, statistics and scale / shift (the file header's row-mapped apply).
 __global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, const float* x2, int C2,
                                                        const float* gamma, const float* beta,
                                                        const double* st1, const double* st2, double inv_count,
                                                        float eps, int silu,
                                                        const float* scale, const float* shift,
                                                        int ld_ss, float* y, int HW, int rows_per_chunk, float* amax,
-                                                       float2* ab_out) {
+                                                       float2* ab_out, const int* src_img) {
   tc::pdl_trigger();
   tc::pdl_wait();
   const int C = C1 + C2;
   const int cpg = C / GN_GROUPS;
   const int C4 = C >> 2;
-  const int b = blockIdx.y;
+  const int bo = blockIdx.y;                                            // the image written
+  const int b = src_img ? __ldcg(src_img + bo) : bo;                    // the image read (coherent: after the dependent-launch wait)
   const int r0 = blockIdx.x * rows_per_chunk;
   const int r1 = min(HW, r0 + rows_per_chunk);
   const int ncol = min(C4, (int)blockDim.x);
@@ -140,7 +145,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, 
   }
   __syncthreads();
   if (ab_out && blockIdx.x == 0)
-    for (int c = threadIdx.x; c < C; c += blockDim.x) ab_out[(long long)b * C + c] = s_aff[c];
+    for (int c = threadIdx.x; c < C; c += blockDim.x) ab_out[(long long)bo * C + c] = s_aff[c];
   float vmax = 0.f;
   if (tr < nrow_par) {
     for (int c4 = tc; c4 < C4; c4 += ncol) {
@@ -148,7 +153,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const float* x1, int C1, 
       const float2 a0 = s_aff[c], a1 = s_aff[c + 1], a2 = s_aff[c + 2], a3 = s_aff[c + 3];
       const float* src = (c < C1) ? (x1 + (long long)b * HW * C1 + c) : (x2 + (long long)b * HW * C2 + (c - C1));
       const int ldx = (c < C1) ? C1 : C2;
-      float* dst = y + (long long)b * HW * C + c;
+      float* dst = y + (long long)bo * HW * C + c;
       auto act = [&](float4 v) {
         float t[4] = {fmaf(v.x, a0.x, a0.y), fmaf(v.y, a1.x, a1.y), fmaf(v.z, a2.x, a2.y), fmaf(v.w, a3.x, a3.y)};
         if (silu) {
@@ -294,7 +299,7 @@ void gn_channel_stats_into(Engine& e, const float* x, int C, int B, int HW, doub
 
 void groupnorm(Engine& e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta, float eps,
                bool silu, const float* scale, const float* shift, int ld_ss, float* y, int B, int HW, cudaStream_t s,
-               const double* st1, const double* st2, float* amax, float2* ab_out) {
+               const double* st1, const double* st2, float* amax, float2* ab_out, const int* src_img) {
   const int C = C1 + C2;
   CDX_CHECK(C % GN_GROUPS == 0, "groupnorm: C=%d not divisible by 32", C);
   CDX_CHECK(C1 % 4 == 0 && C2 % 4 == 0, "groupnorm: channel counts must be multiples of 4 (C1=%d C2=%d)", C1, C2);
@@ -307,7 +312,7 @@ void groupnorm(Engine& e, const float* x1, int C1, const float* x2, int C2, cons
   const int arows = cdiv(HW, achunk);
   achunk = cdiv(HW, arows);
   tc::launch_ex(gn_apply_kernel, dim3((unsigned)achunk, (unsigned)B), dim3(256), (size_t)C * sizeof(float2), s, 1, x1, C1, x2, C2, gamma, beta, st1, st2,
-                1.0 / ((double)HW * (C / GN_GROUPS)), eps, silu ? 1 : 0, scale, shift, ld_ss, y, HW, arows, amax, ab_out);
+                1.0 / ((double)HW * (C / GN_GROUPS)), eps, silu ? 1 : 0, scale, shift, ld_ss, y, HW, arows, amax, ab_out, src_img);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
 }

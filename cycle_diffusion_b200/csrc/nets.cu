@@ -630,13 +630,14 @@ struct Exec {
     return y;
   }
 
+  // src_img (optional device [B]): image b of the result is image src_img[b]'s norm (groupnorm)
   Tensor gn(const Tensor& x, const Tensor* x2, const std::string& name, float eps, bool act, const float* scale = nullptr,
-            const float* shift = nullptr, int ld_ss = 0) {
+            const float* shift = nullptr, int ld_ss = 0, const int* src_img = nullptr) {
     const int C = x.C + (x2 ? x2->C : 0);
     Tensor y = alloc(x.B, x.H, x.W, C);
     y.amax = e.amax_slot();
     groupnorm(e, x.p, x.C, x2 ? x2->p : nullptr, x2 ? x2->C : 0, n.P(name + ".weight"), n.P(name + ".bias"), eps, act, scale, shift, ld_ss,
-              y.p, x.B, x.H * x.W, s, x.stats, x2 ? x2->stats : nullptr, y.amax);
+              y.p, x.B, x.H * x.W, s, x.stats, x2 ? x2->stats : nullptr, y.amax, nullptr, src_img);
     return y;
   }
   Tensor ln(const Tensor& x, const std::string& name) {
@@ -651,8 +652,8 @@ struct Exec {
   // both sources and writes the normalised concat, which the conv then reads as its one source.  `into` (optional): preallocated output.
   Tensor gn_silu_conv3(const Tensor& x, const Tensor* x2, const std::string& norm, float eps, const std::string& conv, const float* scale = nullptr,
                        const float* shift = nullptr, int ld_ss = 0, const float* rowvec = nullptr, int ld_rowvec = 0, const float* residual = nullptr,
-                       Tensor* into = nullptr, float* out_nchw = nullptr) {
-    const Tensor h = gn(x, x2, norm, eps, true, scale, shift, ld_ss);
+                       Tensor* into = nullptr, float* out_nchw = nullptr, const int* src_img = nullptr) {
+    const Tensor h = gn(x, x2, norm, eps, true, scale, shift, ld_ss, src_img);
     return conv3(h, conv, 1, 1, 1, rowvec, ld_rowvec, residual, out_nchw, into);
   }
 
@@ -742,8 +743,17 @@ struct UNetExec : Exec {
   bool oai;
   UNetExec(Net& net, cudaStream_t st) : Exec(net, st), oai(net.kind == NET_UNET_OPENAI) {}
 
-  // ResBlock (OAI:255-275 / IU:241-261).  updown: 0 none, 1 down (avg-pool), 2 up (nearest)
-  Tensor resblock(const Tensor& x, const Tensor* x2, const std::string& p, int updown = 0) {
+  // Plug-and-Play: the row table of output block k's ResBlock in this call, or null when it is not controlled
+  const int* feature_row(int k) const {
+    if (!ctl || !ctl->pnp_feat) return nullptr;
+    for (int i = 0; i < ctl->n_feat; ++i)
+      if (ctl->feat_blocks[i] == k) return ctl->pnp_row;
+    return nullptr;
+  }
+
+  // ResBlock (OAI:255-275 / IU:241-261).  updown: 0 none, 1 down (avg-pool), 2 up (nearest).  feat_row (optional device [B],
+  // Plug-and-Play feature injection): row r's out_layers run on row feat_row[r]'s in_layers output; the skip stays row r's own
+  Tensor resblock(const Tensor& x, const Tensor* x2, const std::string& p, int updown = 0, const int* feat_row = nullptr) {
     const int Cout = n.dim0(p + ".in_layers.2.weight");
     const int eoff = n.emb_off.at(p);
     const int oH = updown == 1 ? x.H / 2 : (updown == 2 ? x.H * 2 : x.H);
@@ -784,8 +794,10 @@ struct UNetExec : Exec {
       residual = xs.p;
     }
     // out_layers: GroupNorm (i-DDPM: scale-shift norm, IU:253-257) + SiLU + conv3x3 + residual, written into `out`
-    if (oai) gn_silu_conv3(h2, nullptr, p + ".out_layers.0", 1e-5f, p + ".out_layers.3", nullptr, nullptr, 0, nullptr, 0, residual, &out);
-    else gn_silu_conv3(h2, nullptr, p + ".out_layers.0", 1e-5f, p + ".out_layers.3", E + eoff, E + eoff + Cout, n.emb_rows, nullptr, 0, residual, &out);
+    if (oai) gn_silu_conv3(h2, nullptr, p + ".out_layers.0", 1e-5f, p + ".out_layers.3", nullptr, nullptr, 0, nullptr, 0, residual, &out, nullptr,
+                           feat_row);
+    else gn_silu_conv3(h2, nullptr, p + ".out_layers.0", 1e-5f, p + ".out_layers.3", E + eoff, E + eoff + Cout, n.emb_rows, nullptr, 0, residual, &out,
+                       nullptr, feat_row);
     return out;
   }
 
@@ -807,7 +819,10 @@ struct UNetExec : Exec {
       a.amax = e.amax_slot();                   // <- max |V| (written by whichever projection produces V)
       bool done = false;
       const bool flash_ok = flash_eligible(e, HW, HW, d, C);
-      const int* srow = (ctl && ctl->self && HW <= ctl->self_max_tokens) ? ctl->qk_row : nullptr;
+      // Prompt-to-Prompt, or Plug-and-Play on layers >= pnp_layer: the controlled rows take their source rows' queries and keys
+      const int* srow = (ctl && ctl->self && HW <= ctl->self_max_tokens)        ? ctl->qk_row
+                        : (ctl && ctl->pnp_attn && st_layer >= ctl->pnp_layer) ? ctl->pnp_row
+                                                                              : nullptr;
       // mutual self-attention: the controlled rows' queries over their source rows' keys and values
       const int* mrow = (ctl && ctl->mutual && st_layer >= ctl->start_layer) ? ctl->kv_row : nullptr;
       ++st_layer;
@@ -1201,7 +1216,7 @@ struct UNetExec : Exec {
         const Tensor skip = hs.back();
         hs.pop_back();
         const std::string bp = S("output_blocks.", bo);
-        h = resblock(h, &skip, bp + ".0");
+        h = resblock(h, &skip, bp + ".0", 0, feature_row(bo));
         int li = 1;
         if (contains(c.attention_ds, c.n_attn, ds)) { h = attn_layer(h, bp + "." + std::to_string(li)); ++li; }
         if (level && i == c.num_res_blocks) {
@@ -1290,9 +1305,10 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
   CDX_CHECK(H % down == 0 && W % down == 0, "unet_forward: %dx%d not divisible by %d", H, W, down);
   UNetExec ex(n, s);
   ex.kv_reuse = reuse_ctx && n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0;
-  CDX_CHECK(!ctl || (!ctl->qk_row && !ctl->kv_row) || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0),
+  CDX_CHECK(!ctl || (!ctl->qk_row && !ctl->kv_row && !ctl->pnp_row) || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0),
             "attention control: SD / LDM U-Nets with a context only");
-  CDX_CHECK(!ctl || !ctl->qk_row || !ctl->kv_row, "attention control: Prompt-to-Prompt and mutual self-attention in one call");
+  CDX_CHECK(!ctl || (!!ctl->qk_row + !!ctl->kv_row + !!ctl->pnp_row) <= 1,
+            "attention control: Prompt-to-Prompt, mutual self-attention and Plug-and-Play are exclusive in one call");
   ex.ctl = ctl;
   if (n.kind == NET_UNET_DDPM) { ex.forward_ddpm(x_nchw, t_dev, out_nchw, B, H, W); return; }
   ex.forward(x_nchw, t_dev, ctx, ctx_len, out_nchw, B, H, W);

@@ -105,6 +105,16 @@ struct AttnControl {
   const int* kv_row = nullptr;          // device [B]
   bool mutual = false;                  // control the self-attention layers >= start_layer in this call
   int start_layer = 0;
+  // Plug-and-Play (Tumanyan et al., 2023; exclusive with qk_row and kv_row).  With `pnp_feat`, the ResBlock output_blocks.k.0 of
+  // each k in feat_blocks normalises row pnp_row[r]'s out_layers input on row r (so its conv adds row r's own skip to row
+  // pnp_row[r]'s out_layers); with `pnp_attn`, the self-attention of every SpatialTransformer whose index in forward order is
+  // >= pnp_layer takes row r's Q and K from row pnp_row[r] and keeps its own V
+  const int* pnp_row = nullptr;         // device [B]
+  bool pnp_feat = false;                // control the ResBlocks of feat_blocks in this call
+  const int* feat_blocks = nullptr;     // host [n_feat]: output-block indices
+  int n_feat = 0;
+  bool pnp_attn = false;                // control the self-attention layers >= pnp_layer in this call
+  int pnp_layer = 0;
 };
 
 // forward executors (enqueue only; caller handles arena dry-run)

@@ -12,7 +12,7 @@ import torch
 
 from . import _cabi
 from ._cabi import lib, check, UnetConfig, VaeConfig, TextConfig, DdimCoef, PixelCoef
-from .attn_control import MutualSelfControl
+from .attn_control import MutualSelfControl, PnPControl
 
 
 def _ptr(t):
@@ -309,11 +309,7 @@ class Engine:
         check(lib.cdx_op_layernorm(self.h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(y), M, Cc, self.stream))
         return y
 
-    def op_groupnorm_ex(self, x1, x2, gamma, beta, eps, silu, scale=None, shift=None):
-        """GroupNorm(32) of the channel concat [x1 | x2] (NHWC [B,H,W,C1], [B,H,W,C2] or None) as the network executors run it,
-        optional gn(x) * (1 + scale) + shift and SiLU.  scale / shift: [B, C] device views with unit column stride and one common
-        row stride (e.g. the two halves of a [B, 2C] embedding projection).  Returns (y, amax, ab): y [B,H,W,C], amax [1] the
-        tracked range slot of y, ab [B, C, 2] the (a, o) table the norm applies, y = silu?(x * a + o)."""
+    def _gn_operands(self, x1, x2, gamma, beta, scale, shift):
         x1, gamma, beta = (_f32c(t, self.device) for t in (x1, gamma, beta))
         B, H, W, C1 = x1.shape
         x2 = _f32c(x2, self.device) if x2 is not None else None
@@ -325,12 +321,33 @@ class Engine:
                 assert t.dtype == torch.float32 and t.device == self.device and tuple(t.shape) == (B, C1 + C2) and t.stride(1) == 1
             assert scale.stride(0) == shift.stride(0), 'scale and shift share one row stride'
             ld_ss = scale.stride(0)
+        return x1, x2, gamma, beta, B, H, W, C1, C2, ld_ss
+
+    def op_groupnorm_ex(self, x1, x2, gamma, beta, eps, silu, scale=None, shift=None):
+        """GroupNorm(32) of the channel concat [x1 | x2] (NHWC [B,H,W,C1], [B,H,W,C2] or None) as the network executors run it,
+        optional gn(x) * (1 + scale) + shift and SiLU.  scale / shift: [B, C] device views with unit column stride and one common
+        row stride (e.g. the two halves of a [B, 2C] embedding projection).  Returns (y, amax, ab): y [B,H,W,C], amax [1] the
+        tracked range slot of y, ab [B, C, 2] the (a, o) table the norm applies, y = silu?(x * a + o)."""
+        x1, x2, gamma, beta, B, H, W, C1, C2, ld_ss = self._gn_operands(x1, x2, gamma, beta, scale, shift)
         y = self.empty(B, H, W, C1 + C2)
         amax = torch.zeros(1, dtype=torch.float32, device=self.device)
         ab = self.empty(B, C1 + C2, 2)
         check(lib.cdx_op_groupnorm_ex(self.h, _ptr(x1), C1, _ptr(x2), C2, _ptr(gamma), _ptr(beta), eps, int(silu), _ptr(scale), _ptr(shift),
                                       ld_ss, _ptr(y), _ptr(amax), _ptr(ab), B, H * W, self.stream))
         return y, amax, ab
+
+    def op_groupnorm_rows(self, x1, x2, gamma, beta, eps, silu, src_rows, scale=None, shift=None):
+        """op_groupnorm_ex's norm twice from one set of statistics (cdx_op_groupnorm_rows): plain, and with the row table src_rows
+        ([B] ints), image b of the second being image src_rows[b]'s norm.  Returns (y, amax, y_rows, amax_rows), amax / amax_rows [1]
+        the tracked range slots."""
+        x1, x2, gamma, beta, B, H, W, C1, C2, ld_ss = self._gn_operands(x1, x2, gamma, beta, scale, shift)
+        rows = [int(r) for r in src_rows]
+        assert len(rows) == B, f'src_rows: {len(rows)} entries for {B} images'
+        y, y_rows = self.empty(B, H, W, C1 + C2), self.empty(B, H, W, C1 + C2)
+        amax, amax_rows = (torch.zeros(1, dtype=torch.float32, device=self.device) for _ in range(2))
+        check(lib.cdx_op_groupnorm_rows(self.h, _ptr(x1), C1, _ptr(x2), C2, _ptr(gamma), _ptr(beta), eps, int(silu), _ptr(scale), _ptr(shift),
+                                        ld_ss, (C.c_int * B)(*rows), _ptr(y), _ptr(amax), _ptr(y_rows), _ptr(amax_rows), B, H * W, self.stream))
+        return y, amax, y_rows, amax_rows
 
     def op_layernorm_ex(self, x, gamma, beta):
         """LayerNorm over the last dim of x [M, C] (eps 1e-5) -> (y, amax [1] the tracked range slot of y)."""
@@ -770,8 +787,9 @@ class UNet(Net):
         target chain is blended with the source chain's x_{t-1} after every step; ones give the unmasked result, zeros give x0.
         attn_control: an attn_control.AttentionControl, Prompt-to-Prompt's "replace" edit on the target chain's cond row
         (cdx_cycle_lockstep_ctl), or its "refine" edit when the control has an own_weight (cdx_cycle_lockstep_refine); or an
-        attn_control.MutualSelfControl, MasaCtrl's mutual self-attention on the target chain's rows (cdx_cycle_lockstep_mutual).
-        Each composes with mask."""
+        attn_control.MutualSelfControl, MasaCtrl's mutual self-attention on the target chain's rows (cdx_cycle_lockstep_mutual); or
+        an attn_control.PnPControl, Plug-and-Play's feature and self-attention injection on the target chain's rows
+        (cdx_cycle_lockstep_pnp).  Each composes with mask."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -780,8 +798,8 @@ class UNet(Net):
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
         mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
-        mutual = isinstance(attn_control, MutualSelfControl)
-        ctl, _token_map, own = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None and not mutual \
+        mutual, pnp = isinstance(attn_control, MutualSelfControl), isinstance(attn_control, PnPControl)
+        ctl, _token_map, own = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None and not (mutual or pnp) \
             else (None, None, None)
         out = e.empty(B, Cc, h, w)
         z = e.empty(B, n + 1, Cc, h, w) if return_z else None
@@ -789,6 +807,11 @@ class UNet(Net):
                 sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask))
         if mutual:
             check(lib.cdx_cycle_lockstep_mutual(*args, attn_control.start_step, attn_control.start_layer))
+            return (out, z) if return_z else out
+        if pnp:
+            blocks = attn_control.feature_blocks
+            check(lib.cdx_cycle_lockstep_pnp(*args, *attn_control.steps(n), attn_control.attention_start_layer,
+                                             (C.c_int * max(len(blocks), 1))(*blocks), len(blocks)))
             return (out, z) if return_z else out
         args += (C.byref(ctl) if ctl is not None else None,)
         if own is None:

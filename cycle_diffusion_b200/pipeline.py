@@ -14,7 +14,7 @@ from dataclasses import dataclass
 
 import torch
 
-from .attn_control import AttentionControl, MutualSelfControl
+from .attn_control import AttentionControl, MutualSelfControl, PnPControl
 from .engine import check_mask
 from .schedule import DDIMSchedule
 
@@ -96,11 +96,12 @@ class CycleDiffusionPipeline:
 
     P2P_KEYS = {'edit_type', 'cross_replace_steps', 'self_replace_steps', 'self_replace_max_tokens', 'token_map', 'equalizer'}
     MUTUAL_KEYS = {'edit_type', 'start_step', 'start_layer'}
+    PNP_KEYS = {'edit_type', 'feature_steps', 'attention_steps', 'feature_blocks', 'attention_start_layer'}
 
     @classmethod
     def _attn_control(cls, kw, source_guidance_scale, two_phase):
-        """cross_attention_kwargs -> AttentionControl, MutualSelfControl or None (no 'edit_type'); ValueError for what the engine
-        cannot do."""
+        """cross_attention_kwargs -> AttentionControl, MutualSelfControl, PnPControl or None (no 'edit_type'); ValueError for what
+        the engine cannot do."""
         if not kw or 'edit_type' not in kw:
             return None
         kind = kw['edit_type']
@@ -116,8 +117,19 @@ class CycleDiffusionPipeline:
                 return MutualSelfControl(kw.get('start_step', 4), kw.get('start_layer', 10))
             except ValueError as err:
                 raise ValueError(f'cross_attention_kwargs: {err}') from None
+        if kind == 'pnp':
+            extra = set(kw) - cls.PNP_KEYS
+            if extra:
+                raise ValueError(f"cross_attention_kwargs: keys {sorted(extra)} do not apply to edit_type='pnp' (it takes feature_steps, "
+                                 f"attention_steps, feature_blocks and attention_start_layer)")
+            if two_phase:
+                raise ValueError('Plug-and-Play needs the lock-step loop: the source chain does not run during the decode (two_phase=False)')
+            try:
+                return PnPControl(**{k: v for k, v in kw.items() if k != 'edit_type'})
+            except ValueError as err:
+                raise ValueError(f'cross_attention_kwargs: {err}') from None
         if kind not in ('replace', 'reweight', 'refine'):
-            raise ValueError(f"edit_type must be 'replace', 'reweight', 'refine' or 'mutual_self', got {kind!r}")
+            raise ValueError(f"edit_type must be 'replace', 'reweight', 'refine', 'mutual_self' or 'pnp', got {kind!r}")
         extra = set(kw) - cls.P2P_KEYS
         if extra:
             raise ValueError(f'cross_attention_kwargs: unsupported keys {sorted(extra)} (LocalBlend: use mask_image)')
@@ -182,7 +194,14 @@ class CycleDiffusionPipeline:
         instead, for non-rigid edits (a pose or a layout change): from loop step start_step on, in the SpatialTransformers from
         index start_layer on (16 in SD v1 / 2.x; the defaults control the decoder's two finest levels), the target rows keep their
         own queries and attend over the source rows' keys and values (attn_control.MutualSelfControl).  Prompt-to-Prompt keys,
-        other keys and two_phase=True raise ValueError; it composes with mask_image."""
+        other keys and two_phase=True raise ValueError; it composes with mask_image.
+        {'edit_type': 'pnp', ['feature_steps': 0.8], ['attention_steps': 0.5], ['feature_blocks': (4,)], ['attention_start_layer': 8]}:
+        Plug-and-Play diffusion features (Tumanyan et al., 2023) instead, for structure-preserving text-guided translation: in the
+        first feature_steps of the loop's steps the ResBlocks of the output blocks feature_blocks give the target rows the source
+        row's features (out_layers of its in_layers output, on the target's own skip), and in the first attention_steps the
+        SpatialTransformers from index attention_start_layer on give them the source row's self-attention queries and keys
+        (attn_control.PnPControl).  source_prompt="" with source_guidance_scale=0 reproduces PnP's unconditional source branch.
+        Other keys, values out of range and two_phase=True raise ValueError; it composes with mask_image."""
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')

@@ -384,7 +384,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         mask: optional [B,1,R,R] in [0,1] at image resolution, 1 = may change (masked editing): pooled to the latent grid, and
         outside it the translated latent stays on the source image's chain (cdx_cycle_lockstep_masked).
         attn_control: optional attn_control.AttentionControl, Prompt-to-Prompt's "replace" edit, or its "refine" edit when the
-        control has an own_weight; or attn_control.MutualSelfControl, MasaCtrl's mutual self-attention (UNet.cycle_lockstep)."""
+        control has an own_weight; attn_control.MutualSelfControl, MasaCtrl's mutual self-attention; or attn_control.PnPControl,
+        Plug-and-Play's feature and self-attention injection (UNet.cycle_lockstep)."""
         assert self.single_member(), 'cycle(): single-member ensembles only (use encode() + forward())'
         with self._precision_scope():
             return self._cycle(image, encode_text, decode_text, mask, attn_control)

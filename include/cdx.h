@@ -369,6 +369,33 @@ int cdx_cycle_lockstep_mutual(cdx_net* unet, const float* x0, const float* c_src
                               const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                               float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                               void* stream, const float* mask, int start_step, int start_layer);
+/* Plug-and-Play diffusion features (PnP, Tumanyan et al., 2023) on the lock-step loop: cdx_cycle_lockstep_masked (mask may be NULL)
+ * where the target chain's rows take the source chain's decoder ResBlock features and self-attention queries and keys, so the real
+ * image's spatial layout is kept while the target prompt sets its appearance.  The source row runs in the same U-Net call at the
+ * same timestep, so no feature cache or separate inversion pass is needed.  Rows are mapped as cdx_cycle_lockstep_mutual maps them:
+ * for sample b the target's cond row r reads the source chain's cond row s, and the target's uncond row (present when tgt_scale is
+ * neither 0 nor 1) reads the source's uncond row, or the source's only row when it has no uncond row.  src_scale 0 is allowed: the
+ * source's only row is then its uncond row, PnP's own unconditional source branch.  At loop step i (0-based, of n_steps):
+ *   - i < feature_steps, for each k of feature_blocks[0 .. n_feature_blocks) (host ints, indices of the net's output blocks): the
+ *     ResBlock output_blocks.k.0 gives row r  skip_r + out_layers(h_s), skip_r row r's own skip path (identity or skip_connection)
+ *     and h_s row s's in_layers output plus its embedding, out_layers(h) = conv3x3(SiLU(GroupNorm(h))).  The GroupNorm before the
+ *     conv writes row r from row s's input and statistics, so the conv reads row s's operand and adds its bias and row r's skip in
+ *     its epilogue: no launch or byte is added, and the norm's range slot stays the max over what it wrote.
+ *   - i < attention_steps, in the self-attention of every SpatialTransformer whose index in forward order (16 in SD v1 / 2.x and the
+ *     LDM text2img net: input 0-5, middle 6, output 7-15) is >= attention_start_layer: row r computes softmax(Q_s K_s^T * scale) . V_r,
+ *     the fused attention kernel reading row s's Q and K tiles (as Prompt-to-Prompt's self-attention control does).
+ * Cross-attention and the source rows run unchanged.  PnP's defaults are feature_steps = int(0.8 n), attention_steps = int(0.5 n),
+ * feature_blocks = {4} (up_blocks[1].resnets[1]) and attention_start_layer = 8 (up_blocks[1].attentions[1]).
+ * feature_steps = attention_steps = 0, or n_feature_blocks = 0 with attention_start_layer >= the net's layer count, gives
+ * cdx_cycle_lockstep_masked's result bit for bit.  CDX_E_INVALID: negative values or step counts above n_steps, a block index
+ * outside the net's output blocks or given twice, nets without SpatialTransformers or a context, and mma modes 0 and 2 (and mode 3
+ * at head width 160) on a controlled attention layer. */
+int cdx_cycle_lockstep_pnp(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                           int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                           const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                           void* stream, const float* mask, int feature_steps, int attention_steps,
+                           int attention_start_layer, const int* feature_blocks, int n_feature_blocks);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -576,6 +603,12 @@ int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, i
 int cdx_op_groupnorm_ex(cdx_engine* e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta,
                         float eps, int silu, const float* scale, const float* shift, int ld_ss, float* y, float* amax_out,
                         float* ab_out, int B, int HW, void* stream);
+/* cdx_op_groupnorm_rows: cdx_op_groupnorm_ex's norm twice from ONE set of statistics: y [B,HW,C] plain, and y_rows [B,HW,C] with a
+ *   row table (src_rows: host [B], each in [0, B)), image b of y_rows being image src_rows[b]'s norm -- bit for bit y[src_rows[b]].
+ *   amax_out / amax_rows_out (optional, device floats): the tracked range slots of y and y_rows. */
+int cdx_op_groupnorm_rows(cdx_engine* e, const float* x1, int C1, const float* x2, int C2, const float* gamma, const float* beta,
+                          float eps, int silu, const float* scale, const float* shift, int ld_ss, const int* src_rows, float* y,
+                          float* amax_out, float* y_rows, float* amax_rows_out, int B, int HW, void* stream);
 int cdx_op_layernorm_ex(cdx_engine* e, const float* x, const float* gamma, const float* beta, float* y, float* amax_out, int M,
                         int C, void* stream);
 int cdx_op_softmax_rows(cdx_engine* e, float* x, int64_t rows, int L, int ld, int causal_nq, void* stream);

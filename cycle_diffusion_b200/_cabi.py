@@ -81,7 +81,19 @@ class LatentChainsDesc(C.Structure):
                 ('x0', _P), ('eout', _P), ('c', DdimCoef), ('noise0', _P), ('sa', C.c_float), ('s1', C.c_float), ('xt', _P), ('xn', _P),
                 ('next', C.c_int), ('noise_next', _P), ('cnext', DdimCoef), ('xn2', _P), ('z_out', _P), ('z_stride', C.c_int64),
                 ('eps_in', _P), ('eps_stride', C.c_int64), ('yt', _P), ('y_out', _P), ('xin', _P), ('pred', C.c_int), ('vsa', C.c_float),
-                ('vs1', C.c_float), ('mask', _P), ('hw', C.c_int)]
+                ('vs1', C.c_float), ('mask', _P), ('hw', C.c_int),
+                ('sg_m', C.c_int), ('sg_rows', C.POINTER(C.c_int)), ('sg_thr', _P), ('sg_nu', _P), ('sg_scale', C.c_float * 8),
+                ('sg_lambda', C.c_float * 8), ('sg_active', C.c_uint), ('sg_apply', C.c_int), ('sg_mu', C.c_float), ('sg_beta', C.c_float),
+                ('sg_beta1', C.c_float)]
+
+
+CDX_SEMANTIC_MAX = 8
+
+
+class SemanticGuidanceC(C.Structure):
+    _fields_ = [('m', C.c_int), ('scale', C.c_float * CDX_SEMANTIC_MAX), ('threshold', C.c_float * CDX_SEMANTIC_MAX),
+                ('cooldown', C.c_int * CDX_SEMANTIC_MAX), ('warmup', C.c_int), ('momentum_scale', C.c_float), ('beta', C.c_float),
+                ('beta1', C.c_float)]
 
 
 _F = C.c_float
@@ -144,6 +156,8 @@ SIGNATURES = {
                                        _I, _I, _P, _P, _I, _I]),
     'cdx_cycle_lockstep_pnp': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
                                     _I, _I, _P, _P, _I, _I, _I, C.POINTER(_I), _I]),
+    'cdx_cycle_lockstep_semantic': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
+                                         _I, _I, _P, _P, _P, C.POINTER(SemanticGuidanceC)]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),

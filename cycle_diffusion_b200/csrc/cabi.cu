@@ -183,6 +183,9 @@ struct ChainLoopArgs {
   // optional, exclusive with ctl: mutual self-attention (cdx.h, cdx_cycle_lockstep_mutual) at steps >= start_step, layers >= start_layer
   bool mutual = false; int start_step = 0, start_layer = 0;
   const PnpLoop* pnp = nullptr;                     // optional, exclusive with ctl and mutual: Plug-and-Play
+  // optional, exclusive with ctl, mutual and pnp: semantic guidance (cdx.h, cdx_cycle_lockstep_semantic), concept contexts
+  // c_edit [n_src, m, L, D]: every target chain of group j runs concept k under c_edit[j, k]
+  const cdx_semantic_guidance* sega = nullptr; const float* c_edit = nullptr;
   int C = 0, h = 0, w = 0;
 };
 
@@ -216,20 +219,36 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   const int chw = a.C * a.h * a.w, n_tgt_chains = a.n_src * a.K;
   const size_t n = (size_t)a.n_src * chw;
   const size_t ctx_n = (size_t)a.L * unet.ucfg.context_dim;
+  if (a.sega) {
+    const cdx_semantic_guidance& g = *a.sega;
+    CDX_CHECK(!a.ctl && !a.mutual && !a.pnp, "semantic guidance and attention control are exclusive in one loop");
+    CDX_CHECK(a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net && !a.scales_on_device,
+              "semantic guidance: needs the lock-step loop with a source chain at every step");
+    CDX_CHECK(ctx_n > 0 && a.c_tgt && a.c_edit, "semantic guidance: needs a net with a context and the concept contexts");
+    CDX_CHECK(a.uc, "semantic guidance: needs the unconditional context (its terms are taken against the uncond row)");
+    CDX_CHECK(g.m >= 1 && g.m <= SEMANTIC_MAX_CONCEPTS, "semantic guidance: m=%d concepts, 1 to %d", g.m, SEMANTIC_MAX_CONCEPTS);
+    for (int k = 0; k < g.m; ++k)
+      CDX_CHECK(g.threshold[k] >= 0.0f && g.threshold[k] < 1.0f, "semantic guidance: threshold[%d]=%g outside [0, 1)", k, g.threshold[k]);
+  }
   // the chain table: all source-chain rows first, then all target-chain rows (the two-model loop runs the two blocks under two
   // nets); inside a block the uncond rows come first, cat([uc, c]) as ddim.py:555-557
   std::vector<Chain> ch((size_t)a.n_src + n_tgt_chains, Chain{-1, -1, 1.f});
   int rows = 0;
-  auto place = [&](Chain* c, int count, const float* scales) {
+  // need_uc: the chains need their uncond row's output even at scale 1 (semantic guidance forms its terms against it)
+  auto place = [&](Chain* c, int count, const float* scales, bool need_uc) {
     for (int k = 0; k < count; ++k) {
       if (!a.scales_on_device && scales) c[k].scale = scales[k];
-      if (a.uc && (a.scales_on_device || (c[k].scale != 0.0f && c[k].scale != 1.0f))) c[k].row2 = rows++;
+      if (a.uc && (a.scales_on_device || (c[k].scale != 0.0f && (c[k].scale != 1.0f || need_uc)))) c[k].row2 = rows++;
     }
     for (int k = 0; k < count; ++k) c[k].row = rows++;
   };
-  if (a.src) place(ch.data(), a.n_src, a.s_scales);
+  if (a.src) place(ch.data(), a.n_src, a.s_scales, false);
   const int rows_src = rows;
-  place(ch.data() + a.n_src, n_tgt_chains, a.t_scales);
+  place(ch.data() + a.n_src, n_tgt_chains, a.t_scales, a.sega != nullptr);
+  // semantic guidance: the m concept rows of every target chain after the whole target block, chain-major, so that no other row moves
+  const int sg_m = a.sega ? a.sega->m : 0;
+  std::vector<int> sg_rows((size_t)n_tgt_chains * sg_m);
+  for (int& r : sg_rows) r = rows++;
   const int loop_steps = a.K ? a.n_steps : a.n_rec;
   CDX_CHECK(!tgt_net || (!unet.pred && !tgt_net->pred), "two-model latent loop: eps-prediction U-Nets only");
   // a masked target chain takes its source chain's x_{t-1} outside the mask, so every step needs one
@@ -301,6 +320,21 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     for (int j = 0; j < a.n_src; ++j) {
       if (a.src) ctx_rows(ch[j], a.c_src, j);
       for (int k = 0; k < a.K; ++k) ctx_rows(ch[a.n_src + (size_t)j * a.K + k], a.c_tgt, j);
+    }
+    for (int t = 0; t < n_tgt_chains; ++t)
+      for (int q = 0; q < sg_m; ++q)
+        copy_dd(e, a.c_edit + ((size_t)(t / a.K) * sg_m + q) * ctx_n, ctx_in + (size_t)sg_rows[(size_t)t * sg_m + q] * ctx_n, ctx_n, s);
+  }
+  // semantic guidance: the concept row table, the thresholds of the step and the momentum of every target chain, fixed for the loop
+  int* sg_rows_dev = nullptr;
+  float *sg_thr = nullptr, *sg_nu = nullptr;
+  if (sg_m) {
+    sg_rows_dev = (int*)e.arena.alloc(sg_rows.size() * sizeof(int));
+    sg_thr = (float*)e.arena.alloc(sg_rows.size() * a.C * sizeof(float));
+    sg_nu = (float*)e.arena.alloc((size_t)n_tgt_chains * chw * sizeof(float));
+    if (!e.dry()) {
+      CDX_CUDA(cudaMemcpyAsync(sg_rows_dev, sg_rows.data(), sg_rows.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+      CDX_CUDA(cudaMemsetAsync(sg_nu, 0, (size_t)n_tgt_chains * chw * sizeof(float), s));
     }
   }
   // attention control: the row table maps each target chain's cond row to its group's source row (every other row to itself); with
@@ -397,6 +431,12 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   LatentChains f;
   f.n = n; f.chw = chw; f.n_src = a.n_src; f.K = a.K; f.chains = chd; f.x0 = a.x0; f.xin = xin; f.mask = a.mask; f.hw = a.h * a.w;
   f.z_stride = (long long)(a.n_rec + 1) * chw;
+  if (sg_m) {
+    const cdx_semantic_guidance& g = *a.sega;
+    f.sg_m = sg_m; f.sg_rows = sg_rows_dev; f.sg_thr = sg_thr; f.sg_nu = sg_nu;
+    for (int q = 0; q < sg_m; ++q) { f.sg_scale[q] = g.scale[q]; f.sg_lambda[q] = g.threshold[q]; }
+    f.sg_mu = g.momentum_scale; f.sg_beta = g.beta; f.sg_beta1 = g.beta1;
+  }
   {
     LatentChains in = f;
     in.src = a.src;
@@ -417,8 +457,12 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.mutual = a.mutual && i >= a.start_step;
       actl.pnp_feat = a.pnp && i < a.pnp->feature_steps;
       actl.pnp_attn = a.pnp && i < a.pnp->attention_steps;
+      const size_t stat0 = e.stat_dry;
       unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true,
                    a.ctl || a.mutual || a.pnp ? &actl : nullptr);
+      CDX_CHECK(!sg_m || !e.dry() || e.stat_dry - stat0 <= e.stat_cap,
+                "semantic guidance: a %d-row U-Net call needs %zu GroupNorm statistics doubles, the pool holds %zu: fewer images or concepts",
+                rows, e.stat_dry - stat0, e.stat_cap);
     } else {
       ps.fork();
       if (src_i) unet_forward(unet, xin, tdev + (size_t)i * rows, nullptr, 0, eout, rows_src, a.h, a.w, s);
@@ -440,6 +484,11 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     }
     st.yt = yb[0]; st.y_out = (i == loop_steps - 1) ? a.x_out : yb[1];
     set_v(unet, a.t_host[i], st);
+    if (sg_m) {                                   // this step's flags, then the thresholds of this step's outputs
+      for (int q = 0; q < sg_m; ++q) st.sg_active |= (unsigned)(i < a.sega->cooldown[q]) << q;
+      st.sg_apply = i >= a.sega->warmup;
+      semantic_thresholds(e, st, s);
+    }
     latent_chains_step(e, st, s);
     if (src_i) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
     std::swap(yb[0], yb[1]);
@@ -838,7 +887,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
                           float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream, const float* mask,
                           const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer,
-                          const PnpLoop* pnp = nullptr) {
+                          const PnpLoop* pnp = nullptr, const cdx_semantic_guidance* sega = nullptr, const float* c_edit = nullptr) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -850,6 +899,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
     a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
     a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer; a.pnp = pnp;
+    a.sega = sega; a.c_edit = c_edit;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -880,6 +930,15 @@ int cdx_cycle_lockstep_pnp(cdx_net* un, const float* x0, const float* c_src, con
   p.blocks = feature_blocks; p.n_blocks = n_feature_blocks;
   return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
                         B, C, h, w, stream, mask, nullptr, nullptr, false, 0, 0, &p);
+}
+
+int cdx_cycle_lockstep_semantic(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                                float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                                float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                                const float* mask, const float* c_edit, const cdx_semantic_guidance* sg) {
+  if (!sg || !c_edit) return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_semantic: null guidance or concept contexts"); });
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, nullptr, nullptr, false, 0, 0, nullptr, sg, c_edit);
 }
 
 int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
@@ -1615,7 +1674,7 @@ int cdx_op_gemm(cdx_engine* eh, const cdx_gemm_desc* d, int* plan_out, void* str
 int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int stage, void* stream) {
   return guard([&] {
     CDX_CHECK(eh && d && d->chains, "op_latent_chains: null argument");
-    CDX_CHECK(stage == 0 || stage == 1, "op_latent_chains: stage %d", stage);
+    CDX_CHECK(stage >= 0 && stage <= 2, "op_latent_chains: stage %d", stage);
     CDX_CHECK(d->chw > 0 && d->n_src > 0 && d->K >= 0 && d->rows >= 0 && (d->src == 0 || d->src == 1) && (d->pred == 0 || d->pred == 1),
               "op_latent_chains: chw=%d n_src=%d K=%d rows=%d src=%d pred=%d", d->chw, d->n_src, d->K, d->rows, d->src, d->pred);
     CDX_CHECK(d->next >= 0 && d->next <= 2 && (d->src || d->next == 0), "op_latent_chains: next=%d without a source chain", d->next);
@@ -1627,21 +1686,36 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
                 "op_latent_chains: chain %zu on rows %d, %d of %d", k, c.row, c.row2, d->rows);
     }
     const bool targets = d->K > 0, reads_x0 = d->src && (stage == 0 || d->next > 0);
-    CDX_CHECK((!d->src && !targets) || d->xin, "op_latent_chains: null xin");
-    CDX_CHECK(!reads_x0 || d->x0, "op_latent_chains: null x0");
-    CDX_CHECK(!(d->src && d->next == 1) || d->noise_next, "op_latent_chains: next == 1 without noise_next");
-    CDX_CHECK(!d->z_out || d->z_stride >= d->chw, "op_latent_chains: z_stride %lld < chw %d", (long long)d->z_stride, d->chw);
-    CDX_CHECK(d->src || !targets || (d->eps_in && d->eps_stride >= d->chw), "op_latent_chains: no source chain and no eps_in (stride %lld)",
-              (long long)d->eps_stride);
+    if (stage != 2) {                      // the threshold stage reads eout and the tables only
+      CDX_CHECK((!d->src && !targets) || d->xin, "op_latent_chains: null xin");
+      CDX_CHECK(!reads_x0 || d->x0, "op_latent_chains: null x0");
+      CDX_CHECK(!(d->src && d->next == 1) || d->noise_next, "op_latent_chains: next == 1 without noise_next");
+      CDX_CHECK(!d->z_out || d->z_stride >= d->chw, "op_latent_chains: z_stride %lld < chw %d", (long long)d->z_stride, d->chw);
+      CDX_CHECK(d->src || !targets || (d->eps_in && d->eps_stride >= d->chw), "op_latent_chains: no source chain and no eps_in (stride %lld)",
+                (long long)d->eps_stride);
+    }
     if (stage == 0) {
       CDX_CHECK(!d->src || (d->noise0 && d->xt && (d->next == 0 || d->xn)), "op_latent_chains: init: null noise0 / xt / xn");
       CDX_CHECK(!targets || d->yt, "op_latent_chains: init: null yt");
-    } else {
+    } else if (stage == 1) {
       CDX_CHECK((!d->src && !targets) || d->eout, "op_latent_chains: step: null eout");
       CDX_CHECK(!d->src || (d->xt && d->xn && (d->next == 0 || d->xn2)), "op_latent_chains: step: null xt / xn / xn2");
       CDX_CHECK(!targets || (d->yt && d->y_out), "op_latent_chains: step: null yt / y_out");
       CDX_CHECK(!d->mask || (d->src && d->hw > 0 && d->hw <= d->chw), "op_latent_chains: a mask needs a source chain and 0 < hw (%d) <= chw",
                 d->hw);
+    }
+    CDX_CHECK(d->sg_m >= 0 && d->sg_m <= SEMANTIC_MAX_CONCEPTS && (stage != 2 || d->sg_m > 0), "op_latent_chains: sg_m=%d at stage %d", d->sg_m,
+              stage);
+    const size_t n_sg = (size_t)d->n_src * d->K * d->sg_m;
+    if (d->sg_m) {
+      CDX_CHECK(targets && d->sg_rows && d->hw > 0 && d->chw % d->hw == 0, "op_latent_chains: concepts need target chains, sg_rows and hw (%d) "
+                "dividing chw", d->hw);
+      CDX_CHECK(stage == 0 || (d->eout && d->sg_thr), "op_latent_chains: concepts: null eout / sg_thr");
+      CDX_CHECK(stage != 1 || d->sg_nu, "op_latent_chains: concepts: null sg_nu");
+      for (size_t k = 0; k < n_sg; ++k)
+        CDX_CHECK(d->sg_rows[k] >= 0 && d->sg_rows[k] < d->rows, "op_latent_chains: concept row %d of %d", d->sg_rows[k], d->rows);
+      for (int q = 0; q < d->sg_m; ++q)
+        CDX_CHECK(d->sg_lambda[q] >= 0.0f && d->sg_lambda[q] < 1.0f, "op_latent_chains: sg_lambda[%d]=%g outside [0, 1)", q, d->sg_lambda[q]);
     }
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
@@ -1650,7 +1724,9 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
     with_arena(e, s, [&] {
       Scope sc(e.arena);
       Chain* chd = (Chain*)e.arena.alloc(ch.size() * sizeof(Chain));
+      int* sg_rows = n_sg ? (int*)e.arena.alloc(n_sg * sizeof(int)) : nullptr;
       if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(chd, ch.data(), ch.size() * sizeof(Chain), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+      if (!e.dry() && n_sg) CDX_CUDA(cudaMemcpyAsync(sg_rows, d->sg_rows, n_sg * sizeof(int), cudaMemcpyHostToDevice, s));
       LatentChains a;
       a.n = (size_t)d->n_src * d->chw; a.chw = d->chw; a.n_src = d->n_src; a.K = d->K;
       a.chains = chd; a.src = d->src;
@@ -1664,7 +1740,11 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
       a.yt = d->yt; a.y_out = d->y_out; a.xin = d->xin;
       a.pred = d->pred; a.vsa = d->vsa; a.vs1 = d->vs1;
       a.mask = d->mask; a.hw = d->hw;
+      a.sg_m = d->sg_m; a.sg_rows = sg_rows; a.sg_thr = d->sg_thr; a.sg_nu = d->sg_nu;
+      for (int q = 0; q < d->sg_m; ++q) { a.sg_scale[q] = d->sg_scale[q]; a.sg_lambda[q] = d->sg_lambda[q]; }
+      a.sg_active = d->sg_active; a.sg_apply = d->sg_apply; a.sg_mu = d->sg_mu; a.sg_beta = d->sg_beta; a.sg_beta1 = d->sg_beta1;
       if (stage == 0) latent_chains_init(e, a, s);
+      else if (stage == 2) semantic_thresholds(e, a, s);
       else latent_chains_step(e, a, s);
     });
   });

@@ -330,9 +330,31 @@ struct LatentChains {
   // m = mask[j*hw + p] for latent pixel p, broadcast over the C channels; m == 1 keeps y and m == 0 takes x exactly.  Kept last
   // so that the offsets of the fields above, and the unmasked kernels' code, do not change.
   const float* mask = nullptr; int hw = 0;
+  // semantic guidance (SEGA; cdx_cycle_lockstep_semantic), sg_m > 0: target chain t has sg_m concept rows sg_rows[t*sg_m + k] at its
+  // own x_t (init and step write them as the chain's rows).  With o_uc the chain's uncond row (row2, or row when it runs on one row
+  // at scale 0) and o_k concept k's row, per element of channel c = r / hw:
+  //   psi_k = sg_scale[k]*(o_k - o_uc);  g_k = (bit k of sg_active and |psi_k| >= sg_thr[(t*sg_m + k)*C + c]) ? psi_k : 0
+  //   G = (g_0 + ... + g_{m-1}) + sg_mu*nu;  nu <- sg_beta*nu + sg_beta1*G  (nu = sg_nu[t*chw + r]);  o-hat += G when sg_apply
+  // the threshold of each (chain, concept, channel) plane written by semantic_thresholds from the same step's eout.  Kept after the
+  // mask so that the earlier offsets, and the code of the kernels without concepts, do not change.
+  int sg_m = 0;
+  const int* sg_rows = nullptr;                  // device [n_src*K*sg_m]
+  float* sg_thr = nullptr;                       // device [n_src*K*sg_m*C]
+  float* sg_nu = nullptr;                        // device [n_src*K, chw], zero before the first step
+  float sg_scale[8] = {};                        // signed edit scales
+  float sg_lambda[8] = {};                       // percentile thresholds in [0, 1)
+  unsigned sg_active = 0;                        // bit k: concept k is before its cooldown step
+  int sg_apply = 0;                              // the step is past the warmup: o-hat += G
+  float sg_mu = 0.f, sg_beta = 0.f, sg_beta1 = 0.f;
 };
+constexpr int SEMANTIC_MAX_CONCEPTS = 8;
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s);
 void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s);
+// SEGA's threshold stage: one launch, one CTA per (target chain, concept, channel) plane of hw elements.  theta = Q(sg_lambda[k],
+// |psi_k| over the plane): r = lambda*(hw - 1) in fp32, the floor(r)-th and ceil(r)-th smallest values found exactly by a radix
+// select over the float bit patterns (re-read from eout each pass: no shared-memory limit on the plane size), then torch.quantile's
+// linear interpolation with ATen's scalar lerp, each op rounded.  Writes a.sg_thr.
+void semantic_thresholds(Engine& e, const LatentChains& a, cudaStream_t s);
 // image-resolution mask [B,1,H,W] -> [B,1,H/f,W/f]: mean of each f x f block, summed row by row then divided by f*f (avg_pool2d)
 void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, int f, cudaStream_t s);
 // paste-back at image resolution: out = m*clamp((dec + 1)*0.5, 0, 1) + (1 - m)*image, mask [B,1,H,W] broadcast over C channels;

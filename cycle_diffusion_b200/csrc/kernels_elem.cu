@@ -280,6 +280,7 @@ __global__ void latent_chains_init_kernel(const LatentChains a) {
       const size_t t = j * a.K + k;
       a.yt[t * a.chw + r] = xT;
       chain_put(a.xin, a.chains[a.n_src + t], r, a.chw, xT);
+      for (int q = 0; q < a.sg_m; ++q) a.xin[(size_t)a.sg_rows[t * a.sg_m + q] * a.chw + r] = xT;      // SEGA concept rows
     }
   }
 }
@@ -287,7 +288,10 @@ __global__ void latent_chains_init_kernel(const LatentChains a) {
 // in a register.  Under v-prediction each target chain forms e_t and pred_x0 from its own x_t and v.  MASK (the driver guarantees a
 // source chain at every step): each target x_{t-1} is blended with the source's x_{t-1}, a posterior sample of q(x_{t-1} | x_t, x0)
 // of the real image at the same noise level (x0 itself on the last step), so the unmasked region stays on the image's trajectory.
-template <int PRED, int MASK>
+// SEGA (a.sg_m > 0): each target chain's guidance-combined output takes its semantic guidance term G (LatentChains), formed from its
+// concept rows, its uncond row, the step's thresholds and its momentum before the e_t / pred_x0 conversion; its concept rows are
+// written with its next x_t.
+template <int PRED, int MASK, int SEGA = 0>
 __global__ void latent_chains_step_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
@@ -313,7 +317,22 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
     for (int k = 0; k < a.K; ++k) {
       const size_t t = j * a.K + k, ti = t * a.chw + r;
       const Chain tc = a.chains[a.n_src + t];
-      const float ot = chain_eps_hat(a.eout, tc, r, a.chw);
+      float ot = chain_eps_hat(a.eout, tc, r, a.chw);
+      if constexpr (SEGA) {
+        const float ou = __ldcg(a.eout + (size_t)(tc.row2 >= 0 ? tc.row2 : tc.row) * a.chw + r);
+        const int C = a.chw / a.hw, ch = (int)r / a.hw;
+        float S = 0.f;
+        for (int q = 0; q < a.sg_m; ++q) {
+          const int tq = (int)t * a.sg_m + q;
+          const float psi = MUL(a.sg_scale[q], SUB(__ldcg(a.eout + (size_t)a.sg_rows[tq] * a.chw + r), ou));
+          const float g = ((a.sg_active >> q) & 1u) && fabsf(psi) >= __ldcg(a.sg_thr + (size_t)tq * C + ch) ? psi : 0.f;
+          S = q ? ADD(S, g) : g;
+        }
+        const float nu = __ldcg(a.sg_nu + ti);
+        const float G = ADD(S, MUL(a.sg_mu, nu));
+        a.sg_nu[ti] = ADD(MUL(a.sg_beta, nu), MUL(a.sg_beta1, G));
+        if (a.sg_apply) ot = ADD(ot, G);
+      }
       const float y = __ldcg(a.yt + ti);
       float et, px0;
       eps_x0<PRED>(ot, y, a.c, a.vsa, a.vs1, et, px0);                                          // ddim.py:634
@@ -326,7 +345,86 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
       }
       a.y_out[ti] = yn;
       chain_put(a.xin, tc, r, a.chw, yn);
+      if constexpr (SEGA)
+        for (int q = 0; q < a.sg_m; ++q) a.xin[(size_t)a.sg_rows[t * a.sg_m + q] * a.chw + r] = yn;
     }
+  }
+}
+
+// SEGA's threshold stage (semantic_thresholds): block b owns plane b = (t*sg_m + k)*C + c, the hw values a = |psi_k| of target chain
+// t, concept k, channel c.  Non-negative floats order as their bit patterns, so the rank-th smallest value is found by a radix select
+// of 8 bits per pass: each pass histograms the values that match the digits found so far and keeps the digit whose bin holds the
+// rank.  The values are recomputed from eout on every pass, so any plane size runs with a 1 KB histogram.  After the last pass the
+// bin is one value, v_lo, and the rank's place among its copies says whether v_hi (rank + 1) is v_lo too; else one more pass takes
+// the smallest value above v_lo.
+constexpr int SEMANTIC_THREADS = 512;
+__device__ __forceinline__ unsigned semantic_abs_bits(const float* ok, const float* ou, int p, float sc) {
+  return __float_as_uint(fabsf(MUL(sc, SUB(__ldcg(ok + p), __ldcg(ou + p)))));
+}
+__global__ void __launch_bounds__(SEMANTIC_THREADS) semantic_threshold_kernel(const LatentChains a) {
+  __shared__ unsigned hist[256];
+  __shared__ unsigned s_digit, s_below, s_count, s_min;
+  const int C = a.chw / a.hw, n = a.hw, plane = blockIdx.x;
+  const int c = plane % C, tq = plane / C, q = tq % a.sg_m, t = tq / a.sg_m;
+  const Chain tc = a.chains[a.n_src + t];
+  const float* ou = a.eout + (size_t)(tc.row2 >= 0 ? tc.row2 : tc.row) * a.chw + (size_t)c * n;
+  const float* ok = a.eout + (size_t)a.sg_rows[tq] * a.chw + (size_t)c * n;
+  const float sc = a.sg_scale[q];
+  const float rk = MUL(a.sg_lambda[q], (float)(n - 1));
+  const float fl = floorf(rk);
+  const unsigned lo = (unsigned)fl, hi = (unsigned)ceilf(rk);
+  const float w = SUB(rk, fl);
+  unsigned prefix = 0, known = 0, want = lo, count = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = threadIdx.x; i < 256; i += SEMANTIC_THREADS) hist[i] = 0;
+    __syncthreads();
+    for (int p = threadIdx.x; p < n; p += SEMANTIC_THREADS) {
+      const unsigned u = semantic_abs_bits(ok, ou, p, sc);
+      if ((u & known) == prefix) atomicAdd(&hist[(u >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {          // warp 0: lane l sums bins [8l, 8l + 8), an exclusive scan finds the lane holding `want`
+      const int lane = threadIdx.x;
+      unsigned cnt[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { cnt[j] = hist[lane * 8 + j]; sum += cnt[j]; }
+      unsigned incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+      }
+      unsigned run = incl - sum;
+      if (want >= run && want < incl) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (want < run + cnt[j]) { s_digit = lane * 8 + j; s_below = run; s_count = cnt[j]; break; }
+          run += cnt[j];
+        }
+      }
+    }
+    __syncthreads();
+    prefix |= s_digit << shift;
+    known |= 255u << shift;
+    want -= s_below;
+    count = s_count;
+  }
+  // prefix = v_lo; `want` is the rank among its `count` copies
+  const bool above = hi != lo && want + 1 >= count;
+  if (above) {
+    if (threadIdx.x == 0) s_min = 0xffffffffu;
+    __syncthreads();
+    unsigned m = 0xffffffffu;
+    for (int p = threadIdx.x; p < n; p += SEMANTIC_THREADS) {
+      const unsigned u = semantic_abs_bits(ok, ou, p, sc);
+      if (u > prefix) m = min(m, u);
+    }
+    atomicMin(&s_min, m);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float vlo = __uint_as_float(prefix), vhi = above ? __uint_as_float(s_min) : vlo;
+    a.sg_thr[plane] = w < 0.5f ? ADD(vlo, MUL(w, SUB(vhi, vlo))) : SUB(vhi, MUL(SUB(vhi, vlo), SUB(1.0f, w)));   // ATen lerp
   }
 }
 
@@ -722,6 +820,16 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
 
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s) { LAUNCH1(latent_chains_init_kernel, a.n, a); }
 void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
+  if (a.sg_m) {
+    if (a.mask) {
+      if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 1>), a.n, a);
+      else LAUNCH1((latent_chains_step_kernel<0, 1, 1>), a.n, a);
+    } else {
+      if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 1>), a.n, a);
+      else LAUNCH1((latent_chains_step_kernel<0, 0, 1>), a.n, a);
+    }
+    return;
+  }
   if (a.mask) {
     if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1>), a.n, a);
     else LAUNCH1((latent_chains_step_kernel<0, 1>), a.n, a);
@@ -729,6 +837,18 @@ void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
     if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0>), a.n, a);
     else LAUNCH1((latent_chains_step_kernel<0, 0>), a.n, a);
   }
+}
+void semantic_thresholds(Engine& e, const LatentChains& a, cudaStream_t s) {
+  CDX_CHECK(a.sg_m >= 1 && a.sg_m <= SEMANTIC_MAX_CONCEPTS && a.hw > 0 && a.chw % a.hw == 0, "semantic_thresholds: m=%d chw=%d hw=%d", a.sg_m,
+            a.chw, a.hw);
+  if (e.dry()) return;
+  const long long planes = (long long)a.n_src * a.K * a.sg_m * (a.chw / a.hw);
+  if (planes == 0) return;
+  ProfScope ps(e, s, PROF_ELEMENTWISE, 0.0, 2.0 * 4.0 * planes * a.hw, 1);     // algorithmic: o_k and o_uc read once
+  ps.note("semantic thresholds %lld planes x %d", planes, a.hw);
+  semantic_threshold_kernel<<<(unsigned)planes, SEMANTIC_THREADS, 0, s>>>(a);
+  CDX_CUDA(cudaGetLastError());
+  e.launches++;
 }
 void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, int f, cudaStream_t s) {
   CDX_CHECK(B >= 1 && f >= 1 && H >= f && W >= f && H % f == 0 && W % f == 0, "mask_pool: %dx%d mask, factor %d", H, W, f);

@@ -13,6 +13,7 @@ import torch
 from . import _cabi
 from ._cabi import lib, check, UnetConfig, VaeConfig, TextConfig, DdimCoef, PixelCoef
 from .attn_control import MutualSelfControl, PnPControl
+from .semantic import SemanticGuidance
 
 
 def _ptr(t):
@@ -423,14 +424,28 @@ class Engine:
         latent_chains_step.  chains: [(row, row2, scale)] for the n_src source chains then the n_src*K target chains; rows: the row
         count of xin / eout; c, cnext: DdimCoef; the other cdx_latent_chains_desc fields are keyword arguments, buffers as contiguous
         float32 tensors on this engine's device (a view at an offset keeps its address).  Each buffer must hold every element the
-        launch may touch; outputs land in the caller's tensors."""
+        launch may touch; outputs land in the caller's tensors.
+        Semantic guidance: sg_rows [(row) * n_src*K*m] (host ints, the concept rows of target chain t at t*m + k) sets sg_m = m;
+        stage 2 is its threshold stage (writes sg_thr), stage 1 then runs the step with the concept terms; sg_scale and sg_lambda are
+        lists of m floats, sg_active / sg_apply / sg_mu / sg_beta / sg_beta1 scalars, sg_thr and sg_nu tensors."""
+        sg_rows = fields.pop('sg_rows', None)
+        m = len(sg_rows) // max(n_src * K, 1) if sg_rows else 0
+        hw = fields.get('hw', 0)
         need = dict(x0=n_src * chw, noise0=n_src * chw, xt=n_src * chw, xn=n_src * chw, noise_next=n_src * chw, xn2=n_src * chw,
                     eout=rows * chw, xin=rows * chw, yt=n_src * K * chw, y_out=n_src * K * chw,
                     z_out=(n_src - 1) * fields.get('z_stride', 0) + chw, eps_in=(n_src - 1) * fields.get('eps_stride', 0) + chw,
-                    mask=n_src * fields.get('hw', 0))
+                    mask=n_src * hw, sg_thr=n_src * K * m * (chw // hw if hw else 0), sg_nu=n_src * K * chw)
         assert len(chains) == n_src * (1 + K), f'op_latent_chains: {len(chains)} chains for n_src={n_src}, K={K}'
         table = (_cabi.LatentChain * len(chains))(*[_cabi.LatentChain(int(r), int(r2), float(s)) for r, r2, s in chains])
         d = _cabi.LatentChainsDesc(chw=chw, n_src=n_src, K=K, rows=rows, chains=table)
+        if sg_rows:
+            assert len(sg_rows) == n_src * K * m, f'op_latent_chains: {len(sg_rows)} concept rows for {n_src * K} target chains'
+            sg_table = (C.c_int * len(sg_rows))(*[int(r) for r in sg_rows])
+            d.sg_m, d.sg_rows = m, sg_table
+        for name in ('sg_scale', 'sg_lambda'):
+            if name in fields:
+                vals = [float(v) for v in fields.pop(name)]
+                setattr(d, name, (C.c_float * 8)(*(vals + [0.0] * (8 - len(vals)))))
         if c is not None:
             d.c = c
         if cnext is not None:
@@ -780,7 +795,8 @@ class UNet(Net):
                                       B, Cc, h, w, e.stream))
         return out
 
-    def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False, mask=None, attn_control=None):
+    def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False, mask=None, attn_control=None,
+                       semantic=None, c_edit=None):
         """Both chains in one loop (one U-Net call + one fused elementwise kernel per step, no z buffer unless asked for):
         x0 [B,C,h,w] -> translated latent [B,C,h,w] (and z [B, n+1, C,h,w] when return_z).  noise as for latent_encode with
         n_rec == sched.refine_steps.  mask [B,1,h,w] in [0,1] (1 = may change): masked editing (cdx_cycle_lockstep_masked), the
@@ -789,7 +805,10 @@ class UNet(Net):
         (cdx_cycle_lockstep_ctl), or its "refine" edit when the control has an own_weight (cdx_cycle_lockstep_refine); or an
         attn_control.MutualSelfControl, MasaCtrl's mutual self-attention on the target chain's rows (cdx_cycle_lockstep_mutual); or
         an attn_control.PnPControl, Plug-and-Play's feature and self-attention injection on the target chain's rows
-        (cdx_cycle_lockstep_pnp).  Each composes with mask."""
+        (cdx_cycle_lockstep_pnp).  Each composes with mask.
+        semantic: a semantic.SemanticGuidance of m concepts, with c_edit [B, m, L, D] (or [m, L, D], every sample's): SEGA's
+        concept terms on the target chain (cdx_cycle_lockstep_semantic); it needs uc, composes with mask, and an attn_control
+        with it raises ValueError."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -798,6 +817,26 @@ class UNet(Net):
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
         mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
+        if semantic is not None:
+            if attn_control is not None:
+                raise ValueError('semantic guidance does not combine with attention control in one loop')
+            if not isinstance(semantic, SemanticGuidance):
+                raise ValueError(f'semantic: expected a semantic.SemanticGuidance, got {type(semantic)}')
+            if c_edit is None:
+                raise ValueError('semantic guidance needs the concept contexts c_edit [B, m, L, D]')
+            c_edit = _f32c(c_edit, e.device)
+            if c_edit.dim() == 3:
+                c_edit = c_edit.unsqueeze(0).expand(B, -1, -1, -1).contiguous()
+            if tuple(c_edit.shape) != (B, semantic.m) + tuple(c_src.shape[1:]):
+                raise ValueError(f'c_edit: shape {tuple(c_edit.shape)}, expected {(B, semantic.m) + tuple(c_src.shape[1:])}')
+            sg = semantic.c_struct(n)
+            out = e.empty(B, Cc, h, w)
+            z = e.empty(B, n + 1, Cc, h, w) if return_z else None
+            check(lib.cdx_cycle_lockstep_semantic(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale),
+                                                  float(tgt_scale), sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T,
+                                                  sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask), _ptr(c_edit),
+                                                  C.byref(sg)))
+            return (out, z) if return_z else out
         mutual, pnp = isinstance(attn_control, MutualSelfControl), isinstance(attn_control, PnPControl)
         ctl, _token_map, own = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None and not (mutual or pnp) \
             else (None, None, None)

@@ -17,6 +17,7 @@ import torch
 from .attn_control import AttentionControl, MutualSelfControl, PnPControl
 from .engine import check_mask
 from .schedule import DDIMSchedule
+from .semantic import SemanticGuidance
 
 
 @dataclass
@@ -172,7 +173,8 @@ class CycleDiffusionPipeline:
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
                  source_guidance_scale=1, num_images_per_prompt=1, eta=0.1, generator=None, prompt_embeds=None, output_type='pt',
                  return_dict=True, callback=None, callback_steps=1, cross_attention_kwargs=None, clip_skip=None, two_phase=False,
-                 mask_image=None, paste_back=False):
+                 mask_image=None, paste_back=False, editing_prompt=None, reverse_editing_direction=False, edit_guidance_scale=5,
+                 edit_threshold=0.9, edit_cooldown_steps=None, edit_warmup_steps=10, edit_momentum_scale=0.1, edit_mom_beta=0.4):
         """mask_image: optional float tensor [B,1,H,W] or [1,1,H,W] in [0,1] at the image's size, 1 = "may change" (diffusers'
         convention).  Outside the mask the latent stays on the source image's own chain (cdx_cycle_lockstep_masked), so the
         unmasked region decodes to the image's VAE reconstruction.  paste_back: additionally composite the output with the input
@@ -201,8 +203,27 @@ class CycleDiffusionPipeline:
         row's features (out_layers of its in_layers output, on the target's own skip), and in the first attention_steps the
         SpatialTransformers from index attention_start_layer on give them the source row's self-attention queries and keys
         (attn_control.PnPControl).  source_prompt="" with source_guidance_scale=0 reproduces PnP's unconditional source branch.
-        Other keys, values out of range and two_phase=True raise ValueError; it composes with mask_image."""
+        Other keys, values out of range and two_phase=True raise ValueError; it composes with mask_image.
+
+        editing_prompt: semantic guidance (SEGA, Brack et al., 2023), named as diffusers' semantic pipelines name it: a str or a list
+        of m <= 8 concept prompts added to (reverse_editing_direction False) or removed from (True) the target image, each with its
+        own edit_guidance_scale, edit_threshold (the percentile in [0, 1) of its term's magnitude per latent plane above which it
+        applies) and edit_cooldown_steps (None: every step); a scalar applies to every concept, a list gives one per concept.
+        edit_warmup_steps, edit_momentum_scale and edit_mom_beta are shared (semantic.SemanticGuidance).  Steps are counted over the
+        loop's int(num_inference_steps * strength) steps.  The concept prompts are broadcast to every image.  It composes with
+        mask_image and precision='autocast'; two_phase=True, an edit_type in cross_attention_kwargs, list lengths other than m and
+        a per-concept warmup list raise ValueError.  Without editing_prompt the edit_* arguments are unused."""
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
+        semantic, concepts = None, None
+        if editing_prompt is not None:
+            concepts = [editing_prompt] if isinstance(editing_prompt, str) else list(editing_prompt)
+            if two_phase:
+                raise ValueError('semantic guidance needs the lock-step loop: its terms are formed at every step of the target chain '
+                                 '(two_phase=False)')
+            if attn_control is not None:
+                raise ValueError('semantic guidance does not combine with a cross_attention_kwargs edit_type in one loop')
+            semantic = SemanticGuidance.for_concepts(len(concepts), edit_guidance_scale, reverse_editing_direction, edit_threshold,
+                                                     edit_cooldown_steps, edit_warmup_steps, edit_momentum_scale, edit_mom_beta)
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')
         if not isinstance(callback_steps, int) or callback_steps <= 0:
@@ -243,6 +264,7 @@ class CycleDiffusionPipeline:
             c_tgt = prompt_embeds if prompt_embeds is not None else g.get_learned_conditioning(prompts)
             c_src = g.get_learned_conditioning(sources)
             uc = g.get_learned_conditioning(B * [''])
+            c_edit = g.get_learned_conditioning(concepts).unsqueeze(0).expand(B, -1, -1, -1).contiguous() if concepts else None
             S = num_inference_steps
             skip = S - min(int(S * strength), S)
             sched = DDIMSchedule(S, eta, skip, g.alphas_cumprod)
@@ -262,7 +284,7 @@ class CycleDiffusionPipeline:
             else:
                 mask = e.mask_pool(mask_image, g.vae.down) if mask_image is not None else None
                 latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise, mask=mask,
-                                                attn_control=attn_control)
+                                                attn_control=attn_control, semantic=semantic, c_edit=c_edit)
             if callback is not None:
                 callback(n_rec - 1, sched.t_loop[-1], latents)
             if paste_back:

@@ -396,6 +396,37 @@ int cdx_cycle_lockstep_pnp(cdx_net* unet, const float* x0, const float* c_src, c
                            float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                            void* stream, const float* mask, int feature_steps, int attention_steps,
                            int attention_start_layer, const int* feature_blocks, int n_feature_blocks);
+/* Semantic guidance (SEGA, Brack et al., 2023; LEDITS++'s editing term) on the lock-step loop: cdx_cycle_lockstep_masked (mask may
+ * be NULL) where concepts are added to or removed from the target chain's image, each where its own guidance is strongest.  Each
+ * target chain gets m concept rows (1 <= m <= CDX_SEMANTIC_MAX), appended after all target rows, that run the U-Net at the chain's
+ * own x_t and timestep under c_edit[b, k] (device [B, m, L, D]).  At loop step i (0-based, of n_steps), with o_uc the chain's uncond
+ * row output (at tgt_scale 1 the chain is given an uncond row; its eps-hat stays the cond row exactly) and o_k concept k's, every
+ * operation one rounded fp32 op:
+ *   psi_k = scale[k] * (o_k - o_uc)                 scale[k] signed: negative removes the concept
+ *   theta = Q(threshold[k], |psi_k| over the h*w plane of each channel), per image: r = threshold*(hw - 1), the floor(r)-th and
+ *           ceil(r)-th smallest values interpolated as torch.quantile does (w = r - floor(r); w < 0.5 ? lo + w*(hi - lo) :
+ *           hi - (hi - lo)*(1 - w))
+ *   g_k   = (i < cooldown[k] and |psi_k| >= theta) ? psi_k : 0;   S = g_0 + g_1 + ... (left to right)
+ *   G     = S + momentum_scale * nu;   nu <- beta * nu + beta1 * G      (nu per target chain, zero at the first step)
+ *   eps-hat += G when i >= warmup   (v nets: on the guidance-combined v, before the conversion)
+ * beta1 = fp32(1 - beta) formed by the caller in double.  The source chain and z_out are untouched but for the last bits the shared
+ * U-Net call moves (fp16-split operands take one exponent per tensor).  One more launch per step, the threshold stage, runs between
+ * the U-Net call and the step kernel.  CDX_E_INVALID: m outside 1..CDX_SEMANTIC_MAX, a threshold outside [0, 1), nets without a
+ * context, uc == NULL, and a row count whose U-Net call needs more GroupNorm statistics than the engine's pool holds. */
+#define CDX_SEMANTIC_MAX 8
+typedef struct cdx_semantic_guidance {
+  int m;
+  float scale[CDX_SEMANTIC_MAX];       /* signed: -edit_guidance_scale with reverse_editing_direction, else +edit_guidance_scale */
+  float threshold[CDX_SEMANTIC_MAX];   /* percentile lambda in [0, 1) */
+  int cooldown[CDX_SEMANTIC_MAX];      /* concept k guides at steps i < cooldown[k] */
+  int warmup;                          /* G is added at steps i >= warmup (the momentum runs from step 0) */
+  float momentum_scale, beta, beta1;
+} cdx_semantic_guidance;
+int cdx_cycle_lockstep_semantic(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                                int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                                const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                                float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                                void* stream, const float* mask, const float* c_edit, const cdx_semantic_guidance* sg);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -654,8 +685,8 @@ typedef struct cdx_gemm_desc {
 } cdx_gemm_desc;
 int cdx_op_gemm(cdx_engine* e, const cdx_gemm_desc* desc, int* plan_out, void* stream);
 
-/* One launch of the latent loops' fused step kernels, the production latent_chains_init (stage 0) or latent_chains_step (stage 1)
- * every latent loop driver runs (tests/test_step_kernels_gpu.py).  n_src element groups of chw elements; group j has a source chain
+/* One launch of the latent loops' fused step kernels, the production latent_chains_init (stage 0), latent_chains_step (stage 1) or
+ * semantic guidance's threshold stage (stage 2) every latent loop driver runs (tests/test_step_kernels_gpu.py).  n_src element groups of chw elements; group j has a source chain
  * (when src) and K target chains j*K + k.  chains: host [n_src + n_src*K] {row, row2, scale}, the source chains first, staged to the
  * device as the drivers stage theirs: `row` is the chain's cond row of xin / eout ([rows, chw]), `row2` its uncond row or -1; a
  * chain on two rows at scale 1 (0) reads its cond (uncond) row unchanged, else eps-hat = e(row2) + scale * (e(row) - e(row2)).
@@ -668,6 +699,12 @@ int cdx_op_gemm(cdx_engine* e, const cdx_gemm_desc* desc, int* plan_out, void* s
  *   step, no src: the noise <- eps_in[j*eps_stride + r]
  *   step:         each target chain from yt with that noise -> y_out and its xin rows; pred == 1: the output is v, converted with
  *                 (vsa, vs1); mask (src only) [n_src, hw], broadcast over the chw / hw channels: y_out = m*y + (1 - m)*xn
+ *   sg_m > 0:     semantic guidance (cdx_cycle_lockstep_semantic).  sg_rows: host [n_src*K*sg_m], the concept rows of target chain
+ *                 t at t*sg_m + k (staged as chains are); a target chain's uncond row is row2, or row when row2 < 0.  Stage 2 (the
+ *                 threshold stage) writes sg_thr [n_src*K*sg_m*C] (C = chw / hw, plane (t*sg_m + k)*C + c) from eout under
+ *                 sg_scale and sg_lambda; stage 1 then adds G to each target chain's eps-hat when sg_apply, from the concepts whose
+ *                 bit is set in sg_active, updates the momentum sg_nu [n_src*K, chw] in place with (sg_mu, sg_beta, sg_beta1), and
+ *                 writes the chain's next x_t to its concept rows too (as does stage 0).
  * Row indices, counts, strides and the stage are checked on the host; buffer extents are the caller's. */
 typedef struct cdx_latent_chain { int row, row2; float scale; } cdx_latent_chain;
 typedef struct cdx_latent_chains_desc {
@@ -688,6 +725,12 @@ typedef struct cdx_latent_chains_desc {
   float* xin;
   int pred; float vsa, vs1;
   const float* mask; int hw;
+  int sg_m;
+  const int* sg_rows;
+  float* sg_thr; float* sg_nu;
+  float sg_scale[CDX_SEMANTIC_MAX]; float sg_lambda[CDX_SEMANTIC_MAX];
+  unsigned sg_active; int sg_apply;
+  float sg_mu, sg_beta, sg_beta1;
 } cdx_latent_chains_desc;
 int cdx_op_latent_chains(cdx_engine* e, const cdx_latent_chains_desc* desc, int stage, void* stream);
 /* One launch of the two-model pixel loop's fused step (pixel_lockstep_step, which cdx_pixel_cycle_lockstep runs): xs / ys [B, chw]

@@ -62,7 +62,8 @@ class GemmDesc(C.Structure):
                 ('C', _P), ('ldc', C.c_int), ('C_lo', _P), ('Ct_hi', _P), ('Ct_lo', _P), ('t_col0', C.c_int), ('ldt', C.c_int64),
                 ('a_amax', _P), ('a2_amax', _P), ('c_amax', _P), ('c_stats', _P), ('w_range', C.c_float),
                 ('batch', C.c_int), ('heads', C.c_int),
-                ('sA_b', C.c_int64), ('sA_h', C.c_int64), ('sB_b', C.c_int64), ('sB_h', C.c_int64), ('sC_b', C.c_int64), ('sC_h', C.c_int64)]
+                ('sA_b', C.c_int64), ('sA_h', C.c_int64), ('sB_b', C.c_int64), ('sB_h', C.c_int64), ('sC_b', C.c_int64), ('sC_h', C.c_int64),
+                ('up', C.c_int)]
 
 
 class AttentionNetDesc(C.Structure):

@@ -1628,6 +1628,8 @@ int cdx_op_gemm(cdx_engine* eh, const cdx_gemm_desc* d, int* plan_out, void* str
               "op_gemm: bad batch / image counts");
     const int batch = d->batch > 0 ? d->batch : 1, heads = d->heads > 0 ? d->heads : 1;
     CDX_CHECK(d->mode == 0 || (!d->b_kn && batch * heads == 1), "op_gemm: a conv3x3 is one unbatched [N][K] product");
+    const int up = d->up > 0 ? d->up : 1;
+    CDX_CHECK(up == 1 || (up == 2 && d->mode == 1), "op_gemm: up=%d (mode %d): a conv3x3 folds a nearest-2x upsample only", d->up, d->mode);
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
     int route = 0;
@@ -1639,7 +1641,7 @@ int cdx_op_gemm(cdx_engine* eh, const cdx_gemm_desc* d, int* plan_out, void* str
       g.M = d->M; g.N = d->N; g.K = d->K;
       g.A = d->A; g.lda = d->lda; g.C1 = d->C1;
       g.A2 = d->A2; g.lda2 = d->lda2; g.C2 = d->C2;
-      g.Hin = d->Hin; g.Win = d->Win; g.Hout = d->Hout; g.Wout = d->Wout; g.stride = d->stride; g.pad = d->pad;
+      g.Hin = d->Hin; g.Win = d->Win; g.Hout = d->Hout; g.Wout = d->Wout; g.stride = d->stride; g.pad = d->pad; g.up = up;
       const float* wk = d->w;
       size_t wn;                                   // weight elements the planes cover (element index = float index)
       if (d->mode == 1) {

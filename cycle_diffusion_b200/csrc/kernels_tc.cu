@@ -933,10 +933,12 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   // floats at ~3 TB/s); a split must buy >= 10 %.  (A model of the kernel's structure, not a fit to measurements.)
   int best_w = TBN, best_s = 1;
   {
-    static std::map<std::array<int64_t, 5>, int> plan_cache;      // exact key (no hashing of packed fields: nothing can collide)
+    // exact key (no hashing of packed fields: nothing can collide) of everything the cost model reads -- M too, through the split-K
+    // traffic term: two shapes of one 128-row band may plan differently, and each must run its own plan whichever was planned first
+    static std::map<std::array<int64_t, 6>, int> plan_cache;
     static std::mutex plan_mutex;                                          // engines on different devices may plan concurrently
     std::lock_guard<std::mutex> plan_lock(plan_mutex);
-    const std::array<int64_t, 5> key = {p.tiles_m, a.N, num_kb, ((a.geglu || a.Ct_hi) ? 1 : 0) | (a.out_nchw ? 2 : 0) | (h16 ? 4 : 0) | (ts ? 8 : 0), e.num_sms};
+    const std::array<int64_t, 6> key = {a.M, p.tiles_m, a.N, num_kb, ((a.geglu || a.Ct_hi) ? 1 : 0) | (a.out_nchw ? 2 : 0) | (h16 ? 4 : 0) | (ts ? 8 : 0), e.num_sms};
     const double kc0 = h16 ? 700.0 : 400.0, kc1 = h16 ? 6.0 : 3.0;
     const int min_kbs = h16 ? 4 : 8;
     auto it = plan_cache.find(key);

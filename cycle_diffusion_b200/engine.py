@@ -396,10 +396,10 @@ class Engine:
         """One contraction through the production GEMM with any of its epilogue terms (cdx_op_gemm in include/cdx.h, whose
         cdx_gemm_desc fields are the keyword arguments).  Every buffer is a float32 tensor (c_stats: float64) on this engine's
         device, passed as it is -- a view at an offset or a column slice keeps its address, so the strides (lda, ldc, ...) are the
-        caller's.  Outputs land in the caller's C / C_lo / Ct_hi / Ct_lo / c_amax / c_stats.  Defaults: alpha 1, stride 1, pad 1,
+        caller's.  Outputs land in the caller's C / C_lo / Ct_hi / Ct_lo / c_amax / c_stats.  Defaults: alpha 1, stride 1, pad 1, up 1,
         one image per row block.  Returns the plan the call ran: dict(kind: 'ffma' or one of GEMM_KINDS, width: tile width
         (FFMA: tile side), splits: split-K factor, amax_fused, stats_fused: side outputs made by the tensor-core epilogue)."""
-        d = _cabi.GemmDesc(alpha=1.0, stride=1, pad=1, batch=1, heads=1, rows_per_batch=1)
+        d = _cabi.GemmDesc(alpha=1.0, stride=1, pad=1, batch=1, heads=1, rows_per_batch=1, up=1)
         for name, v in fields.items():
             if name in self.GEMM_POINTERS:
                 if v is not None:

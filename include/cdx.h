@@ -660,6 +660,8 @@ int cdx_op_produce_norm(cdx_engine* e, const float* x, const float* w, const flo
  * <- max(c_amax, max |stored C|); c_stats (device [M / rows_per_batch, N, 2] doubles) += per-(image, channel) {sum, sum sq}.
  * a_amax / a2_amax: tracked range slots of A / A2 (device floats), or NULL (measured here).  w_range > 0: the fp16 weight planes
  * take the exponent of max(w_range, max |w|), as in a net whose weight exponent comes from a larger weight elsewhere.
+ * up (trailing field; 0 reads as 1): 2 folds a nearest-2x upsample of A into the conv3x3 gather (Hin, Win: the stored map; the FFMA
+ * tiles run it, as the networks' Upsample convs on that path).
  * *plan_out (host): how the call ran -- bit 3 tensor cores; bits 0-2 range fused, statistics fused, split-K; bits 4-5 operand kind
  * (0 SS, 1 TS, 2 fp16 split, 3 one-term fp16); bits 8-15 tile width (FFMA: tile side); bits 16-23 split-K factor. */
 typedef struct cdx_gemm_desc {
@@ -682,6 +684,7 @@ typedef struct cdx_gemm_desc {
   float w_range;
   int batch, heads;
   int64_t sA_b, sA_h, sB_b, sB_h, sC_b, sC_h;
+  int up;
 } cdx_gemm_desc;
 int cdx_op_gemm(cdx_engine* e, const cdx_gemm_desc* desc, int* plan_out, void* stream);
 

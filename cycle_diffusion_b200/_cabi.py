@@ -70,7 +70,8 @@ class AttentionNetDesc(C.Structure):
     _fields_ = [('kind', C.c_int), ('causal', C.c_int), ('qkv', C.c_void_p), ('q', C.c_void_p), ('kv', C.c_void_p), ('k', C.c_void_p),
                 ('v', C.c_void_p), ('B', C.c_int), ('N', C.c_int), ('L', C.c_int), ('ctx_lp', C.c_int), ('heads', C.c_int), ('d', C.c_int),
                 ('scale', C.c_float), ('qk_rows', C.POINTER(C.c_int)), ('kv_rows', C.POINTER(C.c_int)), ('acc_rows', C.POINTER(C.c_int)),
-                ('n_acc', C.c_int), ('slot', C.c_float), ('q_slot', C.c_float), ('out', C.c_void_p)]
+                ('n_acc', C.c_int), ('slot', C.c_float), ('q_slot', C.c_float), ('out', C.c_void_p),
+                ('probe_rows', C.POINTER(C.c_int)), ('probe_spans', C.POINTER(C.c_int)), ('n_probe', C.c_int), ('probe_map', C.c_void_p)]
 
 
 class LatentChain(C.Structure):
@@ -88,6 +89,12 @@ class LatentChainsDesc(C.Structure):
                 ('sg_beta1', C.c_float)]
 
 
+class LatentChainsMaskDesc(LatentChainsDesc):
+    """The whole cdx_latent_chains_desc: LatentChainsDesc plus LEDITS++'s trailing mask fields (the C struct always has them, so every
+    call passes this one)."""
+    _fields_ = [('sg_map', _P), ('sg_mask', C.c_int), ('sg_gh', C.c_int), ('sg_gw', C.c_int), ('w', C.c_int)]
+
+
 CDX_SEMANTIC_MAX = 8
 
 
@@ -95,6 +102,10 @@ class SemanticGuidanceC(C.Structure):
     _fields_ = [('m', C.c_int), ('scale', C.c_float * CDX_SEMANTIC_MAX), ('threshold', C.c_float * CDX_SEMANTIC_MAX),
                 ('cooldown', C.c_int * CDX_SEMANTIC_MAX), ('warmup', C.c_int), ('momentum_scale', C.c_float), ('beta', C.c_float),
                 ('beta1', C.c_float)]
+
+
+class SemanticAttnMaskC(C.Structure):
+    _fields_ = [('intersect', C.c_int), ('n_tokens', C.c_int * CDX_SEMANTIC_MAX)]
 
 
 _F = C.c_float
@@ -159,6 +170,8 @@ SIGNATURES = {
                                     _I, _I, _P, _P, _I, _I, _I, C.POINTER(_I), _I]),
     'cdx_cycle_lockstep_semantic': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
                                          _I, _I, _P, _P, _P, C.POINTER(SemanticGuidanceC)]),
+    'cdx_cycle_lockstep_semantic_attn': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I,
+                                              _I, _I, _I, _P, _P, _P, C.POINTER(SemanticGuidanceC), C.POINTER(SemanticAttnMaskC)]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),

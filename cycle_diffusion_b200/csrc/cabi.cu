@@ -186,6 +186,7 @@ struct ChainLoopArgs {
   // optional, exclusive with ctl, mutual and pnp: semantic guidance (cdx.h, cdx_cycle_lockstep_semantic), concept contexts
   // c_edit [n_src, m, L, D]: every target chain of group j runs concept k under c_edit[j, k]
   const cdx_semantic_guidance* sega = nullptr; const float* c_edit = nullptr;
+  const cdx_semantic_attn_mask* sega_mask = nullptr;    // optional with sega: LEDITS++'s implicit masks (cdx_cycle_lockstep_semantic_attn)
   int C = 0, h = 0, w = 0;
 };
 
@@ -229,6 +230,14 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     CDX_CHECK(g.m >= 1 && g.m <= SEMANTIC_MAX_CONCEPTS, "semantic guidance: m=%d concepts, 1 to %d", g.m, SEMANTIC_MAX_CONCEPTS);
     for (int k = 0; k < g.m; ++k)
       CDX_CHECK(g.threshold[k] >= 0.0f && g.threshold[k] < 1.0f, "semantic guidance: threshold[%d]=%g outside [0, 1)", k, g.threshold[k]);
+  }
+  if (a.sega_mask) {
+    CDX_CHECK(a.sega, "attention masks: semantic guidance only");
+    CDX_CHECK(a.h % 4 == 0 && a.w % 4 == 0 && a.h >= 8 && a.w >= 8, "attention masks: a %dx%d latent, multiples of 4 of at least 8 needed", a.h,
+              a.w);
+    for (int k = 0; k < a.sega->m; ++k)
+      CDX_CHECK(a.sega_mask->n_tokens[k] >= 1 && a.sega_mask->n_tokens[k] <= a.L - 2, "attention masks: n_tokens[%d]=%d outside 1..%d", k,
+                a.sega_mask->n_tokens[k], a.L - 2);
   }
   // the chain table: all source-chain rows first, then all target-chain rows (the two-model loop runs the two blocks under two
   // nets); inside a block the uncond rows come first, cat([uc, c]) as ddim.py:555-557
@@ -328,14 +337,25 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   // semantic guidance: the concept row table, the thresholds of the step and the momentum of every target chain, fixed for the loop
   int* sg_rows_dev = nullptr;
   float *sg_thr = nullptr, *sg_nu = nullptr;
+  // attention masks: each concept row's span and raw map, written by the probe of every step's U-Net call
+  AttnProbe probe;
+  const int sg_mask = a.sega_mask ? 1 + (a.sega_mask->intersect != 0) : 0, gh = a.h / 4, gw = a.w / 4;
   if (sg_m) {
     sg_rows_dev = (int*)e.arena.alloc(sg_rows.size() * sizeof(int));
-    sg_thr = (float*)e.arena.alloc(sg_rows.size() * a.C * sizeof(float));
+    sg_thr = (float*)e.arena.alloc(sg_rows.size() * std::max(a.C, 2) * sizeof(float));
     sg_nu = (float*)e.arena.alloc((size_t)n_tgt_chains * chw * sizeof(float));
     if (!e.dry()) {
       CDX_CUDA(cudaMemcpyAsync(sg_rows_dev, sg_rows.data(), sg_rows.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
       CDX_CUDA(cudaMemsetAsync(sg_nu, 0, (size_t)n_tgt_chains * chw * sizeof(float), s));
     }
+  }
+  if (sg_mask) {
+    std::vector<int> span(sg_rows.size());
+    for (size_t r = 0; r < span.size(); ++r) span[r] = a.sega_mask->n_tokens[r % sg_m];
+    int* span_dev = (int*)e.arena.alloc(span.size() * sizeof(int));
+    if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(span_dev, span.data(), span.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    probe.rows = sg_rows_dev; probe.span = span_dev; probe.n_rows = (int)sg_rows.size(); probe.tokens = gh * gw;
+    probe.map = (float*)e.arena.alloc(sg_rows.size() * gh * gw * sizeof(float));
   }
   // attention control: the row table maps each target chain's cond row to its group's source row (every other row to itself); with
   // a token map, the V context holds A_j . c_tgt[j] on those rows and every other row's own context.  Both fixed for the loop
@@ -436,6 +456,7 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     f.sg_m = sg_m; f.sg_rows = sg_rows_dev; f.sg_thr = sg_thr; f.sg_nu = sg_nu;
     for (int q = 0; q < sg_m; ++q) { f.sg_scale[q] = g.scale[q]; f.sg_lambda[q] = g.threshold[q]; }
     f.sg_mu = g.momentum_scale; f.sg_beta = g.beta; f.sg_beta1 = g.beta1;
+    f.sg_mask = sg_mask; f.sg_map = probe.map; f.sg_gh = gh; f.sg_gw = gw; f.w = a.w;
   }
   {
     LatentChains in = f;
@@ -459,7 +480,7 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.pnp_attn = a.pnp && i < a.pnp->attention_steps;
       const size_t stat0 = e.stat_dry;
       unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true,
-                   a.ctl || a.mutual || a.pnp ? &actl : nullptr);
+                   a.ctl || a.mutual || a.pnp ? &actl : nullptr, sg_mask ? &probe : nullptr);
       CDX_CHECK(!sg_m || !e.dry() || e.stat_dry - stat0 <= e.stat_cap,
                 "semantic guidance: a %d-row U-Net call needs %zu GroupNorm statistics doubles, the pool holds %zu: fewer images or concepts",
                 rows, e.stat_dry - stat0, e.stat_cap);
@@ -887,7 +908,8 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
                           float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream, const float* mask,
                           const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer,
-                          const PnpLoop* pnp = nullptr, const cdx_semantic_guidance* sega = nullptr, const float* c_edit = nullptr) {
+                          const PnpLoop* pnp = nullptr, const cdx_semantic_guidance* sega = nullptr, const float* c_edit = nullptr,
+                          const cdx_semantic_attn_mask* sega_mask = nullptr) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -899,7 +921,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
     a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
     a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer; a.pnp = pnp;
-    a.sega = sega; a.c_edit = c_edit;
+    a.sega = sega; a.c_edit = c_edit; a.sega_mask = sega_mask;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -939,6 +961,17 @@ int cdx_cycle_lockstep_semantic(cdx_net* un, const float* x0, const float* c_src
   if (!sg || !c_edit) return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_semantic: null guidance or concept contexts"); });
   return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
                         B, C, h, w, stream, mask, nullptr, nullptr, false, 0, 0, nullptr, sg, c_edit);
+}
+
+int cdx_cycle_lockstep_semantic_attn(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
+                                     float src_scale, float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps,
+                                     const float* noise, float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                                     void* stream, const float* mask, const float* c_edit, const cdx_semantic_guidance* sg,
+                                     const cdx_semantic_attn_mask* am) {
+  if (!sg || !c_edit || !am)
+    return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_semantic_attn: null guidance, concept contexts or mask settings"); });
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, nullptr, nullptr, false, 0, 0, nullptr, sg, c_edit, am);
 }
 
 int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
@@ -1372,6 +1405,14 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
       if (t) for (int b = 0; b < B; ++b) CDX_CHECK(t[b] >= 0 && t[b] < B, "op_attention_net: row table entry %d = %d outside [0, %d)", b, t[b], B);
     if (d->acc_rows) for (int r = 0; r < d->n_acc; ++r) CDX_CHECK(d->acc_rows[r] >= 0 && d->acc_rows[r] < B, "op_attention_net: acc_rows[%d] outside [0, %d)", r, B);
     const bool tables = d->qk_rows || d->kv_rows || d->acc_rows;
+    const bool probing = d->n_probe > 0;
+    if (probing) {
+      CDX_CHECK(kind == 1 && d->probe_rows && d->probe_spans && d->probe_map && L >= 3, "op_attention_net: the probe needs kind 1, L >= 3, rows, "
+                "spans and a map");
+      for (int i = 0; i < d->n_probe; ++i)
+        CDX_CHECK(d->probe_rows[i] >= 0 && d->probe_rows[i] < B && d->probe_spans[i] >= 1 && d->probe_spans[i] <= L - 2,
+                  "op_attention_net: probe row %d = %d of %d, span %d outside 1..%d", i, d->probe_rows[i], B, d->probe_spans[i], L - 2);
+    }
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
     int plan[7] = {};
@@ -1385,6 +1426,8 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
         return dev;
       };
       const int *qk_dev = stage(d->qk_rows, B), *kv_dev = stage(d->kv_rows, B), *acc_dev = stage(d->acc_rows, d->n_acc);
+      const int *probe_dev = probing ? stage(d->probe_rows, d->n_probe) : nullptr, *span_dev = probing ? stage(d->probe_spans, d->n_probe) : nullptr;
+      ProbeOperands po;
       // a range slot as the network's producer leaves it: max |x| over the tensor, or the caller's (conservative) value
       auto slot_of = [&](float value, const float* x, long long rows, int cols) {
         float* slot = e.amax_slot();
@@ -1474,6 +1517,7 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
             context_split_h16(e, d->kv, (int)Mk, C, kv_slot, k_hi, k_lo, vt_hi, vt_lo, s);
             pl.q_hi = q_hi; pl.q_lo = q_lo; pl.k_hi = k_hi; pl.k_lo = k_lo; pl.vt_hi = vt_hi; pl.vt_lo = vt_lo;
             pl.q_amax = q_slot; pl.k_amax = kv_slot; pl.v_amax = kv_slot;
+            po.fmt = ProbeOperands::H16; po.q = d->q; po.k = k_hi; po.k_lo = k_lo; po.k_amax = kv_slot;
           } else {
             float *q_hi, *q_lo, *k_hi, *k_lo, *vt_hi, *vt_lo;
             tf32_planes(d->q, M, C, C, q_hi, q_lo);
@@ -1484,7 +1528,9 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
             nhwc_to_nchw(e, vr, vt, 1, C, (int)Mk, s);
             tf32_planes(vt, 1, (int)(Mk * C), Mk * C, vt_hi, vt_lo);
             pl.q_hi = q_hi; pl.q_lo = q_lo; pl.k_hi = k_hi; pl.k_lo = k_lo; pl.vt_hi = vt_hi; pl.vt_lo = vt_lo;
+            po.fmt = ProbeOperands::TF32; po.q = q_hi; po.q_lo = q_lo; po.k = k_hi; po.k_lo = k_lo;
           }
+          po.ldq = C; po.ldk = C; po.Lk = Lp;
           done = flash_attention(e, pl, d->out, C, B, N, L, Lp, Lp, heads, dh, d->scale, s, qk_dev, acc_dev, d->n_acc, kv_dev);
           fused_plan(h16 ? (e.attn_one ? 4 : 2) : 3, h16, N, Lp, Lp);
         }
@@ -1495,7 +1541,9 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
             CDX_CUDA(cudaMemcpy2DAsync(kv, (size_t)L * 2 * C * 4, d->kv, (size_t)Lp * 2 * C * 4, (size_t)L * 2 * C * 4, B, cudaMemcpyDeviceToDevice, s));
           attention(e, d->q, C, kv, 2 * C, kv + C, 2 * C, d->out, C, B, N, L, heads, dh, dh, d->scale, s);
           plan[0] = 0;
+          po.fmt = ProbeOperands::F32; po.q = d->q; po.q_lo = nullptr; po.ldq = C; po.k = kv; po.k_lo = nullptr; po.ldk = 2 * C; po.Lk = L;
         }
+        if (probing) attn_probe(e, po, probe_dev, span_dev, d->n_probe, d->probe_map, N, L, heads, dh, d->scale, false, s);
       } else {
         CDX_CHECK(!tables, "op_attention_net: row tables need a fused route");
         attention(e, d->q, C, d->k, C, d->v, C, d->out, C, B, N, L, heads, dh, dh, d->scale, s, d->causal != 0);
@@ -1719,6 +1767,11 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
       for (int q = 0; q < d->sg_m; ++q)
         CDX_CHECK(d->sg_lambda[q] >= 0.0f && d->sg_lambda[q] < 1.0f, "op_latent_chains: sg_lambda[%d]=%g outside [0, 1)", q, d->sg_lambda[q]);
     }
+    CDX_CHECK(d->sg_mask >= 0 && d->sg_mask <= 2 && (!d->sg_mask || d->sg_m), "op_latent_chains: sg_mask=%d with sg_m=%d", d->sg_mask, d->sg_m);
+    if (d->sg_mask && stage != 0)
+      CDX_CHECK(d->sg_map && d->sg_gh >= 2 && d->sg_gw >= 2 && d->w == 4 * d->sg_gw && d->hw == 16 * d->sg_gh * d->sg_gw,
+                "op_latent_chains: sg_mask needs sg_map on an sg_gh x sg_gw >= 2x2 grid of the (4 sg_gh) x (4 sg_gw) latent (w=%d hw=%d, %dx%d)",
+                d->w, d->hw, d->sg_gh, d->sg_gw);
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
     std::vector<Chain> ch(n_chains);
@@ -1745,6 +1798,7 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
       a.sg_m = d->sg_m; a.sg_rows = sg_rows; a.sg_thr = d->sg_thr; a.sg_nu = d->sg_nu;
       for (int q = 0; q < d->sg_m; ++q) { a.sg_scale[q] = d->sg_scale[q]; a.sg_lambda[q] = d->sg_lambda[q]; }
       a.sg_active = d->sg_active; a.sg_apply = d->sg_apply; a.sg_mu = d->sg_mu; a.sg_beta = d->sg_beta; a.sg_beta1 = d->sg_beta1;
+      a.sg_mask = d->sg_mask; a.sg_map = d->sg_map; a.sg_gh = d->sg_gh; a.sg_gw = d->sg_gw; a.w = d->w;
       if (stage == 0) latent_chains_init(e, a, s);
       else if (stage == 2) semantic_thresholds(e, a, s);
       else latent_chains_step(e, a, s);

@@ -230,6 +230,23 @@ bool self_attention_tf32_padded(Engine& e, const float* qk_hi, const float* qk_l
 // both with the exponent of the one slot of the whole projection
 void context_split_h16(Engine& e, const float* kv, int Mk, int C, const float* slot, void* k_hi, void* k_lo, void* vt_hi, void* vt_lo,
                        cudaStream_t s);
+// LEDITS++'s cross-attention probe (attn_probe): the Q and K of one cross-attention layer in the form its route holds them, so the
+// probabilities are those of the operands the layer multiplied.  F32 (unfused routes): fp32 q, fp32 k.  H16 (fused fp16 planes):
+// fp32 q (the projection before its split), K as __half planes of k * 2^e with e = h16_exp_of(*k_amax), k = (hi + lo) * 2^-e (hi
+// only when k_lo is null: mode 5).  TF32 (fused TF32 planes): q = q_hi + q_lo, k = k_hi + k_lo.  Image b's query p at row b*N + p
+// of ldq, its key j at row b*Lk + j of ldk (Lk: the stored keys per image, the padded context on the fused routes); head h at column
+// h*d of both.
+struct ProbeOperands {
+  enum Fmt { F32, H16, TF32 } fmt = F32;
+  const float* q = nullptr; const float* q_lo = nullptr; int ldq = 0;
+  const void* k = nullptr; const void* k_lo = nullptr; int ldk = 0; int Lk = 0;
+  const float* k_amax = nullptr;
+};
+// map[i, p] (= or += with accumulate) sum over heads h (in order) of sum over j in 1..span[i] of softmax_j(scale * q_p . k_j) over
+// all L keys, for the U-Net row rows[i] (device [n_rows] both).  One warp owns each (i, p): the dot in channel order, the softmax
+// sums in a fixed lane order, no atomics, so a row's map does not depend on the other rows or their count.
+void attn_probe(Engine& e, const ProbeOperands& o, const int* rows, const int* span, int n_rows, float* map, int N, int L, int heads, int d,
+                float scale, bool accumulate, cudaStream_t s);
 void split_planes(Engine& e, const float* w, float* hi, float* lo, size_t n, cudaStream_t s);   // hi = rn_tf32(w), lo = rn_tf32(w - hi)
 // fp16 split of w * 2^exp: hi = fp16(w'), lo = fp16(w' - hi)  (hi / lo: __half arrays)
 void split_planes_h16(Engine& e, const float* w, void* hi, void* lo, size_t n, int exp, cudaStream_t s);
@@ -346,6 +363,14 @@ struct LatentChains {
   unsigned sg_active = 0;                        // bit k: concept k is before its cooldown step
   int sg_apply = 0;                              // the step is past the warmup: o-hat += G
   float sg_mu = 0.f, sg_beta = 0.f, sg_beta1 = 0.f;
+  // LEDITS++'s implicit masks (cdx_cycle_lockstep_semantic_attn), sg_mask > 0: concept k of target chain t keeps psi_k at latent
+  // pixel (y, x) where the smoothed cross-attention map of its row, sm(y/4, x/4) (ledits_smooth over sg_map[t*sg_m + k], an sg_gh x
+  // sg_gw grid), reaches sg_thr[(t*sg_m + k)*2]; with sg_mask == 2 also where the channel sum of |psi_k| at (y, x) reaches
+  // sg_thr[(t*sg_m + k)*2 + 1].  The per-channel thresholds are then not used.  Kept last, as the fields above.
+  int sg_mask = 0;
+  const float* sg_map = nullptr;                 // device [n_src*K*sg_m, sg_gh*sg_gw]: the probe's raw maps
+  int sg_gh = 0, sg_gw = 0;
+  int w = 0;                                     // latent width: pixel r % hw = y*w + x
 };
 constexpr int SEMANTIC_MAX_CONCEPTS = 8;
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s);
@@ -353,7 +378,9 @@ void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s);
 // SEGA's threshold stage: one launch, one CTA per (target chain, concept, channel) plane of hw elements.  theta = Q(sg_lambda[k],
 // |psi_k| over the plane): r = lambda*(hw - 1) in fp32, the floor(r)-th and ceil(r)-th smallest values found exactly by a radix
 // select over the float bit patterns (re-read from eout each pass: no shared-memory limit on the plane size), then torch.quantile's
-// linear interpolation with ATen's scalar lerp, each op rounded.  Writes a.sg_thr.
+// linear interpolation with ATen's scalar lerp, each op rounded.  Writes a.sg_thr.  With sg_mask > 0 the planes are instead, per
+// (target chain, concept), the smoothed attention map (sg_gh*sg_gw values) and, with sg_mask == 2, the channel sum of |psi_k| (hw
+// values): one or two CTAs per concept row, still one launch.
 void semantic_thresholds(Engine& e, const LatentChains& a, cudaStream_t s);
 // image-resolution mask [B,1,H,W] -> [B,1,H/f,W/f]: mean of each f x f block, summed row by row then divided by f*f (avg_pool2d)
 void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, int f, cudaStream_t s);

@@ -284,13 +284,42 @@ __global__ void latent_chains_init_kernel(const LatentChains a) {
     }
   }
 }
+// LEDITS++'s implicit masks.  The 3x3 smoothing of a raw attention map m (gh x gw, gh, gw >= 2) with reflect padding of 1 (index -1
+// -> 1, n -> n - 2), as diffusers' GaussianSmoothing(kernel_size=3, sigma=0.5): weights w_ab = fp32(g_a g_b / (sum g)^2), g = (e^-1,
+// 1, e^-1) formed in double (corner, edge, centre below); the nine products in row-major order, each rounded, added left to right.
+// The threshold stage and the step kernel both call it, so the mask the step applies is the one the stage thresholded.
+constexpr float LEDITS_W_CORNER = 0x1.6ffa7p-5f, LEDITS_W_EDGE = 0x1.f42264p-4f, LEDITS_W_CENTRE = 0x1.53e064p-2f;
+__device__ __forceinline__ int ledits_reflect(int i, int n) { return i < 0 ? 1 : i >= n ? n - 2 : i; }
+__device__ __forceinline__ float ledits_smooth(const float* m, int gh, int gw, int y, int x) {
+  float s = 0.f;
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      const float w = (a == 1 && b == 1) ? LEDITS_W_CENTRE : (a == 1 || b == 1) ? LEDITS_W_EDGE : LEDITS_W_CORNER;
+      const float pr = MUL(w, __ldcg(m + (size_t)ledits_reflect(y + a - 1, gh) * gw + ledits_reflect(x + b - 1, gw)));
+      s = (a || b) ? ADD(s, pr) : pr;
+    }
+  return s;
+}
+// sum over channels c = 0, 1, ... of |sc * (o_k - o_uc)| at latent pixel p (ok, ou: the rows' [C, hw] planes), one rounded op each
+__device__ __forceinline__ float ledits_chansum(const float* ok, const float* ou, int C, int hw, int p, float sc) {
+  float s = 0.f;
+  for (int c = 0; c < C; ++c) {
+    const float v = fabsf(MUL(sc, SUB(__ldcg(ok + (size_t)c * hw + p), __ldcg(ou + (size_t)c * hw + p))));
+    s = c ? ADD(s, v) : v;
+  }
+  return s;
+}
+
 // One step of the loop: the source half once per source chain, the target half once per target chain with the recovered noise held
 // in a register.  Under v-prediction each target chain forms e_t and pred_x0 from its own x_t and v.  MASK (the driver guarantees a
 // source chain at every step): each target x_{t-1} is blended with the source's x_{t-1}, a posterior sample of q(x_{t-1} | x_t, x0)
 // of the real image at the same noise level (x0 itself on the last step), so the unmasked region stays on the image's trajectory.
 // SEGA (a.sg_m > 0): each target chain's guidance-combined output takes its semantic guidance term G (LatentChains), formed from its
 // concept rows, its uncond row, the step's thresholds and its momentum before the e_t / pred_x0 conversion; its concept rows are
-// written with its next x_t.
+// written with its next x_t.  SEGA = 1 + a.sg_mask: 1 SEGA's per-channel thresholds, 2 LEDITS++'s
+// attention mask, 3 the attention mask and the channel-summed one.
 template <int PRED, int MASK, int SEGA = 0>
 __global__ void latent_chains_step_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
@@ -325,7 +354,20 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
         for (int q = 0; q < a.sg_m; ++q) {
           const int tq = (int)t * a.sg_m + q;
           const float psi = MUL(a.sg_scale[q], SUB(__ldcg(a.eout + (size_t)a.sg_rows[tq] * a.chw + r), ou));
-          const float g = ((a.sg_active >> q) & 1u) && fabsf(psi) >= __ldcg(a.sg_thr + (size_t)tq * C + ch) ? psi : 0.f;
+          float g;
+          if constexpr (SEGA == 1) {
+            g = ((a.sg_active >> q) & 1u) && fabsf(psi) >= __ldcg(a.sg_thr + (size_t)tq * C + ch) ? psi : 0.f;
+          } else {               // LEDITS++: the concept's attention mask, and with SEGA == 3 its channel-summed mask
+            bool keep = (a.sg_active >> q) & 1u;
+            if (keep) {
+              const int px = (int)r % a.hw, y = px / a.w, x = px - y * a.w;
+              keep = ledits_smooth(a.sg_map + (size_t)tq * a.sg_gh * a.sg_gw, a.sg_gh, a.sg_gw, y / 4, x / 4) >= __ldcg(a.sg_thr + (size_t)tq * 2);
+              if constexpr (SEGA == 3)
+                keep = keep && ledits_chansum(a.eout + (size_t)a.sg_rows[tq] * a.chw, a.eout + (size_t)(tc.row2 >= 0 ? tc.row2 : tc.row) * a.chw, C,
+                                              a.hw, px, a.sg_scale[q]) >= __ldcg(a.sg_thr + (size_t)tq * 2 + 1);
+            }
+            g = keep ? psi : 0.f;
+          }
           S = q ? ADD(S, g) : g;
         }
         const float nu = __ldcg(a.sg_nu + ti);
@@ -361,16 +403,12 @@ constexpr int SEMANTIC_THREADS = 512;
 __device__ __forceinline__ unsigned semantic_abs_bits(const float* ok, const float* ou, int p, float sc) {
   return __float_as_uint(fabsf(MUL(sc, SUB(__ldcg(ok + p), __ldcg(ou + p)))));
 }
-__global__ void __launch_bounds__(SEMANTIC_THREADS) semantic_threshold_kernel(const LatentChains a) {
-  __shared__ unsigned hist[256];
-  __shared__ unsigned s_digit, s_below, s_count, s_min;
-  const int C = a.chw / a.hw, n = a.hw, plane = blockIdx.x;
-  const int c = plane % C, tq = plane / C, q = tq % a.sg_m, t = tq / a.sg_m;
-  const Chain tc = a.chains[a.n_src + t];
-  const float* ou = a.eout + (size_t)(tc.row2 >= 0 ? tc.row2 : tc.row) * a.chw + (size_t)c * n;
-  const float* ok = a.eout + (size_t)a.sg_rows[tq] * a.chw + (size_t)c * n;
-  const float sc = a.sg_scale[q];
-  const float rk = MUL(a.sg_lambda[q], (float)(n - 1));
+// *out <- Q(lambda, the n values val(p)) by the radix select and the lerp above (thread 0 writes).  val returns the bit pattern of a
+// non-negative float
+template <class Val>
+__device__ __forceinline__ void semantic_select(const Val& val, int n, float lambda, float* out, unsigned* hist, unsigned& s_digit,
+                                                unsigned& s_below, unsigned& s_count, unsigned& s_min) {
+  const float rk = MUL(lambda, (float)(n - 1));
   const float fl = floorf(rk);
   const unsigned lo = (unsigned)fl, hi = (unsigned)ceilf(rk);
   const float w = SUB(rk, fl);
@@ -379,7 +417,7 @@ __global__ void __launch_bounds__(SEMANTIC_THREADS) semantic_threshold_kernel(co
     for (int i = threadIdx.x; i < 256; i += SEMANTIC_THREADS) hist[i] = 0;
     __syncthreads();
     for (int p = threadIdx.x; p < n; p += SEMANTIC_THREADS) {
-      const unsigned u = semantic_abs_bits(ok, ou, p, sc);
+      const unsigned u = val(p);
       if ((u & known) == prefix) atomicAdd(&hist[(u >> shift) & 255u], 1u);
     }
     __syncthreads();
@@ -416,7 +454,7 @@ __global__ void __launch_bounds__(SEMANTIC_THREADS) semantic_threshold_kernel(co
     __syncthreads();
     unsigned m = 0xffffffffu;
     for (int p = threadIdx.x; p < n; p += SEMANTIC_THREADS) {
-      const unsigned u = semantic_abs_bits(ok, ou, p, sc);
+      const unsigned u = val(p);
       if (u > prefix) m = min(m, u);
     }
     atomicMin(&s_min, m);
@@ -424,7 +462,41 @@ __global__ void __launch_bounds__(SEMANTIC_THREADS) semantic_threshold_kernel(co
   }
   if (threadIdx.x == 0) {
     const float vlo = __uint_as_float(prefix), vhi = above ? __uint_as_float(s_min) : vlo;
-    a.sg_thr[plane] = w < 0.5f ? ADD(vlo, MUL(w, SUB(vhi, vlo))) : SUB(vhi, MUL(SUB(vhi, vlo), SUB(1.0f, w)));   // ATen lerp
+    *out = w < 0.5f ? ADD(vlo, MUL(w, SUB(vhi, vlo))) : SUB(vhi, MUL(SUB(vhi, vlo), SUB(1.0f, w)));   // ATen lerp
+  }
+}
+// MASKM (LatentChains::sg_mask) 0: SEGA's planes.  1, 2: block b owns concept row tq = b / P (P = MASKM planes per row), plane kind
+// b % P: 0 the smoothed attention map (threshold at sg_thr[tq*2]), 1 the channel sum of |psi_k| (at sg_thr[tq*2 + 1])
+template <int MASKM>
+__global__ void __launch_bounds__(SEMANTIC_THREADS) semantic_threshold_kernel(const LatentChains a) {
+  __shared__ unsigned hist[256];
+  __shared__ unsigned s_digit, s_below, s_count, s_min;
+  const int C = a.chw / a.hw;
+  if constexpr (MASKM == 0) {
+    const int n = a.hw, plane = blockIdx.x;
+    const int c = plane % C, tq = plane / C, q = tq % a.sg_m, t = tq / a.sg_m;
+    const Chain tc = a.chains[a.n_src + t];
+    const float* ou = a.eout + (size_t)(tc.row2 >= 0 ? tc.row2 : tc.row) * a.chw + (size_t)c * n;
+    const float* ok = a.eout + (size_t)a.sg_rows[tq] * a.chw + (size_t)c * n;
+    const float sc = a.sg_scale[q];
+    semantic_select([&](int p) { return semantic_abs_bits(ok, ou, p, sc); }, n, a.sg_lambda[q], a.sg_thr + plane, hist, s_digit, s_below,
+                    s_count, s_min);
+  } else {
+    const int tq = blockIdx.x / MASKM, kind = blockIdx.x % MASKM, q = tq % a.sg_m, t = tq / a.sg_m;
+    float* out = a.sg_thr + (size_t)tq * 2 + kind;
+    if (kind == 0) {
+      const int gh = a.sg_gh, gw = a.sg_gw;
+      const float* mp = a.sg_map + (size_t)tq * gh * gw;
+      semantic_select([&](int p) { return __float_as_uint(ledits_smooth(mp, gh, gw, p / gw, p % gw)); }, gh * gw, a.sg_lambda[q], out, hist,
+                      s_digit, s_below, s_count, s_min);
+    } else {
+      const Chain tc = a.chains[a.n_src + t];
+      const float* ou = a.eout + (size_t)(tc.row2 >= 0 ? tc.row2 : tc.row) * a.chw;
+      const float* ok = a.eout + (size_t)a.sg_rows[tq] * a.chw;
+      const float sc = a.sg_scale[q];
+      semantic_select([&](int p) { return __float_as_uint(ledits_chansum(ok, ou, C, a.hw, p, sc)); }, a.hw, a.sg_lambda[q], out, hist, s_digit,
+                      s_below, s_count, s_min);
+    }
   }
 }
 
@@ -820,6 +892,28 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
 
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s) { LAUNCH1(latent_chains_init_kernel, a.n, a); }
 void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
+  if (a.sg_m && a.sg_mask) {
+    CDX_CHECK(a.sg_mask <= 2 && a.sg_map && a.sg_gh >= 2 && a.sg_gw >= 2 && a.w > 0 && a.hw == (4 * a.sg_gh) * (4 * a.sg_gw) && a.w == 4 * a.sg_gw,
+              "latent_chains_step: mask mode %d over a %dx%d map, hw=%d w=%d", a.sg_mask, a.sg_gh, a.sg_gw, a.hw, a.w);
+    if (a.sg_mask == 1) {
+      if (a.mask) {
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 2>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 1, 2>), a.n, a);
+      } else {
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 2>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 0, 2>), a.n, a);
+      }
+    } else {
+      if (a.mask) {
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 3>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 1, 3>), a.n, a);
+      } else {
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 3>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 0, 3>), a.n, a);
+      }
+    }
+    return;
+  }
   if (a.sg_m) {
     if (a.mask) {
       if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 1>), a.n, a);
@@ -842,11 +936,25 @@ void semantic_thresholds(Engine& e, const LatentChains& a, cudaStream_t s) {
   CDX_CHECK(a.sg_m >= 1 && a.sg_m <= SEMANTIC_MAX_CONCEPTS && a.hw > 0 && a.chw % a.hw == 0, "semantic_thresholds: m=%d chw=%d hw=%d", a.sg_m,
             a.chw, a.hw);
   if (e.dry()) return;
-  const long long planes = (long long)a.n_src * a.K * a.sg_m * (a.chw / a.hw);
+  const long long rows = (long long)a.n_src * a.K * a.sg_m;
+  if (a.sg_mask) {
+    CDX_CHECK(a.sg_mask <= 2 && a.sg_map && a.sg_gh >= 2 && a.sg_gw >= 2 && a.hw == (4 * a.sg_gh) * (4 * a.sg_gw),
+              "semantic_thresholds: mask mode %d over a %dx%d map, hw=%d", a.sg_mask, a.sg_gh, a.sg_gw, a.hw);
+    if (rows == 0) return;
+    const long long blocks = rows * a.sg_mask;
+    ProfScope ps(e, s, PROF_ELEMENTWISE, 0.0, 4.0 * rows * ((double)a.sg_gh * a.sg_gw + (a.sg_mask == 2 ? 2.0 * a.chw : 0.0)), 1);
+    ps.note("semantic attention-mask thresholds %lld rows, %dx%d maps%s", rows, a.sg_gh, a.sg_gw, a.sg_mask == 2 ? " + channel sums" : "");
+    if (a.sg_mask == 1) semantic_threshold_kernel<1><<<(unsigned)blocks, SEMANTIC_THREADS, 0, s>>>(a);
+    else semantic_threshold_kernel<2><<<(unsigned)blocks, SEMANTIC_THREADS, 0, s>>>(a);
+    CDX_CUDA(cudaGetLastError());
+    e.launches++;
+    return;
+  }
+  const long long planes = rows * (a.chw / a.hw);
   if (planes == 0) return;
   ProfScope ps(e, s, PROF_ELEMENTWISE, 0.0, 2.0 * 4.0 * planes * a.hw, 1);     // algorithmic: o_k and o_uc read once
   ps.note("semantic thresholds %lld planes x %d", planes, a.hw);
-  semantic_threshold_kernel<<<(unsigned)planes, SEMANTIC_THREADS, 0, s>>>(a);
+  semantic_threshold_kernel<0><<<(unsigned)planes, SEMANTIC_THREADS, 0, s>>>(a);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
 }

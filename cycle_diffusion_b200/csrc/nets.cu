@@ -694,6 +694,8 @@ struct UNetExec : Exec {
   int ctx_lp = 0;                          // context rows per image, padded for the fused cross-attention
   bool kv_reuse = false, kv_hit = false;   // loop mode: context K / V live in n.ctxkv (kv_hit: already computed)
   const AttnControl* ctl = nullptr;        // attention control of this call, or null
+  const AttnProbe* probe = nullptr;        // cross-attention probe of this call, or null
+  int probed = 0;                          // layers probed so far in this call
   int st_layer = 0;                        // SpatialTransformers run so far in this call (AttnControl::start_layer counts them)
   // the contexts the cross-attention projects: [0] the call's context, [1] the V' context (AttnControl::ctx_v), [2] the refine
   // context (ctx_w); src null when absent.  pad: src zero-padded to ctx_lp rows per image (fused route only); amax: range slot of
@@ -739,6 +741,11 @@ struct UNetExec : Exec {
       if (k_hi) linear_into(x.pad, D, D, nullptr, 0, 0, Mk, n.P(t + ".attn2.to_k.weight"), C, nullptr, nullptr, 0, k_hi, C, k_lo, x.amax);
       linear_into(n.P(t + ".attn2.to_v.weight"), D, D, nullptr, 0, 0, C, x.pad, Mk, nullptr, nullptr, 0, vt_hi, Mk, vt_lo, nullptr, nullptr, slot);
     }
+  }
+  // the probe of one layer: the first probed layer of the call stores the map, later ones add
+  void probe_layer(const ProbeOperands& po, int HW, int heads, int d, float scale) {
+    attn_probe(e, po, probe->rows, probe->span, probe->n_rows, probe->map, HW, ctx_len, heads, d, scale, probed > 0, s);
+    ++probed;
   }
   bool oai;
   UNetExec(Net& net, cudaStream_t st) : Exec(net, st), oai(net.kind == NET_UNET_OPENAI) {}
@@ -930,6 +937,9 @@ struct UNetExec : Exec {
       const bool use_v3 = crow && wmap;
       bool done = false;
       Tensor q;
+      // LEDITS++'s probe: this layer's Q and K as its route multiplied them
+      const bool probe_here = probe && HW == probe->tokens && (p.rfind("input_blocks.", 0) == 0 || p.rfind("output_blocks.", 0) == 0);
+      ProbeOperands po;
       const bool flash_ok = cx[0].pad && flash_eligible(e, HW, ctx_len, d, C);
       CDX_CHECK(!crow || flash_ok, "attention control: cross-attention at HW=%d d=%d would take the unfused route (mma mode "
                 "and head width must run the fused kernel)", HW, d);
@@ -957,11 +967,13 @@ struct UNetExec : Exec {
           void* q_lo = lo ? e.arena.alloc((size_t)M * C * 2) : nullptr;
           split_rows_h16(e, qf.p, M, C, C, q_hi, q_lo, C, qf.amax, s);
           pl.q_hi = q_hi; pl.q_lo = q_lo; pl.q_amax = qf.amax;
+          po.fmt = ProbeOperands::H16; po.q = qf.p;
         } else {
           float* q_hi = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
           float* q_lo = (float*)e.arena.alloc((size_t)M * C * sizeof(float));
           linear_into(n2.p, C, C, nullptr, 0, 0, M, n.P(t + ".attn2.to_q.weight"), C, nullptr, nullptr, 0, q_hi, C, q_lo, n2.amax);
           pl.q_hi = q_hi; pl.q_lo = q_lo;
+          po.fmt = ProbeOperands::TF32; po.q = q_hi; po.q_lo = q_lo;
         }
         if (!kv_hit) {
           context_planes(cx[0], t, C, Mk, a.amax, k_hi, k_lo, vt_hi, vt_lo);
@@ -983,6 +995,10 @@ struct UNetExec : Exec {
           done = flash_attention(e, pl, a.p, C, B, HW, ctx_len, ctx_lp, ctx_lp, heads, d, scale, s, nullptr, ctl->own_rows, ctl->n_own);
           CDX_CHECK(done, "flash cross-attention rejected the refine term (HW=%d d=%d L=%d)", HW, d, ctx_len);
         }
+        if (probe_here) {
+          po.ldq = C; po.k = k_hi; po.k_lo = k_lo; po.ldk = C; po.Lk = ctx_lp; po.k_amax = a.amax;
+          probe_layer(po, HW, heads, d, scale);
+        }
       }
       if (use_v3) a.amax = sum_amax;            // the sum of a convex combination of V' rows and one of V'' rows
       else if (use_v2) a.amax = v2_amax;        // the output is a convex combination of V' rows
@@ -993,6 +1009,10 @@ struct UNetExec : Exec {
         if (!kv_hit) linear_into(cx[0].src, D, D, nullptr, 0, 0, B * ctx_len, n.P(t + ".attn2.to_k.weight"), 2 * C, nullptr, nullptr, 0, kv, 2 * C,
                                  nullptr, cx[0].amax, nullptr, a.amax);
         attention(e, q.p, C, kv, 2 * C, kv + C, 2 * C, a.p, C, B, HW, ctx_len, heads, d, d, scale, s);
+        if (probe_here) {
+          po.fmt = ProbeOperands::F32; po.q = q.p; po.ldq = C; po.k = kv; po.ldk = 2 * C; po.Lk = ctx_len;
+          probe_layer(po, HW, heads, d, scale);
+        }
       }
       h3 = linear(a, t + ".attn2.to_out.0", true, h2.p);
     }
@@ -1297,7 +1317,7 @@ struct VaeExec : Exec {
 }  // namespace
 
 void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* ctx, int ctx_len, float* out_nchw, int B, int H, int W,
-                  cudaStream_t s, bool reuse_ctx, const AttnControl* ctl) {
+                  cudaStream_t s, bool reuse_ctx, const AttnControl* ctl, const AttnProbe* probe) {
   CDX_CHECK(n.kind == NET_UNET_OPENAI || n.kind == NET_UNET_IDDPM || n.kind == NET_UNET_DDPM, "unet_forward on a non-U-Net");
   CDX_CHECK(n.finalized, "unet_forward before finalize");
   if (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0) CDX_CHECK(ctx != nullptr && ctx_len > 0, "unet_forward: the SD/LDM U-Net needs a context");
@@ -1310,8 +1330,14 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
   CDX_CHECK(!ctl || (!!ctl->qk_row + !!ctl->kv_row + !!ctl->pnp_row) <= 1,
             "attention control: Prompt-to-Prompt, mutual self-attention and Plug-and-Play are exclusive in one call");
   ex.ctl = ctl;
+  CDX_CHECK(!probe || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0 && probe->rows && probe->span && probe->map &&
+                       probe->n_rows >= 1 && probe->tokens >= 1),
+            "attention probe: SD / LDM U-Nets with a context, and a row list, spans and a map");
+  ex.probe = probe;
   if (n.kind == NET_UNET_DDPM) { ex.forward_ddpm(x_nchw, t_dev, out_nchw, B, H, W); return; }
   ex.forward(x_nchw, t_dev, ctx, ctx_len, out_nchw, B, H, W);
+  CDX_CHECK(!probe || ex.probed > 0, "attention probe: no cross-attention of %d tokens in the input or output blocks (a %dx%d latent)",
+            probe->tokens, H, W);
   if (ex.kv_reuse && !n.eng->dry()) {
     n.ctxkv.valid = true;
     n.ctxkv.ctx = ctx; n.ctxkv.ctx_v = ctl ? ctl->ctx_v : nullptr; n.ctxkv.ctx_w = ctl ? ctl->ctx_w : nullptr; n.ctxkv.L = ctx_len; n.ctxkv.B = B;

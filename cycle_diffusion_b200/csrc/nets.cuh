@@ -117,11 +117,23 @@ struct AttnControl {
   int pnp_layer = 0;
 };
 
+// Cross-attention probe of one SD / LDM U-Net call (LEDITS++'s implicit masks, driven by the semantic-guidance loop in cabi.cu).  It
+// changes no output: the cross-attention of every SpatialTransformer in the input and output blocks (never the middle block) whose
+// token count is `tokens` also runs attn_probe on the operands its route multiplied, for the listed rows: the first such layer
+// stores map [n_rows, tokens], later ones add.  A call in which no layer matches is an error.
+struct AttnProbe {
+  const int* rows = nullptr;            // device [n_rows]: U-Net rows
+  const int* span = nullptr;            // device [n_rows]: tokens 1..span[i] of row i's context
+  int n_rows = 0;
+  float* map = nullptr;                 // device [n_rows, tokens]
+  int tokens = 0;
+};
+
 // forward executors (enqueue only; caller handles arena dry-run)
 // reuse_ctx: the caller guarantees `ctx` is unchanged since the previous call with reuse_ctx (and n.ctxkv was invalidated
 // at the start of the loop) -> context K / V projections are taken from n.ctxkv instead of being recomputed
 void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* ctx, int ctx_len, float* out_nchw, int B, int H,
-                  int W, cudaStream_t s, bool reuse_ctx = false, const AttnControl* ctl = nullptr);void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int H, int W, cudaStream_t s);
+                  int W, cudaStream_t s, bool reuse_ctx = false, const AttnControl* ctl = nullptr, const AttnProbe* probe = nullptr);void vae_encode(Net& n, const float* img_nchw, float* moments_nchw, int B, int H, int W, cudaStream_t s);
 void vae_decode(Net& n, const float* z_nchw, float* img_nchw, int B, int h, int w, cudaStream_t s);
 void text_encode(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);
 void text_features(Net& n, const int* ids, float* out, int B, int L, cudaStream_t s);                // CLIP.encode_text   -> [B, proj_dim]

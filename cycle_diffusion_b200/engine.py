@@ -427,17 +427,20 @@ class Engine:
         launch may touch; outputs land in the caller's tensors.
         Semantic guidance: sg_rows [(row) * n_src*K*m] (host ints, the concept rows of target chain t at t*m + k) sets sg_m = m;
         stage 2 is its threshold stage (writes sg_thr), stage 1 then runs the step with the concept terms; sg_scale and sg_lambda are
-        lists of m floats, sg_active / sg_apply / sg_mu / sg_beta / sg_beta1 scalars, sg_thr and sg_nu tensors."""
+        lists of m floats, sg_active / sg_apply / sg_mu / sg_beta / sg_beta1 scalars, sg_thr and sg_nu tensors.  LEDITS++'s masks:
+        sg_mask 1 or 2 with sg_map [n_src*K*m, sg_gh*sg_gw] (a tensor), sg_gh, sg_gw and the latent width w; sg_thr then holds 2
+        thresholds per concept row."""
         sg_rows = fields.pop('sg_rows', None)
         m = len(sg_rows) // max(n_src * K, 1) if sg_rows else 0
         hw = fields.get('hw', 0)
         need = dict(x0=n_src * chw, noise0=n_src * chw, xt=n_src * chw, xn=n_src * chw, noise_next=n_src * chw, xn2=n_src * chw,
                     eout=rows * chw, xin=rows * chw, yt=n_src * K * chw, y_out=n_src * K * chw,
                     z_out=(n_src - 1) * fields.get('z_stride', 0) + chw, eps_in=(n_src - 1) * fields.get('eps_stride', 0) + chw,
-                    mask=n_src * hw, sg_thr=n_src * K * m * (chw // hw if hw else 0), sg_nu=n_src * K * chw)
+                    mask=n_src * hw, sg_thr=n_src * K * m * ((chw // hw if hw else 0) if not fields.get('sg_mask') else 2),
+                    sg_nu=n_src * K * chw, sg_map=n_src * K * m * fields.get('sg_gh', 0) * fields.get('sg_gw', 0))
         assert len(chains) == n_src * (1 + K), f'op_latent_chains: {len(chains)} chains for n_src={n_src}, K={K}'
         table = (_cabi.LatentChain * len(chains))(*[_cabi.LatentChain(int(r), int(r2), float(s)) for r, r2, s in chains])
-        d = _cabi.LatentChainsDesc(chw=chw, n_src=n_src, K=K, rows=rows, chains=table)
+        d = _cabi.LatentChainsMaskDesc(chw=chw, n_src=n_src, K=K, rows=rows, chains=table)
         if sg_rows:
             assert len(sg_rows) == n_src * K * m, f'op_latent_chains: {len(sg_rows)} concept rows for {n_src * K} target chains'
             sg_table = (C.c_int * len(sg_rows))(*[int(r) for r in sg_rows])
@@ -508,16 +511,17 @@ class Engine:
     ATTN_ROUTES = ('generic', 'unfused_tc', 'fused_h16', 'fused_tf32', 'fused_one')
 
     def op_attention_net(self, kind, out, B, N, heads, d, scale, qkv=None, q=None, kv=None, k=None, v=None, L=0, ctx_lp=0, causal=False,
-                         qk_rows=None, kv_rows=None, acc_rows=None, slot=0.0, q_slot=0.0):
+                         qk_rows=None, kv_rows=None, acc_rows=None, slot=0.0, q_slot=0.0, probe_rows=None, probe_spans=None, probe_map=None):
         """One attention with its operands prepared as the network executors prepare them (cdx_op_attention_net in include/cdx.h,
         whose descriptor fields are the arguments).  kind: 'self' (qkv [B*N, 3C], one range slot), 'cross' (q [B*N, C], kv
         [B*ctx_lp, 2C] the padded context's K | V) or 'generic' (q, k, v; optional causal mask).  Every buffer is a float32 tensor on
         this engine's device passed as it is; out [B*N, C] (a view inside a larger buffer is fine) is written, or added to for the
         images of acc_rows.  slot / q_slot > 0 replace the measured range slots.  Returns the plan: dict(route, qrows, rag, ksplit,
-        ring, Nks, Nvs)."""
+        ring, Nks, Nvs).  probe_rows / probe_spans (host int lists) with probe_map [n_probe, N] (kind 'cross'): LEDITS++'s probe on
+        the operands the route multiplied, map[i] <- sum over heads of the softmax over tokens 1..probe_spans[i] of image probe_rows[i]."""
         kinds = ('self', 'cross', 'generic')
         assert kind in kinds, kind
-        for name, t in (('out', out), ('qkv', qkv), ('q', q), ('kv', kv), ('k', k), ('v', v)):
+        for name, t in (('out', out), ('qkv', qkv), ('q', q), ('kv', kv), ('k', k), ('v', v), ('probe_map', probe_map)):
             assert t is None or (torch.is_tensor(t) and t.dtype == torch.float32 and t.device == self.device), \
                 f'op_attention_net: {name} must be a float32 tensor on {self.device}'
         rows = lambda r: None if r is None else (C.c_int * max(len(r), 1))(*[int(x) for x in r])
@@ -526,6 +530,11 @@ class Engine:
                                       B=B, N=N, L=L, ctx_lp=ctx_lp, heads=heads, d=d, scale=scale, qk_rows=rows(qk_rows), kv_rows=rows(kv_rows),
                                       acc_rows=rows(acc_rows), n_acc=len(acc_rows) if acc_rows is not None else 0, slot=slot, q_slot=q_slot,
                                       out=ptr(out))
+        if probe_rows is not None:
+            assert probe_spans is not None and len(probe_spans) == len(probe_rows) and probe_map is not None
+            assert probe_map.is_contiguous() and probe_map.numel() >= len(probe_rows) * N, 'op_attention_net: probe_map [n_probe, N]'
+            desc.probe_rows, desc.probe_spans, desc.n_probe = rows(probe_rows), rows(probe_spans), len(probe_rows)
+            desc.probe_map = ptr(probe_map)
         plan = (C.c_int * 7)()
         check(lib.cdx_op_attention_net(self.h, C.byref(desc), plan, self.stream))
         return dict(zip(('route', 'qrows', 'rag', 'ksplit', 'ring', 'Nks', 'Nvs'), [self.ATTN_ROUTES[plan[0]]] + list(plan[1:])))
@@ -807,8 +816,9 @@ class UNet(Net):
         an attn_control.PnPControl, Plug-and-Play's feature and self-attention injection on the target chain's rows
         (cdx_cycle_lockstep_pnp).  Each composes with mask.
         semantic: a semantic.SemanticGuidance of m concepts, with c_edit [B, m, L, D] (or [m, L, D], every sample's): SEGA's
-        concept terms on the target chain (cdx_cycle_lockstep_semantic); it needs uc, composes with mask, and an attn_control
-        with it raises ValueError."""
+        concept terms on the target chain (cdx_cycle_lockstep_semantic), or with use_cross_attn_mask / use_intersect_mask LEDITS++'s
+        implicit masks (cdx_cycle_lockstep_semantic_attn); it needs uc, composes with mask, and an attn_control with it raises
+        ValueError."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -832,10 +842,14 @@ class UNet(Net):
             sg = semantic.c_struct(n)
             out = e.empty(B, Cc, h, w)
             z = e.empty(B, n + 1, Cc, h, w) if return_z else None
-            check(lib.cdx_cycle_lockstep_semantic(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale),
-                                                  float(tgt_scale), sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T,
-                                                  sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w, e.stream, _ptr(mask), _ptr(c_edit),
-                                                  C.byref(sg)))
+            args = (self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), c_src.shape[1], float(src_scale), float(tgt_scale),
+                    sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out), _ptr(z), B, Cc, h, w,
+                    e.stream, _ptr(mask), _ptr(c_edit), C.byref(sg))
+            if semantic.mask_mode:       # LEDITS++'s implicit masks
+                am = semantic.attn_mask_struct(c_src.shape[1])
+                check(lib.cdx_cycle_lockstep_semantic_attn(*args, C.byref(am)))
+            else:
+                check(lib.cdx_cycle_lockstep_semantic(*args))
             return (out, z) if return_z else out
         mutual, pnp = isinstance(attn_control, MutualSelfControl), isinstance(attn_control, PnPControl)
         ctl, _token_map, own = attn_control.c_struct(n, B, c_src.shape[1], e.device) if attn_control is not None and not (mutual or pnp) \

@@ -169,12 +169,24 @@ class CycleDiffusionPipeline:
         except ValueError as err:
             raise ValueError(f'cross_attention_kwargs: {err}') from None
 
+    def _token_counts(self, concepts, given):
+        """LEDITS++'s token span per concept: the caller's edit_token_counts, or the conditioning model's count capped at L - 2."""
+        if given is not None:
+            return given
+        counts = getattr(self.g.cond_stage, 'token_counts', None)
+        if counts is None:
+            raise ValueError('use_cross_attn_mask / use_intersect_mask: the conditioning model has no token_counts(texts); pass '
+                             'edit_token_counts')
+        L = int(self.g.get_learned_conditioning(concepts[:1]).shape[1])
+        return [max(1, min(int(n), L - 2)) for n in counts(concepts)]
+
     @torch.no_grad()
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
                  source_guidance_scale=1, num_images_per_prompt=1, eta=0.1, generator=None, prompt_embeds=None, output_type='pt',
                  return_dict=True, callback=None, callback_steps=1, cross_attention_kwargs=None, clip_skip=None, two_phase=False,
                  mask_image=None, paste_back=False, editing_prompt=None, reverse_editing_direction=False, edit_guidance_scale=5,
-                 edit_threshold=0.9, edit_cooldown_steps=None, edit_warmup_steps=10, edit_momentum_scale=0.1, edit_mom_beta=0.4):
+                 edit_threshold=0.9, edit_cooldown_steps=None, edit_warmup_steps=10, edit_momentum_scale=0.1, edit_mom_beta=0.4,
+                 use_cross_attn_mask=False, use_intersect_mask=False, edit_token_counts=None):
         """mask_image: optional float tensor [B,1,H,W] or [1,1,H,W] in [0,1] at the image's size, 1 = "may change" (diffusers'
         convention).  Outside the mask the latent stays on the source image's own chain (cdx_cycle_lockstep_masked), so the
         unmasked region decodes to the image's VAE reconstruction.  paste_back: additionally composite the output with the input
@@ -212,7 +224,15 @@ class CycleDiffusionPipeline:
         edit_warmup_steps, edit_momentum_scale and edit_mom_beta are shared (semantic.SemanticGuidance).  Steps are counted over the
         loop's int(num_inference_steps * strength) steps.  The concept prompts are broadcast to every image.  It composes with
         mask_image and precision='autocast'; two_phase=True, an edit_type in cross_attention_kwargs, list lengths other than m and
-        a per-concept warmup list raise ValueError.  Without editing_prompt the edit_* arguments are unused."""
+        a per-concept warmup list raise ValueError.  Without editing_prompt the edit_* arguments are unused.
+
+        use_cross_attn_mask / use_intersect_mask: LEDITS++'s implicit masks (Brack et al., 2024; its argument names), both off by
+        default.  Each concept's term is kept where its own cross-attention map (its prompt's tokens, at the U-Net's 1/4-resolution
+        cross-attention layers, smoothed) is in its edit_threshold-th percentile, instead of SEGA's per-channel rule; intersect also
+        requires the term's channel-summed magnitude to be in its percentile (and implies the attention mask).  The tokens of each
+        concept come from the conditioning model's token_counts(concepts) (capped at the context length - 2), or from
+        edit_token_counts (an int or one per concept), which a conditioning callable without token_counts needs.  The latent's sides
+        must be multiples of 4.  A mask flag without editing_prompt raises ValueError."""
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
         semantic, concepts = None, None
         if editing_prompt is not None:
@@ -223,7 +243,11 @@ class CycleDiffusionPipeline:
             if attn_control is not None:
                 raise ValueError('semantic guidance does not combine with a cross_attention_kwargs edit_type in one loop')
             semantic = SemanticGuidance.for_concepts(len(concepts), edit_guidance_scale, reverse_editing_direction, edit_threshold,
-                                                     edit_cooldown_steps, edit_warmup_steps, edit_momentum_scale, edit_mom_beta)
+                                                     edit_cooldown_steps, edit_warmup_steps, edit_momentum_scale, edit_mom_beta,
+                                                     use_cross_attn_mask, use_intersect_mask, self._token_counts(concepts, edit_token_counts)
+                                                     if use_cross_attn_mask or use_intersect_mask else edit_token_counts)
+        elif use_cross_attn_mask or use_intersect_mask:
+            raise ValueError('use_cross_attn_mask / use_intersect_mask mask the semantic guidance terms: pass editing_prompt')
         if strength < 0 or strength > 1:
             raise ValueError(f'The value of strength should in [0.0, 1.0] but is {strength}')
         if not isinstance(callback_steps, int) or callback_steps <= 0:

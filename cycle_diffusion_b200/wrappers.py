@@ -56,16 +56,30 @@ class ClipTextCondStage:
         self.encoder = TextEncoder(engine, self.cfg)
         self.encoder.load_state_dict({k: v for k, v in state_dict.items() if k.startswith(prefix)}, prefix=prefix)
 
+    END_ID = 49407      # CLIP's <|endoftext|> (the OpenCLIP tokenizer's too)
+
     def __call__(self, texts):
         ids = self.tokenizer(list(texts))
         assert ids.dim() == 2 and ids.shape[0] == len(texts), 'tokenizer must return [B, L] ids'
         return self.encoder(ids)
+
+    def token_counts(self, texts):
+        """The prompt's own tokens per text (LEDITS++'s attention masks read tokens 1..n): the position of the first end token after
+        the start token, minus 1 (the whole row when it has none)."""
+        ids = self.tokenizer(list(texts))
+        out = []
+        for row in ids.tolist():
+            end = next((j for j in range(1, len(row)) if row[j] == self.END_ID), len(row))
+            out.append(end - 1)
+        return out
 
 
 class BertTextCondStage(ClipTextCondStage):
     """Same for the LDM text2img-large conditioning model: BERTEmbedder (encoders/modules.py:79-102; 32 x 1280 x_transformer
     encoder over BERT word pieces).  ``tokenizer``: e.g. HF ``BertTokenizerFast`` with ``padding='max_length', max_length=77``
     (modules.py:66-72); the LDM checkpoint keeps the weights under ``cond_stage_model.``."""
+
+    END_ID = 102        # BERT's [SEP]
 
     def __init__(self, engine, state_dict, tokenizer, cfg=None, prefix=''):
         super().__init__(engine, state_dict, tokenizer, cfg or specs.bert_text_config(), prefix)
@@ -104,6 +118,10 @@ class SyntheticTextEncoder:
             g = torch.Generator().manual_seed(seed)
             out.append(torch.randn(self.n_tokens, self.dim, generator=g))
         return torch.stack(out).to(self.device)
+
+    def token_counts(self, texts):
+        """The whitespace word count of each text (the stand-in has no tokenizer)."""
+        return [len(t.split()) for t in texts]
 
 
 def _load_sd(state_dict, ckpt_default, synth_params, seed):

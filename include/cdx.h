@@ -427,6 +427,30 @@ int cdx_cycle_lockstep_semantic(cdx_net* unet, const float* x0, const float* c_s
                                 const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
                                 float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                                 void* stream, const float* mask, const float* c_edit, const cdx_semantic_guidance* sg);
+/* LEDITS++'s implicit masks (Brack et al., 2024) on cdx_cycle_lockstep_semantic: each concept's term is kept only where the concept's
+ * own cross-attention points.  The concept rows' cross-attention probabilities are probed in every SpatialTransformer of the input
+ * and output blocks (never the middle block) whose token count is (h/4)(w/4) -- for SD v1 / 2.x and LDM text2img input blocks 7, 8
+ * and output blocks 3, 4, 5 -- from the operands the layer multiplied.  For concept k of target chain t at loop step i:
+ *   A(p)   = sum over those layers, over heads, over j = 1..n_tokens[k] of softmax_j(scale q_p . k_j) over all L keys
+ *   As     = 3x3 smoothing of A, reflect padding 1, weights fp32(g_a g_b / (sum g)^2), g = (e^-1, 1, e^-1) in double (diffusers'
+ *            GaussianSmoothing(3, 0.5)); products row-major, each rounded, added left to right
+ *   M1(y, x) = As(y/4, x/4) >= Q(threshold[k], As over the (h/4)(w/4) grid)   (the quantile of cdx_cycle_lockstep_semantic)
+ *   intersect: s(y, x) = sum over c ascending of |psi_k(c, y, x)|, M = M1 and s >= Q(threshold[k], s over h*w); else M = M1
+ *   g_k    = (i < cooldown[k] and M(y, x)) ? psi_k : 0     (SEGA's per-channel threshold is not applied)
+ * The sum over concepts, the momentum and the warmup are cdx_cycle_lockstep_semantic's.  One probe launch per probed layer per step,
+ * and the threshold stage stays one launch.  CDX_E_INVALID: everything cdx_cycle_lockstep_semantic rejects, n_tokens[k] outside
+ * 1..L-2, h or w not a multiple of 4 or below 8, and a net with no cross-attention of (h/4)(w/4) tokens in its input or output
+ * blocks. */
+typedef struct cdx_semantic_attn_mask {
+  int intersect;                        /* also the channel-summed mask of |psi_k| */
+  int n_tokens[CDX_SEMANTIC_MAX];       /* concept k's own tokens: 1..n_tokens[k] of its context, after the start token */
+} cdx_semantic_attn_mask;
+int cdx_cycle_lockstep_semantic_attn(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                                     int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                                     const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                                     float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                                     void* stream, const float* mask, const float* c_edit, const cdx_semantic_guidance* sg,
+                                     const cdx_semantic_attn_mask* am);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -612,6 +636,10 @@ typedef struct cdx_attention_net_desc {
   const int* qk_rows; const int* kv_rows; const int* acc_rows; int n_acc;
   float slot, q_slot;
   float* out;
+  /* kind 1 only, optional: LEDITS++'s probe on the operands the route multiplied (cdx_cycle_lockstep_semantic_attn), probe_map
+   * [n_probe, N] <- for image probe_rows[i], sum over heads of sum over j = 1..probe_spans[i] of softmax_j (host lists) */
+  const int* probe_rows; const int* probe_spans; int n_probe;
+  float* probe_map;
 } cdx_attention_net_desc;
 int cdx_op_attention_net(cdx_engine* e, const cdx_attention_net_desc* desc, int* plan_out, void* stream);
 int cdx_op_nchw_to_nhwc(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
@@ -708,6 +736,9 @@ int cdx_op_gemm(cdx_engine* e, const cdx_gemm_desc* desc, int* plan_out, void* s
  *                 sg_scale and sg_lambda; stage 1 then adds G to each target chain's eps-hat when sg_apply, from the concepts whose
  *                 bit is set in sg_active, updates the momentum sg_nu [n_src*K, chw] in place with (sg_mu, sg_beta, sg_beta1), and
  *                 writes the chain's next x_t to its concept rows too (as does stage 0).
+ *   sg_mask > 0:  LEDITS++'s masks (cdx_cycle_lockstep_semantic_attn) instead of the per-channel thresholds: stage 2 writes sg_thr
+ *                 [n_src*K*sg_m, 2], the threshold of the smoothed map and (sg_mask == 2) of the channel-summed |psi_k|; stage 1
+ *                 keeps psi_k where both masks hold.
  * Row indices, counts, strides and the stage are checked on the host; buffer extents are the caller's. */
 typedef struct cdx_latent_chain { int row, row2; float scale; } cdx_latent_chain;
 typedef struct cdx_latent_chains_desc {
@@ -734,6 +765,10 @@ typedef struct cdx_latent_chains_desc {
   float sg_scale[CDX_SEMANTIC_MAX]; float sg_lambda[CDX_SEMANTIC_MAX];
   unsigned sg_active; int sg_apply;
   float sg_mu, sg_beta, sg_beta1;
+  const float* sg_map;          /* [n_src*K*sg_m, sg_gh*sg_gw]: the raw attention maps of the concept rows */
+  int sg_mask;                  /* 0 SEGA's thresholds, 1 LEDITS++'s attention mask, 2 with its channel-summed mask */
+  int sg_gh, sg_gw;             /* the map grid: h/4 x w/4 */
+  int w;                        /* latent width (hw = h*w = 16*sg_gh*sg_gw) */
 } cdx_latent_chains_desc;
 int cdx_op_latent_chains(cdx_engine* e, const cdx_latent_chains_desc* desc, int stage, void* stream);
 /* One launch of the two-model pixel loop's fused step (pixel_lockstep_step, which cdx_pixel_cycle_lockstep runs): xs / ys [B, chw]

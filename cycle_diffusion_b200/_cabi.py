@@ -95,6 +95,33 @@ class LatentChainsMaskDesc(LatentChainsDesc):
     _fields_ = [('sg_map', _P), ('sg_mask', C.c_int), ('sg_gh', C.c_int), ('sg_gw', C.c_int), ('w', C.c_int)]
 
 
+class DpmCoef(C.Structure):
+    _fields_ = [('a', C.c_float), ('b', C.c_float), ('c', C.c_float), ('n', C.c_float), ('order', C.c_int)]
+
+
+class LatentChainsSamplerDesc(LatentChainsMaskDesc):
+    """The whole cdx_latent_chains_desc: LatentChainsMaskDesc plus the edit-friendly inversion's trailing fields."""
+    _fields_ = [('solver', C.c_int), ('dc', DpmCoef), ('d_src', _P), ('d_tgt', _P), ('qa', C.c_float), ('q1', C.c_float)]
+
+
+CDX_SAMPLER_DDIM_POSTERIOR = 0
+CDX_SAMPLER_DDIM_DRAWS = 1
+CDX_SAMPLER_DPMSOLVER_DRAWS = 2
+
+
+class SamplerC(C.Structure):
+    _fields_ = [('kind', C.c_int), ('dpm', C.POINTER(DpmCoef)), ('qa', C.POINTER(C.c_float)), ('q1', C.POINTER(C.c_float))]
+
+
+class MutualControlC(C.Structure):
+    _fields_ = [('start_step', C.c_int), ('start_layer', C.c_int)]
+
+
+class PnpControlC(C.Structure):
+    _fields_ = [('feature_steps', C.c_int), ('attention_steps', C.c_int), ('attention_start_layer', C.c_int),
+                ('feature_blocks', C.POINTER(C.c_int)), ('n_feature_blocks', C.c_int)]
+
+
 CDX_SEMANTIC_MAX = 8
 
 
@@ -172,6 +199,9 @@ SIGNATURES = {
                                          _I, _I, _P, _P, _P, C.POINTER(SemanticGuidanceC)]),
     'cdx_cycle_lockstep_semantic_attn': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I,
                                               _I, _I, _I, _P, _P, _P, C.POINTER(SemanticGuidanceC), C.POINTER(SemanticAttnMaskC)]),
+    'cdx_cycle_lockstep_sampler': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
+                                        _I, _I, _P, C.POINTER(SamplerC), _P, C.POINTER(AttnControl), _P, C.POINTER(MutualControlC),
+                                        C.POINTER(PnpControlC), _P, C.POINTER(SemanticGuidanceC), C.POINTER(SemanticAttnMaskC)]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),

@@ -188,6 +188,8 @@ struct ChainLoopArgs {
   const cdx_semantic_guidance* sega = nullptr; const float* c_edit = nullptr;
   const cdx_semantic_attn_mask* sega_mask = nullptr;    // optional with sega: LEDITS++'s implicit masks (cdx_cycle_lockstep_semantic_attn)
   int C = 0, h = 0, w = 0;
+  // optional: the source chain's sampler (cdx.h, cdx_cycle_lockstep_sampler); NULL or CDX_SAMPLER_DDIM_POSTERIOR is the DPM-Encoder
+  const cdx_sampler* sampler = nullptr;
 };
 
 // RAII: the engine's contractions on the exact-fp32 FFMA path for one scope
@@ -297,6 +299,24 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     for (int i = 0; i < p.n_blocks; ++i) {
       CDX_CHECK(p.blocks[i] >= 0 && p.blocks[i] < n_out, "Plug-and-Play: feature block %d outside the net's %d output blocks", p.blocks[i], n_out);
       for (int j = 0; j < i; ++j) CDX_CHECK(p.blocks[j] != p.blocks[i], "Plug-and-Play: feature block %d given twice", p.blocks[i]);
+    }
+  }
+  // edit-friendly inversion: independent draws of the source's x at every step (solver 1 and 2), the DPM table (solver 2)
+  const int solver = a.sampler ? a.sampler->kind : 0;
+  if (solver) {
+    const cdx_sampler& sp = *a.sampler;
+    CDX_CHECK(solver == CDX_SAMPLER_DDIM_DRAWS || solver == CDX_SAMPLER_DPMSOLVER_DRAWS, "sampler: kind %d", solver);
+    CDX_CHECK(a.src && a.K > 0 && a.n_rec == a.n_steps && !tgt_net && a.noise,
+              "edit-friendly inversion: needs the lock-step loop with a source chain at every step");
+    CDX_CHECK(sp.qa && sp.q1 && sp.qa[0] == a.sa && sp.q1[0] == a.s1,
+              "edit-friendly inversion: the draw scalars qa / q1 must be given, their step 0 the x_T scalars");
+    if (solver == CDX_SAMPLER_DPMSOLVER_DRAWS) {
+      CDX_CHECK(sp.dpm, "SDE-DPM-Solver++: null coefficient table");
+      for (int i = 0; i < a.n_steps; ++i) {
+        const cdx_dpm_coef& d = sp.dpm[i];
+        CDX_CHECK(d.n > 0.f && std::isfinite(d.n) && (d.order == 1 || d.order == 2), "SDE-DPM-Solver++: step %d n=%g order %d", i, d.n, d.order);
+        CDX_CHECK(i > 0 || d.order == 1, "SDE-DPM-Solver++: order %d on the loop's first step (no previous x0-prediction)", d.order);
+      }
     }
   }
   Scope sc(e.arena);
@@ -444,13 +464,20 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
   }
   auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
     if (i_next >= a.n_rec) return 0;
-    return (a.n_steps - 1 - i_next) == 0 ? 2 : 1;                               // ddim.py:583-584
+    return (a.n_steps - 1 - i_next) == 0 ? 2 : solver ? 3 : 1;                  // ddim.py:583-584; 3: an independent draw
   };
+  // solver 2: each chain's previous x0-prediction, written by every step before the second-order steps read it
+  float *d_src = nullptr, *d_tgt = nullptr;
+  if (solver == CDX_SAMPLER_DPMSOLVER_DRAWS) {
+    d_src = (float*)e.arena.alloc(n * sizeof(float));
+    d_tgt = (float*)e.arena.alloc((size_t)n_tgt_chains * chw * sizeof(float));
+  }
   // the noise of a step no source chain recovers: the z_in slots while they last, then `extra`
   const int n_given = a.src ? a.n_rec : a.n_eps;
   LatentChains f;
   f.n = n; f.chw = chw; f.n_src = a.n_src; f.K = a.K; f.chains = chd; f.x0 = a.x0; f.xin = xin; f.mask = a.mask; f.hw = a.h * a.w;
   f.z_stride = (long long)(a.n_rec + 1) * chw;
+  f.solver = solver; f.d_src = d_src; f.d_tgt = d_tgt;
   if (sg_m) {
     const cdx_semantic_guidance& g = *a.sega;
     f.sg_m = sg_m; f.sg_rows = sg_rows_dev; f.sg_thr = sg_thr; f.sg_nu = sg_nu;
@@ -466,6 +493,7 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     in.xt = xb[0]; in.xn = xb[1]; in.yt = yb[0];
     in.next = a.src ? next_kind(0) : 0;
     if (in.next) { in.noise_next = a.noise + n; in.cnext = a.coef[0]; }
+    if (in.next == 3) { in.qa = a.sampler->qa[1]; in.q1 = a.sampler->q1[1]; }
     latent_chains_init(e, in, s);
   }
   const int iters = e.dry() ? std::min(loop_steps, 1) : loop_steps;
@@ -498,6 +526,8 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       if (a.z_out) st.z_out = a.z_out + (size_t)(1 + i) * chw;
       st.next = next_kind(i + 1);
       if (st.next) { st.noise_next = a.noise + (size_t)(2 + i) * n; st.cnext = a.coef[i + 1]; }
+      if (st.next == 3) { st.qa = a.sampler->qa[i + 2]; st.q1 = a.sampler->q1[i + 2]; }
+      if (solver == CDX_SAMPLER_DPMSOLVER_DRAWS) st.dc = a.sampler->dpm[i];
     } else if (i < n_given) {
       st.eps_in = a.z_in + (size_t)(1 + i) * chw; st.eps_stride = (long long)(a.n_eps + 1) * chw;
     } else {
@@ -909,7 +939,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream, const float* mask,
                           const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer,
                           const PnpLoop* pnp = nullptr, const cdx_semantic_guidance* sega = nullptr, const float* c_edit = nullptr,
-                          const cdx_semantic_attn_mask* sega_mask = nullptr) {
+                          const cdx_semantic_attn_mask* sega_mask = nullptr, const cdx_sampler* sampler = nullptr) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -921,7 +951,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
     a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
     a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer; a.pnp = pnp;
-    a.sega = sega; a.c_edit = c_edit; a.sega_mask = sega_mask;
+    a.sega = sega; a.c_edit = c_edit; a.sega_mask = sega_mask; a.sampler = sampler;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -972,6 +1002,23 @@ int cdx_cycle_lockstep_semantic_attn(cdx_net* un, const float* x0, const float* 
     return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_semantic_attn: null guidance, concept contexts or mask settings"); });
   return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
                         B, C, h, w, stream, mask, nullptr, nullptr, false, 0, 0, nullptr, sg, c_edit, am);
+}
+
+int cdx_cycle_lockstep_sampler(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                               float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                               float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                               const cdx_sampler* sampler, const float* mask, const cdx_attn_control* ctl, const float* own_weight,
+                               const cdx_mutual_control* mutual, const cdx_pnp_control* pnp, const float* c_edit,
+                               const cdx_semantic_guidance* sg, const cdx_semantic_attn_mask* am) {
+  if (!sampler) return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_sampler: null sampler"); });
+  PnpLoop p;
+  if (pnp) {
+    p.feature_steps = pnp->feature_steps; p.attention_steps = pnp->attention_steps; p.start_layer = pnp->attention_start_layer;
+    p.blocks = pnp->feature_blocks; p.n_blocks = pnp->n_feature_blocks;
+  }
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, ctl, own_weight, mutual != nullptr, mutual ? mutual->start_step : 0,
+                        mutual ? mutual->start_layer : 0, pnp ? &p : nullptr, sg, c_edit, am, sampler);
 }
 
 int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
@@ -1727,7 +1774,9 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
     CDX_CHECK(stage >= 0 && stage <= 2, "op_latent_chains: stage %d", stage);
     CDX_CHECK(d->chw > 0 && d->n_src > 0 && d->K >= 0 && d->rows >= 0 && (d->src == 0 || d->src == 1) && (d->pred == 0 || d->pred == 1),
               "op_latent_chains: chw=%d n_src=%d K=%d rows=%d src=%d pred=%d", d->chw, d->n_src, d->K, d->rows, d->src, d->pred);
-    CDX_CHECK(d->next >= 0 && d->next <= 2 && (d->src || d->next == 0), "op_latent_chains: next=%d without a source chain", d->next);
+    CDX_CHECK(d->next >= 0 && d->next <= 3 && (d->src || d->next == 0), "op_latent_chains: next=%d without a source chain", d->next);
+    CDX_CHECK(d->solver >= 0 && d->solver <= 2 && (d->solver ? d->next != 1 : d->next != 3), "op_latent_chains: next=%d under solver %d",
+              d->next, d->solver);
     const size_t n_chains = (size_t)d->n_src * (1 + d->K);
     // every row a launch writes or reads: the source chains' when they run, always the target chains'
     for (size_t k = d->src ? 0 : d->n_src; k < n_chains; ++k) {
@@ -1739,7 +1788,7 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
     if (stage != 2) {                      // the threshold stage reads eout and the tables only
       CDX_CHECK((!d->src && !targets) || d->xin, "op_latent_chains: null xin");
       CDX_CHECK(!reads_x0 || d->x0, "op_latent_chains: null x0");
-      CDX_CHECK(!(d->src && d->next == 1) || d->noise_next, "op_latent_chains: next == 1 without noise_next");
+      CDX_CHECK(!(d->src && (d->next == 1 || d->next == 3)) || d->noise_next, "op_latent_chains: next == %d without noise_next", d->next);
       CDX_CHECK(!d->z_out || d->z_stride >= d->chw, "op_latent_chains: z_stride %lld < chw %d", (long long)d->z_stride, d->chw);
       CDX_CHECK(d->src || !targets || (d->eps_in && d->eps_stride >= d->chw), "op_latent_chains: no source chain and no eps_in (stride %lld)",
                 (long long)d->eps_stride);
@@ -1753,6 +1802,9 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
       CDX_CHECK(!targets || (d->yt && d->y_out), "op_latent_chains: step: null yt / y_out");
       CDX_CHECK(!d->mask || (d->src && d->hw > 0 && d->hw <= d->chw), "op_latent_chains: a mask needs a source chain and 0 < hw (%d) <= chw",
                 d->hw);
+      if (d->solver == 2)
+        CDX_CHECK((!d->src || d->d_src) && (!targets || d->d_tgt) && (d->dc.order == 1 || d->dc.order == 2),
+                  "op_latent_chains: solver 2 needs d_src / d_tgt and order 1 or 2 (order %d)", d->dc.order);
     }
     CDX_CHECK(d->sg_m >= 0 && d->sg_m <= SEMANTIC_MAX_CONCEPTS && (stage != 2 || d->sg_m > 0), "op_latent_chains: sg_m=%d at stage %d", d->sg_m,
               stage);
@@ -1799,6 +1851,7 @@ int cdx_op_latent_chains(cdx_engine* eh, const cdx_latent_chains_desc* d, int st
       for (int q = 0; q < d->sg_m; ++q) { a.sg_scale[q] = d->sg_scale[q]; a.sg_lambda[q] = d->sg_lambda[q]; }
       a.sg_active = d->sg_active; a.sg_apply = d->sg_apply; a.sg_mu = d->sg_mu; a.sg_beta = d->sg_beta; a.sg_beta1 = d->sg_beta1;
       a.sg_mask = d->sg_mask; a.sg_map = d->sg_map; a.sg_gh = d->sg_gh; a.sg_gw = d->sg_gw; a.w = d->w;
+      a.solver = d->solver; a.dc = d->dc; a.d_src = d->d_src; a.d_tgt = d->d_tgt; a.qa = d->qa; a.q1 = d->q1;
       if (stage == 0) latent_chains_init(e, a, s);
       else if (stage == 2) semantic_thresholds(e, a, s);
       else latent_chains_step(e, a, s);

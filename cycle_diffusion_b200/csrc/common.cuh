@@ -371,6 +371,15 @@ struct LatentChains {
   const float* sg_map = nullptr;                 // device [n_src*K*sg_m, sg_gh*sg_gw]: the probe's raw maps
   int sg_gh = 0, sg_gw = 0;
   int w = 0;                                     // latent width: pixel r % hw = y*w + x
+  // edit-friendly inversion (cdx_cycle_lockstep_sampler).  solver 0: the DDIM step on the posterior chain; 1: the DDIM step on
+  // independent draws; 2: the SDE-DPM-Solver++ step under dc on independent draws.  Under 1 and 2 the source's next x is next == 3,
+  // q_sample(x0, noise_next, qa, q1), or next == 2, x0; next == 1 is solver 0's.  Solver 2: D = pred_x0 of each chain,
+  // mu = a*x + b*D (+ c*(D - D_prev) at order 2), z = (xn - mu_src) / n, y_next = mu_y + n*z; D_prev is read from d_src / d_tgt
+  // ([n_src, chw] / [n_src*K, chw]) and overwritten with D in place.  Kept last, as the fields above.
+  int solver = 0;
+  cdx_dpm_coef dc{};
+  float* d_src = nullptr; float* d_tgt = nullptr;
+  float qa = 0.f, q1 = 0.f;
 };
 constexpr int SEMANTIC_MAX_CONCEPTS = 8;
 void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s);

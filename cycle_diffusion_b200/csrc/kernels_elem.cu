@@ -260,7 +260,9 @@ __device__ __forceinline__ void chain_put(float* xin, const Chain& ch, size_t r,
 }
 // x_T of every element group, shared by its source chain and its K target chains, and the first U-Net input: drawn from x0
 // (ddim.py:477-479) when the loop has a source chain, else slot 0 of the recovered noises (SDW:153).  Every input was written by the
-// copies and launches just before, so all loads take the coherent path.
+// copies and launches just before, so all loads take the coherent path.  DRAWS (solver 1 and 2): the first next x is next == 3's
+// independent draw instead of next == 1's posterior sample.
+template <int DRAWS = 0>
 __global__ void latent_chains_init_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
@@ -270,8 +272,13 @@ __global__ void latent_chains_init_kernel(const LatentChains a) {
       xT = ADD(MUL(a.sa, x0), MUL(a.s1, __ldcg(a.noise0 + i)));                                // ddim.py:477-479
       if (a.z_out) a.z_out[j * a.z_stride + r] = xT;
       a.xt[i] = xT;
-      if (a.next == 1) a.xn[i] = ddim_posterior_f(x0, xT, __ldcg(a.noise_next + i), a.cnext);
-      else if (a.next == 2) a.xn[i] = x0;
+      if constexpr (DRAWS) {
+        if (a.next == 3) a.xn[i] = ADD(MUL(a.qa, x0), MUL(a.q1, __ldcg(a.noise_next + i)));
+        else if (a.next == 2) a.xn[i] = x0;
+      } else {
+        if (a.next == 1) a.xn[i] = ddim_posterior_f(x0, xT, __ldcg(a.noise_next + i), a.cnext);
+        else if (a.next == 2) a.xn[i] = x0;
+      }
       chain_put(a.xin, a.chains[j], r, a.chw, xT);
     } else {
       xT = __ldcg(a.eps_in + j * a.eps_stride + r);
@@ -320,7 +327,16 @@ __device__ __forceinline__ float ledits_chansum(const float* ok, const float* ou
 // concept rows, its uncond row, the step's thresholds and its momentum before the e_t / pred_x0 conversion; its concept rows are
 // written with its next x_t.  SEGA = 1 + a.sg_mask: 1 SEGA's per-channel thresholds, 2 LEDITS++'s
 // attention mask, 3 the attention mask and the channel-summed one.
-template <int PRED, int MASK, int SEGA = 0>
+// SOLVER (LatentChains::solver): 0 the DDIM step on the posterior chain, 1 the DDIM step on independent draws (next == 3 in place of
+// next == 1), 2 the SDE-DPM-Solver++ step on independent draws.
+// the SDE-DPM-Solver++ mean of one chain at x with x0-prediction D; hist holds the chain's previous D and takes this one
+__device__ __forceinline__ float dpm_mean(const LatentChains& a, float x, float D, float* hist) {
+  float mu = ADD(MUL(a.dc.a, x), MUL(a.dc.b, D));
+  if (a.dc.order == 2) mu = ADD(mu, MUL(a.dc.c, SUB(D, __ldcg(hist))));
+  *hist = D;                                                     // each element's history has one owner thread
+  return mu;
+}
+template <int PRED, int MASK, int SEGA = 0, int SOLVER = 0>
 __global__ void latent_chains_step_kernel(const LatentChains a) {
   GRID_STRIDE(i, a.n) {
     const size_t j = i / a.chw, r = i - j * a.chw;
@@ -332,11 +348,20 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
       xn = __ldcg(a.xn + i);
       float e_t, pred_x0;
       eps_x0<PRED>(o, xt, a.c, a.vsa, a.vs1, e_t, pred_x0);                                     // ddim.py:576
-      const float dir = MUL(a.c.dir_coef, e_t);                                                  // :578
-      eps = DIV(DIV(SUB(SUB(xn, MUL(a.c.sqrt_aprev, pred_x0)), dir), a.c.sigma), 1.0f);         // :579 (temperature 1)
+      if constexpr (SOLVER == 2) {
+        eps = DIV(SUB(xn, dpm_mean(a, xt, pred_x0, a.d_src + i)), a.dc.n);
+      } else {
+        const float dir = MUL(a.c.dir_coef, e_t);                                                // :578
+        eps = DIV(DIV(SUB(SUB(xn, MUL(a.c.sqrt_aprev, pred_x0)), dir), a.c.sigma), 1.0f);       // :579 (temperature 1)
+      }
       if (a.z_out) a.z_out[j * a.z_stride + r] = eps;
-      if (a.next == 1) a.xn2[i] = ddim_posterior_f(__ldcg(a.x0 + i), xn, __ldcg(a.noise_next + i), a.cnext);
-      else if (a.next == 2) a.xn2[i] = __ldcg(a.x0 + i);                                        // ddim.py:583-584
+      if constexpr (SOLVER) {
+        if (a.next == 3) a.xn2[i] = ADD(MUL(a.qa, __ldcg(a.x0 + i)), MUL(a.q1, __ldcg(a.noise_next + i)));
+        else if (a.next == 2) a.xn2[i] = __ldcg(a.x0 + i);
+      } else {
+        if (a.next == 1) a.xn2[i] = ddim_posterior_f(__ldcg(a.x0 + i), xn, __ldcg(a.noise_next + i), a.cnext);
+        else if (a.next == 2) a.xn2[i] = __ldcg(a.x0 + i);                                      // ddim.py:583-584
+      }
       chain_put(a.xin, src, r, a.chw, xn);
     } else {
       eps = __ldcg(a.eps_in + j * a.eps_stride + r);
@@ -378,9 +403,14 @@ __global__ void latent_chains_step_kernel(const LatentChains a) {
       const float y = __ldcg(a.yt + ti);
       float et, px0;
       eps_x0<PRED>(ot, y, a.c, a.vsa, a.vs1, et, px0);                                          // ddim.py:634
-      const float tdir = MUL(a.c.dir_coef, et);                                                 // :638
-      const float noise = MUL(MUL(a.c.sigma, eps), 1.0f);                                       // :642
-      float yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                               // :645
+      float yn;
+      if constexpr (SOLVER == 2) {
+        yn = ADD(dpm_mean(a, y, px0, a.d_tgt + ti), MUL(a.dc.n, eps));
+      } else {
+        const float tdir = MUL(a.c.dir_coef, et);                                               // :638
+        const float noise = MUL(MUL(a.c.sigma, eps), 1.0f);                                     // :642
+        yn = ADD(ADD(MUL(a.c.sqrt_aprev, px0), tdir), noise);                                   // :645
+      }
       if constexpr (MASK) {
         if (m == 0.0f) yn = xn;
         else if (m != 1.0f) yn = ADD(xn, MUL(m, SUB(yn, xn)));
@@ -890,47 +920,57 @@ __global__ void image_metrics_final_kernel(const double* __restrict__ acc, int B
   }
 }
 
-void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s) { LAUNCH1(latent_chains_init_kernel, a.n, a); }
-void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
+void latent_chains_init(Engine& e, const LatentChains& a, cudaStream_t s) {
+  if (a.solver) LAUNCH1(latent_chains_init_kernel<1>, a.n, a);
+  else LAUNCH1(latent_chains_init_kernel<0>, a.n, a);
+}
+template <int SOLVER>
+void launch_step(Engine& e, const LatentChains& a, cudaStream_t s) {
   if (a.sg_m && a.sg_mask) {
     CDX_CHECK(a.sg_mask <= 2 && a.sg_map && a.sg_gh >= 2 && a.sg_gw >= 2 && a.w > 0 && a.hw == (4 * a.sg_gh) * (4 * a.sg_gw) && a.w == 4 * a.sg_gw,
               "latent_chains_step: mask mode %d over a %dx%d map, hw=%d w=%d", a.sg_mask, a.sg_gh, a.sg_gw, a.hw, a.w);
     if (a.sg_mask == 1) {
       if (a.mask) {
-        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 2>), a.n, a);
-        else LAUNCH1((latent_chains_step_kernel<0, 1, 2>), a.n, a);
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 2, SOLVER>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 1, 2, SOLVER>), a.n, a);
       } else {
-        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 2>), a.n, a);
-        else LAUNCH1((latent_chains_step_kernel<0, 0, 2>), a.n, a);
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 2, SOLVER>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 0, 2, SOLVER>), a.n, a);
       }
     } else {
       if (a.mask) {
-        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 3>), a.n, a);
-        else LAUNCH1((latent_chains_step_kernel<0, 1, 3>), a.n, a);
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 3, SOLVER>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 1, 3, SOLVER>), a.n, a);
       } else {
-        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 3>), a.n, a);
-        else LAUNCH1((latent_chains_step_kernel<0, 0, 3>), a.n, a);
+        if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 3, SOLVER>), a.n, a);
+        else LAUNCH1((latent_chains_step_kernel<0, 0, 3, SOLVER>), a.n, a);
       }
     }
     return;
   }
   if (a.sg_m) {
     if (a.mask) {
-      if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 1>), a.n, a);
-      else LAUNCH1((latent_chains_step_kernel<0, 1, 1>), a.n, a);
+      if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 1, SOLVER>), a.n, a);
+      else LAUNCH1((latent_chains_step_kernel<0, 1, 1, SOLVER>), a.n, a);
     } else {
-      if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 1>), a.n, a);
-      else LAUNCH1((latent_chains_step_kernel<0, 0, 1>), a.n, a);
+      if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 1, SOLVER>), a.n, a);
+      else LAUNCH1((latent_chains_step_kernel<0, 0, 1, SOLVER>), a.n, a);
     }
     return;
   }
   if (a.mask) {
-    if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1>), a.n, a);
-    else LAUNCH1((latent_chains_step_kernel<0, 1>), a.n, a);
+    if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 1, 0, SOLVER>), a.n, a);
+    else LAUNCH1((latent_chains_step_kernel<0, 1, 0, SOLVER>), a.n, a);
   } else {
-    if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0>), a.n, a);
-    else LAUNCH1((latent_chains_step_kernel<0, 0>), a.n, a);
+    if (a.pred) LAUNCH1((latent_chains_step_kernel<1, 0, 0, SOLVER>), a.n, a);
+    else LAUNCH1((latent_chains_step_kernel<0, 0, 0, SOLVER>), a.n, a);
   }
+}
+void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s) {
+  CDX_CHECK(a.solver >= 0 && a.solver <= 2, "latent_chains_step: solver %d", a.solver);
+  if (a.solver == 2) launch_step<2>(e, a, s);
+  else if (a.solver == 1) launch_step<1>(e, a, s);
+  else launch_step<0>(e, a, s);
 }
 void semantic_thresholds(Engine& e, const LatentChains& a, cudaStream_t s) {
   CDX_CHECK(a.sg_m >= 1 && a.sg_m <= SEMANTIC_MAX_CONCEPTS && a.hw > 0 && a.chw % a.hw == 0, "semantic_thresholds: m=%d chw=%d hw=%d", a.sg_m,

@@ -13,6 +13,7 @@ import torch
 from . import _cabi
 from ._cabi import lib, check, UnetConfig, VaeConfig, TextConfig, DdimCoef, PixelCoef
 from .attn_control import MutualSelfControl, PnPControl
+from .schedule import EditFriendlySchedule
 from .semantic import SemanticGuidance
 
 
@@ -429,7 +430,8 @@ class Engine:
         stage 2 is its threshold stage (writes sg_thr), stage 1 then runs the step with the concept terms; sg_scale and sg_lambda are
         lists of m floats, sg_active / sg_apply / sg_mu / sg_beta / sg_beta1 scalars, sg_thr and sg_nu tensors.  LEDITS++'s masks:
         sg_mask 1 or 2 with sg_map [n_src*K*m, sg_gh*sg_gw] (a tensor), sg_gh, sg_gw and the latent width w; sg_thr then holds 2
-        thresholds per concept row."""
+        thresholds per concept row.  Edit-friendly inversion: solver 1 or 2, next 3 with the draw scalars qa / q1, and under solver 2
+        dc (a DpmCoef) with the history buffers d_src [n_src*chw] and d_tgt [n_src*K*chw] (tensors)."""
         sg_rows = fields.pop('sg_rows', None)
         m = len(sg_rows) // max(n_src * K, 1) if sg_rows else 0
         hw = fields.get('hw', 0)
@@ -437,10 +439,11 @@ class Engine:
                     eout=rows * chw, xin=rows * chw, yt=n_src * K * chw, y_out=n_src * K * chw,
                     z_out=(n_src - 1) * fields.get('z_stride', 0) + chw, eps_in=(n_src - 1) * fields.get('eps_stride', 0) + chw,
                     mask=n_src * hw, sg_thr=n_src * K * m * ((chw // hw if hw else 0) if not fields.get('sg_mask') else 2),
-                    sg_nu=n_src * K * chw, sg_map=n_src * K * m * fields.get('sg_gh', 0) * fields.get('sg_gw', 0))
+                    sg_nu=n_src * K * chw, sg_map=n_src * K * m * fields.get('sg_gh', 0) * fields.get('sg_gw', 0), d_src=n_src * chw,
+                    d_tgt=n_src * K * chw)
         assert len(chains) == n_src * (1 + K), f'op_latent_chains: {len(chains)} chains for n_src={n_src}, K={K}'
         table = (_cabi.LatentChain * len(chains))(*[_cabi.LatentChain(int(r), int(r2), float(s)) for r, r2, s in chains])
-        d = _cabi.LatentChainsMaskDesc(chw=chw, n_src=n_src, K=K, rows=rows, chains=table)
+        d = _cabi.LatentChainsSamplerDesc(chw=chw, n_src=n_src, K=K, rows=rows, chains=table)
         if sg_rows:
             assert len(sg_rows) == n_src * K * m, f'op_latent_chains: {len(sg_rows)} concept rows for {n_src * K} target chains'
             sg_table = (C.c_int * len(sg_rows))(*[int(r) for r in sg_rows])
@@ -818,7 +821,10 @@ class UNet(Net):
         semantic: a semantic.SemanticGuidance of m concepts, with c_edit [B, m, L, D] (or [m, L, D], every sample's): SEGA's
         concept terms on the target chain (cdx_cycle_lockstep_semantic), or with use_cross_attn_mask / use_intersect_mask LEDITS++'s
         implicit masks (cdx_cycle_lockstep_semantic_attn); it needs uc, composes with mask, and an attn_control with it raises
-        ValueError."""
+        ValueError.
+        sched: a schedule.DDIMSchedule runs the DPM-Encoder chain above; a schedule.EditFriendlySchedule runs LEDITS++'s edit-friendly
+        inversion instead (independent draws of the source's x, stepped by the eta = 1 DDIM step or the SDE-DPM-Solver++ step), with
+        every control above, through cdx_cycle_lockstep_sampler."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -827,18 +833,11 @@ class UNet(Net):
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
         mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
+        if isinstance(sched, EditFriendlySchedule):
+            return self._cycle_sampler(x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z, mask, attn_control, semantic,
+                                       c_edit)
         if semantic is not None:
-            if attn_control is not None:
-                raise ValueError('semantic guidance does not combine with attention control in one loop')
-            if not isinstance(semantic, SemanticGuidance):
-                raise ValueError(f'semantic: expected a semantic.SemanticGuidance, got {type(semantic)}')
-            if c_edit is None:
-                raise ValueError('semantic guidance needs the concept contexts c_edit [B, m, L, D]')
-            c_edit = _f32c(c_edit, e.device)
-            if c_edit.dim() == 3:
-                c_edit = c_edit.unsqueeze(0).expand(B, -1, -1, -1).contiguous()
-            if tuple(c_edit.shape) != (B, semantic.m) + tuple(c_src.shape[1:]):
-                raise ValueError(f'c_edit: shape {tuple(c_edit.shape)}, expected {(B, semantic.m) + tuple(c_src.shape[1:])}')
+            c_edit = self._semantic_contexts(semantic, c_edit, attn_control, B, c_src.shape[1:])
             sg = semantic.c_struct(n)
             out = e.empty(B, Cc, h, w)
             z = e.empty(B, n + 1, Cc, h, w) if return_z else None
@@ -871,6 +870,52 @@ class UNet(Net):
             check(lib.cdx_cycle_lockstep_ctl(*args))
         else:
             check(lib.cdx_cycle_lockstep_refine(*args, _ptr(own)))
+        return (out, z) if return_z else out
+
+    def _semantic_contexts(self, semantic, c_edit, attn_control, B, ctx_shape):
+        if attn_control is not None:
+            raise ValueError('semantic guidance does not combine with attention control in one loop')
+        if not isinstance(semantic, SemanticGuidance):
+            raise ValueError(f'semantic: expected a semantic.SemanticGuidance, got {type(semantic)}')
+        if c_edit is None:
+            raise ValueError('semantic guidance needs the concept contexts c_edit [B, m, L, D]')
+        c_edit = _f32c(c_edit, self.engine.device)
+        if c_edit.dim() == 3:
+            c_edit = c_edit.unsqueeze(0).expand(B, -1, -1, -1).contiguous()
+        if tuple(c_edit.shape) != (B, semantic.m) + tuple(ctx_shape):
+            raise ValueError(f'c_edit: shape {tuple(c_edit.shape)}, expected {(B, semantic.m) + tuple(ctx_shape)}')
+        return c_edit
+
+    def _cycle_sampler(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z, mask, attn_control, semantic, c_edit):
+        """cycle_lockstep under an EditFriendlySchedule: every control through the one entry point cdx_cycle_lockstep_sampler"""
+        e = self.engine
+        B, Cc, h, w = x0.shape
+        n, L = sched.refine_steps, c_src.shape[1]
+        sp, _keep = sched.sampler_struct()
+        ctl = own = mutual = pnp = sg = am = None
+        if semantic is not None:
+            c_edit = self._semantic_contexts(semantic, c_edit, attn_control, B, c_src.shape[1:])
+            sg = semantic.c_struct(n)
+            am = semantic.attn_mask_struct(L) if semantic.mask_mode else None
+        else:
+            c_edit = None
+        blocks = None
+        if isinstance(attn_control, MutualSelfControl):
+            mutual = _cabi.MutualControlC(attn_control.start_step, attn_control.start_layer)
+        elif isinstance(attn_control, PnPControl):
+            blocks = (C.c_int * max(len(attn_control.feature_blocks), 1))(*attn_control.feature_blocks)
+            fs, ats = attn_control.steps(n)
+            pnp = _cabi.PnpControlC(fs, ats, attn_control.attention_start_layer, C.cast(blocks, C.POINTER(C.c_int)),
+                                    len(attn_control.feature_blocks))
+        elif attn_control is not None:
+            ctl, _token_map, own = attn_control.c_struct(n, B, L, e.device)
+        out = e.empty(B, Cc, h, w)
+        z = e.empty(B, n + 1, Cc, h, w) if return_z else None
+        ref = lambda s: C.byref(s) if s is not None else None
+        check(lib.cdx_cycle_lockstep_sampler(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), L, float(src_scale), float(tgt_scale),
+                                             sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out),
+                                             _ptr(z), B, Cc, h, w, e.stream, C.byref(sp), _ptr(mask), ref(ctl), _ptr(own), ref(mutual),
+                                             ref(pnp), _ptr(c_edit), ref(sg), ref(am)))
         return (out, z) if return_z else out
 
     def cycle_fan(self, x0, c_src, c_tgt, uc, src_scales, tgt_scales, sched, noise, return_z=False, mask=None):

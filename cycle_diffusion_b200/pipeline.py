@@ -16,7 +16,7 @@ import torch
 
 from .attn_control import AttentionControl, MutualSelfControl, PnPControl
 from .engine import check_mask
-from .schedule import DDIMSchedule
+from .schedule import DDIMSchedule, EditFriendlySchedule
 from .semantic import SemanticGuidance
 
 
@@ -182,11 +182,11 @@ class CycleDiffusionPipeline:
 
     @torch.no_grad()
     def __call__(self, prompt, source_prompt, image=None, strength=0.8, num_inference_steps=50, guidance_scale=7.5,
-                 source_guidance_scale=1, num_images_per_prompt=1, eta=0.1, generator=None, prompt_embeds=None, output_type='pt',
+                 source_guidance_scale=1, num_images_per_prompt=1, eta=None, generator=None, prompt_embeds=None, output_type='pt',
                  return_dict=True, callback=None, callback_steps=1, cross_attention_kwargs=None, clip_skip=None, two_phase=False,
                  mask_image=None, paste_back=False, editing_prompt=None, reverse_editing_direction=False, edit_guidance_scale=5,
                  edit_threshold=0.9, edit_cooldown_steps=None, edit_warmup_steps=10, edit_momentum_scale=0.1, edit_mom_beta=0.4,
-                 use_cross_attn_mask=False, use_intersect_mask=False, edit_token_counts=None):
+                 use_cross_attn_mask=False, use_intersect_mask=False, edit_token_counts=None, inversion='cycle'):
         """mask_image: optional float tensor [B,1,H,W] or [1,1,H,W] in [0,1] at the image's size, 1 = "may change" (diffusers'
         convention).  Outside the mask the latent stays on the source image's own chain (cdx_cycle_lockstep_masked), so the
         unmasked region decodes to the image's VAE reconstruction.  paste_back: additionally composite the output with the input
@@ -232,7 +232,24 @@ class CycleDiffusionPipeline:
         requires the term's channel-summed magnitude to be in its percentile (and implies the attention mask).  The tokens of each
         concept come from the conditioning model's token_counts(concepts) (capped at the context length - 2), or from
         edit_token_counts (an int or one per concept), which a conditioning callable without token_counts needs.  The latent's sides
-        must be multiples of 4.  A mask flag without editing_prompt raises ValueError."""
+        must be multiples of 4.  A mask flag without editing_prompt raises ValueError.
+
+        inversion: how the source chain is made.  'cycle' (default): CycleDiffusion's DPM-Encoder, a DDIM posterior chain at eta
+        (None: 0.1).  'ddpm' and 'dpmsolver++': LEDITS++'s edit-friendly inversion (Brack et al., 2024), the source's x at every
+        step drawn from q(x_t | x0) on its own and each step's noise recovered from consecutive draws (Huberman-Spiegelglas et al.,
+        2024), stepped by the eta = 1 DDIM step ('ddpm') or the second-order SDE-DPM-Solver++ step ('dpmsolver++',
+        schedule.EditFriendlySchedule).  Both are stochastic by construction: an eta other than 1 raises ValueError.  The generator
+        is drawn from identically under every inversion, and every control above composes with each.  two_phase=True with an
+        edit-friendly inversion raises ValueError."""
+        if inversion not in ('cycle',) + tuple(EditFriendlySchedule.SOLVERS):
+            raise ValueError(f"inversion must be 'cycle', 'ddpm' or 'dpmsolver++', got {inversion!r}")
+        if inversion == 'cycle':
+            eta = 0.1 if eta is None else eta
+        else:
+            if eta is not None and eta != 1:
+                raise ValueError(f'inversion={inversion!r} samples at eta = 1 by construction, got eta={eta}')
+            if two_phase:
+                raise ValueError(f'inversion={inversion!r} runs in the lock-step loop only (two_phase=False)')
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
         semantic, concepts = None, None
         if editing_prompt is not None:
@@ -262,7 +279,7 @@ class CycleDiffusionPipeline:
             if prompt is None:
                 raise ValueError("mask_image='auto' generates the mask from the prompt text: pass prompt")
             mask_image = self.generate_mask(image, source_prompt, prompt, generator=generator, num_inference_steps=num_inference_steps)
-        assert eta > 0, 'CycleDiffusion needs a stochastic sampler (eta > 0), ddim.py:268'
+        assert inversion != 'cycle' or eta > 0, 'CycleDiffusion needs a stochastic sampler (eta > 0), ddim.py:268'
         g, e = self.g, self.engine
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
         sources = [source_prompt] if isinstance(source_prompt, str) else list(source_prompt)
@@ -291,7 +308,8 @@ class CycleDiffusionPipeline:
             c_edit = g.get_learned_conditioning(concepts).unsqueeze(0).expand(B, -1, -1, -1).contiguous() if concepts else None
             S = num_inference_steps
             skip = S - min(int(S * strength), S)
-            sched = DDIMSchedule(S, eta, skip, g.alphas_cumprod)
+            sched = DDIMSchedule(S, eta, skip, g.alphas_cumprod) if inversion == 'cycle' else \
+                EditFriendlySchedule(S, skip, g.alphas_cumprod, solver=inversion)
             x = e.shift_scale(image, -0.5, 2.0)
             moments = g.encode_first_stage(x)
             lat_shape = (B, moments.shape[1] // 2, moments.shape[2], moments.shape[3])

@@ -9,7 +9,7 @@ IEEE fp32 operations.  We therefore evaluate the very same expressions with torc
 import numpy as np
 import torch
 
-from ._cabi import DdimCoef, PixelCoef
+from ._cabi import DdimCoef, DpmCoef, PixelCoef, SamplerC
 
 
 # ------------------------------------------------------------------------------------------ latent models
@@ -76,6 +76,64 @@ class DDIMSchedule:
     def t_array(self):
         import ctypes
         return (ctypes.c_float * len(self.t_loop))(*self.t_loop)
+
+
+class EditFriendlySchedule(DDIMSchedule):
+    """The edit-friendly inversion of LEDITS++ (Brack et al., 2024) on the DDIM schedule's timesteps and loop geometry, so strength
+    and every step-counted control mean what they mean under DDIMSchedule.  solver 'ddpm': the independent draws stepped by the
+    eta = 1 DDIM table (`coef`, inherited); 'dpmsolver++': the same draws stepped by the SDE-DPM-Solver++ table `dpm`, whose
+    x0-prediction reads sqrt_at / sqrt_1m_at_tab from `coef`.
+      qa[k], q1[k]  fp32 sqrt(abar) and sqrt(1 - abar) of loop step k's level, the source's draw x_k = qa[k]*x0 + q1[k]*noise
+                    (the same torch fp32 expression as sqrt_a_T / sqrt_1ma_T, which are qa[0] / q1[0])
+      dpm[i]        DpmCoef of step i from level s = abar(t_i) to level t = the DDIM table's a_prev of the step (abar[0] on the
+                    last), formed in float64 from the fp32 abar and rounded once each (cdx.h, cdx_dpm_coef).  Order 1 on the first
+                    step and, when the loop has fewer than 15 steps, on the last (diffusers' lower_order_final); else order 2."""
+    SOLVERS = {'ddpm': 1, 'dpmsolver++': 2}      # cdx_sampler kinds CDX_SAMPLER_DDIM_DRAWS, CDX_SAMPLER_DPMSOLVER_DRAWS
+
+    def __init__(self, S, skip_steps=0, alphas_cumprod=None, num_ddpm_timesteps=1000, solver='dpmsolver++'):
+        if solver not in self.SOLVERS:
+            raise ValueError(f"solver must be one of {sorted(self.SOLVERS)}, got {solver!r}")
+        super().__init__(S, 1.0, skip_steps, alphas_cumprod, num_ddpm_timesteps)
+        self.solver, self.kind = solver, self.SOLVERS[solver]
+        ac = ldm_alphas_cumprod(num_ddpm_timesteps) if alphas_cumprod is None else alphas_cumprod.to(torch.float32).cpu()
+        alphas = ac[self.timesteps]
+        R = self.refine_steps
+        self.qa, self.q1 = [], []
+        for k in range(R):
+            at = alphas[R - 1 - k]
+            self.qa.append(at.sqrt().item())
+            self.q1.append((1 - at).sqrt().item())
+        self.dpm = [DpmCoef(**c) for c in self.dpm_table(ac, self.timesteps, R)]
+
+    @staticmethod
+    def dpm_table(ac, timesteps, R):
+        """The SDE-DPM-Solver++ coefficients of the R loop steps as dicts (a, b, c, n, order), in float64 from the fp32 abar ac."""
+        lev = [float(ac[timesteps[R - 1 - i]]) for i in range(R)] + [float(ac[0])]     # lev[i]: step i's level; lev[R]: abar[0]
+        alpha = lambda v: np.sqrt(v)
+        sigma = lambda v: np.sqrt(1.0 - v)
+        lam = lambda v: np.log(alpha(v)) - np.log(sigma(v))
+        out = []
+        for i in range(R):
+            s, t = lev[i], lev[i + 1]
+            h = lam(t) - lam(s)
+            em = -np.expm1(-2.0 * h)
+            a = (sigma(t) / sigma(s)) * np.exp(-h)
+            b = alpha(t) * em
+            n = sigma(t) * np.sqrt(em)
+            order = 1 if i == 0 or (i == R - 1 and R < 15) else 2
+            c = 0.5 * b / ((lam(s) - lam(lev[i - 1])) / h) if order == 2 else 0.0
+            out.append(dict(a=float(np.float32(a)), b=float(np.float32(b)), c=float(np.float32(c)), n=float(np.float32(n)), order=order))
+        return out
+
+    def sampler_struct(self):
+        """-> (cdx_sampler, the host arrays it points to, which must outlive the call)"""
+        import ctypes
+        qa = (ctypes.c_float * len(self.qa))(*self.qa)
+        q1 = (ctypes.c_float * len(self.q1))(*self.q1)
+        dpm = (DpmCoef * len(self.dpm))(*self.dpm)
+        sp = SamplerC(kind=self.kind, dpm=ctypes.cast(dpm, ctypes.POINTER(DpmCoef)), qa=ctypes.cast(qa, ctypes.POINTER(ctypes.c_float)),
+                      q1=ctypes.cast(q1, ctypes.POINTER(ctypes.c_float)))
+        return sp, (qa, q1, dpm)
 
 
 def same_schedule(a, b):

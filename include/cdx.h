@@ -451,6 +451,52 @@ int cdx_cycle_lockstep_semantic_attn(cdx_net* unet, const float* x0, const float
                                      float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
                                      void* stream, const float* mask, const float* c_edit, const cdx_semantic_guidance* sg,
                                      const cdx_semantic_attn_mask* am);
+/* Edit-friendly inversion (LEDITS++, Brack et al., 2024; the edit-friendly DDPM noise space of Huberman-Spiegelglas et al., 2024)
+ * on the lock-step loop.  The source chain is not a posterior chain: its x at every loop step k is drawn from q(x_k | x0) on its own,
+ *   x_k = qa[k]*x0 + q1[k]*noise[k]      (k = 0: x_T, qa[0] == sqrt_a_T and q1[0] == sqrt_1ma_T; the last step's next x is x0)
+ * and each step's noise z is recovered from the pair (x_i, x_{i+1}) and the source row's output.  kind:
+ *   CDX_SAMPLER_DDIM_POSTERIOR  cdx_cycle_lockstep's DPM-Encoder chain (qa, q1, dpm unused)
+ *   CDX_SAMPLER_DDIM_DRAWS      the independent draws with coef's DDIM step (coef must be the eta = 1 table): z = (x_{i+1} -
+ *                               sqrt_aprev*D - dir_coef*e_t) / sigma, the target y_{i+1} = sqrt_aprev*D_y + dir_coef*e_y + sigma*z
+ *   CDX_SAMPLER_DPMSOLVER_DRAWS the independent draws with the second-order SDE-DPM-Solver++ step (diffusers' sde-dpmsolver++
+ *                               midpoint update): with D a chain's x0-prediction (formed from coef as the DDIM step forms pred_x0) and
+ *                               D_prev its previous step's, mu = a*x + b*D (+ c*(D - D_prev) when order == 2), one rounded op each;
+ *                               z = (x_{i+1} - mu_src) / n, y_{i+1} = mu_y + n*z.  dpm host [n_steps]; order 2 on step 0 is rejected.
+ * With identical prompts and scales on both chains the target returns x0 up to rounding: each step hands it the source's next x.
+ * Every control of the lock-step loop acts on U-Net rows before the update and composes unchanged: mask (the blend partner is the
+ * source's next x), ctl with own_weight (cdx_cycle_lockstep_refine), mutual (cdx_cycle_lockstep_mutual), pnp (cdx_cycle_lockstep_pnp),
+ * sg with c_edit (cdx_cycle_lockstep_semantic) and am (cdx_cycle_lockstep_semantic_attn), each NULL when off and exclusive as there.
+ * The noise draws are cdx_cycle_lockstep's: noise[0] gives x_T, noise[1 + i] the source's x at loop step i + 1.  With kind
+ * CDX_SAMPLER_DDIM_POSTERIOR every result equals the matching cdx_cycle_lockstep* entry point's.  One launch per step, as there.
+ * CDX_E_INVALID: an unknown kind, qa / q1 / dpm missing for their kinds, qa[0] or q1[0] other than the x_T scalars, a dpm entry with
+ * n <= 0, an order other than 1 or 2, or order 2 on step 0, and everything the matching entry point rejects. */
+#define CDX_SAMPLER_DDIM_POSTERIOR 0
+#define CDX_SAMPLER_DDIM_DRAWS 1
+#define CDX_SAMPLER_DPMSOLVER_DRAWS 2
+typedef struct cdx_dpm_coef { /* one SDE-DPM-Solver++ step s -> t, each formed in double from fp32 abar and rounded once */
+  float a;      /* (sigma_t / sigma_s) * exp(-h), h = lambda_t - lambda_s, lambda = log(alpha) - log(sigma) */
+  float b;      /* alpha_t * -expm1(-2h) */
+  float c;      /* order 2: 0.5 * b / r0, r0 = (lambda_s - lambda_prev) / h; order 1: 0 */
+  float n;      /* sigma_t * sqrt(-expm1(-2h)) */
+  int order;    /* 1 or 2 */
+} cdx_dpm_coef;
+typedef struct cdx_sampler {
+  int kind;                      /* CDX_SAMPLER_* */
+  const cdx_dpm_coef* dpm;       /* host [n_steps], kind CDX_SAMPLER_DPMSOLVER_DRAWS */
+  const float* qa; const float* q1;   /* host [n_steps]: sqrt(abar) and sqrt(1 - abar) of loop step k's level, the draw kinds */
+} cdx_sampler;
+typedef struct cdx_mutual_control { int start_step, start_layer; } cdx_mutual_control;   /* cdx_cycle_lockstep_mutual's */
+typedef struct cdx_pnp_control {                                                        /* cdx_cycle_lockstep_pnp's */
+  int feature_steps, attention_steps, attention_start_layer;
+  const int* feature_blocks; int n_feature_blocks;
+} cdx_pnp_control;
+int cdx_cycle_lockstep_sampler(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                               int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                               const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                               float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                               void* stream, const cdx_sampler* sampler, const float* mask, const cdx_attn_control* ctl,
+                               const float* own_weight, const cdx_mutual_control* mutual, const cdx_pnp_control* pnp,
+                               const float* c_edit, const cdx_semantic_guidance* sg, const cdx_semantic_attn_mask* am);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -769,6 +815,14 @@ typedef struct cdx_latent_chains_desc {
   int sg_mask;                  /* 0 SEGA's thresholds, 1 LEDITS++'s attention mask, 2 with its channel-summed mask */
   int sg_gh, sg_gw;             /* the map grid: h/4 x w/4 */
   int w;                        /* latent width (hw = h*w = 16*sg_gh*sg_gw) */
+  /* edit-friendly inversion (cdx_cycle_lockstep_sampler): solver 0 the DDIM step on the posterior chain (next 0, 1, 2), 1 the DDIM
+   * step on independent draws, 2 the SDE-DPM-Solver++ step under dc on independent draws (next 0, 2, 3).  next == 3: xn (stage 0) /
+   * xn2 (stage 1) = qa*x0 + q1*noise_next.  solver 2, stage 1: d_src [n_src, chw] and d_tgt [n_src*K, chw] hold each chain's
+   * previous x0-prediction, read when dc.order == 2 and overwritten with this step's. */
+  int solver;
+  cdx_dpm_coef dc;
+  float* d_src; float* d_tgt;
+  float qa, q1;
 } cdx_latent_chains_desc;
 int cdx_op_latent_chains(cdx_engine* e, const cdx_latent_chains_desc* desc, int stage, void* stream);
 /* One launch of the two-model pixel loop's fused step (pixel_lockstep_step, which cdx_pixel_cycle_lockstep runs): xs / ys [B, chw]

@@ -148,6 +148,7 @@ SIGNATURES = {
     'cdx_engine_workspace_bytes': (_S, [_P]),
     'cdx_engine_launch_count': (C.c_uint64, [_P]),
     'cdx_engine_set_mma_mode': (_I, [_P, _I]),
+    'cdx_engine_set_persist': (_I, [_P, _I, _I]),
     'cdx_engine_profile': (_I, [_P, _I]),
     'cdx_engine_profile_read': (_I, [_P, _I, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
     'cdx_unet_create': (_I, [_P, C.POINTER(UnetConfig), C.POINTER(_P)]),

@@ -613,6 +613,8 @@ int cdx_engine_create(int device, cdx_engine** out) {
       throw Error(CDX_E_CUDA, "libcdx is built for sm_90a (H100) only; device " + std::to_string(device) + " is sm_" +
                                   std::to_string(prop.major) + std::to_string(prop.minor));
     eng->e.num_sms = prop.multiProcessorCount;
+    const char* persist = getenv("CDX_PERSIST");
+    eng->e.persist = persist == nullptr || atoi(persist) != 0;
     *out = eng;
   });
 }
@@ -637,6 +639,14 @@ int cdx_engine_set_mma_mode(cdx_engine* e, int mode) {
     e->e.flash_attn = mode != 2 && mode != 0;
     e->e.tc_kind = mode == 3 ? 0 : mode >= 4 ? 2 : 1;    // 3 = 3xTF32 contractions, 4 / 5 = single-term fp16, else fp16 split
     e->e.attn_one = mode == 5;                            // 5 = as 4, plus one-term fused attention ("autocast")
+  });
+}
+
+int cdx_engine_set_persist(cdx_engine* e, int enable, int max_ctas) {
+  return guard([&] {
+    CDX_CHECK(e != nullptr && max_ctas >= 0, "set_persist: bad arguments");
+    e->e.persist = enable != 0;
+    e->e.persist_grid = max_ctas;
   });
 }
 

@@ -76,6 +76,8 @@ struct Engine {
   int mma_mode = 1;              // 0 SIMT FFMA (exact fp32), 1 tensor cores (wgmma)
   int tc_kind = 1;               // tensor-core product scheme: 0 3xTF32, 1 3x fp16-split at the f16 rate (default), 2 1x fp16 (fast, not fp32-faithful)
   bool attn_one = false;         // mode 5 ("autocast"): fused fp16 attention with one product term on hi planes only (no lo planes written)
+  bool persist = true;           // persistent tensor-core GEMM for unsplit dense fp16-split work (CDX_PERSIST=0 at creation: one CTA per item)
+  int persist_grid = 0;          // > 0: at most this many persistent CTAs (tests: one CTA walks many work items); 0: one per SM
   // tracked |max| scalars of activation tensors (operand range of the fp16-split GEMMs): a pool of device floats, handed out
   // per tensor by the graph executors and zeroed at the start of every network call
   float* amax_pool = nullptr;

@@ -14,7 +14,8 @@
 // 256 elements (one chunk if the work item has K <= 512): each chunk accumulates in its own register set, which is added into the
 // fp32 total with round-to-nearest adds when the chunk ends.
 //
-// One CTA per work item (tile, K split) of 128 rows x BN (64 or 128) columns; 384 threads = 3 warpgroups:
+// One CTA per work item (tile, K split) of 128 rows x BN (64 or 128) columns -- or, for unsplit dense fp16-split work, one
+// persistent CTA per SM walking the work items (PERSIST, below); 384 threads = 3 warpgroups:
 //   warpgroup 0   TMA producer (one thread): A is a 2D [M,K] row matrix (dense / 1x1 conv / Linear, optionally two
 //                 channel-concatenated sources), or for conv3x3 a 4D box of the NHWC activation -- per (tap, 32-channel block) {32 ch, bw,
 //                 bh, bn} shifted by (dy-1, dx-1): TMA's out-of-bounds zero fill *is* the conv's zero padding, im2col is never
@@ -65,7 +66,10 @@ enum { KIND_SS = 0, KIND_TS = 1, KIND_H16 = 2, KIND_H16_FAST = 3 };
 // and its in-place lo), BN rows each: 32 fp16 = 64 B (64B swizzle) or 32 fp32 = 128 B (128B swizzle).  The ring is as deep as the
 // shared memory allows: the deeper it is, the more operand bytes the producer keeps in flight ahead of the consumers
 // (H16: 7 stages at BN 128, 9 at BN 64; TS / SS: 4 at BN 128, 7 at BN 64).
-template <int KIND, int BN>
+//
+// PERSIST (fp16 split, unsplit dense work items with the staged store): the epilogue has a buffer of its own after the ring, one
+// 32-column box per 32 output columns (64 KB at BN 128, 32 KB at BN 64), and the ring shrinks to fit (5 / 8 stages).
+template <int KIND, int BN, bool PERSIST = false>
 struct Cfg {
   static constexpr bool H16 = KIND == KIND_H16 || KIND == KIND_H16_FAST;
   static constexpr int BK = TBK;                     // K elements per pipeline stage
@@ -75,18 +79,21 @@ struct Cfg {
   static constexpr int B_ROW = H16 ? 64 : 128;       // bytes of one B row of a stage
   static constexpr int B_PLANE = BN * B_ROW;
   static constexpr int STAGE_BYTES = A_BYTES + 2 * B_PLANE;
-  static constexpr int STAGES = (SMEM_MAX - BAR_BYTES - ALIGN_SLACK) / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + ALIGN_SLACK;
+  static constexpr int EPI_BOX = TBM * TBK * 4;
+  static constexpr int EPI_BYTES = PERSIST ? BN / TBK * EPI_BOX : 0;     // the persistent epilogue's own buffer
+  static constexpr int STAGES = (SMEM_MAX - BAR_BYTES - ALIGN_SLACK - EPI_BYTES) / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + BAR_BYTES + ALIGN_SLACK;
   // Staged epilogue: the output tile (and the residual tile, loaded by TMA) as 32-column fp32 boxes of 128 rows (the A box's shape,
   // 128B swizzle), EPI_PER_SLOT to a ring slot, in the slots of ring stages nst, nst + 1, ... after the work item's nst stages.  The
   // producer claims each through its empty barrier, which frees the slot of stage nst + k - STAGES; the last stage's slot is never
   // handed back, so every claimed slot must have held a stage before nst - 1, and for the residual to land while the last wgmmas
-  // run, before nst - 2: STAGES >= 2 + EPI_SLOTS.
-  static constexpr int EPI_BOX = TBM * TBK * 4;
+  // run, before nst - 2: STAGES >= 2 + EPI_SLOTS.  (PERSIST: the boxes live in the epilogue's buffer instead.)
   static constexpr int EPI_PER_SLOT = STAGE_BYTES / EPI_BOX;
   static constexpr int EPI_SLOTS = (BN / TBK + EPI_PER_SLOT - 1) / EPI_PER_SLOT;
-  static_assert(STAGES >= 2 + EPI_SLOTS, "the epilogue's slots never include the last stages' slots");
-  static_assert(STAGES >= 3 && (2 * STAGES + 1) * 8 <= BAR_BYTES, "barrier area holds a full and an empty barrier per stage and bar_res");
+  static_assert(PERSIST || STAGES >= 2 + EPI_SLOTS, "the epilogue's slots never include the last stages' slots");
+  static_assert(!PERSIST || (H16 && STAGES == (BN == 128 ? 5 : 8)), "persistent ring: 5 stages at BN 128, 8 at BN 64 beside the epilogue buffer");
+  static_assert(EPI_BYTES % 1024 == 0, "the barriers after the epilogue buffer stay aligned");
+  static_assert(STAGES >= 3 && (2 * STAGES + 2) * 8 <= BAR_BYTES, "barrier area holds a full and an empty barrier per stage, bar_res and bar_out");
   static_assert(STAGE_BYTES % 1024 == 0 && B_PLANE % 1024 == 0, "stage and plane bases stay 1024-byte aligned (swizzle atoms)");
   static_assert(SMEM_BYTES <= SMEM_MAX, "smem overflow");
 };
@@ -181,31 +188,60 @@ __device__ __forceinline__ TileCoord tile_coord(const TcParams& p, int t, int nu
 
 __device__ __forceinline__ uint32_t tf32_lo(float x, uint32_t hi) { return rn_tf32(__float_as_uint(x - __uint_as_float(hi))); }
 
-template <int KIND, int BN>
+// Timeline probe, compiled in only with -DCDX_GEMM_TIMELINE (tools/gemm_timeline.py builds that variant into a directory of its own):
+// %globaltimer stamps per CTA into a device buffer, TL_SLOTS per CTA at [blockIdx.x * TL_SLOTS]: 0 entry, 1 after pdl_wait, 2 the
+// first stage has landed, 3 the last stage has retired, 4 bar_res passed, 5 the TMA store issued, 6 bulk_wait0 returned.  A
+// persistent CTA stamps 2 at its first work item and 3 - 6 at its last.
+#ifdef CDX_GEMM_TIMELINE
+constexpr int TL_SLOTS = 8;
+__device__ unsigned long long* g_gemm_timeline = nullptr;
+__device__ __forceinline__ void tl_stamp(int k) {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
+  if (g_gemm_timeline) g_gemm_timeline[(size_t)blockIdx.x * TL_SLOTS + k] = t;
+}
+#define TL_STAMP(k) tl_stamp(k)
+#else
+#define TL_STAMP(k) ((void)0)
+#endif
+
+// PERSIST (KIND_H16 / KIND_H16_FAST, unsplit dense work items with the staged store; gemm_tc decides): a grid of at most one CTA
+// per SM, CTA c walking work items t = c, c + gridDim.x, ... of the same raster.  The ring's stage counter and phases run on across
+// the items, so the producer fills item t + gridDim.x's stages as soon as item t's last stage is issued.  The epilogue has its own
+// buffer after the ring: thread 32 (warpgroup 0) stores item j's boxes from it by TMA once the consumers have written them (bar_out),
+// waits only until the store has read the buffer, then TMA-loads item j + 1's residual boxes into it (bar_res: the buffer is free
+// and the residual has landed).  Full completion of the stores is awaited once, after the CTA's last item.  Each output tile is
+// computed by the same stages, wgmmas and epilogue arithmetic as without PERSIST.
+template <int KIND, int BN, bool PERSIST = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapA2,
                const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapBlo,
                const __grid_constant__ CUtensorMap mapR, const __grid_constant__ CUtensorMap mapC, const TcParams p) {
-  using CF = Cfg<KIND, BN>;
+  using CF = Cfg<KIND, BN, PERSIST>;
   constexpr bool H16 = CF::H16, FAST = KIND == KIND_H16_FAST;
   constexpr int BK = CF::BK, KSTEPS = CF::KSTEPS, A_BYTES = CF::A_BYTES, B_PLANE = CF::B_PLANE, STAGE_BYTES = CF::STAGE_BYTES;
   constexpr int STAGES = CF::STAGES, EPI_BOX = CF::EPI_BOX, EPI_PER_SLOT = CF::EPI_PER_SLOT, EPI_SLOTS = CF::EPI_SLOTS;
   constexpr int NACC = BN / 2;                     // fp32 accumulators per thread of an m64nBN tile
+  if (threadIdx.x == 0) TL_STAMP(0);
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // 1024-byte aligned (swizzle atoms)
-  const uint32_t bars = base + STAGES * STAGE_BYTES;
+  const uint32_t epi = base + STAGES * STAGE_BYTES;                // PERSIST: the epilogue's buffer
+  const uint32_t bars = epi + CF::EPI_BYTES;
   auto bar_full = [&](int s) { return bars + 8u * s; };
   auto bar_empty = [&](int s) { return bars + 8u * (STAGES + s); };
   const uint32_t bar_res = bars + 16u * STAGES;    // the epilogue's slots are claimed (and the residual tile has landed)
+  const uint32_t bar_out = bar_res + 8u;           // PERSIST: the consumers have written a work item's output boxes
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = (p.K + BK - 1) / BK;
-  const TileCoord tc_ = tile_coord(p, blockIdx.x, num_kb);
-  const int nst = tc_.kb1 - tc_.kb0;               // stages of this work item (>= 1; K % 32 == 0: every stage is full)
-  const bool staged = staged_store(p);
+  TileCoord tc_ = tile_coord(p, blockIdx.x, num_kb);
+  int nst = tc_.kb1 - tc_.kb0;                     // stages of this work item (>= 1; K % 32 == 0: every stage is full)
+  const bool staged = PERSIST || staged_store(p);
   // shared address of 32-column box k of the staged output / residual tile
-  auto epi_box = [&](int k) { return base + ((nst + k / EPI_PER_SLOT) % STAGES) * STAGE_BYTES + (k % EPI_PER_SLOT) * EPI_BOX; };
+  auto epi_box = [&](int k) {
+    return PERSIST ? epi + k * EPI_BOX : base + ((nst + k / EPI_PER_SLOT) % STAGES) * STAGE_BYTES + (k % EPI_PER_SLOT) * EPI_BOX;
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
@@ -213,10 +249,66 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
       mbar_init(bar_empty(s), 8);                 // one arrival per consumer warp
     }
     mbar_init(bar_res, 1);
+    if (PERSIST) mbar_init(bar_out, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();                     // everything above touched shared memory only
+  if (threadIdx.x == 0) TL_STAMP(1);
+
+  if (PERSIST && warp < 4) {
+    // =========================================================================== TMA producer and epilogue store, persistent
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      int it = 0;                                  // ring stage counter, across the CTA's work items
+      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+        const TileCoord c = tile_coord(p, t, num_kb);
+        for (int kb = c.kb0; kb < c.kb1; ++kb, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(bar_empty(s), ((it / STAGES) & 1) ^ 1);
+          const uint32_t st = base + s * STAGE_BYTES;
+          const int k0 = kb * BK;
+          mbar_expect_tx(bar_full(s), TILE_BYTES + 2 * B_PLANE);
+          if (k0 < p.C1) tma_load_2d(st, &mapA, k0, c.m0, bar_full(s));
+          else tma_load_2d(st, &mapA2, k0 - p.C1, c.m0, bar_full(s));
+          tma_load_2d(st + A_BYTES, &mapB, k0, c.n0, bar_full(s));
+          tma_load_2d(st + A_BYTES + B_PLANE, &mapBlo, k0, c.n0, bar_full(s));
+        }
+      }
+    } else if (threadIdx.x == 32) {
+      const int c0_div = p.geglu ? 2 : 1, ncols = p.geglu ? p.N / 2 : p.N, nbox = p.geglu ? BN / 64 : BN / TBK;
+      auto store = [&](const TileCoord& c) {
+        const int c0 = c.n0 / c0_div;
+        for (int b = 0; b < nbox && c0 + b * TBK < ncols; ++b) tma_store_2d(epi_box(b), &mapC, c0 + b * TBK, c.m0);
+        bulk_commit();
+      };
+      int j = 0;
+      TileCoord prev;
+      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++j) {
+        const TileCoord c = tile_coord(p, t, num_kb);
+        if (j > 0) {
+          mbar_wait(bar_out, (j - 1) & 1);
+          store(prev);
+          bulk_wait_read0();                       // the buffer has been read: it may take item j's residual and output
+        }
+        if (p.residual) {
+          mbar_expect_tx(bar_res, BN * TBM * 4);
+          for (int b = 0; b < BN / TBK; ++b) tma_load_2d(epi_box(b), &mapR, c.n0 + b * TBK, c.m0, bar_res);
+        } else {
+          mbar_arrive(bar_res);
+        }
+        prev = c;
+      }
+      if (j > 0) {
+        mbar_wait(bar_out, (j - 1) & 1);
+        store(prev);
+        TL_STAMP(5);
+        bulk_wait0();                              // written, not only read: a dependent launch reads C after its griddepcontrol.wait
+        TL_STAMP(6);
+      }
+    }
+    return;
+  }
 
   if (warp < 4) {
     // =========================================================================== TMA producer
@@ -283,314 +375,339 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   const int r0 = wg * 64 + wi * 16 + g;            // tile rows r0 and r0 + 8 of this thread
   const int ea = H16 ? h16_a_exp(p) : 0;
   const float asc = exp2i(ea);
-  const int kchunk = (tc_.kb1 - tc_.kb0) <= 2 * CF::KCHUNK ? 2 * CF::KCHUNK : CF::KCHUNK;
-  // conv: pixel of each of this thread's two rows (the epilogue masks rows outside the map)
-  int px[2] = {0, 0}, py[2] = {0, 0}, pb[2] = {0, 0};
-  if (p.mode == 1) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int r = r0 + 8 * i;
-      px[i] = tc_.x0 + r % p.bw; py[i] = tc_.y0 + (r / p.bw) % p.bh; pb[i] = tc_.b0 + r / (p.bw * p.bh);
-    }
-  }
-
-  float acc[NACC], tot[NACC];
-#pragma unroll
-  for (int j = 0; j < NACC; ++j) { acc[j] = 0.f; tot[j] = 0.f; }
-
-  // Software pipeline over the stages of the work item: while the wgmmas of stage it run, stage it + 1's A is split into the
-  // other fragment set; wgmma.wait_group 1 then retires stage it - 1, whose smem slot goes back to the producer.
-  struct Frag { uint32_t h[KSTEPS][4], l[KSTEPS][4]; };     // A fragments of one stage's K steps (rows r0 / r0 + 8), hi / lo
-
-  // wait for stage it to land, then split its A into f
-  auto load_split = [&](int it, Frag& f) {
-    const int s = it % STAGES;
-    mbar_wait(bar_full(s), (it / STAGES) & 1);
-    const uint32_t st = base + s * STAGE_BYTES;
-    if (KIND == KIND_SS) {
-      // raw fp32 B tile -> TF32 hi in place, lo into the second plane (both consumer warpgroups, then a named barrier)
-      const uint32_t sb = st + A_BYTES;
-      const int ct = threadIdx.x - 128;
-#pragma unroll 4
-      for (int i = ct; i < B_PLANE / 16; i += 256) {
-        const uint32_t a = sb + (uint32_t)i * 16u;
-        uint32_t v[4], h[4], l[4];
-        asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(a));
-#pragma unroll
-        for (int c = 0; c < 4; ++c) { h[c] = rn_tf32(v[c]); l[c] = tf32_lo(__uint_as_float(v[c]), h[c]); }
-        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3]) : "memory");
-        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a + B_PLANE), "r"(l[0]), "r"(l[1]), "r"(l[2]), "r"(l[3]) : "memory");
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-    }
-#pragma unroll
-    for (int kk = 0; kk < KSTEPS; ++kk) {
-      if (H16) {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {                 // i: row r0 + 8 i
-          const int r = r0 + 8 * i;
-#pragma unroll
-          for (int hk = 0; hk < 2; ++hk) {            // hk: k 2qd (+1) or 2qd + 8 (+1)
-            const int k = kk * 16 + hk * 8 + 2 * qd;
-            float2 x;
-            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x.x), "=f"(x.y)
-                         : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
-            if (ea != 0) { x.x *= asc; x.y *= asc; }
-            const __half2 h = __floats2half2_rn(x.x, x.y);       // .x (low half) = even k
-            f.h[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&h);
-            if (!FAST) {
-              const float2 hf = __half22float2(h);
-              const __half2 l = __floats2half2_rn(x.x - hf.x, x.y - hf.y);
-              f.l[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&l);
-            }
-          }
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int r = r0 + 8 * i;
-#pragma unroll
-          for (int hk = 0; hk < 2; ++hk) {            // k = 8 kk + qd (+4)
-            const int k = kk * 8 + hk * 4 + qd;
-            float x;
-            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
-                         : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
-            const uint32_t h = rn_tf32(__float_as_uint(x));
-            f.h[kk][hk * 2 + i] = h;
-            f.l[kk][hk * 2 + i] = tf32_lo(x, h);
-          }
-        }
-      }
-    }
-  };
-
-  // the wgmmas of stage it from f: one straight-line batch, small terms first
-  auto mma = [&](int it, const Frag& f) {
-    const uint32_t sb = base + (it % STAGES) * STAGE_BYTES + A_BYTES;
-    const uint64_t bhi = H16 ? make_desc_sw64(sb) : make_desc(sb), blo = H16 ? make_desc_sw64(sb + B_PLANE) : make_desc(sb + B_PLANE);
-    wgmma_pin(acc);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < KSTEPS; ++kk) {
-      const uint64_t adv = (uint64_t)kk * 2u;       // 32 bytes per K step along the B row (64 B fp16 / 128 B fp32)
-      if (H16) {
-        if (!FAST) {
-          Wgmma<BN>::f16_rs(acc, f.l[kk], bhi + adv);
-          Wgmma<BN>::f16_rs(acc, f.h[kk], blo + adv);
-        }
-        Wgmma<BN>::f16_rs(acc, f.h[kk], bhi + adv);
-      } else {
-        Wgmma<BN>::tf32_rs(acc, f.l[kk], bhi + adv);
-        Wgmma<BN>::tf32_rs(acc, f.h[kk], blo + adv);
-        Wgmma<BN>::tf32_rs(acc, f.h[kk], bhi + adv);
-      }
-    }
-    wgmma_commit();
-  };
-
-  // stage it: its fragments are in cur; nxt held stage it - 1's
-  int kin = 0;
-  auto step = [&](int it, const Frag& cur, Frag& nxt) {
-    mma(it, cur);
-    wgmma_wait1();                                  // stage it - 1 has retired: its slot and its fragment set are free
-    if (it > 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_empty((it - 1) % STAGES));
-    }
-    if (it + 1 < nst) load_split(it + 1, nxt);
-    if (++kin == kchunk || it == nst - 1) {        // chunk complete: retire it, round-to-nearest fp32 add into the total
-      wgmma_wait0();
-      wgmma_pin(acc);
-#pragma unroll
-      for (int j = 0; j < NACC; ++j) { tot[j] += acc[j]; acc[j] = 0.f; }
-      kin = 0;
-    }
-  };
-
-  Frag fa, fb;
-  load_split(0, fa);
+  float omax_cta = 0.f;                            // PERSIST: range of C over the CTA's work items
+  int g0 = 0;                                      // PERSIST: ring stage of the work item's first stage
 #pragma unroll 1
-  for (int it = 0; it < nst; it += 2) {
-    step(it, fa, fb);
-    if (it + 1 < nst) step(it + 1, fb, fa);
-  }
-  // (the last stage's slot is not handed back: the producer has loaded everything)
-
-  // ============================================================================= epilogue (straight from registers)
-  // accumulator element j*4 + i*2 + c: tile row r0 + 8 i, column n0 + 8 j + 2 qd + c
-  const bool fin = p.splits == 1;                  // otherwise: raw partial sums to ws[split][M][N]
-  const float alpha = H16 ? p.alpha * exp2i(-ea) * exp2i(-p.b_exp) : p.alpha;
-  long long mrow[2];
-  bool rok[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int r = r0 + 8 * i;
-    if (p.mode != 1) {
-      mrow[i] = (long long)tc_.m0 + r;
-      rok[i] = mrow[i] < p.M;
-    } else {
-      // rows of a tile that overhangs the map's right / bottom edge (or the batch) are not pixels: nothing is stored for them
-      rok[i] = pb[i] < p.B && px[i] < p.W && py[i] < p.H;
-      mrow[i] = ((long long)pb[i] * p.H + py[i]) * p.W + px[i];
-    }
-  }
-  float omax = 0.f;
-  const int n0 = tc_.n0, nend = tc_.nend;
-  if (!fin) {
-    float* const dst = p.ws + (long long)tc_.split * p.M * p.N;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int n = n0 + 8 * j + 2 * qd + c;
-          if (rok[i] && n < nend) dst[mrow[i] * p.N + n] = tot[j * 4 + i * 2 + c];
-        }
-    return;
-  }
-  // pass 1: alpha, bias, per-image row vector
-#pragma unroll
-  for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const int n = n0 + 8 * j + 2 * qd + c;
-      const float bv = (p.bias && n < nend) ? p.bias[n] : 0.f;
+  for (int t = blockIdx.x, item = 0;;) {           // PERSIST: work items t = blockIdx.x, + gridDim.x, ... (item counts them); else one
+    const int kchunk = (tc_.kb1 - tc_.kb0) <= 2 * CF::KCHUNK ? 2 * CF::KCHUNK : CF::KCHUNK;
+    // conv: pixel of each of this thread's two rows (the epilogue masks rows outside the map)
+    int px[2] = {0, 0}, py[2] = {0, 0}, pb[2] = {0, 0};
+    if (p.mode == 1) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        float v = alpha * tot[j * 4 + i * 2 + c] + bv;
-        if (p.rowvec && rok[i] && n < nend) v += p.rowvec[(mrow[i] / p.rows_per_batch) * p.ld_rowvec + n];
-        tot[j * 4 + i * 2 + c] = v;
+        const int r = r0 + 8 * i;
+        px[i] = tc_.x0 + r % p.bw; py[i] = tc_.y0 + (r / p.bw) % p.bh; pb[i] = tc_.b0 + r / (p.bw * p.bh);
       }
     }
-  if (p.out_nchw) {
+
+    float acc[NACC], tot[NACC];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      if (!rok[i]) continue;
-      const long long bimg = mrow[i] / p.rows_per_img, rimg = mrow[i] - bimg * p.rows_per_img;
+    for (int j = 0; j < NACC; ++j) { acc[j] = 0.f; tot[j] = 0.f; }
+
+    // Software pipeline over the stages of the work item: while the wgmmas of stage it run, stage it + 1's A is split into the
+    // other fragment set; wgmma.wait_group 1 then retires stage it - 1, whose smem slot goes back to the producer.
+    struct Frag { uint32_t h[KSTEPS][4], l[KSTEPS][4]; };     // A fragments of one stage's K steps (rows r0 / r0 + 8), hi / lo
+
+    // wait for stage it to land, then split its A into f
+    auto load_split = [&](int it, Frag& f) {
+      const int s = (g0 + it) % STAGES;
+      mbar_wait(bar_full(s), ((g0 + it) / STAGES) & 1);
+      const uint32_t st = base + s * STAGE_BYTES;
+      if (KIND == KIND_SS) {
+        // raw fp32 B tile -> TF32 hi in place, lo into the second plane (both consumer warpgroups, then a named barrier)
+        const uint32_t sb = st + A_BYTES;
+        const int ct = threadIdx.x - 128;
+#pragma unroll 4
+        for (int i = ct; i < B_PLANE / 16; i += 256) {
+          const uint32_t a = sb + (uint32_t)i * 16u;
+          uint32_t v[4], h[4], l[4];
+          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(a));
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int n = n0 + 8 * j + 2 * qd + c;
-          if (n < nend) p.C[(bimg * p.N + n) * p.rows_per_img + rimg] = tot[j * 4 + i * 2 + c];
+          for (int c = 0; c < 4; ++c) { h[c] = rn_tf32(v[c]); l[c] = tf32_lo(__uint_as_float(v[c]), h[c]); }
+          asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3]) : "memory");
+          asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a + B_PLANE), "r"(l[0]), "r"(l[1]), "r"(l[2]), "r"(l[3]) : "memory");
         }
-    }
-    return;
-  }
-  if (p.Ct_hi && n0 >= p.t_col0) {
-    // transposed TF32-plane output (V^T)
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
+      for (int kk = 0; kk < KSTEPS; ++kk) {
+        if (H16) {
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int n = n0 + 8 * j + 2 * qd + c;
-          if (rok[i] && n < nend) {
-            const float o = tot[j * 4 + i * 2 + c];
-            const uint32_t hi = rn_tf32(__float_as_uint(o));
-            const long long at = (long long)(n - p.t_col0) * p.ldt + mrow[i];
-            p.Ct_hi[at] = __uint_as_float(hi);
-            p.Ct_lo[at] = __uint_as_float(tf32_lo(o, hi));
-            omax = fmaxf(omax, fabsf(o));
-          }
-        }
-  } else {
-    float* const dst = p.C + tc_.zb * p.sC_b + tc_.zh * p.sC_h;
-    float* const dst_lo = p.C_lo ? p.C_lo + tc_.zb * p.sC_b + tc_.zh * p.sC_h : nullptr;
-    // one loop body, compiled for each store path: STAGED writes every row and column of the tile into the epilogue's boxes (rows
-    // and columns outside C are clipped by the TMA store), the other path stores the valid elements to global memory
-    auto store_tile = [&](auto staged_c) {
-      constexpr bool STAGED = decltype(staged_c)::value;
-      // GEGLU tiles are [32 value | 32 gate] blocks: accumulator group j (value) pairs with j + 4 (gate)
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        if (p.geglu && (j & 4)) continue;
-        const int n = n0 + 8 * j + 2 * qd;             // even; N % 4 == 0 (eligibility), so n + 1 < nend whenever n < nend
-        const int nout = p.geglu ? (n >> 6) * 32 + (n & 63) : n;
-        // STAGED: the column pair's box and its column in the box (GEGLU: boxes of the BN / 2 output columns)
-        const int box = p.geglu ? j >> 3 : j >> 2, cc = 8 * (j & 3) + 2 * qd;
-        float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          float2 o = make_float2(tot[j * 4 + i * 2], tot[j * 4 + i * 2 + 1]);
-          if (p.geglu) {
-            const float g0 = tot[(j + 4) * 4 + i * 2], g1 = tot[(j + 4) * 4 + i * 2 + 1];
-            o.x *= 0.5f * g0 * (1.f + erff(g0 * 0.70710678118654752440f));     // exact-erf GELU as F.gelu
-            o.y *= 0.5f * g1 * (1.f + erff(g1 * 0.70710678118654752440f));
-          }
-          if (STAGED) {
-            // the 128B-swizzled box layout; the residual box holds its value at the same address
+          for (int i = 0; i < 2; ++i) {                 // i: row r0 + 8 i
             const int r = r0 + 8 * i;
-            const uint32_t a = epi_box(box) + (uint32_t)r * 128u + ((((uint32_t)cc >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(cc & 3) * 4u;
-            if (p.residual) {
-              float2 rv;
-              asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rv.x), "=f"(rv.y) : "r"(a));
-              o.x += rv.x;
-              o.y += rv.y;
-            }
-            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(o.x), "f"(o.y) : "memory");
-          }
-          if (!rok[i] || n >= nend) continue;
-          if (!STAGED && p.residual) {
-            o.x += p.residual[mrow[i] * p.ldr + n];
-            o.y += p.residual[mrow[i] * p.ldr + n + 1];
-          }
-          if (p.c_stats) { cs[0] += o.x; cq[0] += o.x * o.x; cs[1] += o.y; cq[1] += o.y * o.y; }
-          if (!STAGED) {
-            float* const d = dst + mrow[i] * p.ldc + nout;
-            if (dst_lo) {                          // operand planes for a following tensor-core consumer
-              const uint32_t hx = rn_tf32(__float_as_uint(o.x)), hy = rn_tf32(__float_as_uint(o.y));
-              *reinterpret_cast<float2*>(dst_lo + mrow[i] * p.ldc + nout) = make_float2(__uint_as_float(tf32_lo(o.x, hx)), __uint_as_float(tf32_lo(o.y, hy)));
-              o = make_float2(__uint_as_float(hx), __uint_as_float(hy));
-            }
-            *reinterpret_cast<float2*>(d) = o;
-          }
-          omax = fmaxf(omax, fmaxf(fabsf(o.x), fabsf(o.y)));
-        }
-        if (p.c_stats) {
-          // GroupNorm statistics: fold the warp's 16 rows (one image: host-checked), one fp64 atomic per (column, statistic)
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-#pragma unroll
-            for (int o2 = 4; o2 < 32; o2 <<= 1) {
-              cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], o2);
-              cq[c] += __shfl_xor_sync(0xffffffffu, cq[c], o2);
+            for (int hk = 0; hk < 2; ++hk) {            // hk: k 2qd (+1) or 2qd + 8 (+1)
+              const int k = kk * 16 + hk * 8 + 2 * qd;
+              float2 x;
+              asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x.x), "=f"(x.y)
+                           : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
+              if (ea != 0) { x.x *= asc; x.y *= asc; }
+              const __half2 h = __floats2half2_rn(x.x, x.y);       // .x (low half) = even k
+              f.h[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&h);
+              if (!FAST) {
+                const float2 hf = __half22float2(h);
+                const __half2 l = __floats2half2_rn(x.x - hf.x, x.y - hf.y);
+                f.l[kk][hk * 2 + i] = *reinterpret_cast<const uint32_t*>(&l);
+              }
             }
           }
-          const long long mq = __shfl_sync(0xffffffffu, rok[0] ? mrow[0] : -1LL, 0);     // first row of the warp
-          if (g == 0 && mq >= 0 && n < nend) {
-            double* sp = p.c_stats + ((mq / p.rows_per_batch) * p.N + n) * 2;
-            atomicAdd(sp, (double)cs[0]); atomicAdd(sp + 1, (double)cq[0]);
-            atomicAdd(sp + 2, (double)cs[1]); atomicAdd(sp + 3, (double)cq[1]);
+        } else {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int r = r0 + 8 * i;
+#pragma unroll
+            for (int hk = 0; hk < 2; ++hk) {            // k = 8 kk + qd (+4)
+              const int k = kk * 8 + hk * 4 + qd;
+              float x;
+              asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x)
+                           : "r"(st + (uint32_t)r * 128u + ((((uint32_t)k >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 3) * 4u));
+              const uint32_t h = rn_tf32(__float_as_uint(x));
+              f.h[kk][hk * 2 + i] = h;
+              f.l[kk][hk * 2 + i] = tf32_lo(x, h);
+            }
           }
         }
       }
     };
-    if (!staged) {
-      store_tile(std::false_type());
-    } else {
-      mbar_wait(bar_res, 0);                       // the boxes' slots are free and the residual boxes have landed
-      store_tile(std::true_type());
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA store
-      asm volatile("bar.sync 2, 256;" ::: "memory");                 // the consumer warpgroups' rows are all written
-      if (threadIdx.x == 128) {
-        const int c0 = p.geglu ? n0 / 2 : n0, ncols = p.geglu ? p.N / 2 : p.N;
-        for (int b = 0; b < (p.geglu ? BN / 64 : BN / TBK) && c0 + b * TBK < ncols; ++b) {
-          if (p.mode == 0) tma_store_2d(epi_box(b), &mapC, c0 + b * TBK, tc_.m0);
-          else tma_store_4d(epi_box(b), &mapC, c0 + b * TBK, tc_.x0, tc_.y0, tc_.b0);
+
+    // the wgmmas of stage it from f: one straight-line batch, small terms first
+    auto mma = [&](int it, const Frag& f) {
+      const uint32_t sb = base + ((g0 + it) % STAGES) * STAGE_BYTES + A_BYTES;
+      const uint64_t bhi = H16 ? make_desc_sw64(sb) : make_desc(sb), blo = H16 ? make_desc_sw64(sb + B_PLANE) : make_desc(sb + B_PLANE);
+      wgmma_pin(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KSTEPS; ++kk) {
+        const uint64_t adv = (uint64_t)kk * 2u;       // 32 bytes per K step along the B row (64 B fp16 / 128 B fp32)
+        if (H16) {
+          if (!FAST) {
+            Wgmma<BN>::f16_rs(acc, f.l[kk], bhi + adv);
+            Wgmma<BN>::f16_rs(acc, f.h[kk], blo + adv);
+          }
+          Wgmma<BN>::f16_rs(acc, f.h[kk], bhi + adv);
+        } else {
+          Wgmma<BN>::tf32_rs(acc, f.l[kk], bhi + adv);
+          Wgmma<BN>::tf32_rs(acc, f.h[kk], blo + adv);
+          Wgmma<BN>::tf32_rs(acc, f.h[kk], bhi + adv);
         }
-        bulk_commit();
-        bulk_wait0();                              // written, not only read: a dependent launch reads C after its griddepcontrol.wait
+      }
+      wgmma_commit();
+    };
+
+    // stage it: its fragments are in cur; nxt held stage it - 1's
+    int kin = 0;
+    auto step = [&](int it, const Frag& cur, Frag& nxt) {
+      mma(it, cur);
+      wgmma_wait1();                                  // stage it - 1 has retired: its slot and its fragment set are free
+      if (it > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty((g0 + it - 1) % STAGES));
+      }
+      if (it + 1 < nst) load_split(it + 1, nxt);
+      if (++kin == kchunk || it == nst - 1) {        // chunk complete: retire it, round-to-nearest fp32 add into the total
+        wgmma_wait0();
+        wgmma_pin(acc);
+#pragma unroll
+        for (int j = 0; j < NACC; ++j) { tot[j] += acc[j]; acc[j] = 0.f; }
+        kin = 0;
+      }
+    };
+
+    Frag fa, fb;
+    load_split(0, fa);
+    if (threadIdx.x == 128 && item == 0) TL_STAMP(2);
+#pragma unroll 1
+    for (int it = 0; it < nst; it += 2) {
+      step(it, fa, fb);
+      if (it + 1 < nst) step(it + 1, fb, fa);
+    }
+    if (PERSIST) {
+      // the last stage has retired (chunk end): its slot goes back to the producer, which fills the next work item's stages
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty((g0 + nst - 1) % STAGES));
+    }
+    // (otherwise the last stage's slot is not handed back: the producer has loaded everything)
+    if (threadIdx.x == 128) TL_STAMP(3);
+
+    // ============================================================================= epilogue (straight from registers)
+    // accumulator element j*4 + i*2 + c: tile row r0 + 8 i, column n0 + 8 j + 2 qd + c
+    const bool fin = PERSIST || p.splits == 1;       // otherwise: raw partial sums to ws[split][M][N]
+    const float alpha = H16 ? p.alpha * exp2i(-ea) * exp2i(-p.b_exp) : p.alpha;
+    long long mrow[2];
+    bool rok[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = r0 + 8 * i;
+      if (p.mode != 1) {
+        mrow[i] = (long long)tc_.m0 + r;
+        rok[i] = mrow[i] < p.M;
+      } else {
+        // rows of a tile that overhangs the map's right / bottom edge (or the batch) are not pixels: nothing is stored for them
+        rok[i] = pb[i] < p.B && px[i] < p.W && py[i] < p.H;
+        mrow[i] = ((long long)pb[i] * p.H + py[i]) * p.W + px[i];
       }
     }
+    float omax = 0.f;
+    const int n0 = tc_.n0, nend = tc_.nend;
+    if (!fin) {
+      float* const dst = p.ws + (long long)tc_.split * p.M * p.N;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int n = n0 + 8 * j + 2 * qd + c;
+            if (rok[i] && n < nend) dst[mrow[i] * p.N + n] = tot[j * 4 + i * 2 + c];
+          }
+      return;
+    }
+    // pass 1: alpha, bias, per-image row vector
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int n = n0 + 8 * j + 2 * qd + c;
+        const float bv = (p.bias && n < nend) ? p.bias[n] : 0.f;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float v = alpha * tot[j * 4 + i * 2 + c] + bv;
+          if (p.rowvec && rok[i] && n < nend) v += p.rowvec[(mrow[i] / p.rows_per_batch) * p.ld_rowvec + n];
+          tot[j * 4 + i * 2 + c] = v;
+        }
+      }
+    if (!PERSIST && p.out_nchw) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (!rok[i]) continue;
+        const long long bimg = mrow[i] / p.rows_per_img, rimg = mrow[i] - bimg * p.rows_per_img;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int n = n0 + 8 * j + 2 * qd + c;
+            if (n < nend) p.C[(bimg * p.N + n) * p.rows_per_img + rimg] = tot[j * 4 + i * 2 + c];
+          }
+      }
+      return;
+    }
+    if (!PERSIST && p.Ct_hi && n0 >= p.t_col0) {
+      // transposed TF32-plane output (V^T)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int n = n0 + 8 * j + 2 * qd + c;
+            if (rok[i] && n < nend) {
+              const float o = tot[j * 4 + i * 2 + c];
+              const uint32_t hi = rn_tf32(__float_as_uint(o));
+              const long long at = (long long)(n - p.t_col0) * p.ldt + mrow[i];
+              p.Ct_hi[at] = __uint_as_float(hi);
+              p.Ct_lo[at] = __uint_as_float(tf32_lo(o, hi));
+              omax = fmaxf(omax, fabsf(o));
+            }
+          }
+    } else {
+      float* const dst = p.C + tc_.zb * p.sC_b + tc_.zh * p.sC_h;
+      float* const dst_lo = p.C_lo ? p.C_lo + tc_.zb * p.sC_b + tc_.zh * p.sC_h : nullptr;
+      // one loop body, compiled for each store path: STAGED writes every row and column of the tile into the epilogue's boxes (rows
+      // and columns outside C are clipped by the TMA store), the other path stores the valid elements to global memory
+      auto store_tile = [&](auto staged_c) {
+        constexpr bool STAGED = decltype(staged_c)::value;
+        // GEGLU tiles are [32 value | 32 gate] blocks: accumulator group j (value) pairs with j + 4 (gate)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (p.geglu && (j & 4)) continue;
+          const int n = n0 + 8 * j + 2 * qd;             // even; N % 4 == 0 (eligibility), so n + 1 < nend whenever n < nend
+          const int nout = p.geglu ? (n >> 6) * 32 + (n & 63) : n;
+          // STAGED: the column pair's box and its column in the box (GEGLU: boxes of the BN / 2 output columns)
+          const int box = p.geglu ? j >> 3 : j >> 2, cc = 8 * (j & 3) + 2 * qd;
+          float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float2 o = make_float2(tot[j * 4 + i * 2], tot[j * 4 + i * 2 + 1]);
+            if (p.geglu) {
+              const float g0 = tot[(j + 4) * 4 + i * 2], g1 = tot[(j + 4) * 4 + i * 2 + 1];
+              o.x *= 0.5f * g0 * (1.f + erff(g0 * 0.70710678118654752440f));     // exact-erf GELU as F.gelu
+              o.y *= 0.5f * g1 * (1.f + erff(g1 * 0.70710678118654752440f));
+            }
+            if (STAGED) {
+              // the 128B-swizzled box layout; the residual box holds its value at the same address
+              const int r = r0 + 8 * i;
+              const uint32_t a = epi_box(box) + (uint32_t)r * 128u + ((((uint32_t)cc >> 2) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(cc & 3) * 4u;
+              if (p.residual) {
+                float2 rv;
+                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rv.x), "=f"(rv.y) : "r"(a));
+                o.x += rv.x;
+                o.y += rv.y;
+              }
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(o.x), "f"(o.y) : "memory");
+            }
+            if (!rok[i] || n >= nend) continue;
+            if (!STAGED && p.residual) {
+              o.x += p.residual[mrow[i] * p.ldr + n];
+              o.y += p.residual[mrow[i] * p.ldr + n + 1];
+            }
+            if (p.c_stats) { cs[0] += o.x; cq[0] += o.x * o.x; cs[1] += o.y; cq[1] += o.y * o.y; }
+            if (!STAGED) {
+              float* const d = dst + mrow[i] * p.ldc + nout;
+              if (dst_lo) {                          // operand planes for a following tensor-core consumer
+                const uint32_t hx = rn_tf32(__float_as_uint(o.x)), hy = rn_tf32(__float_as_uint(o.y));
+                *reinterpret_cast<float2*>(dst_lo + mrow[i] * p.ldc + nout) = make_float2(__uint_as_float(tf32_lo(o.x, hx)), __uint_as_float(tf32_lo(o.y, hy)));
+                o = make_float2(__uint_as_float(hx), __uint_as_float(hy));
+              }
+              *reinterpret_cast<float2*>(d) = o;
+            }
+            omax = fmaxf(omax, fmaxf(fabsf(o.x), fabsf(o.y)));
+          }
+          if (p.c_stats) {
+            // GroupNorm statistics: fold the warp's 16 rows (one image: host-checked), one fp64 atomic per (column, statistic)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+#pragma unroll
+              for (int o2 = 4; o2 < 32; o2 <<= 1) {
+                cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], o2);
+                cq[c] += __shfl_xor_sync(0xffffffffu, cq[c], o2);
+              }
+            }
+            const long long mq = __shfl_sync(0xffffffffu, rok[0] ? mrow[0] : -1LL, 0);     // first row of the warp
+            if (g == 0 && mq >= 0 && n < nend) {
+              double* sp = p.c_stats + ((mq / p.rows_per_batch) * p.N + n) * 2;
+              atomicAdd(sp, (double)cs[0]); atomicAdd(sp + 1, (double)cq[0]);
+              atomicAdd(sp + 2, (double)cs[1]); atomicAdd(sp + 3, (double)cq[1]);
+            }
+          }
+        }
+      };
+      if (!staged) {
+        store_tile(std::false_type());
+      } else {
+        mbar_wait(bar_res, PERSIST ? item & 1 : 0);  // the boxes' slots are free and the residual boxes have landed
+        if (threadIdx.x == 128) TL_STAMP(4);
+        store_tile(std::true_type());
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA store
+        asm volatile("bar.sync 2, 256;" ::: "memory");                 // the consumer warpgroups' rows are all written
+        if (PERSIST) {
+          if (threadIdx.x == 128) mbar_arrive(bar_out);                // thread 32 stores them
+        } else if (threadIdx.x == 128) {
+          const int c0 = p.geglu ? n0 / 2 : n0, ncols = p.geglu ? p.N / 2 : p.N;
+          for (int b = 0; b < (p.geglu ? BN / 64 : BN / TBK) && c0 + b * TBK < ncols; ++b) {
+            if (p.mode == 0) tma_store_2d(epi_box(b), &mapC, c0 + b * TBK, tc_.m0);
+            else tma_store_4d(epi_box(b), &mapC, c0 + b * TBK, tc_.x0, tc_.y0, tc_.b0);
+          }
+          bulk_commit();
+          TL_STAMP(5);
+          bulk_wait0();                              // written, not only read: a dependent launch reads C after its griddepcontrol.wait
+          TL_STAMP(6);
+        }
+      }
+    }
+    omax_cta = PERSIST ? fmaxf(omax_cta, omax) : omax;
+    if (!PERSIST) break;
+    t += gridDim.x;
+    if (t >= p.total_tiles) break;
+    ++item;
+    g0 += nst;
+    tc_ = tile_coord(p, t, num_kb);
+    nst = tc_.kb1 - tc_.kb0;
   }
   if (p.c_amax) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) omax = fmaxf(omax, __shfl_xor_sync(0xffffffffu, omax, o));
-    if (lane == 0) atomicMax(reinterpret_cast<unsigned int*>(p.c_amax), __float_as_uint(omax));     // non-negative floats order like their bit patterns
+    for (int o = 16; o > 0; o >>= 1) omax_cta = fmaxf(omax_cta, __shfl_xor_sync(0xffffffffu, omax_cta, o));
+    if (lane == 0) atomicMax(reinterpret_cast<unsigned int*>(p.c_amax), __float_as_uint(omax_cta));     // non-negative floats order like their bit patterns
   }
 }
 
@@ -681,9 +798,9 @@ __global__ void amax_rows_scalar_kernel(const float* __restrict__ x, long long r
   if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned int*>(slot), __float_as_uint(m));
 }
 
-template <int KIND, int BN>
+template <int KIND, int BN, bool PERSIST = false>
 void set_smem_attr() {
-  CDX_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<KIND, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<KIND, BN>::SMEM_BYTES));
+  CDX_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<KIND, BN, PERSIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<KIND, BN, PERSIST>::SMEM_BYTES));
 }
 
 // cudaFuncSetAttribute is per DEVICE: remember which devices of this process have it (engines on several devices share the library)
@@ -700,6 +817,10 @@ void ensure_attr(int device) {
     set_smem_attr<KIND_H16, 64>();
     set_smem_attr<KIND_H16_FAST, 128>();
     set_smem_attr<KIND_H16_FAST, 64>();
+    set_smem_attr<KIND_H16, 128, true>();
+    set_smem_attr<KIND_H16, 64, true>();
+    set_smem_attr<KIND_H16_FAST, 128, true>();
+    set_smem_attr<KIND_H16_FAST, 64, true>();
     attr_set[d] = true;
   }
 }
@@ -708,6 +829,13 @@ template <int KIND, int BN>
 void launch_gemm(const TcParams& p, const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB, const CUtensorMap& mBlo,
                  const CUtensorMap& mR, const CUtensorMap& mC, cudaStream_t s) {
   launch_ex(tc_gemm_kernel<KIND, BN>, dim3((unsigned)p.total_tiles), dim3(TC_THREADS), Cfg<KIND, BN>::SMEM_BYTES, s, 1, mA, mA2, mB, mBlo, mR, mC, p);
+}
+
+// persistent grid: `ctas` CTAs walk the p.total_tiles work items
+template <int KIND, int BN>
+void launch_gemm_persist(const TcParams& p, int ctas, const CUtensorMap& mA, const CUtensorMap& mA2, const CUtensorMap& mB,
+                         const CUtensorMap& mBlo, const CUtensorMap& mR, const CUtensorMap& mC, cudaStream_t s) {
+  launch_ex(tc_gemm_kernel<KIND, BN, true>, dim3((unsigned)ctas), dim3(TC_THREADS), Cfg<KIND, BN, true>::SMEM_BYTES, s, 1, mA, mA2, mB, mBlo, mR, mC, p);
 }
 
 }  // namespace
@@ -930,7 +1058,10 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   // Work partition: tile width w (128 or 64 columns: the two wgmma widths compiled in) and split-K factor S, chosen together against
   // wave quantisation of one-CTA-per-work-item launches on num_sms SMs with a cost model in cycles: one k-block of a w-wide tile
   // ~ kc0 + kc1 w, ~3000 per work item for the epilogue, plus the split-K partial-sum traffic (S writes + S reads + 1 write of M*N
-  // floats at ~3 TB/s); a split must buy >= 10 %.  (A model of the kernel's structure, not a fit to measurements.)
+  // floats at ~3 TB/s); a split must buy >= 10 %.  (A model of the kernel's structure, not a fit to measurements.)  Unsplit work
+  // that runs persistent (fp16 split, dense, staged store) overlaps each item's epilogue with the next item's main loop: its ~3000
+  // is charged once per CTA.
+  const bool persist_ok = e.persist && h16 && a.mode == 0 && !a.out_nchw && !a.Cout_lo && !a.Ct_hi;
   int best_w = TBN, best_s = 1;
   {
     // exact key (no hashing of packed fields: nothing can collide) of everything the cost model reads -- M too, through the split-K
@@ -938,7 +1069,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
     static std::map<std::array<int64_t, 6>, int> plan_cache;
     static std::mutex plan_mutex;                                          // engines on different devices may plan concurrently
     std::lock_guard<std::mutex> plan_lock(plan_mutex);
-    const std::array<int64_t, 6> key = {a.M, p.tiles_m, a.N, num_kb, ((a.geglu || a.Ct_hi) ? 1 : 0) | (a.out_nchw ? 2 : 0) | (h16 ? 4 : 0) | (ts ? 8 : 0), e.num_sms};
+    const std::array<int64_t, 6> key = {a.M, p.tiles_m, a.N, num_kb, ((a.geglu || a.Ct_hi) ? 1 : 0) | (a.out_nchw ? 2 : 0) | (h16 ? 4 : 0) | (ts ? 8 : 0) |
+                                        (persist_ok ? 16 : 0), e.num_sms};
     const double kc0 = h16 ? 700.0 : 400.0, kc1 = h16 ? 6.0 : 3.0;
     const int min_kbs = h16 ? 4 : 8;
     auto it = plan_cache.find(key);
@@ -957,7 +1089,8 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
           const int Sx = cdiv(num_kb, kbs);                                  // no empty splits
           if (S > 1 && (Sx != S || kbs < min_kbs || a.out_nchw || a.geglu || a.Ct_hi || (long long)p.tiles_m * tn >= 4LL * e.num_sms)) continue;
           const long long items = (long long)p.tiles_m * tn * S;
-          double cost = (double)cdiv(items, (long long)e.num_sms) * (kbs * (kc0 + kc1 * w) + 3000.0);
+          const double waves = (double)cdiv(items, (long long)e.num_sms);
+          double cost = S == 1 && persist_ok ? waves * kbs * (kc0 + kc1 * w) + 3000.0 : waves * (kbs * (kc0 + kc1 * w) + 3000.0);
           if (S == 1) base = cost;
           else cost += 4000.0 + (2.0 * S + 1.0) * (double)a.M * a.N * 4.0 / 3e12 * 1.8e9;
           if (cost < best - 1e-9 && (S == 1 || cost < 0.9 * base)) { best = cost; best_w = w; best_s = S; }
@@ -1035,9 +1168,15 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
   ensure_attr(e.device);
   ProfScope ps(e, s, a.mode == 1 ? PROF_CONV_TC : PROF_DENSE_TC, 2.0 * a.M * a.N * a.K,
                4.0 * ((double)a.M * a.K / (a.mode == 1 ? 9 : 1) + (double)a.N * a.K + (double)a.M * a.N), 1);
-  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s box%dx%dx%d", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
-          a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "", p.bw, p.bh, p.bn);
-  if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  ps.note("M%d N%d K%d w%d tiles%d S%d %s%s%s%s%s box%dx%dx%d", a.M, a.N, a.K, p.tn_w, tiles, p.splits, h16 ? (fast ? "H16x1" : "H16") : ts ? "TS" : "SS",
+          a.Cout_lo ? " planes" : "", a.geglu ? " geglu" : "", a.residual ? " res" : "", persist_ok && staged_store(p) ? " persist" : "", p.bw, p.bh, p.bn);
+  const bool persist = persist_ok && staged_store(p);
+  const int ctas = (int)std::min<long long>(p.total_tiles, e.persist_grid > 0 ? std::min(e.persist_grid, e.num_sms) : e.num_sms);
+  if (persist && fast && p.tn_w == 128) launch_gemm_persist<KIND_H16_FAST, 128>(p, ctas, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (persist && fast) launch_gemm_persist<KIND_H16_FAST, 64>(p, ctas, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (persist && p.tn_w == 128) launch_gemm_persist<KIND_H16, 128>(p, ctas, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (persist) launch_gemm_persist<KIND_H16, 64>(p, ctas, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
+  else if (fast && p.tn_w == 128) launch_gemm<KIND_H16_FAST, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
   else if (fast) launch_gemm<KIND_H16_FAST, 64>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
   else if (h16 && p.tn_w == 128) launch_gemm<KIND_H16, 128>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
   else if (h16) launch_gemm<KIND_H16, 64>(p, *mA, *mA2, *mB, *mBlo, *mR, *mC, s);
@@ -1057,3 +1196,11 @@ bool gemm_tc(Engine& e, const GemmArgs& a, cudaStream_t s, int* side_done) {
 }
 
 }  // namespace cdx
+
+#ifdef CDX_GEMM_TIMELINE
+// Timeline probe variant only: point the GEMM's stamps at `buf` (TL_SLOTS uint64 per CTA of the largest grid the caller runs; null:
+// no stamps).  Returns 0 on success.
+extern "C" int cdx_gemm_timeline_buffer(void* buf) {
+  return cudaMemcpyToSymbol(cdx::g_gemm_timeline, &buf, sizeof(buf)) == cudaSuccess ? 0 : 1;
+}
+#endif

@@ -80,6 +80,11 @@ class Engine:
         check(lib.cdx_engine_set_mma_mode(self.h, int(mode)))
         self.mma_mode = int(mode)
 
+    def set_persist(self, enable, max_ctas=0):
+        """Persistent tensor-core GEMM for unsplit dense fp16-split work: on by default (CDX_PERSIST=0 at creation: off).
+        max_ctas > 0 caps its grid, so each CTA walks more work items (tests); outputs are bit-identical in every setting."""
+        check(lib.cdx_engine_set_persist(self.h, int(bool(enable)), int(max_ctas)))
+
     # the reference wrappers' `precision` values (SDW:117, txt2img.py --precision {full,autocast}) and the mma mode each selects;
     # None: the engine keeps its current mode
     PRECISIONS = {'full': None, 'autocast': 5}

@@ -76,6 +76,10 @@ int cdx_engine_profile_read(cdx_engine* e, int tag, double* ms, double* flops, d
  *       the paths that use 3xTF32 or FFMA in mode 1 (d = 160 attention, the VAE mid-block, M < 64, the text towers) are
  *       unchanged.  Not bit-compatible with torch.autocast, which rounds every op's output to fp16; at least as accurate. */
 int cdx_engine_set_mma_mode(cdx_engine* e, int mode);
+/* Persistent tensor-core GEMM for unsplit dense fp16-split work (default on; CDX_PERSIST=0 in the environment when the engine is
+ * created turns it off).  enable 0: one CTA per work item.  max_ctas > 0 caps the persistent grid (a CTA then walks more work
+ * items; for tests), 0: one CTA per SM.  Outputs are bit-identical in every setting. */
+int cdx_engine_set_persist(cdx_engine* e, int enable, int max_ctas);
 
 /* ---------------------------------------------------------------- networks ----------------- */
 #define CDX_UNET_OPENAI 1 /* SD v1 / LDM text2img U-Net: OAI:413-742 + attention.py:152-261 */

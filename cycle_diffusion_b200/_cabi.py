@@ -135,6 +135,11 @@ class SemanticAttnMaskC(C.Structure):
     _fields_ = [('intersect', C.c_int), ('n_tokens', C.c_int * CDX_SEMANTIC_MAX)]
 
 
+class LocalBlendC(C.Structure):
+    _fields_ = [('alpha_src', C.c_void_p), ('alpha_tgt', C.c_void_p), ('sub_src', C.c_void_p), ('sub_tgt', C.c_void_p), ('start_step', C.c_int),
+                ('th_blend', C.c_float), ('th_sub', C.c_float)]
+
+
 _F = C.c_float
 _I = C.c_int
 _S = C.c_size_t
@@ -203,6 +208,11 @@ SIGNATURES = {
     'cdx_cycle_lockstep_sampler': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
                                         _I, _I, _P, C.POINTER(SamplerC), _P, C.POINTER(AttnControl), _P, C.POINTER(MutualControlC),
                                         C.POINTER(PnpControlC), _P, C.POINTER(SemanticGuidanceC), C.POINTER(SemanticAttnMaskC)]),
+    'cdx_cycle_lockstep_blend': (_I, [_P, _P, _P, _P, _P, _I, _F, _F, C.POINTER(DdimCoef), C.POINTER(_F), _I, _P, _F, _F, _P, _P, _I, _I,
+                                      _I, _I, _P, C.POINTER(SamplerC), _P, C.POINTER(AttnControl), _P, C.POINTER(MutualControlC),
+                                      C.POINTER(PnpControlC), _P, C.POINTER(SemanticGuidanceC), C.POINTER(SemanticAttnMaskC),
+                                      C.POINTER(LocalBlendC)]),
+    'cdx_local_blend_mask': (_I, [_P, _P, _I, _I, _P, _P, _F, _F, _P, _I, _I, _I, _P]),
     'cdx_mask_pool': (_I, [_P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_mask_composite': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     'cdx_edit_map': (_I, [_P, _P, _P, _P, _I, _F, _F, _F, _P, _I, _I, _P, _I, _I, _I, _I, _P]),
@@ -241,6 +251,7 @@ SIGNATURES = {
     'cdx_op_produce_norm': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P, _P, C.POINTER(_I), _P]),
     'cdx_op_gemm': (_I, [_P, C.POINTER(GemmDesc), C.POINTER(_I), _P]),
     'cdx_op_attention_net': (_I, [_P, C.POINTER(AttentionNetDesc), C.POINTER(_I), _P]),
+    'cdx_op_attention_net_weighted': (_I, [_P, C.POINTER(AttentionNetDesc), C.POINTER(_F), C.POINTER(_I), _P]),
     'cdx_op_latent_chains': (_I, [_P, C.POINTER(LatentChainsDesc), _I, _P]),
     'cdx_op_pixel_lockstep': (_I, [_P, _P, _P, _P, _P, _P, _P, C.POINTER(PixelCoef), _I, _I, _I, _I, _P]),
 }

@@ -11,6 +11,9 @@ MasaCtrl's mutual self-attention (Cao et al., 2023; ``MutualSelfControl``) is th
 the decoder's self-attention layers the target rows keep their own queries and attend over the source row's keys and values
 (cdx_cycle_lockstep_mutual), so the layout follows the target prompt and the content comes from the real image.
 
+Prompt-to-Prompt's LocalBlend (``LocalBlend``) keeps a real-image edit local: at every step the target chain is blended with the
+source chain outside the region the blend words' accumulated cross-attention points to (cdx_cycle_lockstep_blend).
+
 Plug-and-Play diffusion features (Tumanyan et al., 2023; ``PnPControl``) keep the real image's spatial layout for text-guided
 translation: the target rows take the source row's decoder ResBlock features and its self-attention queries and keys
 (cdx_cycle_lockstep_pnp), and the target prompt sets the appearance.
@@ -143,6 +146,140 @@ class PnPControl:
     def steps(self, n):
         """(feature_steps, attention_steps) as step counts of an n-step loop."""
         return int(self.feature_steps * n), int(self.attention_steps * n)
+
+
+def _weights(name, v):
+    if not torch.is_tensor(v) or v.dim() not in (1, 2):
+        raise ValueError(f'{name} must be a tensor [L] or [B, L], got {tuple(v.shape) if torch.is_tensor(v) else type(v)}')
+    v = v.detach().to(torch.float64)
+    if not bool(torch.isfinite(v).all()) or bool((v < 0).any()):
+        raise ValueError(f'{name} must be finite and >= 0')
+    if bool((v.reshape(-1, v.shape[-1]).sum(dim=-1) == 0).any()):
+        raise ValueError(f'{name}: a weight vector is all zero (no blend word in the prompt)')
+
+
+@dataclass(frozen=True)
+class LocalBlend:
+    """Prompt-to-Prompt's LocalBlend.  alpha_src / alpha_tgt: per-token weights [L] or [B, L] of the blend words in the source and
+    the target prompt (P2P's alpha_layers; word_token_weights builds them), finite, >= 0 and not all zero.  sub_src / sub_tgt:
+    optional, both or neither: the subtract words (P2P's substruct_words).  From loop step int(start_blend * n) on, the target
+    chain keeps its own x_{t-1} only where maxpool3x3(R) / max(R) > threshold[0] for the source or the target blend map R (the
+    words' cross-attention summed over the probed layers, heads and every step so far), and not where R_sub / max(R_sub) >
+    threshold[1] for either subtract map; elsewhere it takes the source chain's.  threshold values in [0, 1)."""
+    alpha_src: object
+    alpha_tgt: object
+    sub_src: object = None
+    sub_tgt: object = None
+    start_blend: float = 0.2
+    threshold: tuple = (0.3, 0.3)
+
+    def __post_init__(self):
+        _weights('alpha_src', self.alpha_src)
+        _weights('alpha_tgt', self.alpha_tgt)
+        if (self.sub_src is None) != (self.sub_tgt is None):
+            raise ValueError('sub_src and sub_tgt: give both or neither')
+        if self.sub_src is not None:
+            _weights('sub_src', self.sub_src)
+            _weights('sub_tgt', self.sub_tgt)
+        _fraction('start_blend', self.start_blend)
+        th = self.threshold
+        if not isinstance(th, (tuple, list)) or len(th) != 2 or any(isinstance(t, bool) or not isinstance(t, (int, float)) or
+                                                                      not 0.0 <= float(t) < 1.0 for t in th):
+            raise ValueError(f'threshold must be a pair (th_blend, th_sub) in [0, 1), got {th!r}')
+        object.__setattr__(self, 'threshold', (float(th[0]), float(th[1])))
+
+    def start_step(self, n):
+        """The first blended step of an n-step loop."""
+        return int(self.start_blend * n)
+
+    def vectors(self, B, L, device):
+        """(alpha_src, alpha_tgt, sub_src, sub_tgt) as contiguous float32 [B, L] tensors on `device` (the subtract pair None when
+        not given)."""
+        def one(name, v):
+            if v is None:
+                return None
+            if v.dim() == 1:
+                v = v.unsqueeze(0).expand(B, -1)
+            if tuple(v.shape) != (B, L):
+                raise ValueError(f'{name}: expected [{L}] or [{B}, {L}], got {tuple(v.shape)}')
+            return v.to(device=device, dtype=torch.float32).contiguous()
+        return tuple(one(k, getattr(self, k)) for k in ('alpha_src', 'alpha_tgt', 'sub_src', 'sub_tgt'))
+
+    def c_struct(self, n, B, L, device):
+        """-> (cdx_local_blend for an n-step loop, the device vectors it points to; keep them alive over the call)."""
+        vs = self.vectors(B, L, device)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        return _cabi.LocalBlendC(*[ptr(t) for t in vs], self.start_step(n), self.threshold[0], self.threshold[1]), vs
+
+
+def word_token_weights(prompt_ids, word_ids, L):
+    """P2P's get_word_inds as weights: -> float32 [L] with 1 at every position of every occurrence of the run word_ids in
+    prompt_ids (the prompt's tokens, start token included, so positions are context rows), 0 elsewhere; positions >= L are
+    dropped.  ValueError when the run does not occur below L."""
+    p, w = list(prompt_ids), list(word_ids)
+    if not w:
+        raise ValueError('word_token_weights: an empty word')
+    out = torch.zeros(L, dtype=torch.float32)
+    for i in range(len(p) - len(w) + 1):
+        if p[i: i + len(w)] == w:
+            out[i: min(i + len(w), L)] = 1.0
+    if not bool(out.any()):
+        raise ValueError(f'word_token_weights: the word {w} is not among the first {L} tokens of the prompt')
+    return out
+
+
+def words_weights(token_rows, word_rows, L):
+    """[B, L] float32 from per-prompt token rows and per-prompt word lists (each word a token run): 1 at every occurrence of every
+    word, as P2P sets alpha_layers."""
+    rows = []
+    for ids, words in zip(token_rows, word_rows):
+        r = torch.zeros(L, dtype=torch.float32)
+        for w in words:
+            r = torch.maximum(r, word_token_weights(ids, w, L))
+        rows.append(r)
+    return torch.stack(rows)
+
+
+def word_lists(texts, words):
+    """words: a word (str), a tuple / list of words for every text, or a list with one such entry per text -> one tuple of words
+    per text."""
+    if isinstance(words, str):
+        return [(words,)] * len(texts)
+    words = list(words)
+    if len(words) == len(texts) and all(not isinstance(w, str) for w in words):
+        return [tuple(w) for w in words]
+    if all(isinstance(w, str) for w in words):
+        return [tuple(words)] * len(texts)
+    raise ValueError(f'words: a word, a tuple of words, or one tuple per text ({len(texts)}), got {words!r}')
+
+
+BLEND_KEYS = {'words', 'subtract_words', 'start_blend', 'threshold'}
+
+
+def resolve_local_blend(spec, cond_stage, sources, targets):
+    """A LocalBlend as it is, or {'words': (source_words, target_words), ['subtract_words': (source_words, target_words)],
+    ['start_blend': 0.2], ['threshold': (0.3, 0.3)]} -> LocalBlend, the words turned into per-token weights of the source and target
+    prompts by the conditioning model's word_token_weights(texts, words).  ValueError for anything else."""
+    if isinstance(spec, LocalBlend):
+        return spec
+    if not isinstance(spec, dict):
+        raise ValueError(f'local_blend: a LocalBlend or a dict with words, got {type(spec)}')
+    extra = set(spec) - BLEND_KEYS
+    if extra or 'words' not in spec:
+        raise ValueError(f"local_blend: a dict with 'words' and optionally {sorted(BLEND_KEYS - {'words'})}, got keys {sorted(spec)}")
+    weights = getattr(cond_stage, 'word_token_weights', None)
+    if weights is None:
+        raise ValueError('local_blend: the conditioning model has no word_token_weights(texts, words); pass a LocalBlend')
+
+    def pair(key):
+        p = spec[key]
+        if not isinstance(p, (tuple, list)) or len(p) != 2:
+            raise ValueError(f'local_blend: {key} must be a pair (source words, target words), got {p!r}')
+        return weights(list(sources), p[0]), weights(list(targets), p[1])
+
+    a_src, a_tgt = pair('words')
+    s_src, s_tgt = pair('subtract_words') if spec.get('subtract_words') is not None else (None, None)
+    return LocalBlend(a_src, a_tgt, s_src, s_tgt, spec.get('start_blend', 0.2), spec.get('threshold', (0.3, 0.3)))
 
 
 def replace_token_map(src_ids, tgt_ids, L):

@@ -187,6 +187,7 @@ struct ChainLoopArgs {
   // c_edit [n_src, m, L, D]: every target chain of group j runs concept k under c_edit[j, k]
   const cdx_semantic_guidance* sega = nullptr; const float* c_edit = nullptr;
   const cdx_semantic_attn_mask* sega_mask = nullptr;    // optional with sega: LEDITS++'s implicit masks (cdx_cycle_lockstep_semantic_attn)
+  const cdx_local_blend* blend = nullptr;           // optional, with ctl / own_weight or alone: P2P's LocalBlend (cdx_cycle_lockstep_blend)
   int C = 0, h = 0, w = 0;
   // optional: the source chain's sampler (cdx.h, cdx_cycle_lockstep_sampler); NULL or CDX_SAMPLER_DDIM_POSTERIOR is the DPM-Encoder
   const cdx_sampler* sampler = nullptr;
@@ -240,6 +241,18 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
     for (int k = 0; k < a.sega->m; ++k)
       CDX_CHECK(a.sega_mask->n_tokens[k] >= 1 && a.sega_mask->n_tokens[k] <= a.L - 2, "attention masks: n_tokens[%d]=%d outside 1..%d", k,
                 a.sega_mask->n_tokens[k], a.L - 2);
+  }
+  if (a.blend) {
+    const cdx_local_blend& lb = *a.blend;
+    CDX_CHECK(!a.sega && !a.mutual && !a.pnp, "LocalBlend: Prompt-to-Prompt edits (or none) only, not semantic guidance, MasaCtrl or PnP");
+    CDX_CHECK(a.src && a.K == 1 && a.n_rec == a.n_steps && !tgt_net && !a.scales_on_device,
+              "LocalBlend: needs the lock-step loop with one target chain per source chain (K=%d)", a.K);
+    CDX_CHECK(unet.kind == NET_UNET_OPENAI && ctx_n > 0 && a.c_src && a.c_tgt, "LocalBlend: needs a U-Net with a context and both prompts");
+    CDX_CHECK(lb.alpha_src && lb.alpha_tgt && !lb.sub_src == !lb.sub_tgt, "LocalBlend: null blend-word vector, or one subtract vector alone");
+    CDX_CHECK(a.h % 4 == 0 && a.w % 4 == 0, "LocalBlend: a %dx%d latent, multiples of 4 needed", a.h, a.w);
+    CDX_CHECK(lb.start_step >= 0 && lb.start_step <= a.n_steps, "LocalBlend: start_step=%d (of %d)", lb.start_step, a.n_steps);
+    CDX_CHECK(lb.th_blend >= 0.f && lb.th_blend < 1.f && lb.th_sub >= 0.f && lb.th_sub < 1.f, "LocalBlend: thresholds %g, %g outside [0, 1)",
+              lb.th_blend, lb.th_sub);
   }
   // the chain table: all source-chain rows first, then all target-chain rows (the two-model loop runs the two blocks under two
   // nets); inside a block the uncond rows come first, cat([uc, c]) as ddim.py:555-557
@@ -462,6 +475,57 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.n_feat = a.pnp->n_blocks;
     }
   }
+  // LocalBlend: the probe's entry tables, [0] the rows' own maps and [1] the maps of an edited step, uploaded once.  Entry
+  // (j*n_vec + v)*T + t of image j, vector v (source / target blend words, then source / target subtract words), term t.  A source
+  // vector probes the source row; a target vector the target row, or at an edited step the source row with A_j v (the map P_src A_j
+  // contracted with v) plus, under refine (T = 2), the target row with own_weight_j * v.  The running sums and the step's mask
+  AttnProbe bprobe[2];
+  int bl_terms[2] = {1, 1};
+  const int bl_vec = a.blend ? (a.blend->sub_src ? 4 : 2) : 0;
+  float *bl_run = nullptr, *bl_mask = nullptr;
+  if (a.blend) {
+    const int G = gh * gw, L = a.L;
+    const float* vecs[4] = {a.blend->alpha_src, a.blend->alpha_tgt, a.blend->sub_src, a.blend->sub_tgt};
+    for (int j = 0; j < a.n_src; ++j) {
+      CDX_CHECK(!a.uc || ch[j].scale != 0.0f, "LocalBlend: the source chain at scale 0 has no source-prompt row");
+      CDX_CHECK(!a.uc || ch[a.n_src + j].scale != 0.0f, "LocalBlend: the target chain at scale 0 has no target-prompt row");
+    }
+    bl_terms[1] = a.own_weight ? 2 : 1;
+    for (int tab = 0; tab < (a.ctl ? 2 : 1); ++tab) {
+      const int T = bl_terms[tab], n_ent = a.n_src * bl_vec * T;
+      std::vector<int> rows_h((size_t)n_ent);
+      float* wts = (float*)e.arena.alloc((size_t)n_ent * L * sizeof(float));
+      if (!e.dry()) CDX_CUDA(cudaMemsetAsync(wts, 0, (size_t)n_ent * L * sizeof(float), s));
+      for (int j = 0; j < a.n_src; ++j)
+        for (int v = 0; v < bl_vec; ++v)
+          for (int t = 0; t < T; ++t) {
+            const int idx = (j * bl_vec + v) * T + t, src_row = ch[j].row, tgt_row = ch[a.n_src + j].row;
+            const float* vec = vecs[v] + (size_t)j * L;
+            float* out = wts + (size_t)idx * L;
+            if (!(v & 1)) {                       // source vector: the source row's own map (a refine term 1 stays zero)
+              rows_h[idx] = src_row;
+              if (t == 0) blend_weights(e, vec, nullptr, nullptr, out, L, s);
+            } else if (tab == 0) {
+              rows_h[idx] = tgt_row;
+              blend_weights(e, vec, nullptr, nullptr, out, L, s);
+            } else if (t == 0) {
+              rows_h[idx] = src_row;
+              blend_weights(e, vec, a.ctl->token_map ? a.ctl->token_map + (size_t)j * L * L : nullptr, nullptr, out, L, s);
+            } else {
+              rows_h[idx] = tgt_row;
+              blend_weights(e, vec, nullptr, a.own_weight + (size_t)j * L, out, L, s);
+            }
+          }
+      int* rows_dev = (int*)e.arena.alloc(rows_h.size() * sizeof(int));
+      if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(rows_dev, rows_h.data(), rows_h.size() * sizeof(int), cudaMemcpyHostToDevice, s));   // (pageable: staged)
+      AttnProbe& p = bprobe[tab];
+      p.rows = rows_dev; p.weights = wts; p.n_rows = n_ent; p.tokens = G;
+      p.map = (float*)e.arena.alloc((size_t)n_ent * G * sizeof(float));
+    }
+    bl_run = (float*)e.arena.alloc((size_t)a.n_src * bl_vec * G * sizeof(float));
+    bl_mask = (float*)e.arena.alloc((size_t)a.n_src * a.h * a.w * sizeof(float));
+    if (!e.dry()) CDX_CUDA(cudaMemsetAsync(bl_run, 0, (size_t)a.n_src * bl_vec * G * sizeof(float), s));
+  }
   auto next_kind = [&](int i_next) {             // how x_{t-1} of iteration i_next is obtained (0: that iteration does not exist)
     if (i_next >= a.n_rec) return 0;
     return (a.n_steps - 1 - i_next) == 0 ? 2 : solver ? 3 : 1;                  // ddim.py:583-584; 3: an independent draw
@@ -507,8 +571,9 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       actl.pnp_feat = a.pnp && i < a.pnp->feature_steps;
       actl.pnp_attn = a.pnp && i < a.pnp->attention_steps;
       const size_t stat0 = e.stat_dry;
+      const AttnProbe* pr = sg_mask ? &probe : a.blend ? &bprobe[actl.cross ? 1 : 0] : nullptr;
       unet_forward(unet, xin, tdev + (size_t)i * rows, ctx_in, a.L, eout, rows, a.h, a.w, s, true,
-                   a.ctl || a.mutual || a.pnp ? &actl : nullptr, sg_mask ? &probe : nullptr);
+                   a.ctl || a.mutual || a.pnp ? &actl : nullptr, pr);
       CDX_CHECK(!sg_m || !e.dry() || e.stat_dry - stat0 <= e.stat_cap,
                 "semantic guidance: a %d-row U-Net call needs %zu GroupNorm statistics doubles, the pool holds %zu: fewer images or concepts",
                 rows, e.stat_dry - stat0, e.stat_cap);
@@ -539,6 +604,12 @@ void run_latent_chains(Net& unet, const ChainLoopArgs& a, cudaStream_t s, Net* t
       for (int q = 0; q < sg_m; ++q) st.sg_active |= (unsigned)(i < a.sega->cooldown[q]) << q;
       st.sg_apply = i >= a.sega->warmup;
       semantic_thresholds(e, st, s);
+    }
+    if (a.blend) {                                // this step's maps into the running sums, then the mask the step blends under
+      const int tab = actl.cross ? 1 : 0;
+      local_blend_mask(e, bprobe[tab].map, bl_terms[tab], bl_vec, bl_run, a.mask, a.blend->th_blend, a.blend->th_sub, bl_mask, a.n_src, a.h,
+                       a.w, s);
+      if (i >= a.blend->start_step) st.mask = bl_mask;
     }
     latent_chains_step(e, st, s);
     if (src_i) { float* t0 = xb[0]; xb[0] = xb[1]; xb[1] = xb[2]; xb[2] = t0; }
@@ -949,7 +1020,8 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
                           float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream, const float* mask,
                           const cdx_attn_control* ctl, const float* own_weight, bool mutual, int start_step, int start_layer,
                           const PnpLoop* pnp = nullptr, const cdx_semantic_guidance* sega = nullptr, const float* c_edit = nullptr,
-                          const cdx_semantic_attn_mask* sega_mask = nullptr, const cdx_sampler* sampler = nullptr) {
+                          const cdx_semantic_attn_mask* sega_mask = nullptr, const cdx_sampler* sampler = nullptr,
+                          const cdx_local_blend* blend = nullptr) {
   return guard([&] {
     CDX_CHECK(un && un->owner && x0 && c_src && c_tgt && coef && t_host && noise && x_out, "cycle_lockstep: null argument");
     CDX_CHECK(n_steps >= 1, "cycle_lockstep: n_steps=%d", n_steps);
@@ -961,7 +1033,7 @@ static int cycle_lockstep(cdx_net* un, const float* x0, const float* c_src, cons
     a.coef = coef; a.t_host = t_host; a.n_steps = n_steps; a.n_rec = n_steps; a.noise = noise; a.sa = sqrt_a_T; a.s1 = sqrt_1ma_T;
     a.z_out = z_out; a.x_out = x_out; a.mask = mask; a.ctl = ctl; a.own_weight = own_weight; a.C = C; a.h = h; a.w = w;
     a.mutual = mutual; a.start_step = start_step; a.start_layer = start_layer; a.pnp = pnp;
-    a.sega = sega; a.c_edit = c_edit; a.sega_mask = sega_mask; a.sampler = sampler;
+    a.sega = sega; a.c_edit = c_edit; a.sega_mask = sega_mask; a.sampler = sampler; a.blend = blend;
     with_arena(un->owner->e, S(stream), [&] { run_latent_chains(*un->n, a, S(stream)); });
   });
 }
@@ -1029,6 +1101,19 @@ int cdx_cycle_lockstep_sampler(cdx_net* un, const float* x0, const float* c_src,
   return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
                         B, C, h, w, stream, mask, ctl, own_weight, mutual != nullptr, mutual ? mutual->start_step : 0,
                         mutual ? mutual->start_layer : 0, pnp ? &p : nullptr, sg, c_edit, am, sampler);
+}
+
+int cdx_cycle_lockstep_blend(cdx_net* un, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L, float src_scale,
+                             float tgt_scale, const cdx_ddim_coef* coef, const float* t_host, int n_steps, const float* noise,
+                             float sqrt_a_T, float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w, void* stream,
+                             const cdx_sampler* sampler, const float* mask, const cdx_attn_control* ctl, const float* own_weight,
+                             const cdx_mutual_control* mutual, const cdx_pnp_control* pnp, const float* c_edit,
+                             const cdx_semantic_guidance* sg, const cdx_semantic_attn_mask* am, const cdx_local_blend* blend) {
+  if (!blend) return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_blend: null LocalBlend"); });
+  if (mutual || pnp || c_edit || sg || am)
+    return guard([] { throw Error(CDX_E_INVALID, "cycle_lockstep_blend: LocalBlend runs with Prompt-to-Prompt edits or none"); });
+  return cycle_lockstep(un, x0, c_src, c_tgt, uc, L, src_scale, tgt_scale, coef, t_host, n_steps, noise, sqrt_a_T, sqrt_1ma_T, x_out, z_out,
+                        B, C, h, w, stream, mask, ctl, own_weight, false, 0, 0, nullptr, nullptr, nullptr, nullptr, sampler, blend);
 }
 
 int cdx_latent_loop_ens(cdx_net* un, int mode, const float* x0, const float* c_src, const float* c_tgt, const float* uc, int L,
@@ -1212,6 +1297,10 @@ int cdx_latent_cycle_fan_masked(cdx_net* un, int n_src, int K, const float* x0, 
   });
 }
 
+int cdx_local_blend_mask(cdx_engine* e, const float* maps, int n_terms, int n_vec, float* run, const float* user_mask, float th_blend,
+                         float th_sub, float* mask_out, int B, int h, int w, void* s) {
+  ENG_CALL(e, local_blend_mask(e->e, maps, n_terms, n_vec, run, user_mask, th_blend, th_sub, mask_out, B, h, w, S(s)));
+}
 int cdx_mask_pool(cdx_engine* e, const float* mask, float* out, int B, int H, int W, int f, void* s) {
   ENG_CALL(e, CDX_CHECK(mask && out, "mask_pool: null argument"); mask_pool(e->e, mask, out, B, H, W, f, S(s)));
 }
@@ -1446,7 +1535,7 @@ int cdx_op_attention_accum(cdx_engine* eh, const float* q, const float* k, const
   if (!acc_rows || n_acc < 1) return guard([&] { CDX_CHECK(false, "op_attention_accum: an empty row list"); });
   return op_attention(eh, q, k, v, out, B, Nq, Nk, heads, d, scale, nullptr, acc_rows, n_acc, stream);
 }
-int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* plan_out, void* stream) {
+static int op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, const float* probe_weights, int* plan_out, void* stream) {
   return guard([&] {
     CDX_CHECK(eh && d && d->out && d->kind >= 0 && d->kind <= 2, "op_attention_net: null argument or bad kind");
     const int kind = d->kind, B = d->B, N = d->N, heads = d->heads, dh = d->d, C = heads * dh;
@@ -1464,11 +1553,15 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
     const bool tables = d->qk_rows || d->kv_rows || d->acc_rows;
     const bool probing = d->n_probe > 0;
     if (probing) {
-      CDX_CHECK(kind == 1 && d->probe_rows && d->probe_spans && d->probe_map && L >= 3, "op_attention_net: the probe needs kind 1, L >= 3, rows, "
-                "spans and a map");
+      CDX_CHECK(kind == 1 && d->probe_rows && (probe_weights ? !d->probe_spans : d->probe_spans != nullptr) && d->probe_map && L >= 3,
+                "op_attention_net: the probe needs kind 1, L >= 3, rows, spans or weights and a map");
       for (int i = 0; i < d->n_probe; ++i)
-        CDX_CHECK(d->probe_rows[i] >= 0 && d->probe_rows[i] < B && d->probe_spans[i] >= 1 && d->probe_spans[i] <= L - 2,
-                  "op_attention_net: probe row %d = %d of %d, span %d outside 1..%d", i, d->probe_rows[i], B, d->probe_spans[i], L - 2);
+        CDX_CHECK(d->probe_rows[i] >= 0 && d->probe_rows[i] < B && (probe_weights || (d->probe_spans[i] >= 1 && d->probe_spans[i] <= L - 2)),
+                  "op_attention_net: probe row %d = %d of %d, span %d outside 1..%d", i, d->probe_rows[i], B,
+                  probe_weights ? 0 : d->probe_spans[i], L - 2);
+      if (probe_weights)
+        for (size_t i = 0; i < (size_t)d->n_probe * L; ++i)
+          CDX_CHECK(std::isfinite(probe_weights[i]), "op_attention_net: probe weight %zu is not finite", i);
     }
     Engine& e = eh->e;
     cudaStream_t s = S(stream);
@@ -1483,7 +1576,13 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
         return dev;
       };
       const int *qk_dev = stage(d->qk_rows, B), *kv_dev = stage(d->kv_rows, B), *acc_dev = stage(d->acc_rows, d->n_acc);
-      const int *probe_dev = probing ? stage(d->probe_rows, d->n_probe) : nullptr, *span_dev = probing ? stage(d->probe_spans, d->n_probe) : nullptr;
+      const int *probe_dev = probing ? stage(d->probe_rows, d->n_probe) : nullptr;
+      const int* span_dev = probing && !probe_weights ? stage(d->probe_spans, d->n_probe) : nullptr;
+      float* wts_dev = nullptr;
+      if (probing && probe_weights) {
+        wts_dev = (float*)e.arena.alloc((size_t)d->n_probe * L * sizeof(float));
+        if (!e.dry()) CDX_CUDA(cudaMemcpyAsync(wts_dev, probe_weights, (size_t)d->n_probe * L * sizeof(float), cudaMemcpyHostToDevice, s));
+      }
       ProbeOperands po;
       // a range slot as the network's producer leaves it: max |x| over the tensor, or the caller's (conservative) value
       auto slot_of = [&](float value, const float* x, long long rows, int cols) {
@@ -1600,7 +1699,7 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
           plan[0] = 0;
           po.fmt = ProbeOperands::F32; po.q = d->q; po.q_lo = nullptr; po.ldq = C; po.k = kv; po.k_lo = nullptr; po.ldk = 2 * C; po.Lk = L;
         }
-        if (probing) attn_probe(e, po, probe_dev, span_dev, d->n_probe, d->probe_map, N, L, heads, dh, d->scale, false, s);
+        if (probing) attn_probe(e, po, probe_dev, span_dev, wts_dev, d->n_probe, d->probe_map, N, L, heads, dh, d->scale, false, s);
       } else {
         CDX_CHECK(!tables, "op_attention_net: row tables need a fused route");
         attention(e, d->q, C, d->k, C, d->v, C, d->out, C, B, N, L, heads, dh, dh, d->scale, s, d->causal != 0);
@@ -1609,6 +1708,13 @@ int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* p
     });
     if (plan_out) for (int i = 0; i < 7; ++i) plan_out[i] = plan[i];
   });
+}
+int cdx_op_attention_net(cdx_engine* eh, const cdx_attention_net_desc* d, int* plan_out, void* stream) {
+  return op_attention_net(eh, d, nullptr, plan_out, stream);
+}
+int cdx_op_attention_net_weighted(cdx_engine* eh, const cdx_attention_net_desc* d, const float* probe_weights, int* plan_out, void* stream) {
+  if (!probe_weights) return guard([] { throw Error(CDX_E_INVALID, "op_attention_net_weighted: null probe weights"); });
+  return op_attention_net(eh, d, probe_weights, plan_out, stream);
 }
 int cdx_op_nchw_to_nhwc(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nchw_to_nhwc(eh->e, x, y, B, C, HW, S(stream))); }
 int cdx_op_nhwc_to_nchw(cdx_engine* eh, const float* x, float* y, int B, int C, int HW, void* stream) { ENG_CALL(eh, nhwc_to_nchw(eh->e, x, y, B, C, HW, S(stream))); }

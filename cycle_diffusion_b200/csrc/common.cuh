@@ -246,9 +246,10 @@ struct ProbeOperands {
 };
 // map[i, p] (= or += with accumulate) sum over heads h (in order) of sum over j in 1..span[i] of softmax_j(scale * q_p . k_j) over
 // all L keys, for the U-Net row rows[i] (device [n_rows] both).  One warp owns each (i, p): the dot in channel order, the softmax
-// sums in a fixed lane order, no atomics, so a row's map does not depend on the other rows or their count.
-void attn_probe(Engine& e, const ProbeOperands& o, const int* rows, const int* span, int n_rows, float* map, int N, int L, int heads, int d,
-                float scale, bool accumulate, cudaStream_t s);
+// sums in a fixed lane order, no atomics, so a row's map does not depend on the other rows or their count.  Weighted form
+// (LocalBlend; span null): the inner sum is sum over all j of weights[i, j] * softmax_j (device [n_rows, L]).
+void attn_probe(Engine& e, const ProbeOperands& o, const int* rows, const int* span, const float* weights, int n_rows, float* map, int N, int L,
+                int heads, int d, float scale, bool accumulate, cudaStream_t s);
 void split_planes(Engine& e, const float* w, float* hi, float* lo, size_t n, cudaStream_t s);   // hi = rn_tf32(w), lo = rn_tf32(w - hi)
 // fp16 split of w * 2^exp: hi = fp16(w'), lo = fp16(w' - hi)  (hi / lo: __half arrays)
 void split_planes_h16(Engine& e, const float* w, void* hi, void* lo, size_t n, int exp, cudaStream_t s);
@@ -393,6 +394,15 @@ void latent_chains_step(Engine& e, const LatentChains& a, cudaStream_t s);
 // (target chain, concept), the smoothed attention map (sg_gh*sg_gw values) and, with sg_mask == 2, the channel sum of |psi_k| (hw
 // values): one or two CTAs per concept row, still one launch.
 void semantic_thresholds(Engine& e, const LatentChains& a, cudaStream_t s);
+// Prompt-to-Prompt's LocalBlend (cdx_cycle_lockstep_blend).  blend_weights: one probe weight row out [L] <- A . v (A [L, L]
+// row-major, one fmaf per n ascending), or d * v elementwise, or v.  local_blend_mask: one launch, one CTA per image b.  maps
+// [B*n_vec*n_terms, G] (G = (h/4)(w/4), entry (b*n_vec + v)*n_terms + t); run [B*n_vec, G] += (term 0 + term 1 + ...); then per
+// vector v (0 / 1: blend words of the source / target prompt, 2 / 3: subtract words) its maximum mx_v over the grid, and per cell
+// keep = OR_{v<2} (maxpool3x3(run_v) / mx_v > th_blend) AND NOT OR_{v>=2} (run_v / mx_v > th_sub) (fp32 division; a map whose
+// maximum is 0 adds nothing); mask [B,1,h,w] <- keep of cell (y/4, x/4), times umask [B,1,h,w] when given.
+void blend_weights(Engine& e, const float* v, const float* A, const float* d, float* out, int L, cudaStream_t s);
+void local_blend_mask(Engine& e, const float* maps, int n_terms, int n_vec, float* run, const float* umask, float th_blend, float th_sub,
+                      float* mask, int B, int h, int w, cudaStream_t s);
 // image-resolution mask [B,1,H,W] -> [B,1,H/f,W/f]: mean of each f x f block, summed row by row then divided by f*f (avg_pool2d)
 void mask_pool(Engine& e, const float* mask, float* out, int B, int H, int W, int f, cudaStream_t s);
 // paste-back at image resolution: out = m*clamp((dec + 1)*0.5, 0, 1) + (1 - m)*image, mask [B,1,H,W] broadcast over C channels;

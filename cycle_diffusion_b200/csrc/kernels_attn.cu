@@ -794,11 +794,78 @@ __global__ void __launch_bounds__(PROBE_WARPS * 32) attn_probe_kernel(const Prob
       *o_ = accumulate ? __fadd_rn(*o_, acc[u]) : acc[u];
     }
 }
+// LocalBlend's weighted form of attn_probe_kernel, the same code with the span test replaced by the weights: entry i's softmax sum is
+// sum_j w[i, j] e_j, one fmaf per key in the same lane order (w_j in {0, 1} adds exactly what the span form adds).  A kernel of its
+// own, so that the span form's code is the one LEDITS++ measured and tested.
+template <int FMT>
+__global__ void __launch_bounds__(PROBE_WARPS * 32) attn_probe_weighted_kernel(const ProbeOperands o, const int* rows, const float* wts,
+                                                                                float* map, int N, int L, int heads, int d, float scale,
+                                                                                int accumulate) {
+  extern __shared__ float sm[];
+  const int dp = d + 1, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* sk = sm;                                  // [L][d + 1]
+  float* sq = sk + (size_t)L * dp + warp * d;      // [PROBE_WARPS][d]
+  float* ss = sk + (size_t)L * dp + PROBE_WARPS * d + warp * L;   // [PROBE_WARPS][L] logits
+  const int i = blockIdx.y, b = rows[i];
+  const float* wv = wts + (size_t)i * L;
+  const int p0 = (blockIdx.x * PROBE_WARPS + warp) * PROBE_QPW;
+  const float kscale = FMT == ProbeOperands::H16 ? exp2i(-h16_exp_of(*o.k_amax)) : 1.f;
+  float acc[PROBE_QPW] = {};
+  for (int h = 0; h < heads; ++h) {
+    __syncthreads();
+    for (int x = threadIdx.x; x < L * d; x += blockDim.x) {
+      const int j = x / d, c = x - j * d;
+      sk[j * dp + c] = probe_key<FMT>(o, ((size_t)b * o.Lk + j) * o.ldk + (size_t)h * d + c, kscale);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int u = 0; u < PROBE_QPW; ++u) {
+      const int p = p0 + u;
+      if (p >= N) continue;                      // (warp-uniform; no break, so acc stays in registers)
+      const size_t qi = ((size_t)b * N + p) * o.ldq + (size_t)h * d;
+      for (int c = lane; c < d; c += 32) sq[c] = FMT == ProbeOperands::TF32 ? o.q[qi + c] + o.q_lo[qi + c] : o.q[qi + c];
+      __syncwarp();
+      float mx = -INFINITY;
+      for (int j = lane; j < L; j += 32) {
+        const float* kr = sk + j * dp;
+        float dot = 0.f;
+        for (int c = 0; c < d; ++c) dot = fmaf(sq[c], kr[c], dot);
+        const float sj = __fmul_rn(scale, dot);
+        ss[j] = sj;
+        mx = fmaxf(mx, sj);
+      }
+      for (int m = 16; m; m >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, m));
+      float tot = 0.f, sp = 0.f;
+      for (int j = lane; j < L; j += 32) {
+        const float ej = expf(__fsub_rn(ss[j], mx));
+        tot = __fadd_rn(tot, ej);
+        sp = fmaf(wv[j], ej, sp);
+      }
+      // butterfly: every lane adds the same two partial sums at each level, so all lanes hold the same total
+      for (int m = 16; m; m >>= 1) {
+        tot = __fadd_rn(tot, __shfl_xor_sync(0xffffffffu, tot, m));
+        sp = __fadd_rn(sp, __shfl_xor_sync(0xffffffffu, sp, m));
+      }
+      const float ph = __fdiv_rn(sp, tot);
+      acc[u] = h ? __fadd_rn(acc[u], ph) : ph;
+      __syncwarp();
+    }
+  }
+  if (lane == 0)
+#pragma unroll
+    for (int u = 0; u < PROBE_QPW; ++u) {
+      const int p = p0 + u;
+      if (p >= N) continue;
+      float* o_ = map + (size_t)i * N + p;
+      *o_ = accumulate ? __fadd_rn(*o_, acc[u]) : acc[u];
+    }
+}
 }  // namespace
 
-void attn_probe(Engine& e, const ProbeOperands& o, const int* rows, const int* span, int n_rows, float* map, int N, int L, int heads, int d,
-                float scale, bool accumulate, cudaStream_t s) {
-  CDX_CHECK(rows && span && map && n_rows >= 1 && N >= 1 && L >= 1 && heads >= 1 && d >= 1 && o.q && o.k && o.Lk >= L,
+void attn_probe(Engine& e, const ProbeOperands& o, const int* rows, const int* span, const float* weights, int n_rows, float* map, int N, int L,
+                int heads, int d, float scale, bool accumulate, cudaStream_t s) {
+  CDX_CHECK(!span != !weights, "attn_probe: give spans or weights");
+  CDX_CHECK(rows && map && n_rows >= 1 && N >= 1 && L >= 1 && heads >= 1 && d >= 1 && o.q && o.k && o.Lk >= L,
             "attn_probe: %d rows, N=%d L=%d Lk=%d heads=%d d=%d", n_rows, N, L, o.Lk, heads, d);
   CDX_CHECK(o.fmt != ProbeOperands::H16 || o.k_amax, "attn_probe: fp16 K planes need their range slot");
   CDX_CHECK(o.fmt != ProbeOperands::TF32 || (o.q_lo && o.k_lo), "attn_probe: TF32 planes need both terms");
@@ -806,12 +873,18 @@ void attn_probe(Engine& e, const ProbeOperands& o, const int* rows, const int* s
   CDX_CHECK(smem <= 227 * 1024, "attn_probe: %d keys of width %d need %zu bytes of shared memory", L, d, smem);
   if (e.dry()) return;
   const dim3 grid((unsigned)((N + PROBE_WARPS * PROBE_QPW - 1) / (PROBE_WARPS * PROBE_QPW)), (unsigned)n_rows);
-  auto kernel = o.fmt == ProbeOperands::H16 ? attn_probe_kernel<ProbeOperands::H16>
-                : o.fmt == ProbeOperands::TF32 ? attn_probe_kernel<ProbeOperands::TF32> : attn_probe_kernel<ProbeOperands::F32>;
-  if (smem > 48 * 1024) CDX_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  auto launch = [&](auto kernel, const auto* sel) {
+    if (smem > 48 * 1024) CDX_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, PROBE_WARPS * 32, smem, s>>>(o, rows, sel, map, N, L, heads, d, scale, accumulate ? 1 : 0);
+  };
   ProfScope ps(e, s, PROF_SOFTMAX, 2.0 * n_rows * (double)N * L * heads * d, 4.0 * n_rows * ((double)N * heads * d + (double)L * heads * d), 1);
-  ps.note("attention probe %d rows x %d queries x %d keys, %d heads x %d", n_rows, N, L, heads, d);
-  kernel<<<grid, PROBE_WARPS * 32, smem, s>>>(o, rows, span, map, N, L, heads, d, scale, accumulate ? 1 : 0);
+  ps.note("attention probe %d %s x %d queries x %d keys, %d heads x %d", n_rows, weights ? "weighted rows" : "rows", N, L, heads, d);
+  if (weights)
+    launch(o.fmt == ProbeOperands::H16 ? attn_probe_weighted_kernel<ProbeOperands::H16>
+           : o.fmt == ProbeOperands::TF32 ? attn_probe_weighted_kernel<ProbeOperands::TF32> : attn_probe_weighted_kernel<ProbeOperands::F32>, weights);
+  else
+    launch(o.fmt == ProbeOperands::H16 ? attn_probe_kernel<ProbeOperands::H16>
+           : o.fmt == ProbeOperands::TF32 ? attn_probe_kernel<ProbeOperands::TF32> : attn_probe_kernel<ProbeOperands::F32>, span);
   CDX_CUDA(cudaGetLastError());
   e.launches++;
 }

@@ -1212,3 +1212,95 @@ void image_metrics(Engine& e, const float* a, const float* b, int B, int H, int 
   LAUNCH1(image_metrics_final_kernel, (size_t)B, acc, B, H, W, out);
 }
 }  // namespace cdx
+
+// ------------------------------------------------------------------------------------------------ Prompt-to-Prompt's LocalBlend
+namespace cdx {
+namespace {
+constexpr int BLEND_THREADS = 256;
+__global__ void blend_weights_kernel(const float* v, const float* A, const float* d, float* out, int L) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= L) return;
+  float r = 0.f;
+  if (A) {
+    for (int n = 0; n < L; ++n) r = fmaf(A[(size_t)q * L + n], v[n], r);
+  } else {
+    r = d ? __fmul_rn(d[q], v[q]) : v[q];
+  }
+  out[q] = r;
+}
+// one CTA per image: the running sums, their maxima, the grid mask in shared memory, then the latent mask
+__global__ void __launch_bounds__(BLEND_THREADS) local_blend_mask_kernel(const float* maps, int n_terms, int n_vec, float* run,
+                                                                         const float* umask, float th_blend, float th_sub, float* mask,
+                                                                         int gh, int gw) {
+  extern __shared__ unsigned char cell[];          // [gh*gw]: the grid mask
+  __shared__ float red[BLEND_THREADS];
+  __shared__ float mx[4];
+  const int b = blockIdx.x, G = gh * gw;
+  float* R = run + (size_t)b * n_vec * G;
+  for (int p = threadIdx.x; p < G; p += BLEND_THREADS)
+    for (int v = 0; v < n_vec; ++v) {
+      const float* m = maps + (size_t)(b * n_vec + v) * n_terms * G + p;
+      float wsum = m[0];
+      for (int t = 1; t < n_terms; ++t) wsum = __fadd_rn(wsum, m[(size_t)t * G]);
+      R[(size_t)v * G + p] = __fadd_rn(R[(size_t)v * G + p], wsum);
+    }
+  __syncthreads();
+  // the maximum of each running map (the 3x3 max-pool keeps it); the maps are >= 0
+  for (int v = 0; v < n_vec; ++v) {
+    float m = 0.f;
+    for (int p = threadIdx.x; p < G; p += BLEND_THREADS) m = fmaxf(m, R[(size_t)v * G + p]);
+    red[threadIdx.x] = m;
+    __syncthreads();
+    for (int o = BLEND_THREADS / 2; o > 0; o >>= 1) {
+      if (threadIdx.x < o) red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + o]);
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) mx[v] = red[0];
+    __syncthreads();
+  }
+  for (int p = threadIdx.x; p < G; p += BLEND_THREADS) {
+    const int y = p / gw, x = p - y * gw;
+    bool keep = false;
+    for (int v = 0; v < 2; ++v) {                  // blend words: pooled map / max > th_blend, source OR target
+      const float* r = R + (size_t)v * G;
+      float pm = r[p];
+      for (int yy = max(y - 1, 0); yy <= min(y + 1, gh - 1); ++yy)
+        for (int xx = max(x - 1, 0); xx <= min(x + 1, gw - 1); ++xx) pm = fmaxf(pm, r[yy * gw + xx]);
+      keep |= mx[v] > 0.f && __fdiv_rn(pm, mx[v]) > th_blend;
+    }
+    for (int v = 2; v < n_vec; ++v)                // subtract words: map / max > th_sub removes the cell
+      keep &= !(mx[v] > 0.f && __fdiv_rn(R[(size_t)v * G + p], mx[v]) > th_sub);
+    cell[p] = keep;
+  }
+  __syncthreads();
+  const int w = 4 * gw, hw = 16 * G;
+  for (int i = threadIdx.x; i < hw; i += BLEND_THREADS) {
+    const int y = i / w, x = i - y * w;
+    mask[(size_t)b * hw + i] = cell[(y >> 2) * gw + (x >> 2)] ? (umask ? umask[(size_t)b * hw + i] : 1.f) : 0.f;
+  }
+}
+}  // namespace
+
+void blend_weights(Engine& e, const float* v, const float* A, const float* d, float* out, int L, cudaStream_t s) {
+  CDX_CHECK(v && out && L >= 1 && !(A && d), "blend_weights: L=%d", L);
+  if (e.dry()) return;
+  blend_weights_kernel<<<cdiv(L, 128), 128, 0, s>>>(v, A, d, out, L);
+  CDX_CUDA(cudaGetLastError());
+  e.launches++;
+}
+
+void local_blend_mask(Engine& e, const float* maps, int n_terms, int n_vec, float* run, const float* umask, float th_blend, float th_sub,
+                      float* mask, int B, int h, int w, cudaStream_t s) {
+  CDX_CHECK(maps && run && mask && B >= 1 && h >= 4 && w >= 4 && h % 4 == 0 && w % 4 == 0 && n_terms >= 1 && (n_vec == 2 || n_vec == 4),
+            "local_blend_mask: B=%d %dx%d (multiples of 4) n_terms=%d n_vec=%d", B, h, w, n_terms, n_vec);
+  CDX_CHECK(th_blend >= 0.f && th_blend < 1.f && th_sub >= 0.f && th_sub < 1.f, "local_blend_mask: thresholds %g, %g outside [0, 1)", th_blend,
+            th_sub);
+  const int gh = h / 4, gw = w / 4;
+  CDX_CHECK((size_t)gh * gw <= 48 * 1024, "local_blend_mask: a %dx%d grid", gh, gw);
+  if (e.dry()) return;
+  ProfScope ps(e, s, PROF_ELEMENTWISE, 0.0, 4.0 * B * ((double)n_vec * gh * gw * (n_terms + 2) + (umask ? 2.0 : 1.0) * h * w), 1);
+  local_blend_mask_kernel<<<B, BLEND_THREADS, (size_t)gh * gw, s>>>(maps, n_terms, n_vec, run, umask, th_blend, th_sub, mask, gh, gw);
+  CDX_CUDA(cudaGetLastError());
+  e.launches++;
+}
+}  // namespace cdx

@@ -744,7 +744,7 @@ struct UNetExec : Exec {
   }
   // the probe of one layer: the first probed layer of the call stores the map, later ones add
   void probe_layer(const ProbeOperands& po, int HW, int heads, int d, float scale) {
-    attn_probe(e, po, probe->rows, probe->span, probe->n_rows, probe->map, HW, ctx_len, heads, d, scale, probed > 0, s);
+    attn_probe(e, po, probe->rows, probe->span, probe->weights, probe->n_rows, probe->map, HW, ctx_len, heads, d, scale, probed > 0, s);
     ++probed;
   }
   bool oai;
@@ -1330,9 +1330,9 @@ void unet_forward(Net& n, const float* x_nchw, const float* t_dev, const float* 
   CDX_CHECK(!ctl || (!!ctl->qk_row + !!ctl->kv_row + !!ctl->pnp_row) <= 1,
             "attention control: Prompt-to-Prompt, mutual self-attention and Plug-and-Play are exclusive in one call");
   ex.ctl = ctl;
-  CDX_CHECK(!probe || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0 && probe->rows && probe->span && probe->map &&
+  CDX_CHECK(!probe || (n.kind == NET_UNET_OPENAI && n.ucfg.context_dim > 0 && ctx_len > 0 && probe->rows && !probe->span != !probe->weights && probe->map &&
                        probe->n_rows >= 1 && probe->tokens >= 1),
-            "attention probe: SD / LDM U-Nets with a context, and a row list, spans and a map");
+            "attention probe: SD / LDM U-Nets with a context, and a row list, spans or weights and a map");
   ex.probe = probe;
   if (n.kind == NET_UNET_DDPM) { ex.forward_ddpm(x_nchw, t_dev, out_nchw, B, H, W); return; }
   ex.forward(x_nchw, t_dev, ctx, ctx_len, out_nchw, B, H, W);

@@ -120,10 +120,12 @@ struct AttnControl {
 // Cross-attention probe of one SD / LDM U-Net call (LEDITS++'s implicit masks, driven by the semantic-guidance loop in cabi.cu).  It
 // changes no output: the cross-attention of every SpatialTransformer in the input and output blocks (never the middle block) whose
 // token count is `tokens` also runs attn_probe on the operands its route multiplied, for the listed rows: the first such layer
-// stores map [n_rows, tokens], later ones add.  A call in which no layer matches is an error.
+// stores map [n_rows, tokens], later ones add.  A call in which no layer matches is an error.  LocalBlend's loop gives weights
+// instead of span: entry i's map is then sum_j weights[i, j] * softmax_j of row rows[i].
 struct AttnProbe {
   const int* rows = nullptr;            // device [n_rows]: U-Net rows
   const int* span = nullptr;            // device [n_rows]: tokens 1..span[i] of row i's context
+  const float* weights = nullptr;       // device [n_rows, L], exclusive with span
   int n_rows = 0;
   float* map = nullptr;                 // device [n_rows, tokens]
   int tokens = 0;

@@ -12,7 +12,7 @@ import torch
 
 from . import _cabi
 from ._cabi import lib, check, UnetConfig, VaeConfig, TextConfig, DdimCoef, PixelCoef
-from .attn_control import MutualSelfControl, PnPControl
+from .attn_control import LocalBlend, MutualSelfControl, PnPControl
 from .schedule import EditFriendlySchedule
 from .semantic import SemanticGuidance
 
@@ -147,6 +147,18 @@ class Engine:
         B, _, H, W = mask.shape
         out = self.empty(B, 1, H // f, W // f)
         check(lib.cdx_mask_pool(self.h, _ptr(mask), _ptr(out), B, H, W, int(f), self.stream))
+        return out
+
+    def op_local_blend_mask(self, maps, n_terms, n_vec, run, h, w, th_blend, th_sub, user_mask=None):
+        """LocalBlend's mask stage alone (cdx_local_blend_mask): maps [B*n_vec*n_terms, (h/4)(w/4)] of one step are added into the
+        running sums run [B*n_vec, (h/4)(w/4)] (updated in place) -> the latent mask [B,1,h,w] (times user_mask [B,1,h,w] when given)."""
+        B = run.shape[0] // n_vec
+        for name, t in (('maps', maps), ('run', run), ('user_mask', user_mask)):
+            assert t is None or (torch.is_tensor(t) and t.dtype == torch.float32 and t.device == self.device and t.is_contiguous()), \
+                f'op_local_blend_mask: {name} must be a contiguous float32 tensor on {self.device}'
+        out = self.empty(B, 1, h, w)
+        check(lib.cdx_local_blend_mask(self.h, _ptr(maps), int(n_terms), int(n_vec), _ptr(run), _ptr(user_mask), float(th_blend), float(th_sub),
+                                       _ptr(out), B, h, w, self.stream))
         return out
 
     def mask_composite(self, dec, image, mask):
@@ -519,14 +531,17 @@ class Engine:
     ATTN_ROUTES = ('generic', 'unfused_tc', 'fused_h16', 'fused_tf32', 'fused_one')
 
     def op_attention_net(self, kind, out, B, N, heads, d, scale, qkv=None, q=None, kv=None, k=None, v=None, L=0, ctx_lp=0, causal=False,
-                         qk_rows=None, kv_rows=None, acc_rows=None, slot=0.0, q_slot=0.0, probe_rows=None, probe_spans=None, probe_map=None):
+                         qk_rows=None, kv_rows=None, acc_rows=None, slot=0.0, q_slot=0.0, probe_rows=None, probe_spans=None, probe_map=None,
+                         probe_weights=None):
         """One attention with its operands prepared as the network executors prepare them (cdx_op_attention_net in include/cdx.h,
         whose descriptor fields are the arguments).  kind: 'self' (qkv [B*N, 3C], one range slot), 'cross' (q [B*N, C], kv
         [B*ctx_lp, 2C] the padded context's K | V) or 'generic' (q, k, v; optional causal mask).  Every buffer is a float32 tensor on
         this engine's device passed as it is; out [B*N, C] (a view inside a larger buffer is fine) is written, or added to for the
         images of acc_rows.  slot / q_slot > 0 replace the measured range slots.  Returns the plan: dict(route, qrows, rag, ksplit,
         ring, Nks, Nvs).  probe_rows / probe_spans (host int lists) with probe_map [n_probe, N] (kind 'cross'): LEDITS++'s probe on
-        the operands the route multiplied, map[i] <- sum over heads of the softmax over tokens 1..probe_spans[i] of image probe_rows[i]."""
+        the operands the route multiplied, map[i] <- sum over heads of the softmax over tokens 1..probe_spans[i] of image probe_rows[i].
+        probe_weights (host float tensor [n_probe, L], instead of probe_spans): LocalBlend's weighted probe (cdx_op_attention_net_weighted),
+        map[i] <- sum over heads of sum over j of probe_weights[i, j] * softmax_j of image probe_rows[i]."""
         kinds = ('self', 'cross', 'generic')
         assert kind in kinds, kind
         for name, t in (('out', out), ('qkv', qkv), ('q', q), ('kv', kv), ('k', k), ('v', v), ('probe_map', probe_map)):
@@ -538,13 +553,22 @@ class Engine:
                                       B=B, N=N, L=L, ctx_lp=ctx_lp, heads=heads, d=d, scale=scale, qk_rows=rows(qk_rows), kv_rows=rows(kv_rows),
                                       acc_rows=rows(acc_rows), n_acc=len(acc_rows) if acc_rows is not None else 0, slot=slot, q_slot=q_slot,
                                       out=ptr(out))
+        wts = None
         if probe_rows is not None:
-            assert probe_spans is not None and len(probe_spans) == len(probe_rows) and probe_map is not None
+            assert (probe_spans is None) != (probe_weights is None) and probe_map is not None
+            assert probe_spans is None or len(probe_spans) == len(probe_rows)
             assert probe_map.is_contiguous() and probe_map.numel() >= len(probe_rows) * N, 'op_attention_net: probe_map [n_probe, N]'
             desc.probe_rows, desc.probe_spans, desc.n_probe = rows(probe_rows), rows(probe_spans), len(probe_rows)
             desc.probe_map = ptr(probe_map)
+            if probe_weights is not None:
+                w = torch.as_tensor(probe_weights, dtype=torch.float32).cpu().contiguous()
+                assert tuple(w.shape) == (len(probe_rows), L), f'op_attention_net: probe_weights [{len(probe_rows)}, {L}]'
+                wts = (C.c_float * w.numel()).from_buffer_copy(w.numpy().tobytes())
         plan = (C.c_int * 7)()
-        check(lib.cdx_op_attention_net(self.h, C.byref(desc), plan, self.stream))
+        if wts is not None:
+            check(lib.cdx_op_attention_net_weighted(self.h, C.byref(desc), wts, plan, self.stream))
+        else:
+            check(lib.cdx_op_attention_net(self.h, C.byref(desc), plan, self.stream))
         return dict(zip(('route', 'qrows', 'rag', 'ksplit', 'ring', 'Nks', 'Nvs'), [self.ATTN_ROUTES[plan[0]]] + list(plan[1:])))
 
     def op_nchw_to_nhwc(self, x):
@@ -813,7 +837,7 @@ class UNet(Net):
         return out
 
     def cycle_lockstep(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z=False, mask=None, attn_control=None,
-                       semantic=None, c_edit=None):
+                       semantic=None, c_edit=None, local_blend=None):
         """Both chains in one loop (one U-Net call + one fused elementwise kernel per step, no z buffer unless asked for):
         x0 [B,C,h,w] -> translated latent [B,C,h,w] (and z [B, n+1, C,h,w] when return_z).  noise as for latent_encode with
         n_rec == sched.refine_steps.  mask [B,1,h,w] in [0,1] (1 = may change): masked editing (cdx_cycle_lockstep_masked), the
@@ -829,7 +853,11 @@ class UNet(Net):
         ValueError.
         sched: a schedule.DDIMSchedule runs the DPM-Encoder chain above; a schedule.EditFriendlySchedule runs LEDITS++'s edit-friendly
         inversion instead (independent draws of the source's x, stepped by the eta = 1 DDIM step or the SDE-DPM-Solver++ step), with
-        every control above, through cdx_cycle_lockstep_sampler."""
+        every control above, through cdx_cycle_lockstep_sampler.
+        local_blend: an attn_control.LocalBlend, Prompt-to-Prompt's LocalBlend (cdx_cycle_lockstep_blend): from step
+        int(start_blend * n) on the target chain is kept to where the blend words' cross-attention points, under either schedule.  It
+        composes with mask and with an AttentionControl (replace, reweight, refine) or none; with semantic, MutualSelfControl or
+        PnPControl it raises ValueError."""
         e = self.engine
         x0, c_src, c_tgt, noise = (_f32c(t, e.device) for t in (x0, c_src, c_tgt, noise))
         uc = _f32c(uc, e.device) if uc is not None else None
@@ -838,6 +866,9 @@ class UNet(Net):
         assert noise.shape == (n + 1, B, Cc, h, w), f'noise shape {tuple(noise.shape)}'
         assert c_src.shape == c_tgt.shape
         mask = check_mask(mask, (B, 1, h, w), e.device) if mask is not None else None
+        if local_blend is not None:
+            return self._cycle_blend(x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z, mask, attn_control, semantic,
+                                     local_blend)
         if isinstance(sched, EditFriendlySchedule):
             return self._cycle_sampler(x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z, mask, attn_control, semantic,
                                        c_edit)
@@ -921,6 +952,32 @@ class UNet(Net):
                                              sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out),
                                              _ptr(z), B, Cc, h, w, e.stream, C.byref(sp), _ptr(mask), ref(ctl), _ptr(own), ref(mutual),
                                              ref(pnp), _ptr(c_edit), ref(sg), ref(am)))
+        return (out, z) if return_z else out
+
+    def _cycle_blend(self, x0, c_src, c_tgt, uc, src_scale, tgt_scale, sched, noise, return_z, mask, attn_control, semantic, local_blend):
+        """cycle_lockstep under a LocalBlend: cdx_cycle_lockstep_blend, with the sampler of an EditFriendlySchedule or none"""
+        if not isinstance(local_blend, LocalBlend):
+            raise ValueError(f'local_blend: expected an attn_control.LocalBlend, got {type(local_blend)}')
+        if semantic is not None or isinstance(attn_control, (MutualSelfControl, PnPControl)):
+            raise ValueError('LocalBlend runs with Prompt-to-Prompt edits (replace, reweight, refine) or none, not with semantic guidance, '
+                             'MasaCtrl or Plug-and-Play')
+        e = self.engine
+        B, Cc, h, w = x0.shape
+        n, L = sched.refine_steps, c_src.shape[1]
+        if h % 4 or w % 4:
+            raise ValueError(f'LocalBlend: the latent sides must be multiples of 4, got {h}x{w}')
+        sp, _keep = sched.sampler_struct() if isinstance(sched, EditFriendlySchedule) else (None, None)
+        ctl = own = None
+        if attn_control is not None:
+            ctl, _token_map, own = attn_control.c_struct(n, B, L, e.device)
+        lb, _vecs = local_blend.c_struct(n, B, L, e.device)
+        out = e.empty(B, Cc, h, w)
+        z = e.empty(B, n + 1, Cc, h, w) if return_z else None
+        ref = lambda s: C.byref(s) if s is not None else None
+        check(lib.cdx_cycle_lockstep_blend(self.h, _ptr(x0), _ptr(c_src), _ptr(c_tgt), _ptr(uc), L, float(src_scale), float(tgt_scale),
+                                           sched.coef_array(), sched.t_array(), n, _ptr(noise), sched.sqrt_a_T, sched.sqrt_1ma_T, _ptr(out),
+                                           _ptr(z), B, Cc, h, w, e.stream, ref(sp), _ptr(mask), ref(ctl), _ptr(own), None, None, None, None,
+                                           None, C.byref(lb)))
         return (out, z) if return_z else out
 
     def cycle_fan(self, x0, c_src, c_tgt, uc, src_scales, tgt_scales, sched, noise, return_z=False, mask=None):

@@ -14,7 +14,7 @@ from dataclasses import dataclass
 
 import torch
 
-from .attn_control import AttentionControl, MutualSelfControl, PnPControl
+from .attn_control import AttentionControl, LocalBlend, MutualSelfControl, PnPControl, resolve_local_blend
 from .engine import check_mask
 from .schedule import DDIMSchedule, EditFriendlySchedule
 from .semantic import SemanticGuidance
@@ -106,6 +106,11 @@ class CycleDiffusionPipeline:
         if not kw or 'edit_type' not in kw:
             return None
         kind = kw['edit_type']
+        if kind in ('replace', 'reweight', 'refine') and 'local_blend' in kw:       # CycleDiffusionPipeline._local_blend's key
+            if not isinstance(kw['local_blend'], (LocalBlend, dict)):
+                raise ValueError(f"cross_attention_kwargs: local_blend must be an attn_control.LocalBlend or a dict of words, got "
+                                 f"{type(kw['local_blend'])}")
+            kw = {k: v for k, v in kw.items() if k != 'local_blend'}
         if kind == 'mutual_self':
             extra = set(kw) - cls.MUTUAL_KEYS
             if extra:
@@ -133,7 +138,7 @@ class CycleDiffusionPipeline:
             raise ValueError(f"edit_type must be 'replace', 'reweight', 'refine', 'mutual_self' or 'pnp', got {kind!r}")
         extra = set(kw) - cls.P2P_KEYS
         if extra:
-            raise ValueError(f'cross_attention_kwargs: unsupported keys {sorted(extra)} (LocalBlend: use mask_image)')
+            raise ValueError(f'cross_attention_kwargs: unsupported keys {sorted(extra)}')
         for key in ('cross_replace_steps', 'self_replace_steps'):
             if key not in kw:
                 raise ValueError(f'cross_attention_kwargs: {key} is required with edit_type')
@@ -169,6 +174,24 @@ class CycleDiffusionPipeline:
         except ValueError as err:
             raise ValueError(f'cross_attention_kwargs: {err}') from None
 
+    @staticmethod
+    def _local_blend(kw, source_guidance_scale, guidance_scale, two_phase, editing_prompt):
+        """cross_attention_kwargs['local_blend'] as given (a LocalBlend or a dict of words, resolved once the prompts are known), or
+        None; ValueError where LocalBlend cannot run.  Without an edit_type the dict may hold nothing else."""
+        if not kw or 'local_blend' not in kw:
+            return None
+        if 'edit_type' not in kw and set(kw) != {'local_blend'}:
+            raise ValueError(f"cross_attention_kwargs: keys {sorted(set(kw) - {'local_blend'})} need an edit_type")
+        if two_phase:
+            raise ValueError('LocalBlend needs the lock-step loop: it blends the target chain with the source chain (two_phase=False)')
+        if editing_prompt is not None:
+            raise ValueError('LocalBlend does not combine with semantic guidance (editing_prompt) in one loop')
+        if source_guidance_scale == 0:
+            raise ValueError('LocalBlend needs the source prompt: source_guidance_scale 0 runs no source-prompt row')
+        if guidance_scale == 0:
+            raise ValueError('LocalBlend needs the target prompt: guidance_scale 0 runs no target-prompt row')
+        return kw['local_blend']
+
     def _token_counts(self, concepts, given):
         """LEDITS++'s token span per concept: the caller's edit_token_counts, or the conditioning model's count capped at L - 2."""
         if given is not None:
@@ -202,8 +225,18 @@ class CycleDiffusionPipeline:
         diag(equalizer) (attn_control.replace_token_map builds token_map from two prompts' token ids).  'refine' needs a
         token_map (attn_control.refine_token_map aligns two prompts' token ids) whose column sums lie in [0, 1]: target token j
         takes P_src . A[:, j] and keeps (1 - colsum_j) . eq_j of its own map, so a word the source prompt lacks attends on its own.
-        two_phase=True and a source_guidance_scale of 0 raise ValueError; LocalBlend is mask_image's job.  A dict without
-        'edit_type' is ignored.
+        two_phase=True and a source_guidance_scale of 0 raise ValueError.
+        'local_blend' (with these edit types, or alone): Prompt-to-Prompt's LocalBlend, an attn_control.LocalBlend or
+        {'words': (source_words, target_words), ['subtract_words': (source_words, target_words)], ['start_blend': 0.2],
+        ['threshold': (0.3, 0.3)]}, the words (a word or a tuple of words, for every image) turned into per-token weights by the
+        conditioning model's word_token_weights.  From step int(start_blend * n) of the loop's n steps on, the target chain keeps
+        its own latent only where the blend words' cross-attention, summed over the 1/4-resolution layers and every step so far,
+        is above threshold[0] of its maximum (after a 3x3 max-pool) in the source or the target prompt, and not above threshold[1]
+        for a subtract word; elsewhere it takes the source chain's.  Unlike mask_image, which is fixed for the loop, the mask is
+        recomputed at every step and follows the object; with mask_image the two multiply, and paste_back still pastes outside
+        mask_image.  It composes with every inversion and precision='autocast'; with edit_type 'mutual_self' or 'pnp',
+        editing_prompt, two_phase=True, a source_guidance_scale or guidance_scale of 0, or latent sides that are not multiples of 4
+        it raises ValueError.  Any other dict without 'edit_type' is ignored.
         {'edit_type': 'mutual_self', ['start_step': 4], ['start_layer': 10]}: MasaCtrl's mutual self-attention (Cao et al., 2023)
         instead, for non-rigid edits (a pose or a layout change): from loop step start_step on, in the SpatialTransformers from
         index start_layer on (16 in SD v1 / 2.x; the defaults control the decoder's two finest levels), the target rows keep their
@@ -251,6 +284,7 @@ class CycleDiffusionPipeline:
             if two_phase:
                 raise ValueError(f'inversion={inversion!r} runs in the lock-step loop only (two_phase=False)')
         attn_control = self._attn_control(cross_attention_kwargs, source_guidance_scale, two_phase)
+        blend_spec = self._local_blend(cross_attention_kwargs, source_guidance_scale, guidance_scale, two_phase, editing_prompt)
         semantic, concepts = None, None
         if editing_prompt is not None:
             concepts = [editing_prompt] if isinstance(editing_prompt, str) else list(editing_prompt)
@@ -300,6 +334,7 @@ class CycleDiffusionPipeline:
             sources = [p for p in sources for _ in range(num_images_per_prompt)]
         if len(prompts) == 1 and B > 1:
             prompts, sources = prompts * B, sources * B
+        local_blend = resolve_local_blend(blend_spec, g.cond_stage, sources, prompts) if blend_spec is not None else None
         with e.precision(self.precision):
             rnd = lambda shape: torch.randn(shape, generator=generator)
             c_tgt = prompt_embeds if prompt_embeds is not None else g.get_learned_conditioning(prompts)
@@ -326,7 +361,7 @@ class CycleDiffusionPipeline:
             else:
                 mask = e.mask_pool(mask_image, g.vae.down) if mask_image is not None else None
                 latents = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, source_guidance_scale, guidance_scale, sched, noise, mask=mask,
-                                                attn_control=attn_control, semantic=semantic, c_edit=c_edit)
+                                                attn_control=attn_control, semantic=semantic, c_edit=c_edit, local_blend=local_blend)
             if callback is not None:
                 callback(n_rec - 1, sched.t_loop[-1], latents)
             if paste_back:

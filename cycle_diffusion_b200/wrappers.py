@@ -26,6 +26,7 @@ import numpy as np
 import torch
 
 from . import specs
+from .attn_control import resolve_local_blend
 from .engine import Engine, UNet, VAE, check_mask
 from .ensemble import EnsemblePlan, MemberNoise
 from .schedule import DDIMSchedule, PixelSchedule, same_schedule
@@ -72,6 +73,21 @@ class ClipTextCondStage:
             end = next((j for j in range(1, len(row)) if row[j] == self.END_ID), len(row))
             out.append(end - 1)
         return out
+
+    def word_token_weights(self, texts, words):
+        """LocalBlend's per-token weights of `words` in each text (attn_control.word_token_weights over the tokenizer's ids):
+        words is a word, a tuple of words for every text, or one tuple per text; a word is the token run the tokenizer gives it
+        alone (between its start and end tokens).  -> float32 [B, L]; ValueError when a word is not in its text."""
+        from .attn_control import word_lists, words_weights
+        per_text = word_lists(texts, words)
+        ids = self.tokenizer(list(texts))
+        runs = {w: self._word_run(w) for ws in per_text for w in ws}
+        return words_weights(ids.tolist(), [[runs[w] for w in ws] for ws in per_text], ids.shape[1])
+
+    def _word_run(self, word):
+        row = self.tokenizer([word])[0].tolist()
+        end = next((j for j in range(1, len(row)) if row[j] == self.END_ID), len(row))
+        return row[1:end]
 
 
 class BertTextCondStage(ClipTextCondStage):
@@ -122,6 +138,13 @@ class SyntheticTextEncoder:
     def token_counts(self, texts):
         """The whitespace word count of each text (the stand-in has no tokenizer)."""
         return [len(t.split()) for t in texts]
+
+    def word_token_weights(self, texts, words):
+        """LocalBlend's per-token weights of `words` in each text, whitespace word k being token k + 1 (after the start token), as
+        token_counts counts them; a word of several whitespace words is their run.  -> float32 [B, n_tokens]."""
+        from .attn_control import word_lists, words_weights
+        per_text = word_lists(texts, words)
+        return words_weights([['<start>'] + t.split() for t in texts], [[w.split() for w in ws] for ws in per_text], self.n_tokens)
 
 
 def _load_sd(state_dict, ckpt_default, synth_params, seed):
@@ -391,7 +414,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         sched = DDIMSchedule(self.custom_steps, self.eta, self.skip_steps[0], self.generator.alphas_cumprod)
         return self.white_box_steps != -1 and self.white_box_steps - self.skip_steps[0] - 1 >= sched.refine_steps
 
-    def cycle(self, image, encode_text, decode_text, mask=None, attn_control=None):
+    def cycle(self, image, encode_text, decode_text, mask=None, attn_control=None, local_blend=None):
         """encode(image, encode_text) followed by forward(z, image, encode_text, decode_text) for a single-member ensemble, on the
         engine's lock-step driver (cdx_cycle_lockstep): both chains advance together, one U-Net call per step on the batch
         [source | target uncond | target cond], and the noise recovered at a step is consumed by the target chain at once -- the
@@ -403,10 +426,14 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         outside it the translated latent stays on the source image's chain (cdx_cycle_lockstep_masked).
         attn_control: optional attn_control.AttentionControl, Prompt-to-Prompt's "replace" edit, or its "refine" edit when the
         control has an own_weight; attn_control.MutualSelfControl, MasaCtrl's mutual self-attention; or attn_control.PnPControl,
-        Plug-and-Play's feature and self-attention injection (UNet.cycle_lockstep)."""
+        Plug-and-Play's feature and self-attention injection (UNet.cycle_lockstep).
+        local_blend: optional attn_control.LocalBlend, or a dict {'words': (source_words, target_words), ...}
+        (attn_control.resolve_local_blend, through the conditioning model): Prompt-to-Prompt's LocalBlend on the target chain."""
         assert self.single_member(), 'cycle(): single-member ensembles only (use encode() + forward())'
+        if local_blend is not None:
+            local_blend = resolve_local_blend(local_blend, self.generator.cond_stage, encode_text, decode_text)
         with self._precision_scope():
-            return self._cycle(image, encode_text, decode_text, mask, attn_control)
+            return self._cycle(image, encode_text, decode_text, mask, attn_control, local_blend)
 
     def _latent_mask(self, mask, bsz):
         """Image-resolution mask [B,1,R,R] -> the latent grid (mean over the first stage's f x f blocks), or None."""
@@ -416,7 +443,7 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         mask = check_mask(mask, (bsz, 1, R, R), self.engine.device)
         return self.engine.mask_pool(mask, self.generator.vae.down)
 
-    def _cycle(self, image, encode_text, decode_text, mask=None, attn_control=None):
+    def _cycle(self, image, encode_text, decode_text, mask=None, attn_control=None, local_blend=None):
         g, e = self.generator, self.engine
         bsz = image.shape[0]
         m = self._latent_mask(mask, bsz)                  # checked before the first random draw
@@ -427,7 +454,8 @@ class _StochasticTextWrapperBase(torch.nn.Module):
         sched = DDIMSchedule(self.custom_steps, self.eta, self.skip_steps[0], g.alphas_cumprod)
         noise = self._encode_noise(sched, sched.refine_steps, x0.shape)
         sample = g.unet.cycle_lockstep(x0, c_src, c_tgt, uc, self.encoder_unconditional_guidance_scales[0],
-                                       self.decoder_unconditional_guidance_scales[0], sched, noise, mask=m, attn_control=attn_control)
+                                       self.decoder_unconditional_guidance_scales[0], sched, noise, mask=m, attn_control=attn_control,
+                                       local_blend=local_blend)
         return e.shift_scale(g.decode_first_stage(sample), 1.0, 0.5)
 
     def forward(self, z_ensemble, original_img, encode_text, decode_text):

@@ -501,6 +501,45 @@ int cdx_cycle_lockstep_sampler(cdx_net* unet, const float* x0, const float* c_sr
                                void* stream, const cdx_sampler* sampler, const float* mask, const cdx_attn_control* ctl,
                                const float* own_weight, const cdx_mutual_control* mutual, const cdx_pnp_control* pnp,
                                const float* c_edit, const cdx_semantic_guidance* sg, const cdx_semantic_attn_mask* am);
+/* Prompt-to-Prompt's LocalBlend (Hertz et al., 2022; its AttentionStore and LocalBlend.get_mask) on the lock-step loop of
+ * cdx_cycle_lockstep_sampler (same arguments; sampler may be NULL, the DPM-Encoder chain; mutual, pnp, c_edit, sg and am must be
+ * NULL): at each loop step the target chain is kept to where the blend words' cross-attention points.  K = 1: one source and one
+ * target chain per image b.  The cond rows of both chains are probed (the attention probe of cdx_cycle_lockstep_semantic_attn, same
+ * layers) with per-token weights, each map as the row attended with it:
+ *   W_src,v(p) = sum over layers, heads, j of P_src(p, j) v_src[b, j]                       (v: alpha or sub, source prompt)
+ *   W_tgt,v(p) = the same of P_src with weights A_b v_tgt[b]  (+ P_tgt with own_weight[b] * v_tgt[b] under refine)
+ *                at steps i < ctl->cross_steps (A_b = ctl->token_map, identity when NULL), else of P_tgt with v_tgt[b]
+ * and R_v += W_v from the loop's first step on.  On the (h/4) x (w/4) grid, per image:
+ *   blend = OR over src, tgt of  maxpool3x3(R_alpha) / max(R_alpha) > th_blend      (stride 1, padding never wins)
+ *   sub   = OR over src, tgt of  R_sub / max(R_sub) > th_sub                          (only with the subtract pair)
+ *   m     = blend AND NOT sub, nearest x4 to h x w, times mask when given               (a map whose max is 0 adds nothing)
+ * At steps i >= start_step the target's x_{t-1} is blended with the source's under m (cdx_cycle_lockstep_masked's blend); before,
+ * the loop runs exactly as without LocalBlend.  Weight vectors: device [B, ctx_len], finite and >= 0 (not checked here).  One probe
+ * launch per probed layer and one mask launch per step.  CDX_E_INVALID: a NULL blend or alpha vector, one subtract vector without
+ * the other, start_step outside 0..n_steps, thresholds outside [0, 1), h or w not a multiple of 4, a source or target chain at
+ * scale 0 with uc (no prompt row), and every control other than ctl / own_weight. */
+typedef struct cdx_local_blend {
+  const float* alpha_src;   /* device [B, ctx_len]: blend-word weights on the source prompt's tokens (P2P's alpha_layers) */
+  const float* alpha_tgt;   /* device [B, ctx_len]: on the target prompt's tokens */
+  const float* sub_src;     /* optional device [B, ctx_len]: subtract-word weights (P2P's substruct_layers), both or neither */
+  const float* sub_tgt;
+  int start_step;           /* loop steps i >= start_step blend: int(start_blend * n_steps) */
+  float th_blend, th_sub;   /* in [0, 1) */
+} cdx_local_blend;
+int cdx_cycle_lockstep_blend(cdx_net* unet, const float* x0, const float* c_src, const float* c_tgt, const float* uc,
+                             int ctx_len, float src_scale, float tgt_scale, const cdx_ddim_coef* coef,
+                             const float* t_host, int n_steps, const float* noise, float sqrt_a_T,
+                             float sqrt_1ma_T, float* x_out, float* z_out, int B, int C, int h, int w,
+                             void* stream, const cdx_sampler* sampler, const float* mask, const cdx_attn_control* ctl,
+                             const float* own_weight, const cdx_mutual_control* mutual, const cdx_pnp_control* pnp,
+                             const float* c_edit, const cdx_semantic_guidance* sg, const cdx_semantic_attn_mask* am,
+                             const cdx_local_blend* blend);
+/* LocalBlend's mask stage alone (one launch): maps device [B*n_vec*n_terms, (h/4)(w/4)], entry (b*n_vec + v)*n_terms + t, vectors
+ * v = 0, 1 the blend words of the source and target prompt, 2, 3 (n_vec == 4) the subtract words; run device [B*n_vec, (h/4)(w/4)]
+ * += (term 0 + term 1 + ...) in fp32; mask_out device [B,1,h,w] <- cdx_cycle_lockstep_blend's m from run (times user_mask
+ * [B,1,h,w] when given). */
+int cdx_local_blend_mask(cdx_engine* e, const float* maps, int n_terms, int n_vec, float* run, const float* user_mask, float th_blend,
+                         float th_sub, float* mask_out, int B, int h, int w, void* stream);
 /* Helpers of masked editing (image resolution, one [B,1,H,W] mask broadcast over the channels):
  * cdx_mask_pool: mask [B,1,H,W] -> out [B,1,H/f,W/f], the mean of each f x f block (f = the first stage's factor: 8 for KL-f8,
  *   4 for VQ-f4), summed row by row then divided by f*f as torch.nn.functional.avg_pool2d(mask, f) does.  H, W multiples of f.
@@ -692,6 +731,10 @@ typedef struct cdx_attention_net_desc {
   float* probe_map;
 } cdx_attention_net_desc;
 int cdx_op_attention_net(cdx_engine* e, const cdx_attention_net_desc* desc, int* plan_out, void* stream);
+/* cdx_op_attention_net with LocalBlend's weighted probe (cdx_cycle_lockstep_blend): probe_spans must be NULL and probe_weights (host
+ * [n_probe, L], finite) gives probe_map[i] <- sum over heads of sum over j of probe_weights[i, j] softmax_j of image probe_rows[i]. */
+int cdx_op_attention_net_weighted(cdx_engine* e, const cdx_attention_net_desc* desc, const float* probe_weights, int* plan_out,
+                                  void* stream);
 int cdx_op_nchw_to_nhwc(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 int cdx_op_nhwc_to_nchw(cdx_engine* e, const float* x, float* y, int B, int C, int HW, void* stream);
 /* The normalisation kernels in the forms the network executors call them, with their side outputs (tests/test_norms_gpu.py).
